@@ -1,14 +1,15 @@
 #!/usr/bin/env python
 """bench.py -- SdBG-construction hot path (count -> seq2sdbg) on synthetic 150 bp reads, k=27.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 One "step" = one pass of the hot path over one batch of reads: canonical (k+1)-mer edge extraction, LSD
 radix sort, solid-edge counting + mercy bookkeeping, then seq2sdbg item extraction, radix sort and SdBG
 emission from the device-resident solid edges.  `value` is whole-job edges/s with the read library already
 in HBM; `e2e` is the same metric through the host-buffer C ABI (mhb_build_host: count -> device mercy edges -> seq2sdbg), H2D/D2H
 inside the timed region.  `--impl reference` times the unmodified reference's OpenMP path
-(oracle/_ref/megahit_core_ref count + seq2sdbg) on the host cores on a bounded sample.
+(oracle/_ref/megahit_core_ref count + seq2sdbg) on the host cores on a bounded sample.  `--dump-outputs DIR` writes what
+the last timed step computed as DIR/<name>.npy (see dump_outputs), so that two builds can be compared on the same inputs.
 """
 from __future__ import annotations
 
@@ -33,28 +34,12 @@ GENOME_PER_READ = 5  # 5 Mb of genome per 1 M reads ~ 30x coverage (SURVEY.md 8d
 ERR = 0.01
 
 
-def ncu_traffic(n_reads: int, k: int):
-    """DRAM bytes (read + write) of one launch of the dominant kernel from a committed `ncu --set full` capture of this
-    same workload (profiles/radix_traffic.json, written by scripts/ncu_traffic.py); None when no capture matches."""
-    p = os.path.join(ROOT, "profiles", "radix_traffic.json")
-    if not os.path.exists(p):
-        return None, None
-    try:
-        j = json.load(open(p))
-        for e in j.get("captures", []):
-            if e.get("reads") == n_reads and e.get("k") == k:
-                return float(e["dram_bytes_per_launch"]), e.get("source")
-    except Exception:
-        pass
-    return None, None
-
-
 def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         j = json.load(open(p))
         return float(j["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
 class ClockSampler:
@@ -194,6 +179,36 @@ def bind_to_gpu_numa(local: int):
     return "unbound"
 
 
+DUMP_SAMPLE = 1 << 20  # SdBG stream bytes and about this many edge words sampled by --dump-outputs
+
+
+def dump_outputs(d, plan, s2s, n_edges_out):
+    """Writes what the timed path handed back in its last step as float64 / float32 .npy files under d (every value is
+    an integer the float holds exactly; about 23 MB in all at k = 27): the SdBG bucket table {byte offset, items, tips, large
+    multiplicities} and totals, the multiplicity histogram of the count stage (`.counting`), a seeded sample of the SdBG
+    item stream with its byte positions, and the solid + mercy edges whose content hashes into a fixed range, sorted
+    (the device writes the edges in no fixed order, so a sample by position would not be comparable)."""
+    import torch
+    os.makedirs(d, exist_ok=True)
+    totals = s2s.totals.cpu().numpy()
+    n_bytes = int(totals[0])
+    pos = np.unique(np.random.default_rng(0).integers(0, max(1, n_bytes), size=DUMP_SAMPLE if n_bytes else 0))
+    vals = s2s.bytes[torch.from_numpy(pos).to(s2s.bytes.device)].cpu().numpy()
+    WE = plan.WE
+    e = plan.edges[: n_edges_out * WE].view(-1, WE).to(torch.int64) & 0xFFFFFFFF
+    h = torch.zeros(len(e), dtype=torch.int64, device=e.device)
+    for j in range(WE):
+        h = (h * 0x9E3779B1 + e[:, j]) & 0xFFFFFFFF
+    keep = h < int((1 << 32) * min(1.0, DUMP_SAMPLE / max(1, n_edges_out * WE)))
+    edges = e[keep].cpu().numpy()
+    edges = edges[np.lexsort(edges.T[::-1])] if len(edges) else edges.reshape(0, WE)
+    out = {"sdbg_bucket_table": s2s.table.view(-1, 4).cpu().numpy(), "sdbg_totals": totals,
+           "counting_hist": plan.mul_hist.cpu().numpy(), "sdbg_bytes_sample_pos": pos,
+           "sdbg_bytes_sample": vals.astype(np.float32), "edges_sample": edges}
+    for name, a in out.items():
+        np.save(os.path.join(d, name + ".npy"), a if a.dtype == np.float32 else a.astype(np.float64))
+
+
 # ------------------------------------------------------------------------------------------------
 # our arm
 # ------------------------------------------------------------------------------------------------
@@ -233,6 +248,7 @@ def ours(args):
     s2s = dev.S2sPlan(int((n_solid + n_mercy0) * 1.05) + 1024, k + 1, k, device)
 
     mercy_ev = []
+    last = {}
 
     def step(timed=False):
         # count (extract, partition/sort, solid edges, mercy marks) -> mercy edges -> seq2sdbg over solid + mercy edges:
@@ -244,6 +260,7 @@ def ours(args):
             e.record()
             mercy_ev.append(e)
         s2s.run(plan.edges, None, ns + nm, plan.WE, timed=timed, aux=plan.aux, n_aux=ns)
+        last["n_edges_out"] = ns + nm
         return ns
 
     for _ in range(max(0, args.warmup - 1)):
@@ -269,6 +286,8 @@ def ours(args):
     torch.cuda.synchronize()
     clk = clocks.stop()
     ms_per_step = e0.elapsed_time(e1) / args.steps
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, plan, s2s, last["n_edges_out"])
     value = n_edges / (ms_per_step * 1e-3)
 
     # stage split of the count stage
@@ -294,12 +313,11 @@ def ours(args):
     spass = np.array(sort_ms["s2s"])
     n_items = s2s.n_items
     s2s_achieved = 2.0 * n_items * s2s.W * 4 / (float(spass.mean()) * 1e-3) / 1e9
-    traffic, traffic_src = ncu_traffic(n_reads, k)
     roofline = {
         "bound": "hbm", "kernel": f"radix passes over the count records ({S} B): k_radix_pass3<{plan.WR}> (stable, look-back); "
                                    "the first pass of a sort is k_part_unstable (no look-back) for 8/12-byte records",
         "achieved": achieved, "peak": peak,
-        "unit": "GB/s", "frac": achieved / peak, "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
+        "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_src,
         "algorithmic_bytes_per_launch": 2 * n_edges * S, "avg_launch_ms": avg_pass_ms,
         "per_pass_ms": [float(x) for x in cpass.mean(axis=0)],
         "per_pass_frac": [float(2.0 * n_edges * S / (x * 1e-3) / 1e9 / peak) for x in cpass.mean(axis=0)],
@@ -369,12 +387,12 @@ def ours(args):
         "metric": METRIC, "value": value, "unit": "edges/s", "n_gpus": 1, "steps": args.steps, "warmup": args.warmup,
         "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u32",
         "data": "synthetic",
-        "config": {"workload": f"synthetic {n_reads}x{L}bp reads (30x, 1% subst.), k={k}, m={m}, 1xB200 single-GPU "
+        "config": {"workload": f"synthetic {n_reads}x{L}bp reads (30x, 1% subst.), k={k}, m={m}, 1xH100 single-GPU "
                                "sdbg_build: count (extract + partition/sort + solid count + mercy marks) + mercy-edge "
                                "generation + seq2sdbg (extract+radix+emit) over solid + mercy edges; the seq2sdbg extract skips the $-items the count stage's in/out flags prove the emitter would discard (same bytes out)",
                    "count_mode": count_mode, "host_affinity": args.affinity,
                    "n_edge_records": n_edges, "n_solid_edges": int(n_solid), "n_sdbg_sort_items": int(n_items),
-                   "l2_note": "inputs (>= 4.9 GB per kernel) exceed the 126 MB L2, no explicit flush needed"},
+                   "l2_note": "inputs (>= 4.9 GB per kernel) exceed the 50 MB L2, no explicit flush needed"},
         "stage_ms": stage, "stage_roofline": stage_roofline,
         "roofline": roofline, "cpu_baseline": cpu, "clocks": clk,
         "e2e": {"value": e2e_v, "unit": "edges/s", "h2d_bytes_per_step": int(h2d), "d2h_bytes_per_step": int(d2h),
@@ -396,6 +414,8 @@ def main():
     ap.add_argument("--sample-reads", type=int, default=1_000_000, help="bounded CPU sample (reference arm / cpu_baseline)")
     ap.add_argument("--e2e-steps", type=int, default=2)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed to DIR/<name>.npy")
     ap.add_argument("--count-mode", default=None, choices=["sort", "hashed", "auto"],
                     help="count stage algorithm (default: $MHB_COUNT_MODE, else hashed where supported)")
     args = ap.parse_args()

@@ -1,5 +1,5 @@
 /*
- * mhb.h -- C ABI of libmhb (megahit_b200): the B200-native SdBG-construction hot path of MEGAHIT.
+ * mhb.h -- C ABI of libmhb (megahit_b200): the H100-native (sm_90a) SdBG-construction hot path of MEGAHIT.
  *
  * Plain pointers and sizes only; no C++ or torch types.  Status: 0 = ok, non-zero = error
  * (mhb_last_error() returns the message).  There is NO CPU fallback: every compute entry point fails

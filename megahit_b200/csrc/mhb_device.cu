@@ -1,5 +1,5 @@
 // mhb_device.cu -- device-level C ABI (see include/mhb.h, layer 1): kernel launches on caller-owned
-// device memory.  Built for sm_100a only; there is no host fallback.
+// device memory.  Built for sm_90a only; there is no host fallback.
 #include <cuda_runtime.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -27,7 +27,7 @@ int mhb_set_error(int code, const char *fmt, ...) {
   return code;
 }
 extern "C" const char *mhb_last_error(void) { return g_err; }
-extern "C" const char *mhb_version(void) { return "megahit_b200 0.1 (sm_100a; formats of megahit v1.2.9)"; }
+extern "C" const char *mhb_version(void) { return "megahit_b200 0.1 (sm_90a; formats of megahit v1.2.9)"; }
 extern "C" int mhb_device_count(void) {
   int n = 0;
   if (cudaGetDeviceCount(&n) != cudaSuccess) {
@@ -81,7 +81,7 @@ int mhb_sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, dev);
-    if (g_sm_count <= 0) g_sm_count = 148;
+    if (g_sm_count <= 0) g_sm_count = 132;
     if (g_bound_device < 0) g_bound_device = dev;  // first compute call: the process stays on this device
   }
   return g_sm_count;
@@ -353,8 +353,8 @@ extern "C" int mhb_count_mark_mercy(void *stream, const mhb_dev_reads *reads, ui
   u64 g64 = (rv.n_reads + 7) / 8;
   if (g64 > (u64)sm_count() * 16) g64 = (u64)sm_count() * 16;
   const int grid = (int)g64;
-  // rolling record builder (4 positions per lane, three of them by shifting): 6.5 vs 7.4 ms on the bench workload
-  // (profiles/r2a_bench_roll.json); MHB_EXTRACT_ROLL=0 selects the per-position kernel
+  // rolling record builder (4 positions per lane, three of them by shifting); MHB_EXTRACT_ROLL=0 selects the
+  // per-position kernel
   static const bool roll = !(getenv("MHB_EXTRACT_ROLL") && !strcmp(getenv("MHB_EXTRACT_ROLL"), "0"));
   if (roll && W == 2 && WR == 2 && k + 1 >= 17) {
     k_mark_mercy_roll<<<grid, 256, 0, st>>>(rv, k, filter, fwords, table, cap, first_0_out, last_0_in);

@@ -1178,8 +1178,7 @@ static int build_host_impl(const mhb_build_args *args, mhb_build_result *res, bo
 
   // ---- H2D ----
   // Fixed-length libraries are uploaded in C pieces on a copy stream and the edges of piece i are extracted while piece
-  // i+1 is still crossing PCIe, instead of upload-then-extract (C = 4; MHB_H2D_CHUNKS=1 restores the single copy;
-  // measured e2e 115.7 -> 112.5 ms on the bench workload, profiles/r2a_bench_chunks.json).
+  // i+1 is still crossing PCIe, instead of upload-then-extract (C = 4; MHB_H2D_CHUNKS=1 restores the single copy).
   static const int h2d_chunks_env = getenv("MHB_H2D_CHUNKS") ? atoi(getenv("MHB_H2D_CHUNKS")) : 4;
   const bool chunked = h2d_chunks_env > 1 && ix.fixed_len >= k + 1 && n_reads >= (uint64_t)h2d_chunks_env * 64;
   t.start();

@@ -1,4 +1,4 @@
-// mhb_kernels.cuh -- device-side building blocks (sm_100a) shared by the kernel translation units.
+// mhb_kernels.cuh -- device-side building blocks (sm_90a) shared by the kernel translation units.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -10,7 +10,7 @@
 //                             (edges sharing a 12-base prefix share their leading byte), and the has_in / has_out logic
 //                             is an OR over search outcomes, so each rank answers the searches that land in its own
 //                             bucket range from local HBM and the per-position answer bits are exchanged instead of
-//                             the edges (round 1 bisected the peers' edge arrays over NVLink: 219 ms at 8 GPUs)
+//                             the edges (instead of bisecting the peers' edge arrays over NVLink)
 //   mhb_mercy_count_planes    OR the answer planes of all ranks into (A, O, N) and count the mercy edges
 #include <cuda_runtime.h>
 #include <stdio.h>

@@ -469,7 +469,7 @@ __global__ void __launch_bounds__(kEmitThreads)
 // finds the first non-empty bucket of its range, a suffix pass over the 1024 ranges gives the first non-empty bucket
 // behind each range, then the thread walks its range backwards.  (The first version let every bucket scan forward for
 // its successor: fine while all buckets are populated, but a rank of a multi-GPU build owns one contiguous range, and
-// its last bucket then walked tens of thousands of empty buckets in one thread - 6 ms at 2 GPUs, 11 ms at 8.)
+// its last bucket then walked tens of thousands of empty buckets in one thread.)
 __global__ void __launch_bounds__(1024) k_bucket_finalize(const u64 *bucket_start, const u64 *totals, u64 *bucket_table) {
   constexpr u32 PER = MHB_NUM_BUCKETS / 1024;
   __shared__ u32 s_first[1024];

@@ -1,8 +1,7 @@
 // mhb_sort3.cuh -- radix pass v3: the same one-sweep LSD pass as k_radix_pass (mhb_sort.cuh: ticketed tiles, warp
 // ranking, decoupled look-back, shared-memory reorder, coalesced scatter, next digit's histogram fused into the
-// scatter) rebuilt around the instruction budget.  v2 was issue-bound at ~125 thread-instructions per record
-// (profiles/r1_radix_v2_*.txt: 24 % issue-active with 2 CTAs/SM, DRAM traffic 1.01x algorithmic), of which only ~26
-// are the eight ballots.  v3 removes what surrounded them:
+// scatter) rebuilt around the instruction budget.  v2 is issue-bound at ~125 thread-instructions per record, of which
+// only ~26 are the eight ballots.  v3 removes what surrounded them:
 //   * one tile ticket is prefetched a whole tile ahead (the global atomic's latency is never exposed);
 //   * per-warp digit counters are read by ALL lanes before the leader bumps them (no shuffle, no divergent load);
 //   * the prefix over warps, the tile scan and the fold of the digit's start run as ONE pass of 256 threads
@@ -35,9 +34,10 @@ namespace mhb {
 //   bit  13   batched loads in the reorder only; bit 14: in the warp-base loop only (bit 6 = both + the asm scatter)
 //   bit  12   (with bit 7) the scan over the digit totals also runs early, on the early histogram: one barrier and the
 //             per-warp total loop leave the critical path between ranking and the reorder
-// Measured on B200, 1.23 G 8-byte records, ms per pass (profiles/r1d_sort_sweep.txt): v2 7.24; v3 base 6.93;
-// + prefetch 6.72; + early publish 6.44 (default); wider look-back windows (8, 16) 6.8-7.6; batched loads 7.1-7.3;
-// OR-match ranking 7.3.
+// Measured on an H100 SXM (80 GB HBM3, 400 W power limit), bench.py at 10 M reads: the three radix passes of the count
+// stage over 1.23 G 8-byte records take 25.4 ms with 0x180 (early publish + a first look-back window of 1, the
+// default), 26.6 ms with 0x082 (256 threads x 18 records, 3 CTAs/SM), 28.7-29.6 ms with 0x080 (early publish), 29.0 ms
+// with 0x1080, 34.5-35.0 ms with 0x000 (v3 base); v2 (cfg 0) 28.0 ms.
 template <int WR, int CFG>
 struct SortCfg3 {
   static constexpr int GEOM = CFG & 3;
@@ -480,8 +480,8 @@ __global__ void __launch_bounds__(SortCfg3<WR, CFG>::THREADS, SortCfg3<WR, CFG>:
 
     // ---- global offsets by decoupled look-back.  All CTAs run the same phases almost in step, so the nearest
     // predecessors are still "partial" when a tile looks back and the walk to the last "inclusive" descriptor is long
-    // (profiles/r1b: 25 % of all warp samples were this loop + the CTA waiting for it at B4 when it fetched 2
-    // descriptors per L2 round trip).  After the two prefetched descriptors the walk therefore fetches LBW at a
+    // (when it fetched 2 descriptors per L2 round trip, this loop and the CTA waiting for it at B4 were a quarter of
+    // all warp samples).  After the two prefetched descriptors the walk therefore fetches LBW at a
     // time - all loads in flight together, one round trip per LBW predecessors.
     if constexpr (CDESC) {
       if (tid < 256) {

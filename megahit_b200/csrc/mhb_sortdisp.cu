@@ -22,8 +22,8 @@ using namespace mhb;
 // Radix-pass variants.  0..3 = v2 geometries (mhb_sort.cuh); 256 + bits = v3 (mhb_sort3.cuh, see SortCfg3 for the
 // bit field).  Only the listed v3 combinations are instantiated (all for 8- and 12-byte records, the first one for
 // every record width).
-#define MHB_V3_DEFAULT 0x080
-#define MHB_V3_LIST(X) X(0x080) X(0x000) X(0x180) X(0x1080) X(0x082)
+#define MHB_V3_DEFAULT 0x180
+#define MHB_V3_LIST(X) X(0x180) X(0x080) X(0x000) X(0x1080) X(0x082)
 static bool v3_listed(int bits) {
 #define X(B) \
   if (bits == B) return true;

@@ -670,8 +670,8 @@ def bench(args, bin_dev, bin_words, rank, world, device, metric, clocks=None):
     dist.all_reduce(nbytes)
     if rank == 0:
         from .lib import count_record_words
-        peak = 6650.0
-        src = "fallback (B200_PROFILING.md 6.65 TB/s)"
+        peak = 3350.0
+        src = "H100 SXM data sheet (3.35 TB/s HBM3)"
         pk = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")
         if os.path.exists(pk):
             peak, src = float(json.load(open(pk))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
@@ -685,14 +685,14 @@ def bench(args, bin_dev, bin_words, rank, world, device, metric, clocks=None):
             "metric": metric, "value": n_edges / (ms_per_step * 1e-3), "unit": "edges/s", "n_gpus": world,
             "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_per_step, "higher_is_better": True,
             "scaling": "weak", "vs_baseline": None, "dtype": "u32", "data": "synthetic",
-            "config": {"workload": f"synthetic {n_reads}x{L}bp reads PER GPU (30x, 1% subst.), k={k}, m={m}, {world}xB200: "
+            "config": {"workload": f"synthetic {n_reads}x{L}bp reads PER GPU (30x, 1% subst.), k={k}, m={m}, {world}xH100: "
                                    "top-byte range partition (balanced from the all-reduced histogram), one fused partition+"
                                    "exchange pass per stage storing into the owners' buffers over NVLink (CUDA IPC peer "
                                    "memory), then per-GPU radix sort / count / mercy / seq2sdbg emit",
                        "parallelism": f"bucket-range x{world}", "n_edge_records": n_edges,
                        "records_owned_per_rank": [int(o[0]) for o in owns],
                        "solid_edges_per_rank": [int(o[1]) for o in owns], "mercy_edges_per_rank": [int(o[2]) for o in owns],
-                       "l2_note": "inputs (>= 4.9 GB per kernel) exceed the 126 MB L2, no explicit flush needed"},
+                       "l2_note": "inputs (>= 4.9 GB per kernel) exceed the 50 MB L2, no explicit flush needed"},
             "stage_ms_max_over_ranks": stage,
             "roofline": {"bound": "hbm", "kernel": f"k_radix_pass<{S // 4}> (count records, {S} B), slowest rank",
                          "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": None,

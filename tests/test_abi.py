@@ -27,7 +27,7 @@ def test_library_exports_every_declared_symbol():
 
 def test_version_and_error_strings():
     L = lib.load()
-    assert b"sm_100a" in L.mhb_version()
+    assert b"sm_90a" in L.mhb_version()
     assert isinstance(L.mhb_last_error(), bytes)
 
 

@@ -7,8 +7,10 @@
   far above kmsort's insertion-sort threshold, where the reference's result depends on kmsort's order among tied
   records (a stable sort gives other bytes - checked on the oracle, tests/test_oracle_r2s.py);
 * the oracle on the intermediate state (solid-edge bits are not visible through the ABI; the SdBG is);
-* the reference binary itself on the GPU box at 300 k reads, through the CLI (`megahit_core read2sdbg`).
+* what the reference binary writes at 300 k reads (oracle/gen_golden_cli.py -> tests/golden_cli/cli.json), through the
+  CLI (`megahit_core read2sdbg`).
 """
+import json
 import os
 import subprocess
 
@@ -17,13 +19,13 @@ import pytest
 
 from conftest import ROOT
 from megahit_b200 import formats as F
-from megahit_b200 import lib, synth
+from megahit_b200 import lib
+from oracle import gen_golden_cli as GC
 from oracle import oracle as O
 from test_oracle_r2s import R2S, r2s_reads
 
 pytestmark = pytest.mark.gpu
 
-REF = os.path.join(ROOT, "oracle", "_ref", "megahit_core_ref")
 OURS = os.path.join(ROOT, "megahit_b200", "bin", "megahit_core")
 
 
@@ -31,7 +33,7 @@ def gpu_cases():
     out = []
     for r in R2S["runs"]:
         if r["m"] > 1 and r["k"] > 237:
-            continue  # stage-1 records wider than 17 words: forwarded to the reference by the CLI (test below)
+            continue  # stage-1 records wider than 17 words: the CLI forwards these to the reference binary
         out.append(pytest.param(r, id=f"{r['lib'].split('/')[-1]}-k{r['k']}-m{r['m']}-mercy{r['mercy']}"))
     return out
 
@@ -92,43 +94,14 @@ def _run(cmd, **kw):
     return r
 
 
-def _sdbg_digest(p):
-    info, stream, table = F.canonical_sdbg(p)
-    return {"sdbg": F.sha256(stream), "k": info.k, "wpt": info.words_per_tip_label, "items": int(table[:, 0].sum()),
-            "tips": int(table[:, 1].sum()), "large": int(table[:, 2].sum())}
-
-
 @pytest.mark.parametrize("m,mercy", [(2, True), (1, False)])
 def test_cli_read2sdbg_matches_reference_binary_at_300k_reads(tmp_path, m, mercy):
-    """the sub-command itself, against the reference binary run on the same box; buckets of ~600 stage-1 records
-    (kmsort's radix levels decide the tie order), 37 M stage-1 records, 70+ M stage-2 items"""
-    if not os.path.exists(REF):
-        pytest.fail("oracle/_ref/megahit_core_ref is missing (built in the container, travels with the snapshot)")
-    n_reads, L = 300_000, 150
-    b = synth.synth_reads(n_reads, L, 5 * n_reads, 0.01, seed=777)
-    libp = str(tmp_path / "reads.lib")
-    F.write_lib(libp, b, n_reads, n_reads * L, L)
-    res = {}
-    for name, core in (("ref", REF), ("ours", OURS)):
-        p = str(tmp_path / name)
-        cmd = [core, "read2sdbg", "-k", "27", "-m", str(m), "--host_mem", "3e10", "--mem_flag", "1", "--output_prefix", p,
-               "--num_cpu_threads", str(min(32, os.cpu_count() or 8)), "--read_lib_file", libp]
-        _run(cmd + (["--need_mercy"] if mercy else []))
-        res[name] = _sdbg_digest(p)
-        if m > 1:
-            res[name]["counting"] = F.file_sha256(p + ".counting")
-        assert os.path.exists(p + ".mercy_cand.0")
-    assert res["ours"] == res["ref"]
-
-
-def test_cli_forwards_wide_stage1_to_reference(tmp_path):
-    """k = 255 with min count 2: stage-1 records of 19 words are outside the device sort; the CLI hands the command to
-    the reference binary (MHB_REFERENCE_CORE) instead of failing"""
-    if not os.path.exists(REF):
-        pytest.fail("oracle/_ref/megahit_core_ref is missing")
-    gold = [r for r in R2S["runs"] if r["k"] == 255 and r["m"] == 2][0]
-    p = str(tmp_path / "o")
-    env = dict(os.environ, MHB_REFERENCE_CORE=REF)
-    _run([OURS, "read2sdbg", "-k", "255", "-m", "2", "--host_mem", "3e10", "--output_prefix", p, "--num_cpu_threads", "4",
-          "--read_lib_file", os.path.join(ROOT, "tests", gold["lib"], "reads.lib"), "--need_mercy"], env=env)
-    assert _sdbg_digest(p)["sdbg"] == gold["sdbg_sha256"]
+    """the sub-command itself, against the digests of what the reference binary writes for the same library; buckets of
+    ~600 stage-1 records (kmsort's radix levels decide the tie order), 37 M stage-1 records, 70+ M stage-2 items"""
+    ref = json.load(open(os.path.join(ROOT, "tests", "golden_cli", "cli.json")))["read2sdbg_300k"][f"m{m}"]
+    libp = GC.r2s_lib(tmp_path)
+    p = str(tmp_path / "ours")
+    _run([OURS, "read2sdbg", "-k", "27", "-m", str(m), "--host_mem", "3e10", "--mem_flag", "1", "--output_prefix", p,
+          "--num_cpu_threads", str(min(32, os.cpu_count() or 8)), "--read_lib_file", libp] + (["--need_mercy"] if mercy else []))
+    assert os.path.exists(p + ".mercy_cand.0")
+    assert GC.r2s_digest(p, m) == ref
