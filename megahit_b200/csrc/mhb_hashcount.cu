@@ -6,8 +6,9 @@
 //   1. three stable radix passes on the three leading key bytes (the same k_radix_pass3 the sort uses) group the
 //      records by their leading 24 key bits - 3 x 2NS bytes instead of 7 x 2NS;
 //   2. k_bucket_bounds finds the 65 537 boundaries of the reference's 16-bit buckets (base_engine.h kNumBuckets) by
-//      binary search, and every bucket is cut into slices of ~6000 records whose boundaries are moved to the next
-//      change of the 24-bit prefix: a slice is contiguous and key-closed;
+//      binary search, and every bucket is cut into slices of ~7500 records whose boundaries are moved to the next
+//      change of the 24-bit prefix: a slice is contiguous and key-closed.  k_slice_plan computes every slice's range
+//      once;
 //   3. k_hash_count: a CTA takes a slice and aggregates it in a shared-memory open-addressing table keyed by the
 //      remaining 42 record bits: occurrence counts first, then, for the keys that reached the solid threshold, the
 //      4 + 4 prev/next tallies (has_in / has_out, :279-305) in a second sweep over the same records (L2 hits); the solid
@@ -33,12 +34,14 @@ namespace {
 
 constexpr int kHcHist = 1024;                  // multiplicities < kHcHist are histogrammed in shared memory
 constexpr u64 kHcEmpty = ~0ull;
-constexpr int kHcBatch = 4;                    // records per thread in flight while streaming a slice
+constexpr int kHcBatch = 8;                    // records per thread in flight while streaming a slice
 constexpr u32 kRemBits = 42;                   // record bits 47..6
 constexpr u32 kHcHotCount = 256;               // keys this frequent may wrap a byte tally: they get exact 32-bit tallies
 constexpr int kHcHotRound = 32;                // ... this many at a time
 constexpr int kHcMaxProbes = 48;               // longer probe sequences = the table is too full for this sub-range
 constexpr int kHcStack = 72;
+constexpr u32 kHcHistDone = 1u << 31;          // stack entry flag: the parent already histogrammed this sub-range's keys
+constexpr u32 kHcPrefetchChunk = 16384;        // bytes per cp.async.bulk.prefetch.L2
 
 __device__ __forceinline__ u64 rec_key64(const uint2 r) { return ((u64)r.x << 32) | r.y; }
 
@@ -55,8 +58,45 @@ __global__ void k_bucket_bounds(const uint2 *__restrict__ recs, u64 n, u64 *__re
   bounds[b] = lo;
 }
 
-// Geometry of the hash kernel: THREADS per CTA, 2^LOG_SLOTS table slots, CTAS per SM.  The per-slice fixed costs
-// (barriers, table sweeps, the ordering scan) are amortised over more records by the larger geometries.
+// first index q in [p, hi] that may start a slice: q == lo, q == hi, or the 24-bit prefix changes between q-1 and q
+// (records with equal keys share their prefix, so they never straddle such a boundary).  The records are sorted on
+// that prefix, so q is the first record in [p, hi) whose prefix exceeds that of record p-1.
+__device__ __forceinline__ u64 hc_align(const uint2 *__restrict__ recs, u64 p, u64 lo, u64 hi) {
+  if (p <= lo) return lo;
+  if (p >= hi) return hi;
+  const u32 pre = recs[p - 1].x >> 8;
+  u64 a = p, z = hi;
+  while (a < z) {
+    const u64 mid = (a + z) >> 1;
+    if ((recs[mid].x >> 8) > pre) z = mid;
+    else a = mid + 1;
+  }
+  return a;
+}
+
+// The slice plan, one thread per bucket: bucket b (16-bit prefix) is cut into slice_off[b+1] - slice_off[b] slices of
+// equal length whose boundaries are moved forward with hc_align.  plan[s] = [lo, hi) of slice s (empty when a 24-bit
+// group longer than a slice swallowed it); slice_base[s] = lo / m + s is where its solid entries go in the scratch list
+// (a slice of n records holds at most n / m solid keys and floor is super-additive: the areas never overlap).
+__global__ void k_slice_plan(const uint2 *__restrict__ recs, const u64 *__restrict__ bounds, const u64 *__restrict__ slice_off,
+                             int m, ulonglong2 *__restrict__ plan, u64 *__restrict__ slice_base, u32 *__restrict__ slice_bucket) {
+  const u32 b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= 65536u) return;
+  const u64 s0 = slice_off[b], ns = slice_off[b + 1] - s0;
+  if (!ns) return;
+  const u64 blo = bounds[b], bhi = bounds[b + 1], step = (bhi - blo + ns - 1) / ns;
+  u64 lo = blo;
+  for (u64 i = 0; i < ns; ++i) {
+    const u64 hi = i + 1 == ns ? bhi : hc_align(recs, blo + (i + 1) * step, blo, bhi);
+    plan[s0 + i] = make_ulonglong2(lo, hi);
+    slice_base[s0 + i] = lo / (u64)m + s0 + i;
+    slice_bucket[s0 + i] = b;
+    lo = hi;
+  }
+}
+
+// Geometry of the hash kernel: THREADS per CTA, 2^LOG_SLOTS table slots, CTAS per SM.  HcGeomB below is the one
+// instantiated: on H100 at 10 M reads it beat 256 x 2048 x 3 CTAs and 1024 x 8192 x 1 CTA (DESIGN.md 4.3).
 template <int THREADS_, int LOG_SLOTS_, int CTAS_>
 struct HcGeom {
   static constexpr int THREADS = THREADS_, LOG_SLOTS = LOG_SLOTS_, SLOTS = 1 << LOG_SLOTS_, CTAS = CTAS_;
@@ -75,14 +115,16 @@ struct HcShared {
   u64 sorted[G::MAX_SOLID];    // rem42 << 22 | cnt16 << 6 | aux
   u64 tmp[G::MAX_SOLID];
   u32 cell_base[G::CELLS];
-  u32 cell_cur[G::CELLS];
+  u32 cell_cur[G::CELLS];      // all zero between sub-ranges; the judge counts the solid keys per cell here
   u32 cta_hist[kHcHist];
   u32 wide[kHcHotRound][8];    // exact tallies of the hot keys of the current round
-  uint16_t hot_slot[G::MAX_SOLID];
+  uint16_t hot_rank[G::MAX_SOLID];  // rank (entry in `sorted`) of each hot key
   u64 st_prefix[kHcStack];
-  u32 st_bits[kHcStack];
+  u32 st_bits[kHcStack];       // key bits fixed by the prefix | kHcHistDone
   u32 warp_sum[G::THREADS / 32];
-  u32 n_solid, n_hot, overflow, bucket, out_cursor, sp;
+  ulonglong2 nx_range[2];      // [lo, hi) of the slice after the current one, by slice parity
+  u32 nx_sl[2];                // its id
+  u32 n_solid[2], n_hot[2], overflow[2];  // by sub-range parity: a word is reset while the other one is in use
 };
 
 __device__ __forceinline__ u32 lane_lt_mask() { return (1u << (threadIdx.x & 31)) - 1u; }
@@ -91,6 +133,16 @@ __device__ __forceinline__ u32 lane_lt_mask() { return (1u << (threadIdx.x & 31)
 // MATCH.ANY-driven loop over the groups of lanes that hit the same address; with ~1 lane per address that is overhead.
 __device__ __forceinline__ void smem_add(u32 *p, u32 v) {
   asm volatile("red.shared.add.u32 [%0], %1;" ::"r"((u32)__cvta_generic_to_shared(p)), "r"(v) : "memory");
+}
+
+// records [lo, hi) into L2 ahead of their sweep (no shared memory, no completion to wait for).  The range is cut to
+// whole 16-byte units inside it: it never reaches past the records.
+__device__ __forceinline__ void hc_prefetch_l2(const uint2 *recs, u64 lo, u64 hi) {
+  const u64 a0 = (u64)(recs + lo) & ~15ull, a1 = (u64)(recs + hi) & ~15ull;
+  for (u64 a = a0; a < a1; a += kHcPrefetchChunk) {
+    const u32 sz = (u32)(a1 - a < kHcPrefetchChunk ? a1 - a : kHcPrefetchChunk);
+    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(a), "r"(sz) : "memory");
+  }
 }
 
 template <class G>
@@ -112,31 +164,23 @@ __device__ __forceinline__ u32 hc_insert(HcShared<G> &s, u64 r) {
   }
   return G::SLOTS;
 }
+// slot of key r, SLOTS when absent
 template <class G>
-__device__ __forceinline__ u32 hc_find(const HcShared<G> &s, u64 r) {
+__device__ __forceinline__ u32 hc_lookup(const HcShared<G> &s, u64 r) {
   u32 h = hc_hash<G>(r);
-  while (s.keys[h] != r) h = (h + 1) & (G::SLOTS - 1);
-  return h;
-}
-
-// take the multiplicity histogram contribution of the occupied slots back (a sub-range that has to be split after
-// it was judged)
-template <class G>
-__device__ __forceinline__ void hc_hist_undo(HcShared<G> &s, u64 *mul_hist) {
-  for (u32 i = threadIdx.x; i < (u32)G::SLOTS; i += G::THREADS) {
-    if (s.keys[i] == kHcEmpty) continue;
-    const u32 c = s.cnt[i];
-    const u32 c16 = c > 65535u ? 65535u : c;
-    if (c16 < (u32)kHcHist) atomicAdd(&s.cta_hist[c16], 0xFFFFFFFFu);
-    else atomicAdd((unsigned long long *)&mul_hist[c16], ~0ull);
+  while (true) {
+    const u64 cur = s.keys[h];
+    if (cur == r) return h;
+    if (cur == kHcEmpty) return G::SLOTS;
+    h = (h + 1) & (G::SLOTS - 1);
   }
 }
 
-// exclusive scan of s.cell_base[0 .. CELLS) in place (CELLS = 2 * THREADS); also primes cell_cur
+// exclusive scan of the cell counts in s.cell_cur[0 .. CELLS) (CELLS = 2 * THREADS) into cell_base; cell_cur = cell_base
 template <class G>
 __device__ __forceinline__ void hc_scan_cells(HcShared<G> &s) {
   const u32 t = threadIdx.x, lane = t & 31, w = t >> 5;
-  const u32 a = s.cell_base[2 * t], b = s.cell_base[2 * t + 1];
+  const u32 a = s.cell_cur[2 * t], b = s.cell_cur[2 * t + 1];
   u32 v = a + b;
 #pragma unroll
   for (int d = 1; d < 32; d <<= 1) {
@@ -167,105 +211,83 @@ __device__ __forceinline__ bool hc_any_byte_ge(u32 w, u32 m) {
   return (w & 0xFFu) >= m || ((w >> 8) & 0xFFu) >= m || ((w >> 16) & 0xFFu) >= m || (w >> 24) >= m;
 }
 
-// first index q in [p, hi] that may start a slice: q == lo, q == hi, or the 24-bit prefix changes between q-1 and q
-// (records with equal keys share their prefix, so they never straddle such a boundary).  Block-wide.
-template <int THREADS>
-__device__ __forceinline__ u64 hc_align(const uint2 *__restrict__ recs, u64 p, u64 lo, u64 hi, u32 *s_min) {
-  if (p <= lo) return lo;
-  if (p >= hi) return hi;
-  for (u64 q0 = p; q0 < hi; q0 += THREADS) {
-    __syncthreads();
-    if (threadIdx.x == 0) *s_min = 0xFFFFFFFFu;
-    __syncthreads();
-    const u64 q = q0 + threadIdx.x;
-    if (q < hi && (recs[q].x >> 8) != (recs[q - 1].x >> 8)) atomicMin(s_min, threadIdx.x);
-    __syncthreads();
-    const u32 f = *s_min;
-    if (f != 0xFFFFFFFFu) return q0 + f;
-  }
-  return hi;
-}
-
-// Work unit = a SLICE of the prefix-sorted records: bucket b (16-bit prefix) is cut into ceil(n_b / T) slices whose
-// boundaries are moved forward to the next change of the 24-bit prefix, so that a slice is a contiguous, key-closed
-// range read once with every lane busy.  slice_off[b] = first slice id of bucket b (exclusive scan of the per-bucket
-// slice counts).  list: slice s's solid entries go to list[a_s / m + s ...) with a_s the slice's first record (a slice
-// of n records holds at most n / m solid keys and floor is super-additive: the areas never overlap).
+// Work unit = a SLICE of the prefix-sorted records (k_slice_plan), taken by ticket.  Thread 0 holds the ticket of the
+// slice after the next one: while the CTA sweeps slice i it loads the plan entry of slice i+1 and takes the ticket of
+// slice i+2, and once the sweep is done it prefetches slice i+1's records into L2, so that they arrive while slice i
+// is judged, ordered and written.
 // One sweep per slice: occurrence count and the 4 + 4 prev / next tallies (kmer_counter.cpp:279-295) of every key, the
-// tallies as byte fields; only keys with >= 256 occurrences ("hot": a byte could wrap) get a second sweep with exact
-// 32-bit tallies, 32 keys at a time.
+// tallies as byte fields; the judge then reads every slot once (histogram, solid keys, flags) and empties it.  Keys
+// with >= 256 occurrences ("hot": a byte could wrap) get exact 32-bit tallies in a second sweep, 32 keys at a time.
 template <class G>
 __global__ void __launch_bounds__(G::THREADS, G::CTAS)
-    k_hash_count(const uint2 *__restrict__ recs, const u64 *__restrict__ bounds, const u64 *__restrict__ slice_off,
-                 const u64 *__restrict__ n_slices_dev, int m, u32 *ticket, u64 *__restrict__ list,
-                 u32 *__restrict__ slice_count, u64 *__restrict__ slice_base, u32 *__restrict__ slice_bucket, u64 *mul_hist,
-                 u32 *err_flag) {
+    k_hash_count(const uint2 *__restrict__ recs, const ulonglong2 *__restrict__ plan, const u64 *__restrict__ n_slices_dev,
+                 int m, u32 *ticket, u64 *__restrict__ list, u32 *__restrict__ slice_count, u64 *mul_hist, u32 *err_flag) {
   constexpr int THREADS = G::THREADS, SLOTS = G::SLOTS, MAX_SOLID = G::MAX_SOLID, CELLS = G::CELLS;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   HcShared<G> &s = *reinterpret_cast<HcShared<G> *>(smem_raw);
   const u32 tid = threadIdx.x;
   for (u32 i = tid; i < kHcHist; i += THREADS) s.cta_hist[i] = 0;
+  for (u32 i = tid; i < (u32)CELLS; i += THREADS) s.cell_cur[i] = 0;
   for (u32 i = tid; i < (u32)SLOTS; i += THREADS) {
     s.keys[i] = kHcEmpty;
     s.cnt[i] = 0;
     s.pt[i] = 0;
     s.nt[i] = 0;
   }
-  __syncthreads();
   const u64 n_slices = *n_slices_dev;
   const u32 um = (u32)m;
-  while (true) {
-    if (tid == 0) {
-      const u32 sl = atomicAdd(ticket, 1u);
-      s.bucket = sl;
-      if (sl < n_slices) {  // bucket of this slice: last b with slice_off[b] <= sl
-        u32 a = 0, z = 65536;
-        while (z - a > 1) {
-          const u32 mid = (a + z) >> 1;
-          if (slice_off[mid] <= sl) a = mid; else z = mid;
-        }
-        s.sp = a;
-      }
+  const u32 cshift = 22 + (kRemBits - G::LOG_CELLS);  // entry bits 63..22 hold the remainder
+  u32 tk = 0;  // thread 0: ticket of the slice after the next one
+  if (tid == 0) {
+    s.n_solid[0] = s.n_solid[1] = s.n_hot[0] = s.n_hot[1] = s.overflow[0] = s.overflow[1] = 0;
+    const u32 t0 = atomicAdd(ticket, 1u);
+    s.nx_sl[0] = t0;
+    if (t0 < n_slices) {
+      const ulonglong2 r = plan[t0];
+      s.nx_range[0] = r;
+      hc_prefetch_l2(recs, r.x, r.y);
+      tk = atomicAdd(ticket, 1u);
+    } else {
+      tk = t0;
     }
-    __syncthreads();
-    const u32 sl = s.bucket;
+  }
+  __syncthreads();
+  u32 q = 0;  // sub-ranges done by this CTA; its parity selects the control words
+  for (u32 it = 0;; ++it) {
+    const u32 sl = s.nx_sl[it & 1];
     if (sl >= n_slices) break;
-    const u32 b = s.sp;
-    __syncthreads();
-    const u64 blo = bounds[b], bhi = bounds[b + 1];
-    const u64 n_in_b = slice_off[b + 1] - slice_off[b], idx = sl - slice_off[b];
-    const u64 step = (bhi - blo + n_in_b - 1) / n_in_b;
-    const u64 lo = hc_align<THREADS>(recs, blo + idx * step, blo, bhi, &s.overflow);
-    const u64 hi = idx + 1 == n_in_b ? bhi : hc_align<THREADS>(recs, blo + (idx + 1) * step, blo, bhi, &s.overflow);
-    __syncthreads();
-    const u64 base = lo / (u64)m + sl;
-    if (tid == 0) {
-      slice_base[sl] = base;
-      slice_bucket[sl] = b;
-      s.out_cursor = 0;
-      s.st_prefix[0] = 0;
-      s.st_bits[0] = 0;
-      s.sp = 1;
+    const ulonglong2 rg = s.nx_range[it & 1];
+    const u64 lo = rg.x, hi = rg.y;
+    // thread 0: the next slice's plan entry and the ticket after it are in flight during this slice's sweep
+    ulonglong2 nx = make_ulonglong2(0, 0);
+    u32 ntk = tk;
+    if (tid == 0 && tk < n_slices) {
+      nx = plan[tk];
+      ntk = atomicAdd(ticket, 1u);
     }
-    if (hi <= lo) {  // a 24-bit group longer than a slice swallowed this one
-      if (tid == 0) slice_count[sl] = 0;
+    auto publish_next = [&]() {
+      if (tid != 0) return;
+      s.nx_sl[(it + 1) & 1] = tk;
+      if (tk < n_slices) {
+        s.nx_range[(it + 1) & 1] = nx;
+        hc_prefetch_l2(recs, nx.x, nx.y);
+      }
+      tk = ntk;
+    };
+    if (hi <= lo) {  // a 24-bit group longer than a slice swallowed this one (its count stays 0)
+      publish_next();
       __syncthreads();
       continue;
     }
-    __syncthreads();
-    while (s.sp > 0) {
-      // ---------------- one key sub-range: the records whose remainder starts with `prefix` (`bits` bits) -------
-      const u32 sp = s.sp - 1;
-      const u64 prefix = s.st_prefix[sp];
-      const u32 bits = s.st_bits[sp];
-      __syncthreads();
-      if (tid == 0) {
-        s.sp = sp;
-        s.n_solid = 0;
-        s.n_hot = 0;
-        s.overflow = 0;
-      }
-      __syncthreads();
+    const u64 base = lo / (u64)m + sl;  // = slice_base[sl]
+    u32 out_cursor = 0, sp = 0;
+    u64 prefix = 0;
+    u32 bits = 0;
+    bool hist_done = false, first = true;
+    while (true) {
+      // ---------------- one key sub-range: the records whose remainder starts with `prefix` (`bits` bits) ---------
+      const u32 par = q & 1;
+      ++q;
       // ---- the sweep: occurrence counts and byte tallies ----
       for (u64 i0 = lo + tid; i0 < hi; i0 += (u64)THREADS * kHcBatch) {
         uint2 v[kHcBatch];
@@ -283,159 +305,177 @@ __global__ void __launch_bounds__(G::THREADS, G::CTAS)
           if (bits && (r >> (kRemBits - bits)) != prefix) continue;
           const u32 h = hc_insert<G>(s, r);
           if (h == (u32)SLOTS) {
-            s.overflow = 1;
+            s.overflow[par] = 1;
             continue;
           }
           smem_add(&s.cnt[h], 1u);
-          const u32 p = (u32)(key >> 3) & 7u, nx = (u32)key & 7u;
+          const u32 p = (u32)(key >> 3) & 7u, nx_ = (u32)key & 7u;
           if (p < 4) smem_add(&s.pt[h], 1u << (8 * p));
-          if (nx < 4) smem_add(&s.nt[h], 1u << (8 * nx));
+          if (nx_ < 4) smem_add(&s.nt[h], 1u << (8 * nx_));
         }
-        if (s.overflow) break;
+        if (s.overflow[par]) break;
       }
+      if (first) publish_next();
+      first = false;
       __syncthreads();
-      bool failed = s.overflow != 0;
-      u32 ns = 0;
-      if (!failed) {
-        // ---- judge: multiplicity histogram; the keys that reached the solid threshold get a rank and their flags ----
-        for (u32 i0 = 0; i0 < (u32)SLOTS; i0 += THREADS) {
-          const u32 slot = i0 + tid;
-          const bool on = s.keys[slot] != kHcEmpty;
-          const u32 c = on ? s.cnt[slot] : 0u;
-          const u32 c16 = c > 65535u ? 65535u : c;
+      const bool overflowed = s.overflow[par] != 0;
+      if (tid == 0) s.n_solid[par ^ 1] = s.n_hot[par ^ 1] = s.overflow[par ^ 1] = 0;
+      // ---- judge: every slot is read once and emptied; unless the table overflowed, the multiplicity histogram, and
+      // the keys that reached the solid threshold get a rank, their flags and their counting-sort cell ----
+      const bool count_hist = !overflowed && !hist_done;
+      for (u32 slot = tid; slot < (u32)SLOTS; slot += THREADS) {
+        const u64 key = s.keys[slot];
+        const bool on = key != kHcEmpty;
+        u32 c = 0, ptv = 0, ntv = 0;
+        if (on) {
+          c = s.cnt[slot];
+          ptv = s.pt[slot];
+          ntv = s.nt[slot];
+          s.keys[slot] = kHcEmpty;
+          s.cnt[slot] = 0;
+          s.pt[slot] = 0;
+          s.nt[slot] = 0;
+        }
+        if (overflowed) continue;
+        const u32 c16 = c > 65535u ? 65535u : c;
+        if (count_hist) {
           const u32 ones = __ballot_sync(0xffffffffu, on && c16 == 1u), twos = __ballot_sync(0xffffffffu, on && c16 == 2u);
           if (on && c16 > 2u) {
             if (c16 < (u32)kHcHist) smem_add(&s.cta_hist[c16], 1u);
             else atomicAdd((unsigned long long *)&mul_hist[c16], 1ull);
           }
-          const bool solid = on && c >= um;
-          const u32 sm_ = __ballot_sync(0xffffffffu, solid);
-          u32 wbase = 0;
           if ((tid & 31) == 0) {
-            if (ones) atomicAdd(&s.cta_hist[1], (u32)__popc(ones));
-            if (twos) atomicAdd(&s.cta_hist[2], (u32)__popc(twos));
-            if (sm_) wbase = atomicAdd(&s.n_solid, (u32)__popc(sm_));
-          }
-          wbase = __shfl_sync(0xffffffffu, wbase, 0);
-          if (solid) {
-            const u32 rank = wbase + __popc(sm_ & lane_lt_mask());
-            if (rank < (u32)MAX_SOLID) {
-              u64 e = (s.keys[slot] << 22) | ((u64)c16 << 6);
-              if (c >= kHcHotCount) {  // byte tallies may have wrapped: exact tallies in a second sweep
-                const u32 hi_ = atomicAdd(&s.n_hot, 1u);
-                if (hi_ < (u32)MAX_SOLID) s.hot_slot[hi_] = (uint16_t)slot;
-                s.pt[slot] = hi_;   // index among the hot keys
-                s.nt[slot] = rank;  // where its entry lives
-              } else {
-                e |= (hc_any_byte_ge(s.pt[slot], um) ? 0ull : 1ull) | (hc_any_byte_ge(s.nt[slot], um) ? 0ull : 2ull);
-              }
-              s.sorted[rank] = e;
-            }
+            if (ones) smem_add(&s.cta_hist[1], (u32)__popc(ones));
+            if (twos) smem_add(&s.cta_hist[2], (u32)__popc(twos));
           }
         }
-        __syncthreads();
-        ns = s.n_solid;
-        if (ns > (u32)MAX_SOLID) {  // too many solid keys for the ordering buffers: take the histogram back, split
-          hc_hist_undo<G>(s, mul_hist);
-          failed = true;
+        const bool solid = on && c >= um;
+        const u32 sm_ = __ballot_sync(0xffffffffu, solid);
+        if (!sm_) continue;
+        u32 wbase = 0;
+        if ((tid & 31) == 0) wbase = atomicAdd(&s.n_solid[par], (u32)__popc(sm_));
+        wbase = __shfl_sync(0xffffffffu, wbase, 0);
+        if (solid) {
+          const u32 rank = wbase + __popc(sm_ & lane_lt_mask());
+          if (rank < (u32)MAX_SOLID) {
+            u64 e = (key << 22) | ((u64)c16 << 6);
+            if (c >= kHcHotCount) {  // byte tallies may have wrapped: exact tallies in a second sweep
+              s.hot_rank[atomicAdd(&s.n_hot[par], 1u)] = (uint16_t)rank;
+            } else {
+              e |= (hc_any_byte_ge(ptv, um) ? 0ull : 1ull) | (hc_any_byte_ge(ntv, um) ? 0ull : 2ull);
+            }
+            s.sorted[rank] = e;
+            smem_add(&s.cell_cur[(u32)((e << bits) >> cshift)], 1u);
+          }
         }
       }
+      __syncthreads();
+      const u32 ns = s.n_solid[par];
+      const bool failed = overflowed || ns > (u32)MAX_SOLID;
       if (!failed && ns) {
-        const u32 n_hot = s.n_hot;
-        for (u32 h0 = 0; h0 < n_hot; h0 += kHcHotRound) {
-          // ---- exact prev / next tallies of up to 32 hot keys: one more sweep over the slice ----
-          for (u32 i = tid; i < (u32)kHcHotRound * 8; i += THREADS) s.wide[i >> 3][i & 7] = 0;
-          __syncthreads();
-          for (u64 i0 = lo + tid; i0 < hi; i0 += (u64)THREADS * kHcBatch) {
-            uint2 v[kHcBatch];
-#pragma unroll
-            for (int j = 0; j < kHcBatch; ++j) {
-              const u64 i = i0 + (u64)j * THREADS;
-              v[j] = i < hi ? recs[i] : make_uint2(0, 0);
-            }
-#pragma unroll
-            for (int j = 0; j < kHcBatch; ++j) {
-              const u64 i = i0 + (u64)j * THREADS;
-              if (i >= hi) break;
-              const u64 key = rec_key64(v[j]);
-              const u64 r = (key >> 6) & ((1ull << kRemBits) - 1);
-              if (bits && (r >> (kRemBits - bits)) != prefix) continue;
-              const u32 slot = hc_find<G>(s, r);
-              const u32 c = s.cnt[slot];
-              if (c < kHcHotCount || c < um) continue;
-              const u32 hidx = s.pt[slot] - h0;
-              if (hidx >= (u32)kHcHotRound) continue;
-              const u32 p = (u32)(key >> 3) & 7u, nx = (u32)key & 7u;
-              if (p < 4) smem_add(&s.wide[hidx][p], 1u);
-              if (nx < 4) smem_add(&s.wide[hidx][4 + nx], 1u);
-            }
+        const u32 n_hot = s.n_hot[par];
+        if (n_hot) {
+          // ---- exact prev / next tallies of the hot keys: the emptied table holds them alone (pt = index among
+          // them), one more sweep over the slice per 32 of them ----
+          for (u32 i = tid; i < n_hot; i += THREADS) {
+            const u64 r = s.sorted[s.hot_rank[i]] >> 22;
+            u32 h = hc_hash<G>(r);  // distinct keys, at most SLOTS / 4 of them: a free slot is always found
+            while (atomicCAS((unsigned long long *)&s.keys[h], kHcEmpty, r) != kHcEmpty) h = (h + 1) & (SLOTS - 1);
+            s.pt[h] = i;
           }
-          __syncthreads();
-          for (u32 i = tid; i < (u32)kHcHotRound && h0 + i < n_hot; i += THREADS) {
-            bool has_in = false, has_out = false;
+          for (u32 h0 = 0; h0 < n_hot; h0 += kHcHotRound) {
+            for (u32 i = tid; i < (u32)kHcHotRound * 8; i += THREADS) s.wide[i >> 3][i & 7] = 0;
+            __syncthreads();
+            for (u64 i0 = lo + tid; i0 < hi; i0 += (u64)THREADS * kHcBatch) {
+              uint2 v[kHcBatch];
 #pragma unroll
-            for (int c = 0; c < 4; ++c) {
-              has_in = has_in || s.wide[i][c] >= um;
-              has_out = has_out || s.wide[i][4 + c] >= um;
+              for (int j = 0; j < kHcBatch; ++j) {
+                const u64 i = i0 + (u64)j * THREADS;
+                v[j] = i < hi ? recs[i] : make_uint2(0, 0);
+              }
+#pragma unroll
+              for (int j = 0; j < kHcBatch; ++j) {
+                const u64 i = i0 + (u64)j * THREADS;
+                if (i >= hi) break;
+                const u64 key = rec_key64(v[j]);
+                const u64 r = (key >> 6) & ((1ull << kRemBits) - 1);
+                if (bits && (r >> (kRemBits - bits)) != prefix) continue;
+                const u32 slot = hc_lookup<G>(s, r);
+                if (slot == (u32)SLOTS) continue;
+                const u32 hidx = s.pt[slot] - h0;
+                if (hidx >= (u32)kHcHotRound) continue;
+                const u32 p = (u32)(key >> 3) & 7u, nx_ = (u32)key & 7u;
+                if (p < 4) smem_add(&s.wide[hidx][p], 1u);
+                if (nx_ < 4) smem_add(&s.wide[hidx][4 + nx_], 1u);
+              }
             }
-            s.sorted[s.nt[s.hot_slot[h0 + i]]] |= (has_in ? 0ull : 1ull) | (has_out ? 0ull : 2ull);
+            __syncthreads();
+            for (u32 i = tid; i < (u32)kHcHotRound && h0 + i < n_hot; i += THREADS) {
+              bool has_in = false, has_out = false;
+#pragma unroll
+              for (int c = 0; c < 4; ++c) {
+                has_in = has_in || s.wide[i][c] >= um;
+                has_out = has_out || s.wide[i][4 + c] >= um;
+              }
+              s.sorted[s.hot_rank[h0 + i]] |= (has_in ? 0ull : 1ull) | (has_out ? 0ull : 2ull);
+            }
+            __syncthreads();
           }
-          __syncthreads();
+          for (u32 i = tid; i < (u32)SLOTS; i += THREADS) {  // empty the table again (the next sweep follows barriers)
+            s.keys[i] = kHcEmpty;
+            s.pt[i] = 0;
+          }
         }
         // ---- order the solid keys: counting sort on the next key bits, ties ranked inside their cell ----
-        for (u32 i = tid; i < (u32)CELLS; i += THREADS) s.cell_base[i] = 0;
-        __syncthreads();
-        const u32 cshift = 22 + (kRemBits - G::LOG_CELLS);  // entry bits 63..22 hold the remainder
-        for (u32 i = tid; i < ns; i += THREADS) smem_add(&s.cell_base[(u32)((s.sorted[i] << bits) >> cshift)], 1u);
-        __syncthreads();
         hc_scan_cells<G>(s);
         for (u32 i = tid; i < ns; i += THREADS) {
           const u64 e = s.sorted[i];
           s.tmp[atomicAdd(&s.cell_cur[(u32)((e << bits) >> cshift)], 1u)] = e;
         }
         __syncthreads();
-        const u32 at = s.out_cursor;
+        for (u32 i = tid; i < (u32)CELLS; i += THREADS) s.cell_cur[i] = 0;  // not read again before the next judge
         for (u32 i = tid; i < ns; i += THREADS) {
           const u64 e = s.tmp[i];
           const u32 c = (u32)((e << bits) >> cshift);
           const u32 b0 = s.cell_base[c], b1 = c + 1 < (u32)CELLS ? s.cell_base[c + 1] : ns;
           u32 r = b0;
           for (u32 j = b0; j < b1; ++j) r += s.tmp[j] < e ? 1u : 0u;
-          list[base + at + r] = e;
+          list[base + out_cursor + r] = e;
+        }
+        out_cursor += ns;
+      }
+      if (failed) {
+        // split this sub-range in four (ascending order is kept: the smallest child is popped first).  Unless the table
+        // overflowed, the judge has histogrammed its keys already: the children, which partition them, must not.
+        for (u32 i = tid; i < (u32)CELLS; i += THREADS) s.cell_cur[i] = 0;
+        if (bits + 2 > kRemBits || sp + 4 > (u32)kHcStack) {
+          if (tid == 0) atomicExch(err_flag, 1u);
+        } else {
+          const u32 flag = (hist_done || !overflowed) ? kHcHistDone : 0u;
+          if (tid == 0)
+            for (int c = 3; c >= 0; --c) {
+              s.st_prefix[sp + 3 - c] = (prefix << 2) | (u64)c;
+              s.st_bits[sp + 3 - c] = (bits + 2) | flag;
+            }
+          sp += 4;
         }
         __syncthreads();
-        if (tid == 0) s.out_cursor = at + ns;
       }
-      // ---- clear the table ----
-      for (u32 i = tid; i < (u32)SLOTS; i += THREADS) {
-        s.keys[i] = kHcEmpty;
-        s.cnt[i] = 0;
-        s.pt[i] = 0;
-        s.nt[i] = 0;
-      }
-      __syncthreads();
-      if (tid == 0 && failed) {  // split this sub-range in four (ascending order is kept: the smallest child is popped first)
-        if (bits + 2 > kRemBits || s.sp + 4 > (u32)kHcStack) atomicExch(err_flag, 1u);
-        else
-          for (int c = 3; c >= 0; --c) {
-            s.st_prefix[s.sp] = (prefix << 2) | (u64)c;
-            s.st_bits[s.sp] = bits + 2;
-            ++s.sp;
-          }
-      }
-      __syncthreads();
+      if (sp == 0) break;
+      --sp;
+      prefix = s.st_prefix[sp];
+      bits = s.st_bits[sp] & ~kHcHistDone;
+      hist_done = (s.st_bits[sp] & kHcHistDone) != 0;
     }
     // ---- the slice is complete ----
-    if (tid == 0) slice_count[sl] = s.out_cursor;
-    __syncthreads();
+    if (tid == 0) slice_count[sl] = out_cursor;
   }
+  __syncthreads();
   for (u32 i = tid; i < kHcHist; i += THREADS)
     if (s.cta_hist[i]) atomicAdd((unsigned long long *)&mul_hist[i], (unsigned long long)s.cta_hist[i]);
 }
 
-using HcGeomA = HcGeom<256, 11, 3>;
 using HcGeomB = HcGeom<512, 12, 2>;
-using HcGeomC = HcGeom<1024, 13, 1>;
 
 // per-bucket slice counts: ceil(n_b / T) (0 for an empty bucket)
 __global__ void k_slice_counts(const u64 *__restrict__ bounds, u32 T, u32 *__restrict__ cnt) {
@@ -486,43 +526,32 @@ int scan_counts(cudaStream_t st, const u32 *in, u64 n, u64 *out, u64 *total_dev,
   return MHB_OK;
 }
 
-// MHB_HC_GEOM = A | B | C selects the kernel geometry, MHB_HC_SLICE the records per slice (tuning hooks)
-static int hc_geom() {
-  static const int g = getenv("MHB_HC_GEOM") ? (getenv("MHB_HC_GEOM")[0] == 'A' ? 0 : (getenv("MHB_HC_GEOM")[0] == 'C' ? 2 : 1)) : 1;
-  return g;
-}
-static u32 hc_slice_records() {
-  const u32 def = hc_geom() == 0 ? HcGeomA::SLICE : (hc_geom() == 1 ? HcGeomB::SLICE : HcGeomC::SLICE);
-  static const u32 v = getenv("MHB_HC_SLICE") ? (u32)atoi(getenv("MHB_HC_SLICE")) : 0;
-  return v >= 256 && v <= 64000 ? v : def;
-}
-#define kHcSliceRecords hc_slice_records()
-
 template <class G>
-static int launch_hash_count(cudaStream_t st, const uint2 *recs, const u64 *bounds, const u64 *slice_off, const u64 *n_slices_dev,
-                             int m, u32 *misc, u64 *list, u32 *slice_count, u64 *slice_base, u32 *slice_bucket, u64 *mul_hist) {
+static int launch_hash_count(cudaStream_t st, const uint2 *recs, const ulonglong2 *plan, const u64 *n_slices_dev, int m, u32 *misc,
+                             u64 *list, u32 *slice_count, u64 *mul_hist) {
   static int bps = 0;
   const size_t smem = sizeof(HcShared<G>);
   if (!bps) {
     CK(cudaFuncSetAttribute(k_hash_count<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_hash_count<G>, G::THREADS, smem));
     if (bps < 1) return mhb_set_error(MHB_ERR_CUDA, "hash-count kernel does not fit an SM (%zu B shared memory)", smem);
-    if (getenv("MHB_VERBOSE")) fprintf(stderr, "[mhb] hash count: %d threads, %d slots, %zu B smem, %d CTA/SM, slice %u\n", G::THREADS, G::SLOTS, smem, bps, kHcSliceRecords);
+    if (getenv("MHB_VERBOSE")) fprintf(stderr, "[mhb] hash count: %d threads, %d slots, %zu B smem, %d CTA/SM, slice %u\n", G::THREADS, G::SLOTS, smem, bps, G::SLICE);
   }
-  k_hash_count<G><<<sm_count() * bps, G::THREADS, smem, st>>>(recs, bounds, slice_off, n_slices_dev, m, misc, list, slice_count,
-                                                             slice_base, slice_bucket, mul_hist, misc + 1);
+  k_hash_count<G><<<sm_count() * bps, G::THREADS, smem, st>>>(recs, plan, n_slices_dev, m, misc, list, slice_count, mul_hist,
+                                                             misc + 1);
   CK_LAUNCH();
   return MHB_OK;
 }
 
 struct HcLayout {
-  size_t sort_ws, off_bounds, off_bcnt, off_soff, off_bsum, off_misc, off_scount, off_sdst, off_sbase, off_sbucket, off_list, total;
+  size_t sort_ws, off_bounds, off_bcnt, off_soff, off_bsum, off_misc, off_scount, off_sdst, off_sbase, off_sbucket, off_plan,
+      off_list, total;
   uint64_t max_slices;
 };
 HcLayout hc_layout(uint64_t n, int32_t m) {
   HcLayout L;
   auto pad = [](size_t x) { return (x + 255) & ~(size_t)255; };
-  L.max_slices = n / 256 + 65536 + 2;  // 256 = smallest slice size hc_slice_records() admits
+  L.max_slices = n / HcGeomB::SLICE + 65536 + 2;  // sum over the buckets of ceil(n_b / SLICE) <= n / SLICE + 65536
   L.sort_ws = pad(mhb_sort_workspace_bytes(n, 2));
   size_t p = L.sort_ws;
   L.off_bounds = p;
@@ -543,6 +572,8 @@ HcLayout hc_layout(uint64_t n, int32_t m) {
   p += pad(L.max_slices * 8);
   L.off_sbucket = p;
   p += pad(L.max_slices * 4);
+  L.off_plan = p;
+  p += pad(L.max_slices * 16);
   L.off_list = p;
   p += pad((size_t)(n / (uint64_t)(m < 1 ? 1 : m) + L.max_slices + 8) * 8);
   L.total = p;
@@ -586,25 +617,22 @@ extern "C" int mhb_count_solid_hashed(void *stream, uint32_t *recs_a, uint32_t *
   u64 *slice_dst = (u64 *)(w + L.off_sdst);
   u64 *slice_base = (u64 *)(w + L.off_sbase);
   u32 *slice_bucket = (u32 *)(w + L.off_sbucket);
+  ulonglong2 *plan = (ulonglong2 *)(w + L.off_plan);
   u64 *list = (u64 *)(w + L.off_list);
   u64 *n_slices_dev = (u64 *)(misc + 2);
   CK(cudaMemsetAsync(misc, 0, 256, st));
   CK(cudaMemsetAsync(slice_count, 0, L.max_slices * 4, st));
-  // 2. bucket boundaries, slices per bucket
+  // 2. bucket boundaries, slices per bucket, the slice plan
   k_bucket_bounds<<<(65537 + 255) / 256, 256, 0, st>>>(recs, n, bounds);
   CK_LAUNCH();
-  k_slice_counts<<<65536 / 256, 256, 0, st>>>(bounds, kHcSliceRecords, bcnt);
+  k_slice_counts<<<65536 / 256, 256, 0, st>>>(bounds, HcGeomB::SLICE, bcnt);
   CK_LAUNCH();
   if (int rc = scan_counts(st, bcnt, 65536, slice_off, n_slices_dev, bsum)) return rc;
   CK(cudaMemcpyAsync(slice_off + 65536, n_slices_dev, 8, cudaMemcpyDeviceToDevice, st));
+  k_slice_plan<<<65536 / 256, 256, 0, st>>>(recs, bounds, slice_off, m, plan, slice_base, slice_bucket);
+  CK_LAUNCH();
   // 3. per-slice hash aggregation
-  {
-    int rc;
-    if (hc_geom() == 0) rc = launch_hash_count<HcGeomA>(st, recs, bounds, slice_off, n_slices_dev, m, misc, list, slice_count, slice_base, slice_bucket, mul_hist);
-    else if (hc_geom() == 2) rc = launch_hash_count<HcGeomC>(st, recs, bounds, slice_off, n_slices_dev, m, misc, list, slice_count, slice_base, slice_bucket, mul_hist);
-    else rc = launch_hash_count<HcGeomB>(st, recs, bounds, slice_off, n_slices_dev, m, misc, list, slice_count, slice_base, slice_bucket, mul_hist);
-    if (rc) return rc;
-  }
+  if (int rc = launch_hash_count<HcGeomB>(st, recs, plan, n_slices_dev, m, misc, list, slice_count, mul_hist)) return rc;
   // 4. offsets + edges (the scan runs over the allocated maximum; unused slice ids hold zero)
   if (int rc = scan_counts(st, slice_count, L.max_slices, slice_dst, n_solid_out, bsum)) return rc;
   k_hash_gather<<<sm_count() * 4, 256, 0, st>>>(list, n_slices_dev, slice_count, slice_dst, slice_base, slice_bucket,
