@@ -182,7 +182,7 @@ int mhb_count_solid(void *stream, const uint32_t *sorted_records, uint64_t n, ui
                     uint32_t *edges_out, uint8_t *aux_out, uint64_t capacity_edges, uint64_t *mul_hist,
                     uint64_t *n_solid_out, void *scratch, size_t scratch_bytes);
 
-/* A4 + A5 without the full sort, for 8-byte count records (11 <= k <= 28) and 1 <= m <= 1024: the records are grouped
+/* A4 + A5 without the full sort, for 8-byte count records (13 <= k <= 28) and 1 <= m <= 1024: the records are grouped
  * by their leading 24 key bits with three radix passes (record bytes 5, 6, 7), cut into key-closed slices inside the
  * reference's 16-bit buckets, and every slice is aggregated by a hash table in shared memory - occurrence counts,
  * prev/next tallies of the keys that reach m, a counting sort of the slice's solid keys.  Same outputs, bit for bit,

@@ -1,5 +1,5 @@
 // mhb_hashcount.cu -- solid-edge counting by radix PARTITION + per-bucket HASH AGGREGATION (A4 + A5 for 8-byte count
-// records, i.e. k <= 28), an alternative to "sort all records by all 7 key bytes, then run-length count".
+// records, i.e. 13 <= k <= 28), an alternative to "sort all records by all 7 key bytes, then run-length count".
 //
 // Why: the run-length count (kmer_counter.cpp:254-305) needs equal (k+1)-mers to meet, not a total order of the 1.23 G
 // records; only the SOLID edges (5 % of the distinct ones on the bench workload) have to come out sorted.  So:
@@ -18,8 +18,8 @@
 //      distribution, only speed does;
 //   4. a scan over the per-slice solid counts + k_hash_gather write the `.edges`-format records (PackEdge, :32-52),
 //      the aux flags and the multiplicity histogram exactly as mhb_count_solid does.
-// Output is bit-identical to sort + mhb_count_solid (tests/test_gpu_parity.py).  HBM traffic of the count stage falls
-// from (7 x 2 + 1) NS to (3 x 2 + 1) NS bytes.
+// Output is bit-identical to sort + mhb_count_solid and to the NumPy reference (tests/test_gpu_count.py).  HBM traffic
+// of the count stage falls from (7 x 2 + 1) NS to (3 x 2 + 1) NS bytes.
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <string.h>
@@ -595,7 +595,7 @@ extern "C" int mhb_count_solid_hashed(void *stream, uint32_t *recs_a, uint32_t *
                                       const uint64_t *hist_byte5, uint32_t *edges_out, uint8_t *aux_out,
                                       uint64_t capacity_edges, uint64_t *mul_hist, uint64_t *n_solid_out, void *ws,
                                       size_t ws_bytes) {
-  if (!mhb_count_hashed_supported(k, m)) return mhb_set_error(MHB_ERR_ARG, "hashed count needs 8-byte records (11 <= k <= 28) and 1 <= m <= %d", kHcHist);
+  if (!mhb_count_hashed_supported(k, m)) return mhb_set_error(MHB_ERR_ARG, "hashed count needs 8-byte records (13 <= k <= 28) and 1 <= m <= %d", kHcHist);
   if (!mul_hist || !n_solid_out || !ws) return mhb_set_error(MHB_ERR_ARG, "bad args");
   if (n == 0) return MHB_OK;
   if (n >= (1ull << 40)) return mhb_set_error(MHB_ERR_ARG, "too many records for one hashed count call");

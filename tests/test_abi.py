@@ -61,3 +61,17 @@ def test_no_cpu_fallback():
     with pytest.raises(lib.MhbError, match="no CUDA device"):
         lib.s2s_host(np.zeros(2, np.uint32), np.array([0, 2], np.uint64), np.array([30], np.uint32),
                      np.array([1], np.uint16), 21)
+
+
+def test_hashed_count_supported_range():
+    """the hashed count needs 8-byte records (13 <= k <= 28) and 1 <= m <= 1024; outside that range a call is refused
+    with MHB_ERR_ARG before it touches any pointer"""
+    L = lib.load()
+    for k, m in ((13, 2), (28, 2), (21, 1), (27, 1024)):
+        assert L.mhb_count_hashed_supported(k, m) == 1, (k, m)
+    for k, m in ((12, 2), (29, 2), (11, 2), (31, 2), (27, 0), (27, 1025), (27, -1)):
+        assert L.mhb_count_hashed_supported(k, m) == 0, (k, m)
+        rc = L.mhb_count_solid_hashed(None, None, None, 100, k, m, None, None, None, 0, None, None, None, 0)
+        assert rc == 1 and b"13 <= k <= 28" in L.mhb_last_error(), (k, m)
+    assert all(lib.count_record_words(k) == 2 for k in range(13, 29))
+    assert lib.count_record_words(12) == 1 and lib.count_record_words(29) == 3

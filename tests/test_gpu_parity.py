@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 from conftest import GOLDEN, golden_cases
+from count_reference import count_records_reference
 from megahit_b200 import formats as F
 from megahit_b200 import lib, synth
 
@@ -525,10 +526,11 @@ def _count_both_ways(recs: np.ndarray, k: int, m: int):
 @pytest.mark.parametrize("case", ["reads30x", "all_distinct", "one_bucket_many_keys", "one_key_huge", "few_keys_high_mult",
                                   "k21_reads", "m1", "m5", "tiny"])
 def test_hashed_count_matches_sort_and_count(case):
-    """mhb_count_solid_hashed (2 partition passes + per-bucket hash aggregation) gives the edges, aux flags, multiplicity
-    histogram and solid count of the full sort + mhb_count_solid, on real extractions and on adversarial key sets: a bucket
-    with more distinct keys than the table holds (sub-range retries), one key repeated beyond the 16-bit tally fields
-    (clamping between chunks), multiplicities above the shared-memory histogram"""
+    """mhb_count_solid_hashed (2 partition passes + per-bucket hash aggregation) and the full sort + mhb_count_solid both
+    give the edges, aux flags, multiplicity histogram and solid count of the NumPy reference (tests/count_reference.py),
+    on real extractions and on adversarial key sets: a bucket with more distinct keys than the table holds (sub-range
+    retries), one key repeated beyond the 16-bit tally fields (clamping between chunks), multiplicities above the
+    shared-memory histogram.  The cases aimed at single branches of the hash kernel are in tests/test_gpu_count.py."""
     torch = _torch()
     import ctypes as C
     import zlib
@@ -578,6 +580,9 @@ def test_hashed_count_matches_sort_and_count(case):
     (e0, a0, h0, n0), (e1, a1, h1, n1) = _count_both_ways(recs, k, m)
     assert n0 == n1 and (n0 > 0 or case == "all_distinct")
     assert (e0 == e1).all() and (a0 == a1).all() and (h0 == h1).all()
+    ref_e, ref_a, ref_h, ref_n = count_records_reference(recs, k, m)
+    assert n0 == ref_n
+    assert (e0.view(np.uint32) == ref_e.reshape(-1)).all() and (a0 == ref_a).all() and (h0 == ref_h).all()
 
 
 @pytest.mark.parametrize("words,n", [(2, 1), (2, 6911), (2, 700_001), (3, 450_007), (2, 3_000_000)])
