@@ -422,6 +422,9 @@ typedef struct {
   uint64_t *cand_ids;     /* want_edges: malloc'ed n_cand */
   int64_t *counting;      /* want_edges: malloc'ed 65536 */
   double t_total_ms, t_h2d_ms, t_count_ms, t_mercy_ms, t_s2s_ms, t_d2h_ms;
+  /* mhb_read2sdbg_host: passes over bucket ranges its stage 1 / stage 2 sort took (1 = the whole library at once, 0 = the
+   * stage did not run); mhb_build_host leaves both 0 */
+  uint32_t n_rounds_s1, n_rounds_s2;
 } mhb_build_result;
 
 /* A13: when the resident plan does not fit in device memory (cudaMalloc fails), or a round cap is set with
@@ -437,8 +440,17 @@ int mhb_build_host(const mhb_build_args *args, mhb_build_result *res);
  * builds the SdBG from the marked occurrences.  Same argument / result structs as mhb_build_host: want_edges is
  * ignored (this route writes no edges); res->counting (malloc'ed, 65536) = what stage 1 dumps to P.counting (zero for
  * m == 1), res->n_solid = distinct stage-2 items, t_count_ms / t_mercy_ms = bucket partition / kmsort emulation.
- * Stage 1 handles k <= 237 (records of at most 17 words); larger k with m > 1 returns MHB_ERR_ARG. */
+ * Stage 1 handles k <= 237 (records of at most 17 words); larger k with m > 1 returns MHB_ERR_ARG.
+ * Libraries larger than device memory: the package, its offsets, the solid / mercy bit planes and the multiplicity
+ * histogram stay resident; each stage decides on its own, from its exact record / item count and the free device memory
+ * (an arena cached by earlier host-level calls counts as free), whether it sorts the whole library at once or runs in
+ * rounds over contiguous ranges of 16-bit bucket ids (as the reference's Lv1 passes, base_engine.cpp:54-141, :254-281).
+ * res->n_rounds_s1 / n_rounds_s2 report the plan; the output does not depend on it.  A single bucket larger than a round
+ * returns MHB_ERR_NOMEM, as does a library whose resident part alone does not fit. */
 int mhb_read2sdbg_host(const mhb_build_args *args, mhb_build_result *res);
+/* Caps the stage-1 records / stage-2 items of one read2sdbg round regardless of memory (0 = derive from free device
+ * memory).  Independent of mhb_set_round_limit / mhb_set_s2s_round_limit.  The result does not depend on the caps. */
+int mhb_set_r2s_round_limit(uint64_t max_s1_records, uint64_t max_s2_items);
 
 /* `megahit_core iterate` (SURVEY.md 8f N2; main_iterate.cpp:117-221, iterate/contig_flank_index.h:16-221,
  * iterate/kmer_collector.h:37-79): the iterative edges for k + step - every (k+step+1)-mer of a read whose step+1

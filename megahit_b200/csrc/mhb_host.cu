@@ -141,6 +141,30 @@ extern "C" int mhb_release(void) {
   return MHB_OK;
 }
 
+size_t mhb_arena_bytes(void) { return g_arena.cap; }
+
+int SdbgStitch::append(void *stream, const uint8_t *d_bytes, uint64_t cap_bytes, const uint64_t *d_table,
+                       const uint64_t *d_totals) {
+  cudaStream_t st = (cudaStream_t)stream;
+  uint64_t rt[16];
+  CK(cudaMemcpyAsync(rt, d_totals, sizeof(rt), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(round_table.data(), d_table, round_table.size() * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  if (rt[0] > cap_bytes) return mhb_set_error(MHB_ERR_NOMEM, "internal: SdBG byte stream exceeds capacity");
+  const size_t base = bytes.size();
+  bytes.resize(base + rt[0]);
+  if (rt[0]) CK(cudaMemcpy(bytes.data() + base, d_bytes, rt[0], cudaMemcpyDeviceToHost));
+  for (size_t b = 0; b < (size_t)MHB_NUM_BUCKETS; ++b)
+    if (round_table[4 * b + 1]) {
+      table[4 * b + 0] = round_table[4 * b + 0] + base;
+      table[4 * b + 1] = round_table[4 * b + 1];
+      table[4 * b + 2] = round_table[4 * b + 2];
+      table[4 * b + 3] = round_table[4 * b + 3];
+    }
+  for (int i = 0; i < 16; ++i) tot[i] += rt[i];
+  return MHB_OK;
+}
+
 
 // ------------------------------------------------------------------------------------------------
 // The count stage on extracted records resident in d_a: either the LSD sort on every key byte followed by the
@@ -803,9 +827,7 @@ static int s2s_host_rounds(const mhb_s2s_args *args, mhb_s2s_result *res, const 
   if (n_ranges < 0) return MHB_ERR_NOMEM;
   res->t_extract_ms = t.stop();
 
-  std::vector<uint8_t> h_bytes;
-  std::vector<uint64_t> h_table((size_t)MHB_NUM_BUCKETS * 4), h_round_table((size_t)MHB_NUM_BUCKETS * 4);
-  uint64_t tot[16] = {0};
+  SdbgStitch out;
   for (int ri = 0; ri < n_ranges; ++ri) {
     t.start();
     CK(cudaMemsetAsync(d_hist0, 0, 256 * 8, st));
@@ -823,34 +845,19 @@ static int s2s_host_rounds(const mhb_s2s_args *args, mhb_s2s_result *res, const 
     res->t_sort_ms += t.stop();
     t.start();
     CKR(mhb_s2s_emit(st, in_b ? d_b : d_a, n_round, k, d_bytes, cap_bytes, d_table, d_totals, d_scratch, scratch_bytes));
-    uint64_t rt[16];
-    CK(cudaMemcpyAsync(rt, d_totals, sizeof(rt), cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(h_round_table.data(), d_table, h_round_table.size() * 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    if (rt[0] > cap_bytes) return mhb_set_error(MHB_ERR_NOMEM, "internal: SdBG byte stream exceeds capacity");
-    const size_t base = h_bytes.size();
-    h_bytes.resize(base + rt[0]);
-    if (rt[0]) CK(cudaMemcpy(h_bytes.data() + base, d_bytes, rt[0], cudaMemcpyDeviceToHost));
-    for (size_t b = 0; b < (size_t)MHB_NUM_BUCKETS; ++b)
-      if (h_round_table[4 * b + 1]) {
-        h_table[4 * b + 0] = h_round_table[4 * b + 0] + base;
-        h_table[4 * b + 1] = h_round_table[4 * b + 1];
-        h_table[4 * b + 2] = h_round_table[4 * b + 2];
-        h_table[4 * b + 3] = h_round_table[4 * b + 3];
-      }
-    for (int i = 0; i < 16; ++i) tot[i] += rt[i];
+    CKR(out.append(st, d_bytes, cap_bytes, d_table, d_totals));
     res->t_emit_ms += t.stop();
   }
-  res->n_bytes = tot[0];
-  res->n_items = tot[1];
-  res->n_tips = tot[2];
-  res->n_large_mul = tot[3];
-  for (int i = 0; i < 9; ++i) res->w_count[i] = tot[4 + i];
-  res->ones_in_last = tot[13];
-  memcpy(res->bucket_table, h_table.data(), sizeof(res->bucket_table));
-  res->bytes = (uint8_t *)malloc(std::max<size_t>(1, h_bytes.size()));
+  res->n_bytes = out.tot[0];
+  res->n_items = out.tot[1];
+  res->n_tips = out.tot[2];
+  res->n_large_mul = out.tot[3];
+  for (int i = 0; i < 9; ++i) res->w_count[i] = out.tot[4 + i];
+  res->ones_in_last = out.tot[13];
+  memcpy(res->bucket_table, out.table.data(), sizeof(res->bucket_table));
+  res->bytes = (uint8_t *)malloc(std::max<size_t>(1, out.bytes.size()));
   if (!res->bytes) return mhb_set_error(MHB_ERR_NOMEM, "host malloc failed");
-  if (!h_bytes.empty()) memcpy(res->bytes, h_bytes.data(), h_bytes.size());
+  if (!out.bytes.empty()) memcpy(res->bytes, out.bytes.data(), out.bytes.size());
   res->t_total_ms = t_all.stop();
   return MHB_OK;
 }

@@ -537,6 +537,48 @@ __global__ void __launch_bounds__(256) k_r2s_s1_extract(PkgView pv, u32 k, u32 *
   }
 }
 
+// Stage 1 in rounds (libraries whose records do not fit the device at once; base_engine.cpp:54-141, :254-281 plan Lv1
+// passes over bucket ranges the same way).  One warp per read, lane = emission index; the record's 16-bit bucket id is
+// the top of key word 0.  No atomics on the records and no reordering: a round's records come out in the same order
+// k_r2s_s1_extract gives them, so the stable bucket partition and kmsort see the reference's bucket input order.
+//   kS1Hist : hist[bucket id] += 1 over the whole library (the round planner's input)
+//   kS1Count: per_read[r] = number of records of read r with bucket id in [lo, hi]
+//   kS1Write: those records, stored from off[r] on (off = exclusive scan of the counts)
+enum { kS1Hist = 0, kS1Count = 1, kS1Write = 2 };
+template <int NW, int MODE>
+__global__ void __launch_bounds__(256) k_r2s_s1_range(PkgView pv, u32 k, u32 lo, u32 hi, unsigned long long *__restrict__ hist,
+                                                     u32 *__restrict__ per_read, const u64 *__restrict__ off, u32 *__restrict__ recs) {
+  const u32 lane = lane_id(), lt = lanemask_lt();
+  const u64 n_warps = (u64)gridDim.x * 8;
+  for (u64 r = ((u64)blockIdx.x * 256 + threadIdx.x) >> 5; r < pv.n_reads; r += n_warps) {
+    const u32 L = pv.L(r);
+    u64 run = MODE == kS1Write ? off[r] : 0;
+    if (L >= k + 1) {
+      const u32 n_e = L - k + 4, nwords = div_ceil(L, 16);
+      const u32 *s = pv.ptr(r);
+      const u64 base = pv.base(r);
+      for (u32 e0 = 0; e0 < n_e; e0 += 32) {
+        const u32 e = e0 + lane;
+        u32 rec[NW + 2];
+        bool in = false;
+        if (e < n_e) {
+          u32 p, want;
+          s1_emission(L, k, e, p, want);
+          make_s1_record<NW>(s, nwords, L, k, p, want, base, rec);
+          const u32 b = rec[0] >> 16;
+          if (MODE == kS1Hist) atomicAdd(&hist[b], 1ull);
+          in = b >= lo && b <= hi;
+        }
+        if (MODE == kS1Hist) continue;
+        const u32 mask = __ballot_sync(0xffffffffu, in);
+        if (MODE == kS1Write && in) st_rec<NW + 2>(recs, run + __popc(mask & lt), rec);
+        run += __popc(mask);
+      }
+    }
+    if (MODE == kS1Count && lane == 0) per_read[r] = (u32)run;
+  }
+}
+
 // first record of every 16-bit bucket in records sorted by their two leading bytes: bstart[b], b = 0..65536
 __global__ void k_r2s_bucket_bounds(const u32 *__restrict__ recs, u64 n, u32 rw, u64 *__restrict__ bstart) {
   const u32 b = blockIdx.x * blockDim.x + threadIdx.x;
@@ -833,11 +875,14 @@ MHB_HD u32 r2s_edge_types(const u32 *is_solid, bool sure, u64 b, u32 i, u32 L, u
   return types;
 }
 
-// WRITE = false: total number of items -> *cursor.  WRITE = true: items appended at recs[*cursor ...] in no
-// particular order (whole-record sort keys).  One thread per (k+1)-mer position.
-template <int W, bool WRITE>
+// MODE kS2Count: total number of items -> *cursor.  kS2Write: items appended at recs[*cursor ...] in no particular
+// order (whole-record sort keys).  For stage 2 in rounds: kS2Hist adds every item's 16-bit bucket id (top of word 0)
+// to hist[65536]; kS2Range appends only the items whose bucket id lies in [lo, hi].  One thread per (k+1)-mer position.
+enum { kS2Count = 0, kS2Write = 1, kS2Hist = 2, kS2Range = 3 };
+template <int W, int MODE>
 __global__ void __launch_bounds__(256) k_r2s_s2_extract(PkgView pv, u32 k, const u32 *__restrict__ is_solid, int sure, u64 n_edges,
-                                                       u32 *__restrict__ recs, unsigned long long *__restrict__ cursor, u64 capacity) {
+                                                       u32 *__restrict__ recs, unsigned long long *__restrict__ cursor, u64 capacity,
+                                                       u32 lo = 0, u32 hi = 0, unsigned long long *__restrict__ hist = nullptr) {
   const u32 lane = lane_id();
   u64 t0 = (u64)blockIdx.x * 256 + threadIdx.x;
   const u64 step = (u64)gridDim.x * 256;
@@ -860,8 +905,33 @@ __global__ void __launch_bounds__(256) k_r2s_s2_extract(PkgView pv, u32 k, const
       if (types) pal = edge_is_palindrome<W>(pv.ptr(r), div_ceil(L, 16), k, i) ? 1u : 0u;
     }
     const u32 cnt = (u32)__popc(types) * (pal ? 1u : 2u);
-    if (!WRITE) {
+    if (MODE == kS2Count) {
       local_total += cnt;
+      continue;
+    }
+    if (MODE == kS2Hist || MODE == kS2Range) {
+      // one (type, strand) slot at a time: a warp-aggregated append per slot for the items in range
+      const u32 *s = pv.ptr(r);
+      const u32 nwords = div_ceil(L, 16);
+      for (u32 slot = 0; slot < 6; ++slot) {
+        const u32 type = slot >> 1, strand = slot & 1u;
+        u32 rec[W];
+        bool in = false;
+        if (((types >> type) & 1u) && (strand == 0 || !pal)) {
+          make_r2s_item<W>(s, nwords, k, i, strand, type, rec);
+          const u32 b = rec[0] >> 16;
+          if (MODE == kS2Hist) atomicAdd(&hist[b], 1ull);
+          in = b >= lo && b <= hi;
+        }
+        if (MODE == kS2Hist) continue;
+        const u32 mask = __ballot_sync(0xffffffffu, in);
+        if (!mask) continue;
+        unsigned long long wbase = 0;
+        if (lane == 0) wbase = atomicAdd(cursor, (unsigned long long)__popc(mask));
+        wbase = __shfl_sync(0xffffffffu, wbase, 0);
+        const u64 dst = wbase + __popc(mask & lanemask_lt());
+        if (in && dst < capacity) st_rec<W>(recs, dst, rec);
+      }
       continue;
     }
     u32 inc = cnt;
@@ -889,7 +959,7 @@ __global__ void __launch_bounds__(256) k_r2s_s2_extract(PkgView pv, u32 k, const
       }
     }
   }
-  if (!WRITE) {
+  if (MODE == kS2Count) {
     for (int d = 16; d; d >>= 1) local_total += __shfl_xor_sync(0xffffffffu, local_total, d);
     if (lane == 0 && local_total) atomicAdd(cursor, local_total);
   }

@@ -82,7 +82,8 @@ class BuildResult(C.Structure):
                 ("ones_in_last", C.c_uint64), ("edges", C.POINTER(C.c_uint32)), ("cand_ids", C.POINTER(C.c_uint64)),
                 ("counting", C.POINTER(C.c_int64)),
                 ("t_total_ms", C.c_double), ("t_h2d_ms", C.c_double), ("t_count_ms", C.c_double),
-                ("t_mercy_ms", C.c_double), ("t_s2s_ms", C.c_double), ("t_d2h_ms", C.c_double)]
+                ("t_mercy_ms", C.c_double), ("t_s2s_ms", C.c_double), ("t_d2h_ms", C.c_double),
+                ("n_rounds_s1", C.c_uint32), ("n_rounds_s2", C.c_uint32)]
 
 
 class CountOpts(C.Structure):
@@ -123,7 +124,7 @@ class IterateOpts(C.Structure):
 SYMBOLS = [
     "mhb_last_error", "mhb_version", "mhb_device_count", "mhb_launch_count", "mhb_count_record_words", "mhb_words_per_edge",
     "mhb_s2s_record_words", "mhb_count_sort_bytes", "mhb_s2s_sort_bytes", "mhb_sort_workspace_bytes",
-    "mhb_count_extract", "mhb_check_fixed_len", "mhb_count_extract_range", "mhb_set_round_limit", "mhb_set_s2s_round_limit", "mhb_plan_rounds", "mhb_plan_rounds16", "mhb_sort_records", "mhb_sort_records_relaxed", "mhb_sort_pass_ms", "mhb_set_sort_cfg", "mhb_partition_scatter", "mhb_partition_scatter_hist", "mhb_plan_partition", "mhb_compact_tip_edges", "mhb_dev_malloc", "mhb_dev_free",
+    "mhb_count_extract", "mhb_check_fixed_len", "mhb_count_extract_range", "mhb_set_round_limit", "mhb_set_s2s_round_limit", "mhb_set_r2s_round_limit", "mhb_plan_rounds", "mhb_plan_rounds16", "mhb_sort_records", "mhb_sort_records_relaxed", "mhb_sort_pass_ms", "mhb_set_sort_cfg", "mhb_partition_scatter", "mhb_partition_scatter_hist", "mhb_plan_partition", "mhb_compact_tip_edges", "mhb_dev_malloc", "mhb_dev_free",
     "mhb_ipc_export", "mhb_ipc_open", "mhb_ipc_close", "mhb_count_solid_scratch_bytes", "mhb_count_solid", "mhb_count_hashed_supported", "mhb_count_hashed_workspace_bytes", "mhb_count_solid_hashed", "mhb_tipset_bytes",
     "mhb_tipset_build", "mhb_count_mark_mercy", "mhb_count_tip_edges", "mhb_s2s_extract", "mhb_s2s_extract_range",
     "mhb_s2s_emit_scratch_bytes", "mhb_s2s_emit", "mhb_set_device", "mhb_count_host", "mhb_s2s_host", "mhb_build_host", "mhb_free",
@@ -307,6 +308,14 @@ def set_s2s_round_limit(max_items: int = 0):
     _check(L.mhb_set_s2s_round_limit(int(max_items)))
 
 
+def set_r2s_round_limit(s1: int = 0, s2: int = 0):
+    """Cap the stage-1 records / stage-2 items per round of read2sdbg (0 = derive from free device memory); independent
+    of the count and seq2sdbg caps.  The result does not depend on the caps."""
+    L = load()
+    L.mhb_set_r2s_round_limit.argtypes = [C.c_uint64, C.c_uint64]
+    _check(L.mhb_set_r2s_round_limit(int(s1), int(s2)))
+
+
 def mercy_host(k: int, edges: np.ndarray, cand_bin: np.ndarray) -> np.ndarray:
     """GenMercyEdges on the device from host buffers: sorted `.edges` records + the `.cand` image -> mercy edge records."""
     L = load()
@@ -461,6 +470,7 @@ def read2sdbg_host(bin_words: np.ndarray, n_reads: int, k: int, m: int, need_mer
         "bytes": bytes(np.ctypeslib.as_array(r.bytes, (max(r.n_bytes, 1),))[: r.n_bytes]),
         "ms": {"total": r.t_total_ms, "h2d": r.t_h2d_ms, "s1_records_partition": r.t_count_ms, "kmsort": r.t_mercy_ms,
                "stage2": r.t_s2s_ms, "d2h": r.t_d2h_ms},
+        "n_rounds_s1": int(r.n_rounds_s1), "n_rounds_s2": int(r.n_rounds_s2),
     }
     L.mhb_free(r.bytes)
     L.mhb_free(r.bucket_table)
