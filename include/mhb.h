@@ -483,6 +483,45 @@ typedef struct {
 
 int mhb_iterate_host(const mhb_iterate_args *args, mhb_iterate_result *res);
 
+/* `megahit_core buildlib` (SURVEY.md 8f N3; sequence_lib.cpp:8-91, fastx_reader.cpp, kseq.h:193-246): FASTA/FASTQ text
+ * in, the `.bin` read library out, byte-identical to the reference.  Each stream is parsed on the device in chunks
+ * (line index, speculative record walk with a fix-up pass, TrimN, 2-bit packing; `pe` streams zipped by a kernel); a
+ * record that does not end inside a chunk is carried to the next one, and one larger than a chunk grows the chunk.
+ * The reference's batch rules are kept: a malformed record (quality of another length, a '+' line ending the file)
+ * ends the current batch of 4 Mi reads / 2^28 bases, and ends the library when it is the first record of a batch.
+ * type: "pe" (data[0], data[1] read in lockstep; the longer file's surplus is dropped), "se" or "interleaved"
+ * (data[0]); another type returns MHB_ERR_ARG "Valid types: pe, se, interleaved", an odd interleaved library
+ * MHB_ERR_ARG "PE library number of reads is odd: N!".  res->bin (the `.bin` image, ready for mhb_build_host /
+ * mhb_read2sdbg_host) and the per-library arrays are malloc'ed: free them with mhb_buildlib_free. */
+typedef struct {
+  const char *type;
+  const uint8_t *data[2];
+  uint64_t size[2];
+} mhb_buildlib_lib;
+
+typedef struct {
+  const mhb_buildlib_lib *libs;
+  uint32_t n_libs;
+} mhb_buildlib_args;
+
+typedef struct {
+  uint32_t *bin;
+  uint64_t bin_words;
+  uint64_t n_reads, n_bases; /* P.lib_info line 1 (an empty read stored as "A" counts one base) */
+  uint32_t n_libs;
+  uint64_t *lib_begin, *lib_end; /* per library: first read, one past its last read */
+  uint32_t *lib_max_len;
+  uint64_t n_chunks;             /* stream chunks parsed */
+  uint64_t n_walk_passes;        /* record-walk passes over all chunks (1 per chunk when every segment guessed right) */
+  double t_total_ms;
+} mhb_buildlib_result;
+
+int mhb_buildlib_host(const mhb_buildlib_args *args, mhb_buildlib_result *res);
+void mhb_buildlib_free(mhb_buildlib_result *res);
+/* Caps the text bytes of one parsed chunk (0 = the default, 256 MiB).  A record that does not fit grows its chunk.  The
+ * output does not depend on the cap. */
+int mhb_set_buildlib_chunk(uint64_t bytes);
+
 /* A11 from host buffers (SeqToSdbg::GenMercyEdges, seq_to_sdbg.cpp:171-357, as `seq2sdbg --need_mercy` runs it between
  * loading `.edges` / `.cand` and the sort): edges = n_edges sorted `.edges`-format records, cand_bin = the `.cand` image
  * (`.bin` record format, reads in the reversed orientation KmerCounter wrote them, kmer_counter.cpp:387-401).
@@ -551,6 +590,11 @@ int mhb_seq2sdbg_run(const mhb_seq2sdbg_opts *opts);
 int mhb_iterate_run(const mhb_iterate_opts *opts);
 /* writes P.sdbg.0, P.sdbg_info, P.counting (m > 1) and the (empty) P.mercy_cand.<i> temp files of the reference */
 int mhb_read2sdbg_run(const mhb_read2sdbg_opts *opts);
+/* `megahit_core buildlib lib_file out_prefix`: writes P.bin and P.lib_info.  The lib file is parsed with the reference's
+ * istream operations (a metadata line, `>> type`, `>> file(s)`, the rest of the line).  Inputs are read sequentially
+ * with read() (FIFOs work; nothing is seeked or mmap'ed).  Plain text only: gzip input and stdin are the CLI's to
+ * forward to the reference. */
+int mhb_buildlib_run(const char *lib_file, const char *out_prefix);
 
 /* `count` on n_gpus GPUs of this node (fixed-length read libraries; anything else, or n_gpus <= 1, runs mhb_count_run).
  * One worker process per GPU is forked; each takes a contiguous block of the reads, the records meet on the rank that
@@ -590,6 +634,11 @@ int mhb_selftest_r2s_s1_group(const uint32_t *recs, uint64_t n, uint32_t k, int3
                               int64_t *counting);
 /* `iterate` with the device code's __host__ __device__ building blocks driven serially on the host (CPU tests only) */
 int mhb_selftest_iterate(const mhb_iterate_args *args, mhb_iterate_result *res);
+/* buildlib: the line walk, TrimN and packing of the device code run serially over one whole stream (no batch rules).
+ * Per record (up to cap): trimmed length (0xFFFFFFFF = malformed record) and first kept position; bin_out = the `.bin`
+ * records of the well-formed ones. */
+int mhb_selftest_fastx(const uint8_t *text, uint64_t n, uint32_t *len_out, uint32_t *bpos_out, uint64_t cap,
+                       uint64_t *n_rec_out, uint32_t *bin_out, uint64_t bin_cap, uint64_t *bin_words_out);
 int mhb_selftest_r2s_mercy_read(uint32_t fixed_len, uint64_t n_reads, uint64_t r, uint32_t k, const uint32_t *is_solid,
                                 const uint32_t *no_in, const uint32_t *no_out, const uint32_t *any, uint32_t *mercy,
                                 uint32_t *added_out);

@@ -120,6 +120,21 @@ class IterateOpts(C.Structure):
                 ("num_cpu_threads", C.c_int32), ("k", C.c_uint32), ("step", C.c_uint32), ("output_prefix", C.c_char_p)]
 
 
+class BuildlibLib(C.Structure):
+    _fields_ = [("type", C.c_char_p), ("data", C.c_void_p * 2), ("size", C.c_uint64 * 2)]
+
+
+class BuildlibArgs(C.Structure):
+    _fields_ = [("libs", C.POINTER(BuildlibLib)), ("n_libs", C.c_uint32)]
+
+
+class BuildlibResult(C.Structure):
+    _fields_ = [("bin", C.POINTER(C.c_uint32)), ("bin_words", C.c_uint64), ("n_reads", C.c_uint64), ("n_bases", C.c_uint64),
+                ("n_libs", C.c_uint32), ("lib_begin", C.POINTER(C.c_uint64)), ("lib_end", C.POINTER(C.c_uint64)),
+                ("lib_max_len", C.POINTER(C.c_uint32)), ("n_chunks", C.c_uint64), ("n_walk_passes", C.c_uint64),
+                ("t_total_ms", C.c_double)]
+
+
 # every symbol include/mhb.h declares (tests/test_abi.py checks the header against this list)
 SYMBOLS = [
     "mhb_last_error", "mhb_version", "mhb_device_count", "mhb_launch_count", "mhb_count_record_words", "mhb_words_per_edge",
@@ -132,6 +147,7 @@ SYMBOLS = [
     "mhb_release", "mhb_count_run", "mhb_count_run_multi", "mhb_seq2sdbg_run", "mhb_selftest_count_record", "mhb_selftest_count_records_roll", "mhb_selftest_s2s_record",
     "mhb_iterate_host", "mhb_iterate_run", "mhb_selftest_iterate", "mhb_s2s_extract_edges_pruned", "mhb_s2s_emit_fmt", "mhb_read2sdbg_host", "mhb_read2sdbg_run", "mhb_selftest_r2s_s1_record", "mhb_selftest_r2s_item",
     "mhb_selftest_kmsort", "mhb_selftest_kmsort_smem", "mhb_selftest_r2s_s1_group", "mhb_selftest_r2s_mercy_read",
+    "mhb_buildlib_host", "mhb_buildlib_free", "mhb_set_buildlib_chunk", "mhb_buildlib_run", "mhb_selftest_fastx",
 ]
 
 
@@ -245,6 +261,13 @@ def load():
                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.mhb_selftest_r2s_mercy_read.argtypes = [C.c_uint32, C.c_uint64, C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p,
                                               C.c_void_p, C.c_void_p, C.POINTER(C.c_uint32)]
+    L.mhb_buildlib_host.argtypes = [C.POINTER(BuildlibArgs), C.POINTER(BuildlibResult)]
+    L.mhb_buildlib_free.argtypes = [C.POINTER(BuildlibResult)]
+    L.mhb_buildlib_free.restype = None
+    L.mhb_set_buildlib_chunk.argtypes = [C.c_uint64]
+    L.mhb_buildlib_run.argtypes = [C.c_char_p, C.c_char_p]
+    L.mhb_selftest_fastx.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64),
+                                     C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
     _lib = L
     return L
 
@@ -609,3 +632,57 @@ def selftest_kmsort(recs: np.ndarray, nw: int, smem: bool = False, cap: int = 65
     else:
         _check(load().mhb_selftest_kmsort(recs.ctypes.data, len(recs), nw))
     return recs
+
+
+def set_buildlib_chunk(n_bytes: int) -> None:
+    """Cap the text bytes of one parsed buildlib chunk (0 = default); the output does not depend on it."""
+    _check(load().mhb_set_buildlib_chunk(n_bytes))
+
+
+def buildlib_host(libs) -> dict:
+    """`buildlib` from in-memory text: libs = [(type, [bytes, ...])] with one buffer for se / interleaved and two for pe.
+    Returns the `.bin` image (uint32 array) and what P.lib_info holds."""
+    L = load()
+    arr = (BuildlibLib * max(len(libs), 1))()
+    keep = []
+    for i, (typ, datas) in enumerate(libs):
+        arr[i].type = typ.encode()
+        for j, d in enumerate(datas[:2]):
+            b = C.create_string_buffer(bytes(d), max(len(d), 1))
+            keep.append(b)
+            arr[i].data[j] = C.cast(b, C.c_void_p)
+            arr[i].size[j] = len(d)
+    a = BuildlibArgs(arr, len(libs))
+    r = BuildlibResult()
+    _check(L.mhb_buildlib_host(C.byref(a), C.byref(r)))
+    n = len(libs)
+    out = {
+        "bin": np.ctypeslib.as_array(r.bin, (max(r.bin_words, 1),))[: r.bin_words].copy(),
+        "n_reads": int(r.n_reads), "n_bases": int(r.n_bases),
+        "lib_begin": [int(r.lib_begin[i]) for i in range(n)], "lib_end": [int(r.lib_end[i]) for i in range(n)],
+        "lib_max_len": [int(r.lib_max_len[i]) for i in range(n)],
+        "n_chunks": int(r.n_chunks), "n_walk_passes": int(r.n_walk_passes), "ms": r.t_total_ms,
+    }
+    L.mhb_buildlib_free(C.byref(r))
+    return out
+
+
+def buildlib_run(lib_file: str, out_prefix: str) -> None:
+    """`megahit_core buildlib lib_file out_prefix`: writes out_prefix.bin and out_prefix.lib_info."""
+    _check(load().mhb_buildlib_run(lib_file.encode(), out_prefix.encode()))
+
+
+def selftest_fastx(text: bytes) -> dict:
+    """The device code's line walk, TrimN and packing run serially on the host over one stream (CPU tests only)."""
+    L = load()
+    buf = C.create_string_buffer(bytes(text), max(len(text), 1))
+    cap = text.count(b"\n") + 2
+    lens = np.zeros(cap, np.uint32)
+    bpos = np.zeros(cap, np.uint32)
+    bin_cap = 2 * cap + len(text) // 16 + 16
+    binw = np.zeros(bin_cap, np.uint32)
+    n_rec = C.c_uint64()
+    n_w = C.c_uint64()
+    _check(L.mhb_selftest_fastx(C.cast(buf, C.c_void_p), len(text), lens.ctypes.data, bpos.ctypes.data, cap, C.byref(n_rec),
+                                binw.ctypes.data, bin_cap, C.byref(n_w)))
+    return {"len": lens[: n_rec.value].copy(), "bpos": bpos[: n_rec.value].copy(), "bin": binw[: n_w.value].tobytes()}
