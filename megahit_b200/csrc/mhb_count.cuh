@@ -1,6 +1,9 @@
 // mhb_count.cuh -- `count` stage kernels: edge extraction, solid-edge counting, mercy bookkeeping.
 // Reference: voutcn/megahit src/sorting/kmer_counter.cpp (line numbers cited per kernel).
 #pragma once
+#include <stdlib.h>
+#include <string.h>
+
 #include "mhb.h"
 #include "mhb_kernels.cuh"
 
@@ -256,20 +259,63 @@ static __global__ void __launch_bounds__(1024) k_scan_u64(u64 *v, u64 nb, u64 *t
 
 // ------------------------------------------------------------------------------------------------
 // tip set: the solid edges that lack an incoming or outgoing solid neighbour (aux != 0), as
-//   u64 capacity (power of two), u64 filter_words (power of two),
-//   u32 filter[filter_words]           one-bit-per-hash prefilter (~32 bits per tip edge, L2 resident)
-//   u32 table[capacity][1 + W]         open addressing: flags (0 = empty) followed by the (k+1)-mer
+//   TipsetHeader (32 bytes)
+//   u32 filter[fold * filter_words]    blocked Bloom prefilter in global memory: one word per key, filter_bits bits
+//   u32 folded[filter_words]           (fold > 1 only) word i = OR of filter words [i*fold, (i+1)*fold)
+//   u32 table[capacity][slot words]    open addressing: flags (0 = empty), the (k+1)-mer, padding to 16 B for W = 2
+// A key's word is the multiply-high range reduction of one hash, so with fold words per folded word the folded filter
+// is the same blocked Bloom filter at 1/fold of the size: a key that passes the large filter passes the folded one.
+// When the tip set is resident, every mark CTA copies the folded filter (<= kTipFilterSmemWords words) into shared
+// memory and probes it first; only what passes it probes the large filter (L2), and only what passes that probes the
+// table.  Otherwise the kernels probe the large filter (~32 bits per tip edge) directly.  The table is the authority:
+// the filters only spare the mark kernels work, so their geometry changes speed, never a mark.
 // ------------------------------------------------------------------------------------------------
-__host__ __device__ inline u64 tipset_capacity(u64 n_tip) {
-  u64 c = 1024;
-  while (c < 2 * n_tip) c <<= 1;
-  return c;
+struct TipsetHeader {
+  u64 capacity;      // table slots, a power of two
+  u64 filter_words;  // words of the (folded) filter, a multiple of 4 (16-byte copies)
+  u32 fold;          // the global filter has fold * filter_words words
+  u32 filter_bits;   // bits set per key: 2 or 3
+  u32 resident;      // 1: the mark kernels probe the folded filter in shared memory first
+  u32 reserved;
+};
+static_assert(sizeof(TipsetHeader) == 32, "tip set header");
+static constexpr u64 kTipFilterSmemWords = 224 * 1024 / 4;  // 224 KiB of the 227 KiB an H100 CTA may have
+static constexpr u64 kTipMul = 0x9E3779B97F4A7C15ull;
+
+struct TipsetPlan {
+  u64 capacity, filter_words;
+  u32 fold, filter_bits, resident;
+  __host__ __device__ u64 global_words() const { return fold * filter_words; }
+  __host__ __device__ u64 folded_words() const { return fold > 1 ? filter_words : 0; }
+};
+
+// spec = $MHB_TIPSET_FILTER: "global" leaves out the shared-memory level; a number N makes the filter N words in one
+// level (fold 1; resident when it fits shared memory); anything else (or NULL) sizes it from n_tip: ~16 bits per tip
+// edge up to the shared-memory budget, folded from a global filter of >= 32 bits per tip edge, resident while the
+// budget holds >= 3 bits per tip edge (<= ~24 % false positives in shared memory).
+inline TipsetPlan tipset_plan(u64 n_tip, const char *spec) {
+  TipsetPlan p;
+  p.capacity = 1024;
+  while (p.capacity < 2 * n_tip) p.capacity <<= 1;
+  char *end = nullptr;
+  const unsigned long long forced = spec && *spec ? strtoull(spec, &end, 10) : 0ull;
+  if (forced > 0 && end && *end == '\0') {
+    p.filter_words = (forced + 3) & ~3ull;
+    p.fold = 1;
+    p.resident = p.filter_words <= kTipFilterSmemWords;
+  } else {
+    const u64 want = ((n_tip + 1) / 2 + 3) & ~3ull;
+    p.filter_words = want < 1024 ? 1024 : (want > kTipFilterSmemWords ? kTipFilterSmemWords : want);
+    p.fold = (u32)((n_tip + p.filter_words - 1) / p.filter_words);
+    if (p.fold < 1) p.fold = 1;
+    p.resident = 3 * n_tip <= 32 * kTipFilterSmemWords && !(spec && !strcmp(spec, "global"));
+  }
+  // 3 bits per key where the probed filter holds >= 5 bits per tip edge, else 2 (fewer false positives)
+  const u64 probed_words = p.resident ? p.filter_words : p.global_words();
+  p.filter_bits = 32 * probed_words >= 5 * n_tip ? 3 : 2;
+  return p;
 }
-__host__ __device__ inline u64 tipset_filter_words(u64 n_tip) {
-  u64 c = 1024;
-  while (c < n_tip) c <<= 1;
-  return c;
-}
+__host__ __device__ constexpr u32 tipset_slot_words(u32 W) { return W == 2 ? 4u : W + 1; }
 
 template <int W>
 __device__ __forceinline__ u32 hash_key(const u32 (&key)[W]) {
@@ -282,9 +328,31 @@ __device__ __forceinline__ u32 hash_key(const u32 (&key)[W]) {
   h *= 0x2C1B3C6Du;
   return h ^ (h >> 13);
 }
-__device__ __forceinline__ u32 hash2(u32 h) {  // second, independent-ish hash for the bit filter
-  h *= 0xC2B2AE3Du;
-  return h ^ (h >> 16);
+
+// filter hash of a (k+1)-mer (key words left-aligned, unused bits zero): for W <= 2 one 64-bit multiply of the
+// right-aligned 2(k+1)-bit value
+__device__ __forceinline__ u64 tip_filter_hash64(u64 key, u32 K1) { return (key >> (64 - 2 * K1)) * kTipMul; }
+template <int W>
+__device__ __forceinline__ u64 tip_filter_hash(const u32 (&key)[W], u32 K1) {
+  if constexpr (W == 1) {
+    return (u64)(key[0] >> (32 - 2 * K1)) * kTipMul;
+  } else if constexpr (W == 2) {
+    return tip_filter_hash64(((u64)key[0] << 32) | key[1], K1);
+  } else {
+    u64 a = 0;
+#pragma unroll
+    for (int j = 0; j < W; j += 2) {
+      a = (a ^ (((u64)key[j] << 32) | (j + 1 < W ? key[j + 1] : 0u))) * kTipMul;
+      a ^= a >> 32;
+    }
+    return a * kTipMul;
+  }
+}
+// word = multiply-high range reduction of the upper half; bit positions from bits 17..31 of the lower half
+__device__ __forceinline__ u32 tip_filter_word(u64 h, u32 n_words) { return __umulhi((u32)(h >> 32), n_words); }
+__device__ __forceinline__ u32 tip_filter_mask(u64 h, u32 bits) {
+  const u32 lo = (u32)h;
+  return (1u << (lo >> 27)) | (1u << ((lo >> 22) & 31u)) | (bits > 2 ? 1u << ((lo >> 17) & 31u) : 0u);
 }
 
 static __global__ void k_count_tips(const uint8_t *aux, u64 n, unsigned long long *out) {
@@ -297,22 +365,22 @@ static __global__ void k_count_tips(const uint8_t *aux, u64 n, unsigned long lon
 
 template <int W>
 __global__ void k_tipset_insert(const u32 *__restrict__ edges, const uint8_t *__restrict__ aux, u64 n, u32 k,
-                                u32 *filter, u64 filter_words, u32 *table, u64 cap) {
+                                u32 *filter, TipsetPlan plan, u32 *table) {
   const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n || aux[i] == 0) return;
-  const u32 WE = words_per_edge(k);
+  const u32 WE = words_per_edge(k), SW = tipset_slot_words(W);
   u32 key[W];
 #pragma unroll
   for (int j = 0; j < W; ++j) {
     const u32 keep = 2 * (k + 1) - 32 * j;
     key[j] = edges[i * WE + j] & top_mask(keep > 32 ? 32 : keep);
   }
-  const u32 h = hash_key<W>(key);
-  const u32 fb = hash2(h) & (u32)(filter_words * 32 - 1);
-  atomicOr(&filter[fb >> 5], 1u << (fb & 31));
-  u64 slot = h & (cap - 1);
+  const u64 fh = tip_filter_hash<W>(key, k + 1);
+  atomicOr(&filter[tip_filter_word(fh, (u32)plan.global_words())], tip_filter_mask(fh, plan.filter_bits));
+  const u64 cap = plan.capacity;
+  u64 slot = hash_key<W>(key) & (cap - 1);
   while (true) {
-    u32 *e = table + slot * (W + 1);
+    u32 *e = table + slot * SW;
     if (atomicCAS(e, 0u, (u32)aux[i]) == 0u) {
 #pragma unroll
       for (int j = 0; j < W; ++j) e[1 + j] = key[j];
@@ -322,164 +390,261 @@ __global__ void k_tipset_insert(const u32 *__restrict__ edges, const uint8_t *__
   }
 }
 
-// K-mercy (kmer_counter.cpp:307-367): per read min/max over the occurrences of tip edges.
-// One warp per read, straight from global memory (the library is ~3 % of the count stage's traffic and
-// L1 serves the re-reads), kMercyUnroll positions per lane per round so that the bit-filter probes of a
-// whole 150 bp read are in flight together; the kernel is bound by L2 latency, not bandwidth.
-static constexpr int kMercyUnroll = 4;
-
-template <int W, int WR>
-__global__ void __launch_bounds__(256)
-    k_mark_mercy(ReadsView rv, u32 k, const u32 *__restrict__ filter, u64 filter_words, const u32 *__restrict__ table,
-                 u64 cap, u32 *first_0_out, u32 *last_0_in) {
-  const u32 lane = lane_id();
-  const u32 K1 = k + 1;
-  const u32 fmask = (u32)(filter_words * 32 - 1);
-  for (u64 r = (u64)blockIdx.x * 8 + (threadIdx.x >> 5); r < rv.n_reads; r += (u64)gridDim.x * 8) {
-    const u32 *rec0 = rv.bin + rv.rec_start(r);
-    const u32 L = rec0[0];
-    const u32 *s = rec0 + 1;
-    const u32 nwords = div_ceil(L, 16);
-    u32 first = 0xFFFFFFFFu;
-    long long last = -1;
-    if (L >= K1) {
-      const u32 n_e = L - k;
-      for (u32 q0 = 0; q0 < n_e; q0 += 32 * kMercyUnroll) {
-        u32 key[kMercyUnroll][W], strand[kMercyUnroll], fw[kMercyUnroll], h[kMercyUnroll];
-        bool live[kMercyUnroll];
-#pragma unroll
-        for (int u = 0; u < kMercyUnroll; ++u) {
-          const u32 q = q0 + 32 * u + lane;
-          live[u] = q < n_e;
-          h[u] = 0;
-          fw[u] = 0;
-          strand[u] = 0;
-          if (live[u]) {
-            u32 rec[WR];
-            make_count_record<W, WR>(s, nwords, L, k, q, rec, strand[u]);
-#pragma unroll
-            for (int j = 0; j < W; ++j) {
-              const u32 keep = 2 * K1 - 32 * j;
-              key[u][j] = rec[j] & top_mask(keep > 32 ? 32 : keep);
-            }
-            h[u] = hash_key<W>(key[u]);
-            fw[u] = filter[(hash2(h[u]) & fmask) >> 5];
-          }
-        }
-#pragma unroll
-        for (int u = 0; u < kMercyUnroll; ++u) {
-          if (!live[u] || !((fw[u] >> (hash2(h[u]) & 31)) & 1u)) continue;
-          u64 slot = h[u] & (cap - 1);
-          u32 flags = 0;
-          while (true) {
-            const u32 *e = table + slot * (W + 1);
-            const u32 f = e[0];
-            if (f == 0) break;
-            bool eq = true;
-#pragma unroll
-            for (int j = 0; j < W; ++j) eq = eq && e[1 + j] == key[u][j];
-            if (eq) {
-              flags = f;
-              break;
-            }
-            slot = (slot + 1) & (cap - 1);
-          }
-          if (flags) {
-            const u32 off = L - K1 - (q0 + 32 * u + lane);  // offset in the reversed (package) read
-            // no in, strand 0 -> last; no in, strand 1 -> first; no out, strand 0 -> first; no out, strand 1 -> last
-            const bool to_last = ((flags & 1u) && strand[u] == 0) || ((flags & 2u) && strand[u] == 1);
-            const bool to_first = ((flags & 1u) && strand[u] == 1) || ((flags & 2u) && strand[u] == 0);
-            if (to_last) last = last > (long long)off ? last : (long long)off;
-            if (to_first) first = first < off + 1 ? first : off + 1;
-          }
-        }
-      }
-    }
-    for (int d = 16; d; d >>= 1) {
-      const u32 f2 = __shfl_xor_sync(0xffffffffu, first, d);
-      const long long l2 = __shfl_xor_sync(0xffffffffu, last, d);
-      first = first < f2 ? first : f2;
-      last = last > l2 ? last : l2;
-    }
-    if (lane == 0) {
-      first_0_out[r] = first;
-      last_0_in[r] = last < 0 ? 0xFFFFFFFFu : (u32)last;
-    }
+static __global__ void k_tipset_fold(const u32 *__restrict__ filter, u64 n, u32 fold, u32 *__restrict__ folded) {
+  for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) {
+    u32 w = 0;
+    for (u32 j = 0; j < fold; ++j) w |= filter[i * fold + j];
+    folded[i] = w;
   }
 }
 
-// Rolling variant of k_mark_mercy for 8-byte records (opt-in with MHB_EXTRACT_ROLL=1): a lane re-derives four
-// consecutive canonical (k+1)-mers with make_count_records_roll and probes the filter for all four at once.
-static __global__ void __launch_bounds__(256)
-    k_mark_mercy_roll(ReadsView rv, u32 k, const u32 *__restrict__ filter, u64 filter_words, const u32 *__restrict__ table,
-                      u64 cap, u32 *first_0_out, u32 *last_0_in) {
-  constexpr int W = 2;
+// K-mercy (kmer_counter.cpp:307-367): per read min/max over the occurrences of tip edges.
+// A persistent grid of one kMarkThreads CTA per SM (the folded filter takes the SM's shared memory); a warp walks whole
+// reads straight from global memory (L1 serves the re-reads).  With a resident tip set a position costs the cheap
+// filter hash and one shared-memory load; the global filter (L2) is probed only on a hit there, hash_key and the
+// table probe only on a hit in both.  Otherwise the same code probes the global filter first.
+static constexpr int kMarkThreads = 1024;
+
+struct TipsetDev {
+  const u32 *filter;  // the global filter
+  const u32 *table;
+  u32 n1, n2, filter_bits;  // words of the first / second filter level probed (n2 = 0: no second level)
+  u64 cap;
+  bool smem;
+};
+// reads the header; copies the folded filter to s_filter when the tip set is resident and it fits the dynamic shared
+// memory launched.  The first level is then s_filter and the second the global filter; otherwise the global filter
+// is the only level.
+__device__ __forceinline__ TipsetDev tipset_open(const void *tipset, u32 smem_words, u32 *s_filter) {
+  const TipsetHeader hd = *reinterpret_cast<const TipsetHeader *>(tipset);
+  TipsetPlan p;
+  p.capacity = hd.capacity;
+  p.filter_words = hd.filter_words;
+  p.fold = hd.fold;
+  TipsetDev t;
+  t.filter = reinterpret_cast<const u32 *>((const char *)tipset + sizeof(TipsetHeader));
+  t.table = t.filter + p.global_words() + p.folded_words();
+  t.filter_bits = hd.filter_bits;
+  t.cap = hd.capacity;
+  t.smem = hd.resident && hd.filter_words <= smem_words;
+  t.n1 = t.smem ? (u32)hd.filter_words : (u32)p.global_words();
+  t.n2 = t.smem && hd.fold > 1 ? (u32)p.global_words() : 0u;
+  if (t.smem) {
+    const uint4 *src = reinterpret_cast<const uint4 *>(t.filter + (hd.fold > 1 ? p.global_words() : 0));
+    for (u32 i = threadIdx.x; i < t.n1 / 4; i += blockDim.x) reinterpret_cast<uint4 *>(s_filter)[i] = src[i];
+    __syncthreads();
+  }
+  return t;
+}
+
+// the per-read result: no in, strand 0 -> last; no in, strand 1 -> first; no out, strand 0 -> first; no out,
+// strand 1 -> last (off = offset in the reversed (package) read)
+__device__ __forceinline__ void mercy_note(u32 flags, u32 strand, u32 off, u32 &first, long long &last) {
+  const bool to_last = ((flags & 1u) && strand == 0) || ((flags & 2u) && strand == 1);
+  const bool to_first = ((flags & 1u) && strand == 1) || ((flags & 2u) && strand == 0);
+  if (to_last) last = last > (long long)off ? last : (long long)off;
+  if (to_first) first = first < off + 1 ? first : off + 1;
+}
+__device__ __forceinline__ void mercy_store(u64 r, u32 first, long long last, u32 *first_0_out, u32 *last_0_in) {
+  for (int d = 16; d; d >>= 1) {
+    const u32 f2 = __shfl_xor_sync(0xffffffffu, first, d);
+    const long long l2 = __shfl_xor_sync(0xffffffffu, last, d);
+    first = first < f2 ? first : f2;
+    last = last > l2 ? last : l2;
+  }
+  if (lane_id() == 0) {
+    first_0_out[r] = first;
+    last_0_in[r] = last < 0 ? 0xFFFFFFFFu : (u32)last;
+  }
+}
+
+static constexpr int kMercyUnroll = 4;
+// wide keys need more than the 64 registers a thread of a 1024-thread CTA may have
+__host__ __device__ constexpr int mark_threads(int W) { return W <= 3 ? kMarkThreads : 256; }
+
+template <int W, int WR>
+__global__ void __launch_bounds__(mark_threads(W), 1)
+    k_mark_mercy(ReadsView rv, u32 k, const void *__restrict__ tipset, u32 smem_words, u32 *first_0_out, u32 *last_0_in) {
+  extern __shared__ __align__(16) u32 s_filter[];
+  const TipsetDev ts = tipset_open(tipset, smem_words, s_filter);
   const u32 lane = lane_id();
-  const u32 K1 = k + 1;
-  const u32 fmask = (u32)(filter_words * 32 - 1);
-  for (u64 r = (u64)blockIdx.x * 8 + (threadIdx.x >> 5); r < rv.n_reads; r += (u64)gridDim.x * 8) {
-    const u32 *rec0 = rv.bin + rv.rec_start(r);
-    const u32 L = rec0[0];
-    const u32 *s = rec0 + 1;
-    const u32 nwords = div_ceil(L, 16);
-    u32 first = 0xFFFFFFFFu;
-    long long last = -1;
-    if (L >= K1) {
-      const u32 n_e = L - k;
-      for (u32 q0 = 0; q0 < n_e; q0 += 128) {
-        const u32 q = q0 + 4 * lane;
-        u32 key[4][W], strand[4] = {0, 0, 0, 0}, fw[4] = {0, 0, 0, 0}, h[4] = {0, 0, 0, 0};
-        bool live[4] = {false, false, false, false};
-        if (q < n_e) {
-          u64 rec[4];
-          make_count_records_roll<4>(s, nwords, L, k, q, rec, strand);
+  const u32 K1 = k + 1, SW = tipset_slot_words(W);
+  constexpr u32 NW = mark_threads(W) / 32;
+  auto scan = [&](const u32 *__restrict__ filter) {
+    for (u64 r = (u64)blockIdx.x * NW + (threadIdx.x >> 5); r < rv.n_reads; r += (u64)gridDim.x * NW) {
+      const u32 *rec0 = rv.bin + rv.rec_start(r);
+      const u32 L = rec0[0];
+      const u32 *s = rec0 + 1;
+      const u32 nwords = div_ceil(L, 16);
+      u32 first = 0xFFFFFFFFu;
+      long long last = -1;
+      if (L >= K1) {
+        const u32 n_e = L - k;
+        for (u32 q0 = 0; q0 < n_e; q0 += 32 * kMercyUnroll) {
+          u32 key[kMercyUnroll][W], strand[kMercyUnroll];
+          u64 fh[kMercyUnroll];
+          bool hit[kMercyUnroll];
 #pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            live[u] = q + u < n_e;
-            key[u][0] = (u32)(rec[u] >> 32);
-            key[u][1] = (u32)rec[u] & ~63u;  // drop prev/next: the (k+1)-mer alone, as the tip set stores it
-            if (live[u]) {
-              h[u] = hash_key<W>(key[u]);
-              fw[u] = filter[(hash2(h[u]) & fmask) >> 5];
+          for (int u = 0; u < kMercyUnroll; ++u) {
+            const u32 q = q0 + 32 * u + lane;
+            hit[u] = false;
+            strand[u] = 0;
+            if (q < n_e) {
+              u32 rec[WR];
+              make_count_record<W, WR>(s, nwords, L, k, q, rec, strand[u]);
+#pragma unroll
+              for (int j = 0; j < W; ++j) {
+                const u32 keep = 2 * K1 - 32 * j;
+                key[u][j] = rec[j] & top_mask(keep > 32 ? 32 : keep);
+              }
+              fh[u] = tip_filter_hash<W>(key[u], K1);
+              const u32 mask = tip_filter_mask(fh[u], ts.filter_bits);
+              hit[u] = (filter[tip_filter_word(fh[u], ts.n1)] & mask) == mask;
             }
           }
-        }
+          if (ts.n2) {
 #pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          if (!live[u] || !((fw[u] >> (hash2(h[u]) & 31)) & 1u)) continue;
-          u64 slot = h[u] & (cap - 1);
-          u32 flags = 0;
-          while (true) {
-            const u32 *e = table + slot * (W + 1);
-            const u32 f = e[0];
-            if (f == 0) break;
-            if (e[1] == key[u][0] && e[2] == key[u][1]) {
-              flags = f;
-              break;
+            for (int u = 0; u < kMercyUnroll; ++u) {
+              const u32 mask = tip_filter_mask(fh[u], ts.filter_bits);
+              if (hit[u]) hit[u] = (ts.filter[tip_filter_word(fh[u], ts.n2)] & mask) == mask;
             }
-            slot = (slot + 1) & (cap - 1);
           }
-          if (flags) {
-            const u32 off = L - K1 - (q + u);  // offset in the reversed (package) read
-            const bool to_last = ((flags & 1u) && strand[u] == 0) || ((flags & 2u) && strand[u] == 1);
-            const bool to_first = ((flags & 1u) && strand[u] == 1) || ((flags & 2u) && strand[u] == 0);
-            if (to_last) last = last > (long long)off ? last : (long long)off;
-            if (to_first) first = first < off + 1 ? first : off + 1;
+#pragma unroll
+          for (int u = 0; u < kMercyUnroll; ++u) {
+            if (!hit[u]) continue;
+            u64 slot = hash_key<W>(key[u]) & (ts.cap - 1);
+            u32 flags = 0;
+            while (true) {
+              const u32 *e = ts.table + slot * SW;
+              const u32 f = e[0];
+              if (f == 0) break;
+              bool eq = true;
+#pragma unroll
+              for (int j = 0; j < W; ++j) eq = eq && e[1 + j] == key[u][j];
+              if (eq) {
+                flags = f;
+                break;
+              }
+              slot = (slot + 1) & (ts.cap - 1);
+            }
+            if (flags) mercy_note(flags, strand[u], L - K1 - (q0 + 32 * u + lane), first, last);
           }
         }
       }
+      mercy_store(r, first, last, first_0_out, last_0_in);
     }
-    for (int d = 16; d; d >>= 1) {
-      const u32 f2 = __shfl_xor_sync(0xffffffffu, first, d);
-      const long long l2 = __shfl_xor_sync(0xffffffffu, last, d);
-      first = first < f2 ? first : f2;
-      last = last > l2 ? last : l2;
-    }
-    if (lane == 0) {
-      first_0_out[r] = first;
-      last_0_in[r] = last < 0 ? 0xFFFFFFFFu : (u32)last;
-    }
+  };
+  if (ts.smem)
+    scan(s_filter);
+  else
+    scan(ts.filter);
+}
+
+// The canonical (k+1)-mers (low 64 - 2(k+1) bits zero) and strands of R consecutive positions q.. of a read,
+// 17 <= k+1 <= 29: make_count_records_roll without the prev/next bases and the forward string S, which the marks do not
+// need.  Entries for positions past the read's end are garbage.
+template <int R>
+__device__ __forceinline__ void canon_keys_roll(const u32 *s, u32 nwords, u32 k, u32 q, u64 (&key)[R], u32 (&strand)[R]) {
+  const u32 K1 = k + 1;
+  const u32 T = 64u - 2u * K1;  // 6..30
+  const u32 w0 = q >> 4, sh = (q & 15) * 2;
+  const u32 x0 = s[w0];
+  const u32 x1 = (w0 + 1 < nwords) ? s[w0 + 1] : 0u;
+  const u32 x2 = (w0 + 2 < nwords) ? s[w0 + 2] : 0u;
+  const u32 x3 = (w0 + 3 < nwords) ? s[w0 + 3] : 0u;
+  const u64 S = ((((u64)fshl(x0, x1, sh) << 32) | fshl(x1, x2, sh)) >> T) << T;
+  u64 B = ((~S) >> T) << T;                                         // complement(S)
+  u64 A = (((u64)rev2((u32)S) << 32) | rev2((u32)(S >> 32))) << T;  // reverse(S)
+  const u32 pi = q + K1;
+  const u32 wa = (pi >> 4) - w0;  // 1 or 2
+  u32 LA = fshl(wa == 1 ? x1 : x2, wa == 1 ? x2 : x3, (pi & 15) * 2);
+  const u64 lowmask = ~((1ull << T) - 1ull);
+#pragma unroll
+  for (int j = 0; j < R; ++j) {
+    const bool st = B < A;
+    key[j] = st ? B : A;
+    strand[j] = st ? 1u : 0u;
+    const u32 b = LA >> 30;
+    B = (B << 2) | (u64)((3u - b) << T);
+    A = ((A >> 2) & lowmask) | ((u64)b << 62);
+    LA <<= 2;
   }
+}
+
+// Rolling variant of k_mark_mercy for 8-byte records (17 <= k+1 <= 29, the default there; MHB_EXTRACT_ROLL=0 selects
+// k_mark_mercy<2, 2>): a lane re-derives four consecutive canonical (k+1)-mers with canon_keys_roll and probes the
+// filter for all four; the table probes of the hits are issued together as single 16-byte slot loads.
+static __global__ void __launch_bounds__(kMarkThreads, 1)
+    k_mark_mercy_roll(ReadsView rv, u32 k, const void *__restrict__ tipset, u32 smem_words, u32 *first_0_out,
+                      u32 *last_0_in) {
+  extern __shared__ __align__(16) u32 s_filter[];
+  const TipsetDev ts = tipset_open(tipset, smem_words, s_filter);
+  const u32 lane = lane_id();
+  const u32 K1 = k + 1;
+  constexpr u32 NW = kMarkThreads / 32;
+  const uint4 *table = reinterpret_cast<const uint4 *>(ts.table);
+  auto scan = [&](const u32 *__restrict__ filter) {
+    for (u64 r = (u64)blockIdx.x * NW + (threadIdx.x >> 5); r < rv.n_reads; r += (u64)gridDim.x * NW) {
+      const u32 *rec0 = rv.bin + rv.rec_start(r);
+      const u32 L = rec0[0];
+      const u32 *s = rec0 + 1;
+      const u32 nwords = div_ceil(L, 16);
+      u32 first = 0xFFFFFFFFu;
+      long long last = -1;
+      if (L >= K1) {
+        const u32 n_e = L - k;
+        for (u32 q0 = 0; q0 < n_e; q0 += 128) {
+          const u32 q = q0 + 4 * lane;
+          u64 rec[4];
+          u32 strand[4] = {0, 0, 0, 0};
+          bool hit[4] = {false, false, false, false};
+          if (q < n_e) {
+            canon_keys_roll<4>(s, nwords, k, q, rec, strand);
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+              const u64 fh = tip_filter_hash64(rec[u], K1);
+              const u32 mask = tip_filter_mask(fh, ts.filter_bits);
+              hit[u] = q + u < n_e && (filter[tip_filter_word(fh, ts.n1)] & mask) == mask;
+            }
+          }
+          if (!(hit[0] | hit[1] | hit[2] | hit[3])) continue;
+          if (ts.n2) {
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+              const u64 fh = tip_filter_hash64(rec[u], K1);
+              const u32 mask = tip_filter_mask(fh, ts.filter_bits);
+              if (hit[u]) hit[u] = (ts.filter[tip_filter_word(fh, ts.n2)] & mask) == mask;
+            }
+            if (!(hit[0] | hit[1] | hit[2] | hit[3])) continue;
+          }
+          u64 slot[4];
+          uint4 e[4];
+#pragma unroll
+          for (int u = 0; u < 4; ++u) {
+            if (!hit[u]) continue;
+            const u32 key[2] = {(u32)(rec[u] >> 32), (u32)rec[u]};
+            slot[u] = hash_key<2>(key) & (ts.cap - 1);
+            e[u] = table[slot[u]];
+          }
+#pragma unroll
+          for (int u = 0; u < 4; ++u) {
+            if (!hit[u]) continue;
+            const u32 k0 = (u32)(rec[u] >> 32), k1 = (u32)rec[u];
+            while (e[u].x != 0 && !(e[u].y == k0 && e[u].z == k1)) {
+              slot[u] = (slot[u] + 1) & (ts.cap - 1);
+              e[u] = table[slot[u]];
+            }
+            if (e[u].x) mercy_note(e[u].x, strand[u], L - K1 - (q + u), first, last);
+          }
+        }
+      }
+      mercy_store(r, first, last, first_0_out, last_0_in);
+    }
+  };
+  if (ts.smem)
+    scan(s_filter);
+  else
+    scan(ts.filter);
 }
 
 

@@ -287,8 +287,14 @@ extern "C" size_t mhb_count_solid_scratch_bytes(uint64_t n) {
 // ------------------------------------------------------------------------------------------------
 // count: mercy bookkeeping
 // ------------------------------------------------------------------------------------------------
+// the filter plan of a tip set of n_tip edges ($MHB_TIPSET_FILTER is read at every call, so that one process can time
+// two plans against each other; the mark kernels take the plan from the tip set's header, not from here)
+static TipsetPlan tipset_plan_env(uint64_t n_tip) { return tipset_plan(n_tip, getenv("MHB_TIPSET_FILTER")); }
+
 extern "C" size_t mhb_tipset_bytes(uint64_t n_tip_edges, uint32_t k) {
-  return 16 + tipset_filter_words(n_tip_edges) * 4 + tipset_capacity(n_tip_edges) * (size_t)(count_key_words(k) + 1) * 4;
+  const TipsetPlan p = tipset_plan_env(n_tip_edges);
+  return sizeof(TipsetHeader) + (p.global_words() + p.folded_words()) * 4 +
+         p.capacity * (size_t)tipset_slot_words(count_key_words(k)) * 4;
 }
 
 // a few device words for scalar results, allocated once per device (cudaMallocAsync/cudaFreeAsync per call
@@ -321,19 +327,47 @@ extern "C" int mhb_tipset_build(void *stream, const uint32_t *edges, const uint8
                                 void *tipset, size_t tipset_bytes, uint64_t n_tip_edges) {
   if (tipset_bytes < mhb_tipset_bytes(n_tip_edges, k)) return mhb_set_error(MHB_ERR_ARG, "tipset too small");
   cudaStream_t st = (cudaStream_t)stream;
-  const u64 hdr[2] = {tipset_capacity(n_tip_edges), tipset_filter_words(n_tip_edges)};
-  const u64 cap = hdr[0], fwords = hdr[1];
+  const TipsetPlan plan = tipset_plan_env(n_tip_edges);
+  TipsetHeader hdr;
+  memset(&hdr, 0, sizeof(hdr));
+  hdr.capacity = plan.capacity;
+  hdr.filter_words = plan.filter_words;
+  hdr.fold = plan.fold;
+  hdr.filter_bits = plan.filter_bits;
+  hdr.resident = plan.resident;
   CK(cudaMemsetAsync(tipset, 0, mhb_tipset_bytes(n_tip_edges, k), st));
-  CK(cudaMemcpyAsync(tipset, hdr, 16, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(tipset, &hdr, sizeof(hdr), cudaMemcpyHostToDevice, st));
   if (n_solid == 0) return MHB_OK;
-  u32 *filter = (u32 *)((char *)tipset + 16);
-  u32 *table = filter + fwords;
+  u32 *filter = (u32 *)((char *)tipset + sizeof(TipsetHeader));
+  u32 *table = filter + plan.global_words() + plan.folded_words();
   const u32 W = count_key_words(k);
   const u64 g = (n_solid + 255) / 256;
 #define M(WW) \
-  if (W == WW) k_tipset_insert<WW><<<(unsigned)g, 256, 0, st>>>(edges, aux, n_solid, k, filter, fwords, table, cap);
+  if (W == WW) k_tipset_insert<WW><<<(unsigned)g, 256, 0, st>>>(edges, aux, n_solid, k, filter, plan, table);
   MHB_FOR_W(M)
 #undef M
+  CK_LAUNCH();
+  if (plan.fold > 1) {
+    k_tipset_fold<<<(unsigned)((plan.filter_words + 255) / 256), 256, 0, st>>>(filter, plan.filter_words, plan.fold,
+                                                                              filter + plan.global_words());
+    CK_LAUNCH();
+  }
+  return MHB_OK;
+}
+
+// persistent grid of `threads`-thread CTAs with smem_words words of dynamic shared memory for the filter
+template <class Kernel>
+static int launch_mark(Kernel kern, int threads, const ReadsView &rv, uint32_t k, const void *tipset, u32 smem_words,
+                       uint32_t *first_0_out, uint32_t *last_0_in, cudaStream_t st) {
+  const size_t smem = (size_t)smem_words * 4;
+  CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  int bps = 0;
+  CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, kern, threads, smem));
+  if (bps < 1) return mhb_set_error(MHB_ERR_CUDA, "mercy-mark kernel: no CTA of %d threads and %zu B fits an SM", threads, smem);
+  const u64 warps = threads / 32;
+  u64 grid = (u64)sm_count() * bps;
+  if (grid > (rv.n_reads + warps - 1) / warps) grid = (rv.n_reads + warps - 1) / warps;
+  kern<<<(unsigned)grid, threads, smem, st>>>(rv, k, tipset, smem_words, first_0_out, last_0_in);
   CK_LAUNCH();
   return MHB_OK;
 }
@@ -347,30 +381,21 @@ extern "C" int mhb_count_mark_mercy(void *stream, const mhb_dev_reads *reads, ui
   cudaStream_t st = (cudaStream_t)stream;
   const ReadsView rv = make_reads_view(reads);
   const u32 W = count_key_words(k), WR = count_record_words(k);
-  const u64 cap = tipset_capacity(n_tip_edges), fwords = tipset_filter_words(n_tip_edges);
-  const u32 *filter = (const u32 *)((const char *)tipset + 16);
-  const u32 *table = filter + fwords;
-  u64 g64 = (rv.n_reads + 7) / 8;
-  if (g64 > (u64)sm_count() * 16) g64 = (u64)sm_count() * 16;
-  const int grid = (int)g64;
+  const TipsetPlan plan = tipset_plan_env(n_tip_edges);
+  const u32 smem_words = plan.resident ? (u32)plan.filter_words : 0u;
   // rolling record builder (4 positions per lane, three of them by shifting); MHB_EXTRACT_ROLL=0 selects the
   // per-position kernel
   static const bool roll = !(getenv("MHB_EXTRACT_ROLL") && !strcmp(getenv("MHB_EXTRACT_ROLL"), "0"));
-  if (roll && W == 2 && WR == 2 && k + 1 >= 17) {
-    k_mark_mercy_roll<<<grid, 256, 0, st>>>(rv, k, filter, fwords, table, cap, first_0_out, last_0_in);
-    CK_LAUNCH();
-    return MHB_OK;
-  }
+  if (roll && W == 2 && WR == 2 && k + 1 >= 17)
+    return launch_mark(k_mark_mercy_roll, kMarkThreads, rv, k, tipset, smem_words, first_0_out, last_0_in, st);
 #define M(WW)                                                                                                          \
   if (W == WW && WR == WW)                                                                                             \
-    k_mark_mercy<WW, WW><<<grid, 256, 0, st>>>(rv, k, filter, fwords, table, cap, first_0_out, last_0_in);              \
+    return launch_mark(k_mark_mercy<WW, WW>, mark_threads(WW), rv, k, tipset, smem_words, first_0_out, last_0_in, st);                   \
   else if (W == WW && WR == WW + 1)                                                                                    \
-    k_mark_mercy<WW, WW + 1><<<grid, 256, 0, st>>>(rv, k, filter, fwords, table, cap, first_0_out, last_0_in);          \
+    return launch_mark(k_mark_mercy<WW, WW + 1>, mark_threads(WW), rv, k, tipset, smem_words, first_0_out, last_0_in, st);               \
   else
   MHB_FOR_W(M) return mhb_set_error(MHB_ERR_ARG, "unsupported k=%u", k);
 #undef M
-  CK_LAUNCH();
-  return MHB_OK;
 }
 
 // ------------------------------------------------------------------------------------------------
