@@ -122,6 +122,20 @@ int mhb_sort_records(void *stream, uint32_t *a, uint32_t *b, uint64_t n, uint32_
 int mhb_sort_records_relaxed(void *stream, uint32_t *a, uint32_t *b, uint64_t n, uint32_t words, const uint8_t *bytes,
                              uint32_t n_bytes, const uint64_t *first_hist, void *ws, size_t ws_bytes, int *result_in_b);
 
+/* The seq2sdbg item sort: the contract of mhb_sort_records_relaxed on mhb_s2s_sort_bytes(k) (ascending on those bytes,
+ * a permutation of the input, order among equal keys unspecified) for n items of mhb_s2s_record_words(k) words.  For
+ * 9 <= k <= 38 it runs two radix passes on the 16-bit bucket (the first eight bases) and finishes every bucket in shared
+ * memory (up to 403 M items; larger sorts are the full relaxed sort); a, b must then be 16-byte aligned.  first_hist
+ * (may be NULL): the 256-bin histogram of record byte mhb_s2s_sort_hist_byte(n, k), as the extract kernels make it.  ws: mhb_s2s_sort_workspace_bytes(n, k) bytes.  May
+ * synchronise the stream once.  Leaves ONE entry in the mhb_sort_pass_ms ring (its global passes). */
+int mhb_s2s_sort(void *stream, uint32_t *a, uint32_t *b, uint64_t n, uint32_t k, const uint64_t *first_hist, void *ws,
+                 size_t ws_bytes, int *result_in_b);
+size_t mhb_s2s_sort_workspace_bytes(uint64_t n, uint32_t k);
+int mhb_s2s_sort_hist_byte(uint64_t n, uint32_t k);
+/* buckets the last mhb_s2s_sort of this process left to the radix engine and their items; buckets it sorted with the
+ * large shared-memory geometry after the small one (any pointer may be NULL) */
+void mhb_s2s_sort_stats(uint64_t *n_oversized, uint64_t *oversized_items, uint64_t *n_large);
+
 /* Fused partition + exchange for the multi-GPU path: ONE stable radix pass whose per-digit destinations are arbitrary
  * device byte addresses (bin_addr_dev[256], device memory) = where the first record of digit d coming from THIS call
  * goes.  The digit of a record is owner_of_byte_dev[record byte `byte`] (256-entry device table mapping the record's
@@ -617,6 +631,8 @@ int mhb_selftest_count_records_roll(const uint32_t *read_words, uint32_t nwords,
                                     uint64_t *rec4_out, uint32_t *strand4_out);
 int mhb_selftest_s2s_record(const uint32_t *seq_words, uint32_t nwords, uint32_t L, uint32_t k, uint32_t strand,
                             uint32_t offset, uint32_t mult, uint32_t *rec_out);
+/* the 64-bit in-bucket key mhb_s2s_sort orders n seq2sdbg records by (9 <= k <= 38) */
+int mhb_selftest_s2s_local_key(const uint32_t *recs, uint64_t n, uint32_t k, uint64_t *keys_out);
 
 /* read2sdbg building blocks on host arrays (same __host__ __device__ code as the kernels): stage-1 record e of a
  * package-orientation read (rec_out: key words + 2), stage-2 item (seq2sdbg layout) + palindrome flag, kmsort of one

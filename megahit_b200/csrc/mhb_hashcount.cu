@@ -45,19 +45,6 @@ constexpr u32 kHcPrefetchChunk = 16384;        // bytes per cp.async.bulk.prefet
 
 __device__ __forceinline__ u64 rec_key64(const uint2 r) { return ((u64)r.x << 32) | r.y; }
 
-// bounds[b] = first record whose 16-bit prefix is >= b (b = 0..65536); the records are sorted on that prefix
-__global__ void k_bucket_bounds(const uint2 *__restrict__ recs, u64 n, u64 *__restrict__ bounds) {
-  const u32 b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b > 65536u) return;
-  u64 lo = 0, hi = n;
-  while (lo < hi) {
-    const u64 mid = (lo + hi) >> 1;
-    if ((recs[mid].x >> 16) < b) lo = mid + 1;
-    else hi = mid;
-  }
-  bounds[b] = lo;
-}
-
 // first index q in [p, hi] that may start a slice: q == lo, q == hi, or the 24-bit prefix changes between q-1 and q
 // (records with equal keys share their prefix, so they never straddle such a boundary).  The records are sorted on
 // that prefix, so q is the first record in [p, hi) whose prefix exceeds that of record p-1.
@@ -623,7 +610,7 @@ extern "C" int mhb_count_solid_hashed(void *stream, uint32_t *recs_a, uint32_t *
   CK(cudaMemsetAsync(misc, 0, 256, st));
   CK(cudaMemsetAsync(slice_count, 0, L.max_slices * 4, st));
   // 2. bucket boundaries, slices per bucket, the slice plan
-  k_bucket_bounds<<<(65537 + 255) / 256, 256, 0, st>>>(recs, n, bounds);
+  k_bucket_bounds<2><<<(65537 + 255) / 256, 256, 0, st>>>(reinterpret_cast<const u32 *>(recs), n, bounds);
   CK_LAUNCH();
   k_slice_counts<<<65536 / 256, 256, 0, st>>>(bounds, HcGeomB::SLICE, bcnt);
   CK_LAUNCH();

@@ -730,7 +730,7 @@ extern "C" int mhb_count_host(const mhb_count_args *args, mhb_count_result *res)
 // ================================================================================================
 namespace {
 size_t s2s_round_bytes(uint64_t n, uint32_t W, uint32_t k) {
-  return 2 * Arena::pad((size_t)n * W * 4 + 16) + Arena::pad(mhb_sort_workspace_bytes(n, W)) +
+  return 2 * Arena::pad((size_t)n * W * 4 + 16) + Arena::pad(mhb_s2s_sort_workspace_bytes(n, k)) +
          Arena::pad(mhb_s2s_emit_scratch_bytes(n, k)) + Arena::pad((size_t)n * (4ull + 4ull * words_per_tip_label(k)) + 16);
 }
 }  // namespace
@@ -744,8 +744,6 @@ static int s2s_host_rounds(const mhb_s2s_args *args, mhb_s2s_result *res, const 
   const uint32_t k = args->k;
   const uint64_t ns = args->n_seqs;
   const uint32_t W = s2s_record_words(k), WPT = words_per_tip_label(k);
-  uint8_t sort_bytes[72];
-  const uint32_t n_sort = mhb_s2s_sort_bytes(k, sort_bytes);
   const int top_byte = (int)(4 * W - 1);
   cudaStream_t st = 0;
   Timer t_all(st), t(st);
@@ -781,7 +779,7 @@ static int s2s_host_rounds(const mhb_s2s_args *args, mhb_s2s_result *res, const 
   uint64_t *d_cursor = g_arena.take<uint64_t>(8);
   uint32_t *d_a = g_arena.take<uint32_t>((size_t)max_items * W + 4);
   uint32_t *d_b = g_arena.take<uint32_t>((size_t)max_items * W + 4);
-  const size_t ws_bytes = mhb_sort_workspace_bytes(max_items, W);
+  const size_t ws_bytes = mhb_s2s_sort_workspace_bytes(max_items, k);
   const size_t scratch_bytes = mhb_s2s_emit_scratch_bytes(max_items, k);
   const uint64_t cap_bytes = max_items * (4ull + 4ull * WPT) + 16;
   char *d_ws = g_arena.take<char>(ws_bytes);
@@ -832,7 +830,7 @@ static int s2s_host_rounds(const mhb_s2s_args *args, mhb_s2s_result *res, const 
     t.start();
     CK(cudaMemsetAsync(d_hist0, 0, 256 * 8, st));
     CK(cudaMemsetAsync(d_cursor, 0, 64, st));
-    CKR(mhb_s2s_extract_range(st, &seqs, k, d_a, n_items, r_lo[ri], r_hi[ri], d_cursor, max_items, d_hist0, sort_bytes[0]));
+    CKR(mhb_s2s_extract_range(st, &seqs, k, d_a, n_items, r_lo[ri], r_hi[ri], d_cursor, max_items, d_hist0, mhb_s2s_sort_hist_byte(max_items, k)));
     uint64_t n_round = 0;
     CK(cudaMemcpyAsync(&n_round, d_cursor, 8, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
@@ -841,7 +839,9 @@ static int s2s_host_rounds(const mhb_s2s_args *args, mhb_s2s_result *res, const 
     if (n_round == 0) continue;
     t.start();
     int in_b = 0;
-    CKR(mhb_sort_records_impl(st, d_a, d_b, n_round, W, sort_bytes, n_sort, d_hist0, d_ws, ws_bytes, &in_b, nullptr));
+    // the histogram is of the byte a sort of max_items items starts with: pass it only if this round's sort does too
+    const bool hist_ok = mhb_s2s_sort_hist_byte(n_round, k) == mhb_s2s_sort_hist_byte(max_items, k);
+    CKR(mhb_s2s_sort(st, d_a, d_b, n_round, k, hist_ok ? d_hist0 : nullptr, d_ws, ws_bytes, &in_b));
     res->t_sort_ms += t.stop();
     t.start();
     CKR(mhb_s2s_emit(st, in_b ? d_b : d_a, n_round, k, d_bytes, cap_bytes, d_table, d_totals, d_scratch, scratch_bytes));
@@ -894,9 +894,7 @@ extern "C" int mhb_s2s_host(const mhb_s2s_args *args, mhb_s2s_result *res) {
   Timer t_all(st), t(st);
   t_all.start();
   const uint32_t W = s2s_record_words(k);
-  uint8_t sort_bytes[72];
-  const uint32_t n_sort = mhb_s2s_sort_bytes(k, sort_bytes);
-  const size_t ws_bytes = mhb_sort_workspace_bytes(n_items, W);
+  const size_t ws_bytes = mhb_s2s_sort_workspace_bytes(n_items, k);
   const size_t scratch_bytes = mhb_s2s_emit_scratch_bytes(n_items, k);
   // worst case bytes per sort item: 2 + 2 + 4*WPT (every item a large-multiplicity tip)
   const uint64_t cap_bytes = n_items * (4ull + 4ull * res->words_per_tip_label) + 16;
@@ -950,11 +948,11 @@ extern "C" int mhb_s2s_host(const mhb_s2s_args *args, mhb_s2s_result *res) {
   seqs.fixed_stride = 0;
 
   t.start();
-  CKR(mhb_s2s_extract(st, &seqs, k, d_a, n_items, d_hist0, sort_bytes[0]));
+  CKR(mhb_s2s_extract(st, &seqs, k, d_a, n_items, d_hist0, mhb_s2s_sort_hist_byte(n_items, k)));
   res->t_extract_ms = t.stop();
   t.start();
   int in_b = 0;
-  CKR(mhb_sort_records_impl(st, d_a, d_b, n_items, W, sort_bytes, n_sort, d_hist0, d_ws, ws_bytes, &in_b, nullptr));
+  CKR(mhb_s2s_sort(st, d_a, d_b, n_items, k, d_hist0, d_ws, ws_bytes, &in_b));
   res->t_sort_ms = t.stop();
   t.start();
   CKR(mhb_s2s_emit(st, in_b ? d_b : d_a, n_items, k, d_bytes, cap_bytes, d_table, d_totals, d_scratch, scratch_bytes));
@@ -1136,8 +1134,8 @@ static int build_host_impl(const mhb_build_args *args, mhb_build_result *res, bo
   Timer t_all(st), t(st);
   t_all.start();
 
-  uint8_t cbytes[72], sbytes[72];
-  const uint32_t n_csort = mhb_count_sort_bytes(k, cbytes), n_ssort = mhb_s2s_sort_bytes(k, sbytes);
+  uint8_t cbytes[72];
+  const uint32_t n_csort = mhb_count_sort_bytes(k, cbytes);
   const int32_t m = args->m;
   const uint64_t cap_edges = n / (uint64_t)std::max(1, m) + 1;
   const size_t bin_bytes = (args->bin_words * 4 + 15) & ~(size_t)15;
@@ -1320,7 +1318,7 @@ static int build_host_impl(const mhb_build_args *args, mhb_build_result *res, bo
   const uint64_t n_seqs = n_solid + n_mercy;
   const uint64_t n_items = n_seqs * 6;  // 2 strands x (k+1 - k + 2)
   res->n_sort_items = n_items;
-  const size_t s_ws = mhb_sort_workspace_bytes(n_items, W2), s_scr = mhb_s2s_emit_scratch_bytes(n_items, k);
+  const size_t s_ws = mhb_s2s_sort_workspace_bytes(n_items, k), s_scr = mhb_s2s_emit_scratch_bytes(n_items, k);
   const uint64_t cap_bytes = n_items * (4ull + 4ull * WPT) + 16;
   const size_t s2s_work = 2 * Arena::pad((size_t)n_items * W2 * 4 + 16) + Arena::pad(s_ws) + Arena::pad(s_scr) + Arena::pad(cap_bytes);
   char *sw = work;
@@ -1353,16 +1351,18 @@ static int build_host_impl(const mhb_build_args *args, mhb_build_result *res, bo
   uint64_t n_sorted = n_items;
   if (!no_prune) {
     CK(cudaMemsetAsync(d_nsolid + 4, 0, 8, st));
-    CKR(mhb_s2s_extract_edges_pruned(st, d_all_edges, d_aux, n_seqs, n_solid, k, s_a, n_items, d_nsolid + 4, d_hist1, sbytes[0]));
+    CKR(mhb_s2s_extract_edges_pruned(st, d_all_edges, d_aux, n_seqs, n_solid, k, s_a, n_items, d_nsolid + 4, d_hist1, mhb_s2s_sort_hist_byte(n_items, k)));
     CK(cudaMemcpyAsync(&n_sorted, d_nsolid + 4, 8, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     if (n_sorted > n_items) return mhb_set_error(MHB_ERR_CUDA, "internal: pruned item count exceeds 6 per edge");
     res->n_sort_items = n_sorted;
   } else {
-    CKR(mhb_s2s_extract(st, &seqs, k, s_a, n_items, d_hist1, sbytes[0]));
+    CKR(mhb_s2s_extract(st, &seqs, k, s_a, n_items, d_hist1, mhb_s2s_sort_hist_byte(n_items, k)));
   }
   int s_in_b = 0;
-  CKR(mhb_sort_records_impl(st, s_a, s_b, n_sorted, W2, sbytes, n_ssort, d_hist1, s_wsp, s_ws, &s_in_b, nullptr));
+  // the extraction histogrammed the byte a sort of n_items (the bound) starts with; the pruned count may start with another
+  const bool hist_ok = mhb_s2s_sort_hist_byte(n_sorted, k) == mhb_s2s_sort_hist_byte(n_items, k);
+  CKR(mhb_s2s_sort(st, s_a, s_b, n_sorted, k, hist_ok ? d_hist1 : nullptr, s_wsp, s_ws, &s_in_b));
   CKR(mhb_s2s_emit(st, s_in_b ? s_b : s_a, n_sorted, k, d_bytes, cap_bytes, d_table, d_totals, s_scrp, s_scr));
   uint64_t totals[16];
   CK(cudaMemcpyAsync(totals, d_totals, sizeof(totals), cudaMemcpyDeviceToHost, st));

@@ -11,6 +11,13 @@ int mhb_set_error(int code, const char *fmt, ...);
 int mhb_sort_records_impl(void *stream, uint32_t *a, uint32_t *b, uint64_t n, uint32_t words, const uint8_t *bytes,
                           uint32_t n_bytes, const uint64_t *first_hist, void *ws, size_t ws_bytes, int *result_in_b,
                           double *pass_ms_host);
+// relaxed: as mhb_sort_records_relaxed (1) or mhb_sort_records (0), + per-pass timings as above
+int mhb_sort_records_ex(void *stream, uint32_t *a, uint32_t *b, uint64_t n, uint32_t words, const uint8_t *bytes,
+                        uint32_t n_bytes, const uint64_t *first_hist, void *ws, size_t ws_bytes, int *result_in_b,
+                        double *pass_ms_host, int relaxed);
+// mhb_sort_records_relaxed without an entry in the per-pass timing ring (a sort inside another sort)
+int mhb_sort_records_untraced(void *stream, uint32_t *a, uint32_t *b, uint64_t n, uint32_t words, const uint8_t *bytes,
+                              uint32_t n_bytes, const uint64_t *first_hist, void *ws, size_t ws_bytes, int *result_in_b);
 
 // bytes held by the arena the host-level calls keep between calls (mhb_release frees it)
 size_t mhb_arena_bytes(void);

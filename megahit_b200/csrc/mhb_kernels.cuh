@@ -137,6 +137,20 @@ MHB_HD void make_s2s_record(const u32 *s, u32 nwords, u32 L, u32 k, u32 strand, 
   rec[W - 1] |= 65535u - counting;
 }
 
+// Key of a seq2sdbg sort record INSIDE its 16-bit bucket (the first eight bases): the 2k - 16 key bits below the
+// bucket followed by the four flag bits (non-dollar, prev), left-aligned in 64 bits.  Comparing these keys orders two
+// records of one bucket exactly as mhb_s2s_sort_bytes does: the zero fill between the k-mer and the flags is constant
+// and the multiplicity bits are not sorted.  9 <= k <= 38 (W = 2 or 3): 2k - 12 <= 64 bits.
+template <int W>
+MHB_HD u64 s2s_local_key(const u32 (&r)[W], u32 k) {
+  u32 w2 = 0;
+  if constexpr (W >= 3) w2 = r[2];
+  const u64 top = ((u64)r[0] << 48) | ((u64)r[1] << 16) | (w2 >> 16);  // the record from bit 16 on
+  const u32 kb = 2 * k - 16;
+  const u64 flags = (r[W - 1] >> 16) & 15u;
+  return (top & ~(~0ull >> kb)) | (flags << (60 - kb));
+}
+
 #if defined(__CUDACC__)
 // ------------------------------------------------------------------------------------------------
 // record load/store (AoS, WR words; 8- and 16-byte records use vector accesses)
@@ -190,6 +204,21 @@ __device__ __forceinline__ void st_rec(u32 *base, u64 idx, const u32 (&r)[WR]) {
 template <int WR>
 __device__ __forceinline__ u32 rec_byte(const u32 (&r)[WR], int b) {
   return (pick<WR>(r, (u32)(WR - 1 - (b >> 2))) >> (8 * (b & 3))) & 255u;
+}
+
+// bounds[b] = first record whose 16-bit prefix (top half of word 0) is >= b, b = 0..65536; the W-word records are
+// sorted on that prefix
+template <int W>
+__global__ void k_bucket_bounds(const u32 *__restrict__ recs, u64 n, u64 *__restrict__ bounds) {
+  const u32 b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b > 65536u) return;
+  u64 lo = 0, hi = n;
+  while (lo < hi) {
+    const u64 mid = (lo + hi) >> 1;
+    if ((recs[mid * W] >> 16) < b) lo = mid + 1;
+    else hi = mid;
+  }
+  bounds[b] = lo;
 }
 
 __device__ __forceinline__ u32 lane_id() { return threadIdx.x & 31; }

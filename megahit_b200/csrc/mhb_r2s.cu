@@ -205,7 +205,7 @@ size_t s1_pass_bytes(uint64_t n, uint32_t RW) {
 // device bytes of one stage-2 pass over n items: items, sort buffer and workspace, run collapse, emitter scratch + stream
 size_t s2_pass_bytes(uint64_t n, uint32_t W, uint32_t k) {
   const uint64_t n_tiles = (n + kDdTile - 1) / kDdTile;
-  return 2 * pad((size_t)n * W * 4 + 16) + pad(mhb_sort_workspace_bytes(n, W)) + pad(n_tiles * 4) + pad(n_tiles * 8) +
+  return 2 * pad((size_t)n * W * 4 + 16) + pad(mhb_s2s_sort_workspace_bytes(n, k)) + pad(n_tiles * 4) + pad(n_tiles * 8) +
          pad((n_tiles / 4096 + 4) * 8) + pad((size_t)n * 8) + pad(mhb_s2s_emit_scratch_bytes(n, k)) +
          pad((size_t)n * (4ull + 4ull * words_per_tip_label(k)) + 16);
 }
@@ -466,11 +466,9 @@ int s2_sort_emit(cudaStream_t st, uint32_t k, BigBufs &big, S2Bufs &sb, uint64_t
                  unsigned long long *d_counter, PhaseTrace &tr, uint64_t *n_u_out, uint64_t *cap_bytes) {
   const uint32_t W = s2s_record_words(k), WPT = words_per_tip_label(k);
   DevBuf &a = big.a, &b = big.b, &ws = big.ws;
-  const size_t ws_bytes = mhb_sort_workspace_bytes(n, W);
-  uint8_t sbytes[80];
-  const uint32_t n_sb = mhb_s2s_sort_bytes(k, sbytes);
+  const size_t ws_bytes = mhb_s2s_sort_workspace_bytes(n, k);
   int in_b = 0;
-  CKR(mhb_sort_records_relaxed(st, a.as<u32>(), b.as<u32>(), n, W, sbytes, n_sb, nullptr, ws.p, ws_bytes, &in_b));
+  CKR(mhb_s2s_sort(st, a.as<u32>(), b.as<u32>(), n, k, nullptr, ws.p, ws_bytes, &in_b));
   tr.mark("s2.sort");
   const u32 *sorted = in_b ? b.as<u32>() : a.as<u32>();
   u32 *uniq = in_b ? a.as<u32>() : b.as<u32>();
@@ -642,10 +640,10 @@ extern "C" int mhb_read2sdbg_host(const mhb_build_args *args, mhb_build_result *
       // size the shared buffers for stage 2 as well when that fits: ~1.6 items per edge position on a 30x library, 2.2
       // to be safe (stage 2 reallocates when its count launch says more)
       const size_t rec1 = pad((size_t)ix.n_s1 * RW * 4 + 16), ws1 = pad(mhb_sort_workspace_bytes(ix.n_s1, RW));
-      const size_t rec2 = pad((size_t)est_items * W * 4 + 16), ws2 = pad(mhb_sort_workspace_bytes(est_items, W));
+      const size_t rec2 = pad((size_t)est_items * W * 4 + 16), ws2 = pad(mhb_s2s_sort_workspace_bytes(est_items, k));
       const bool share = s1_one - 2 * rec1 - ws1 + 2 * std::max(rec1, rec2) + std::max(ws1, ws2) <= avail;
       CKR(run_stage1(st, pv, ix, k, m, mercy, so, d_hist.as<unsigned long long>(), tr, big,
-                     share ? (size_t)est_items * W * 4 + 16 : 0, share ? mhb_sort_workspace_bytes(est_items, W) : 0));
+                     share ? (size_t)est_items * W * 4 + 16 : 0, share ? mhb_s2s_sort_workspace_bytes(est_items, k) : 0));
       res->n_rounds_s1 = 1;
     } else {
       if (!max_n) {
@@ -708,7 +706,7 @@ extern "C" int mhb_read2sdbg_host(const mhb_build_args *args, mhb_build_result *
   } else if (!s2_rounds) {
     S2Bufs sb;
     DevBuf &a = big.a, &b = big.b, &ws = big.ws;
-    const size_t rec_bytes = (size_t)n_items * W * 4 + 16, ws_bytes = mhb_sort_workspace_bytes(n_items, W);
+    const size_t rec_bytes = (size_t)n_items * W * 4 + 16, ws_bytes = mhb_s2s_sort_workspace_bytes(n_items, k);
     CKR(a.ensure(rec_bytes, "stage-2 items"));
     CKR(b.ensure(rec_bytes, "stage-2 items (sort buffer)"));
     CKR(ws.ensure(ws_bytes, "sort workspace"));
@@ -777,7 +775,7 @@ extern "C" int mhb_read2sdbg_host(const mhb_build_args *args, mhb_build_result *
     CKR(plan_bucket_ranges(h_h16, max_items, &ranges));
     CKR(big.a.ensure((size_t)max_items * W * 4 + 16, "stage-2 items"));
     CKR(big.b.ensure((size_t)max_items * W * 4 + 16, "stage-2 items (sort buffer)"));
-    CKR(big.ws.ensure(mhb_sort_workspace_bytes(max_items, W), "sort workspace"));
+    CKR(big.ws.ensure(mhb_s2s_sort_workspace_bytes(max_items, k), "sort workspace"));
     S2Bufs sb;
     SdbgStitch out;
     uint64_t seen = 0;

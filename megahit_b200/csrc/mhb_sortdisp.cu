@@ -228,19 +228,31 @@ uint64_t g_trace_seq = 0;
 }  // namespace
 
 // relaxed != 0: the first pass may be the unstable partition pass (mhb_part.cuh) - the order among records whose sorted
-// bytes are ALL equal is then unspecified; MHB_SORT_STABLE_FIRST=1 keeps the stable pass everywhere (A/B hook)
-int mhb_sort_records_ex(void *stream, uint32_t *a, uint32_t *b, uint64_t n, uint32_t words, const uint8_t *bytes,
-                        uint32_t n_bytes, const uint64_t *first_hist, void *ws, size_t ws_bytes, int *result_in_b,
-                        double *pass_ms_host, int relaxed);
+// bytes are ALL equal is then unspecified; MHB_SORT_STABLE_FIRST=1 keeps the stable pass everywhere (A/B hook).
+// trace: the sort takes a slot of the per-pass timing ring (mhb_sort_pass_ms); the sorts a larger sort runs inside
+// itself (mhb_s2s_sort's oversized buckets) do not, so that the ring keeps one entry per sort a caller issued.
+static int sort_records_core(void *stream, uint32_t *a, uint32_t *b, uint64_t n, uint32_t words, const uint8_t *bytes,
+                             uint32_t n_bytes, const uint64_t *first_hist, void *ws, size_t ws_bytes, int *result_in_b,
+                             double *pass_ms_host, int relaxed, bool trace);
 int mhb_sort_records_impl(void *stream, uint32_t *a, uint32_t *b, uint64_t n, uint32_t words, const uint8_t *bytes,
                           uint32_t n_bytes, const uint64_t *first_hist, void *ws, size_t ws_bytes, int *result_in_b,
                           double *pass_ms_host) {
   // the library's own stages tally or minimise over records with equal sort keys: their order is irrelevant
-  return mhb_sort_records_ex(stream, a, b, n, words, bytes, n_bytes, first_hist, ws, ws_bytes, result_in_b, pass_ms_host, 1);
+  return sort_records_core(stream, a, b, n, words, bytes, n_bytes, first_hist, ws, ws_bytes, result_in_b, pass_ms_host, 1, true);
 }
 int mhb_sort_records_ex(void *stream, uint32_t *a, uint32_t *b, uint64_t n, uint32_t words, const uint8_t *bytes,
-                          uint32_t n_bytes, const uint64_t *first_hist, void *ws, size_t ws_bytes, int *result_in_b,
+                        uint32_t n_bytes, const uint64_t *first_hist, void *ws, size_t ws_bytes, int *result_in_b,
                         double *pass_ms_host, int relaxed) {
+  return sort_records_core(stream, a, b, n, words, bytes, n_bytes, first_hist, ws, ws_bytes, result_in_b, pass_ms_host, relaxed, true);
+}
+int mhb_sort_records_untraced(void *stream, uint32_t *a, uint32_t *b, uint64_t n, uint32_t words, const uint8_t *bytes,
+                              uint32_t n_bytes, const uint64_t *first_hist, void *ws, size_t ws_bytes, int *result_in_b) {
+  return sort_records_core(stream, a, b, n, words, bytes, n_bytes, first_hist, ws, ws_bytes, result_in_b, nullptr, 1, false);
+}
+static int sort_records_core(void *stream, uint32_t *a, uint32_t *b, uint64_t n, uint32_t words, const uint8_t *bytes,
+                             uint32_t n_bytes, const uint64_t *first_hist, void *ws, size_t ws_bytes, int *result_in_b,
+                             double *pass_ms_host, int relaxed, bool trace) {
+  if (pass_ms_host && !trace) return mhb_set_error(MHB_ERR_ARG, "per-pass times need a traced sort");
   static const bool stable_first = getenv("MHB_SORT_STABLE_FIRST") != nullptr;
   if (stable_first) relaxed = 0;
   if (words < 1 || words > 17 || n_bytes > 72 || !result_in_b)
@@ -266,15 +278,18 @@ int mhb_sort_records_ex(void *stream, uint32_t *a, uint32_t *b, uint64_t n, uint
 #undef M
     CK_LAUNCH();
   }
-  SortTrace &tr = g_trace[g_trace_seq++ & 3];
-  if (!tr.created) {
-    for (int i = 0; i < 74; ++i) CK(cudaEventCreate(&tr.ev[i]));
-    tr.created = true;
+  SortTrace *tr = nullptr;
+  if (trace) {
+    tr = &g_trace[g_trace_seq++ & 3];
+    if (!tr->created) {
+      for (int i = 0; i < 74; ++i) CK(cudaEventCreate(&tr->ev[i]));
+      tr->created = true;
+    }
+    tr->n_passes = n_bytes;
+    tr->words = words;
+    tr->n = n;
+    CK(cudaEventRecord(tr->ev[0], st));
   }
-  tr.n_passes = n_bytes;
-  tr.words = words;
-  tr.n = n;
-  CK(cudaEventRecord(tr.ev[0], st));
   u32 *in = a, *out = b;
   for (u32 p = 0; p < n_bytes; ++p) {
     k_hist_scan256<<<1, 256, 0, st>>>(hist + (u64)p * 256, bin_base, (u64)(uintptr_t)out, words * 4);
@@ -291,17 +306,17 @@ int mhb_sort_records_ex(void *stream, uint32_t *a, uint32_t *b, uint64_t n, uint
 #undef M
     }
     if (rc) return rc;
-    CK(cudaEventRecord(tr.ev[p + 1], st));
+    if (tr) CK(cudaEventRecord(tr->ev[p + 1], st));
     u32 *t = in;
     in = out;
     out = t;
   }
   *result_in_b = (in == b) ? 1 : 0;
   if (pass_ms_host) {
-    CK(cudaEventSynchronize(tr.ev[n_bytes]));
+    CK(cudaEventSynchronize(tr->ev[n_bytes]));
     for (u32 p = 0; p < n_bytes; ++p) {
       float ms = 0;
-      CK(cudaEventElapsedTime(&ms, tr.ev[p], tr.ev[p + 1]));
+      CK(cudaEventElapsedTime(&ms, tr->ev[p], tr->ev[p + 1]));
       pass_ms_host[p] = ms;
     }
   }

@@ -38,6 +38,18 @@ def sort_records(a: torch.Tensor, b: torch.Tensor, n: int, words: int, sort_byte
     return b if in_b.value else a
 
 
+def s2s_sort(a: torch.Tensor, b: torch.Tensor, n: int, k: int, first_hist=None, ws=None):
+    """The seq2sdbg item sort (mhb_s2s_sort) of n items in a; b is the other buffer (same size, 16-byte aligned).
+    first_hist: histogram of record byte lib.s2s_sort_hist_byte(n, k), or None.  Returns the tensor holding the result."""
+    L = lib.load()
+    need = L.mhb_s2s_sort_workspace_bytes(n, k)
+    if ws is None or ws.numel() < need:
+        ws = torch.empty(need, dtype=torch.uint8, device=a.device)
+    in_b = C.c_int(0)
+    lib._check(L.mhb_s2s_sort(_stream(), _ptr(a), _ptr(b), n, k, _ptr(first_hist), _ptr(ws), ws.numel(), C.byref(in_b)))
+    return b if in_b.value else a
+
+
 class CountPlan:
     """`count` (extract -> sort -> solid edges [-> mercy bookkeeping]) for a fixed-length read library
     resident on the device."""
@@ -183,7 +195,7 @@ class S2sPlan:
         i32 = dict(dtype=torch.int32, device=device)
         self.a = torch.empty(n * self.W + 4, **i32)
         self.b = torch.empty(n * self.W + 4, **i32)
-        self.ws = torch.empty(L.mhb_sort_workspace_bytes(n, self.W), dtype=torch.uint8, device=device)
+        self.ws = torch.empty(L.mhb_s2s_sort_workspace_bytes(n, k), dtype=torch.uint8, device=device)
         self.scratch = torch.empty(L.mhb_s2s_emit_scratch_bytes(n, k), dtype=torch.uint8, device=device)
         wpt = (k + 15) // 16
         self.cap_bytes = n * (4 + 4 * wpt) + 16
@@ -211,10 +223,10 @@ class S2sPlan:
         if timed:
             ev[0].record()
         lib._check(self.L.mhb_s2s_extract(_stream(), C.byref(seqs), self.k, _ptr(self.a), self.n_items, _ptr(self.hist0),
-                                          self.sort_bytes[0]))
+                                          lib.s2s_sort_hist_byte(self.n_items, self.k)))
         if timed:
             ev[1].record()
-        srt = sort_records(self.a, self.b, self.n_items, self.W, self.sort_bytes, self.hist0, self.ws, relaxed=True)
+        srt = s2s_sort(self.a, self.b, self.n_items, self.k, self.hist0, self.ws)
         if timed:
             ev[2].record()
         lib._check(self.L.mhb_s2s_emit(_stream(), _ptr(srt), self.n_items, self.k, _ptr(self.bytes), self.cap_bytes,
@@ -232,12 +244,15 @@ class S2sPlan:
         if timed:
             ev[0].record()
         lib._check(self.L.mhb_s2s_extract_edges_pruned(_stream(), _ptr(edges), _ptr(aux), n_edges, n_aux, self.k, _ptr(self.a),
-                                                       cap, _ptr(self.cursor), _ptr(self.hist0), self.sort_bytes[0]))
-        self.n_items = int(self.cursor.item())  # the one host read-back of the stage (launch geometry of the sort)
+                                                       cap, _ptr(self.cursor), _ptr(self.hist0),
+                                                       lib.s2s_sort_hist_byte(cap, self.k)))
+        self.n_items = int(self.cursor.item())  # host read-back of the item count (launch geometry of the sort)
         assert self.n_items <= cap
         if timed:
             ev[1].record()
-        srt = sort_records(self.a, self.b, self.n_items, self.W, self.sort_bytes, self.hist0, self.ws, relaxed=True)
+        # the histogram is of the byte a sort of `cap` items starts with; pass it only if this sort starts there too
+        same = lib.s2s_sort_hist_byte(self.n_items, self.k) == lib.s2s_sort_hist_byte(cap, self.k)
+        srt = s2s_sort(self.a, self.b, self.n_items, self.k, self.hist0 if same else None, self.ws)
         if timed:
             ev[2].record()
         lib._check(self.L.mhb_s2s_emit(_stream(), _ptr(srt), self.n_items, self.k, _ptr(self.bytes), self.cap_bytes,

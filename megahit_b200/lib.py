@@ -148,6 +148,8 @@ SYMBOLS = [
     "mhb_iterate_host", "mhb_iterate_run", "mhb_selftest_iterate", "mhb_s2s_extract_edges_pruned", "mhb_s2s_emit_fmt", "mhb_read2sdbg_host", "mhb_read2sdbg_run", "mhb_selftest_r2s_s1_record", "mhb_selftest_r2s_item",
     "mhb_selftest_kmsort", "mhb_selftest_kmsort_smem", "mhb_selftest_r2s_s1_group", "mhb_selftest_r2s_mercy_read",
     "mhb_buildlib_host", "mhb_buildlib_free", "mhb_set_buildlib_chunk", "mhb_buildlib_run", "mhb_selftest_fastx",
+    "mhb_s2s_sort", "mhb_s2s_sort_workspace_bytes", "mhb_s2s_sort_hist_byte", "mhb_s2s_sort_stats",
+    "mhb_selftest_s2s_local_key",
 ]
 
 
@@ -177,6 +179,14 @@ def load():
     L.mhb_sort_records.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_uint32,
                                    C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_int)]
     L.mhb_sort_records_relaxed.argtypes = L.mhb_sort_records.argtypes
+    L.mhb_s2s_sort.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_size_t,
+                               C.POINTER(C.c_int)]
+    L.mhb_s2s_sort_workspace_bytes.argtypes = [C.c_uint64, C.c_uint32]
+    L.mhb_s2s_sort_workspace_bytes.restype = C.c_size_t
+    L.mhb_s2s_sort_hist_byte.argtypes = [C.c_uint64, C.c_uint32]
+    L.mhb_s2s_sort_stats.argtypes = [C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
+    L.mhb_s2s_sort_stats.restype = None
+    L.mhb_selftest_s2s_local_key.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p]
     L.mhb_count_solid.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p,
                                   C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
     L.mhb_count_hashed_workspace_bytes.restype = C.c_size_t
@@ -385,6 +395,27 @@ def s2s_sort_bytes(k: int) -> list[int]:
     buf = (C.c_uint8 * 80)()
     n = load().mhb_s2s_sort_bytes(C.c_uint32(k), buf)
     return list(buf[:n])
+
+
+def s2s_sort_hist_byte(n: int, k: int) -> int:
+    """record byte the extract kernels histogram for an mhb_s2s_sort of n items"""
+    return load().mhb_s2s_sort_hist_byte(C.c_uint64(n), C.c_uint32(k))
+
+
+def s2s_sort_stats() -> tuple[int, int, int]:
+    """(buckets, items) the last mhb_s2s_sort left to the radix engine, and the buckets it passed from the small to the
+    large shared-memory geometry"""
+    a, b, c = C.c_uint64(), C.c_uint64(), C.c_uint64()
+    load().mhb_s2s_sort_stats(C.byref(a), C.byref(b), C.byref(c))
+    return a.value, b.value, c.value
+
+
+def selftest_s2s_local_key(recs: np.ndarray, k: int) -> np.ndarray:
+    """host run of the in-bucket key of mhb_s2s_sort for (n, W) uint32 records"""
+    recs = np.ascontiguousarray(recs, dtype=np.uint32)
+    keys = np.zeros(len(recs), dtype=np.uint64)
+    _check(load().mhb_selftest_s2s_local_key(recs.ctypes.data, len(recs), k, keys.ctypes.data))
+    return keys
 
 
 # ------------------------------------------------------------------------------------------------
