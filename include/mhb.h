@@ -384,6 +384,29 @@ int mhb_plan_rounds(const uint64_t *hist256, uint64_t max_records, uint32_t *lo_
 int mhb_plan_rounds16(const uint64_t *hist256, const uint64_t *sub_hist, uint64_t max_records, uint32_t *lo16_out,
                       uint32_t *hi16_out, uint32_t cap_out);
 
+/* Read libraries larger than device memory (mhb_count_host, mhb_iterate_host, and mhb_build_host through its staged
+ * route): the `.bin` image stays in host memory and every pass over the reads streams it through the device in chunks
+ * that end on read boundaries (two pinned staging buffers, two device chunk slots; upload of chunk i overlaps the kernels
+ * of chunk i-1 and the host fill of chunk i+1).  The library is resident whenever it was before; it is streamed when the
+ * resident part alone does not fit, when the plan next to it fails (count: one bucket exceeds the room left; iterate:
+ * a cudaMalloc of the resident path fails), or when a chunk cap is set.  The output does not depend on it.
+ * mhb_plan_read_chunks (host only, no GPU needed): cuts the reads into contiguous chunks [first[i], first[i+1]) whose
+ * image is at most max_chunk_bytes each, except that a read larger than the cap gets a chunk of its own.  first_read_out
+ * (may be NULL) needs room for n_chunks + 1 entries (cap_out).  Returns n_chunks (0 for an empty library), or -1
+ * (mhb_last_error).
+ * mhb_read_stream_decide (host only): 1 when the library is streamed, given the bytes of its resident part, the device
+ * bytes available for it, whether the plan next to it failed and the chunk cap.
+ * mhb_set_read_chunk_limit: 0 = automatic; otherwise every library is streamed in chunks of at most that many bytes.
+ * mhb_read_stream_stats / _times: the last mhb_count_host / mhb_iterate_host call - chunks (0 = the library was
+ * resident), passes over the reads, bytes copied host to device; copy-engine and compute-stream busy time, the host
+ * threads' fill time and the wall time of those passes (ms). */
+int mhb_plan_read_chunks(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, uint64_t max_chunk_bytes,
+                         uint64_t *first_read_out, uint32_t cap_out);
+int mhb_read_stream_decide(uint64_t resident_bytes, uint64_t avail_bytes, int plan_failed, uint64_t chunk_limit);
+int mhb_set_read_chunk_limit(uint64_t bytes);
+int mhb_read_stream_stats(uint64_t *n_chunks, uint64_t *n_passes, uint64_t *h2d_bytes);
+int mhb_read_stream_times(double *h2d_ms, double *kernel_ms, double *fill_ms, double *pass_ms);
+
 typedef struct {
   uint32_t k;
   const uint32_t *words;    /* host package-orientation sequences, word aligned */

@@ -354,28 +354,57 @@ extern "C" int mhb_set_s2s_round_limit(uint64_t max_items_per_round) {
 // next to the resident read library: extract that range -> sort -> solid edges -> append to the host result.  Rounds
 // ascend, so the concatenated edges are sorted.  Tip edges (aux != 0) of all rounds are collected on the host and the
 // mercy bookkeeping runs once at the end over the whole library.
-static int count_host_rounds(const mhb_count_args *args, mhb_count_result *res, const BinIndex &ix, uint64_t max_records) {
+//
+// stream: the `.bin` image stays in host memory and every pass over the reads (leading-byte histogram, second-byte
+// histograms of oversized bytes, one pass per round, mercy marks) streams it through the device in chunks
+// (ReadStream); the round buffers get the memory the resident image would have taken.  A resident call switches to
+// streaming when the library alone does not fit or when one bucket exceeds the round that fits next to it.
+static int count_host_rounds(const mhb_count_args *args, mhb_count_result *res, const BinIndex &ix, uint64_t max_records,
+                             bool stream = false) {
   const uint32_t k = args->k;
   const int32_t m = args->m;
   const uint64_t n = ix.n_edges, n_reads = args->n_reads;
   const uint32_t WR = count_record_words(k), WE = words_per_edge(k);
   uint8_t sort_bytes[72];
   const uint32_t n_sort = mhb_count_sort_bytes(k, sort_bytes);
+  (void)n_sort;
   const int top_byte = (int)(4 * WR - 1);
   cudaStream_t st = 0;
   Timer t_all(st), t(st);
   t_all.start();
+  const uint64_t round_cap = max_records;  // the caller's cap (0 = derive from memory)
+  auto restart_streamed = [&]() {
+    const uint32_t we = res->words_per_edge;
+    const uint64_t ne = res->n_edge_records;
+    memset(res, 0, sizeof(*res));
+    res->words_per_edge = we;
+    res->n_edge_records = ne;
+    return count_host_rounds(args, res, ix, round_cap, true);
+  };
+  if (!stream && read_chunk_limit()) stream = true;
 
   const size_t bin_bytes = (args->bin_words * 4 + 15) & ~(size_t)15;
-  size_t fixed = Arena::pad(bin_bytes + 16) + Arena::pad((n_reads + 2) * 8) + Arena::pad(65536 * 8) + 2 * Arena::pad(256 * 8) +
-                 Arena::pad(64) + 8192;
+  const size_t small = Arena::pad(65536 * 8) + 2 * Arena::pad(256 * 8) + Arena::pad(64) + 8192;
+  size_t fixed = Arena::pad(bin_bytes + 16) + Arena::pad((n_reads + 2) * 8) + small;
   if (!ix.fixed_len) fixed += 2 * Arena::pad((n_reads + 1) * 8);
   if (args->want_mercy) fixed += 2 * Arena::pad((size_t)(n_reads + 1) * 4);
+  ReadStream rs;
+  uint64_t chunk_reads = n_reads;  // reads the per-read arrays hold
+  if (stream) {
+    const uint64_t cap = read_chunk_limit() ? read_chunk_limit() : read_chunk_auto_bytes();
+    CKR(rs.init(args->bin, args->bin_words, n_reads, ix.fixed_len, ix.rec_off.data(), ix.edge_off.data(), cap));
+    chunk_reads = rs.max_chunk_reads();
+    fixed = Arena::pad(rs.device_bytes()) + Arena::pad((chunk_reads + 2) * 8) + Arena::pad(256 * 256 * 8) + small;
+    if (args->want_mercy) fixed += 2 * Arena::pad((size_t)(chunk_reads + 1) * 4);
+  }
   if (!max_records) {
     size_t free_b = 0, total_b = 0;
     CK(cudaMemGetInfo(&free_b, &total_b));
     const size_t avail = (size_t)((double)(free_b + g_arena.cap) * 0.92);
-    if (avail <= fixed) return mhb_set_error(MHB_ERR_NOMEM, "the read library alone (%zu bytes) does not fit the device", fixed);
+    if (!stream && mhb_read_stream_decide(fixed, avail, 0, read_chunk_limit())) return restart_streamed();
+    if (avail <= fixed)
+      return mhb_set_error(MHB_ERR_NOMEM, "the read library's %s (%zu bytes) does not fit the device",
+                           stream ? "chunk buffers" : "image", fixed);
     uint64_t lo = 1, hi = n;  // largest round that fits (round_bytes is monotone)
     while (lo < hi) {
       const uint64_t mid = lo + (hi - lo + 1) / 2;
@@ -388,21 +417,28 @@ static int count_host_rounds(const mhb_count_args *args, mhb_count_result *res, 
   const uint64_t cap_edges = max_records / (uint64_t)std::max(1, m) + 1;
   CKR(g_arena.reserve(fixed + round_bytes(max_records, WR, WE, m, k)));
 
-  uint32_t *d_bin = g_arena.take<uint32_t>(bin_bytes / 4 + 4);
-  uint64_t *d_per_read = g_arena.take<uint64_t>(n_reads + 2);
+  uint32_t *d_bin = nullptr;
+  uint64_t *d_sub = nullptr;  // streamed: second-byte histograms of the oversized leading bytes, one pass for all
+  if (stream) {
+    rs.bind(g_arena.take<char>(rs.device_bytes()));
+    d_sub = g_arena.take<uint64_t>(256 * 256);
+  } else {
+    d_bin = g_arena.take<uint32_t>(bin_bytes / 4 + 4);
+  }
+  uint64_t *d_per_read = g_arena.take<uint64_t>(chunk_reads + 2);
   uint64_t *d_mul_hist = g_arena.take<uint64_t>(65536);
   uint64_t *d_hist0 = g_arena.take<uint64_t>(256);
   uint64_t *d_hist_top = g_arena.take<uint64_t>(256);
   uint64_t *d_scalars = g_arena.take<uint64_t>(8);  // [0] n_solid, [1] round total
   uint64_t *d_rec_off = nullptr, *d_edge_off = nullptr;
   uint32_t *d_first = nullptr, *d_last = nullptr;
-  if (!ix.fixed_len) {
+  if (!ix.fixed_len && !stream) {
     d_rec_off = g_arena.take<uint64_t>(n_reads + 1);
     d_edge_off = g_arena.take<uint64_t>(n_reads + 1);
   }
   if (args->want_mercy) {
-    d_first = g_arena.take<uint32_t>(n_reads + 1);
-    d_last = g_arena.take<uint32_t>(n_reads + 1);
+    d_first = g_arena.take<uint32_t>(chunk_reads + 1);
+    d_last = g_arena.take<uint32_t>(chunk_reads + 1);
   }
   uint32_t *d_a = g_arena.take<uint32_t>((size_t)max_records * WR + 4);
   uint32_t *d_b = g_arena.take<uint32_t>((size_t)max_records * WR + 4);
@@ -412,10 +448,12 @@ static int count_host_rounds(const mhb_count_args *args, mhb_count_result *res, 
   uint8_t *d_aux = g_arena.take<uint8_t>(cap_edges);
 
   t.start();
-  if (args->bin_words) CK(cudaMemcpyAsync(d_bin, args->bin, args->bin_words * 4, cudaMemcpyHostToDevice, st));
-  if (!ix.fixed_len && n_reads) {
-    CK(cudaMemcpyAsync(d_rec_off, ix.rec_off.data(), (n_reads + 1) * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_edge_off, ix.edge_off.data(), (n_reads + 1) * 8, cudaMemcpyHostToDevice, st));
+  if (!stream) {
+    if (args->bin_words) CK(cudaMemcpyAsync(d_bin, args->bin, args->bin_words * 4, cudaMemcpyHostToDevice, st));
+    if (!ix.fixed_len && n_reads) {
+      CK(cudaMemcpyAsync(d_rec_off, ix.rec_off.data(), (n_reads + 1) * 8, cudaMemcpyHostToDevice, st));
+      CK(cudaMemcpyAsync(d_edge_off, ix.edge_off.data(), (n_reads + 1) * 8, cudaMemcpyHostToDevice, st));
+    }
   }
   CK(cudaMemsetAsync(d_mul_hist, 0, 65536 * 8, st));
   CK(cudaMemsetAsync(d_hist_top, 0, 256 * 8, st));
@@ -428,27 +466,62 @@ static int count_host_rounds(const mhb_count_args *args, mhb_count_result *res, 
   reads.fixed_len = ix.fixed_len;
   reads.rec_off = d_rec_off;
   reads.edge_off = d_edge_off;
+  // one pass over the reads: the resident library in one view, or every chunk of the stream in turn
+  auto over_reads = [&](const std::function<int(const mhb_dev_reads &, uint64_t)> &fn) -> int {
+    if (!stream) return fn(reads, 0);
+    return rs.pass(st, [&](const ReadChunkView &c) {
+      mhb_dev_reads v;
+      v.bin = c.bin;
+      v.bin_words = c.bin_words;
+      v.n_reads = c.n_reads;
+      v.fixed_len = ix.fixed_len;
+      v.rec_off = c.rec_off;
+      v.edge_off = c.aux_off;
+      return fn(v, c.first_read);
+    });
+  };
 
   // ---- plan: histogram of the leading byte over the whole library (+ of the second byte inside every leading byte
   // that alone exceeds a round), then greedy contiguous ranges of bucket ids ----
   t.start();
   uint64_t h_top[256];
-  CKR(mhb_count_extract_range(st, &reads, k, 0, 65535, 0, d_per_read, nullptr, d_hist_top, top_byte, d_scalars + 1));
+  CKR(over_reads([&](const mhb_dev_reads &v, uint64_t) {
+    return mhb_count_extract_range(st, &v, k, 0, 65535, 0, d_per_read, nullptr, d_hist_top, top_byte, d_scalars + 1);
+  }));
   CK(cudaMemcpyAsync(h_top, d_hist_top, sizeof(h_top), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   std::vector<uint64_t> h_sub;
+  std::vector<uint32_t> over;  // leading bytes that alone exceed a round
   for (uint32_t b = 0; b < 256; ++b) {
     if (h_top[b] <= max_records) continue;
     if (WR * 4 < 2) return mhb_set_error(MHB_ERR_NOMEM, "leading byte 0x%02x exceeds a round and the record has no second byte", b);
     if (h_sub.empty()) h_sub.assign(256 * 256, 0);
+    over.push_back(b);
+    if (stream) continue;
     CK(cudaMemsetAsync(d_hist0, 0, 256 * 8, st));
     CKR(mhb_count_extract_range(st, &reads, k, b << 8, (b << 8) | 255u, 0, d_per_read, nullptr, d_hist0, top_byte - 1, d_scalars + 1));
     CK(cudaMemcpyAsync(h_sub.data() + (size_t)b * 256, d_hist0, 256 * 8, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
   }
+  if (stream && !over.empty()) {  // every oversized byte in the same pass: one launch per byte per chunk
+    CK(cudaMemsetAsync(d_sub, 0, over.size() * 256 * 8, st));
+    CKR(over_reads([&](const mhb_dev_reads &v, uint64_t) {
+      for (size_t j = 0; j < over.size(); ++j)
+        CKR(mhb_count_extract_range(st, &v, k, over[j] << 8, (over[j] << 8) | 255u, 0, d_per_read, nullptr, d_sub + j * 256,
+                                    top_byte - 1, d_scalars + 1));
+      return MHB_OK;
+    }));
+    for (size_t j = 0; j < over.size(); ++j)
+      CK(cudaMemcpyAsync(h_sub.data() + (size_t)over[j] * 256, d_sub + j * 256, 256 * 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+  }
   std::vector<uint32_t> r_lo(65536), r_hi(65536);
   const int n_ranges = mhb_plan_rounds16(h_top, h_sub.empty() ? nullptr : h_sub.data(), max_records, r_lo.data(), r_hi.data(), 65536);
-  if (n_ranges < 0) return MHB_ERR_NOMEM;  // message set by the planner
+  if (n_ranges < 0) {
+    // one bucket exceeds the round that fits next to the resident library: stream it, which leaves more room
+    if (!stream && !round_cap) return restart_streamed();
+    return MHB_ERR_NOMEM;  // message set by the planner
+  }
   std::vector<std::pair<uint32_t, uint32_t>> ranges;
   for (int i = 0; i < n_ranges; ++i) ranges.push_back({r_lo[i], r_hi[i]});
   res->t_extract_ms = t.stop();
@@ -458,17 +531,38 @@ static int count_host_rounds(const mhb_count_args *args, mhb_count_result *res, 
   std::vector<uint8_t> h_tip_aux, h_aux;
   uint64_t n_solid_total = 0;
   for (const auto &rg : ranges) {
-    // ---- extract the range ----
+    // ---- extract the range: per view, count its in-range records, then write them at the round's cursor ----
     t.start();
     uint64_t n_round = 0;
-    CKR(mhb_count_extract_range(st, &reads, k, rg.first, rg.second, 0, d_per_read, nullptr, nullptr, 0, d_scalars + 1));
-    CK(cudaMemcpyAsync(&n_round, d_scalars + 1, 8, cudaMemcpyDeviceToHost, st));
+    if (stream) {
+      uint64_t expect = 0;  // the round's size is known from the histograms: an empty round needs no pass
+      for (uint32_t id = rg.first; id <= rg.second;) {
+        const uint32_t b = id >> 8;
+        if (!h_sub.empty() && h_top[b] > max_records) {
+          expect += h_sub[(size_t)b * 256 + (id & 255)];
+          ++id;
+        } else {
+          expect += h_top[b];
+          id = (b + 1) << 8;
+        }
+      }
+      if (expect == 0) continue;
+    }
     CK(cudaMemsetAsync(d_hist0, 0, 256 * 8, st));
     CK(cudaMemsetAsync(d_scalars, 0, 8, st));
-    CK(cudaStreamSynchronize(st));
-    if (n_round > max_records) return mhb_set_error(MHB_ERR_NOMEM, "internal: round of %llu records exceeds its plan", (unsigned long long)n_round);
+    CKR(over_reads([&](const mhb_dev_reads &v, uint64_t) {
+      uint64_t n_view = 0;
+      CKR(mhb_count_extract_range(st, &v, k, rg.first, rg.second, 0, d_per_read, nullptr, nullptr, 0, d_scalars + 1));
+      CK(cudaMemcpyAsync(&n_view, d_scalars + 1, 8, cudaMemcpyDeviceToHost, st));
+      CK(cudaStreamSynchronize(st));
+      if (n_round + n_view > max_records)
+        return mhb_set_error(MHB_ERR_NOMEM, "internal: round of %llu records exceeds its plan", (unsigned long long)(n_round + n_view));
+      if (n_view)
+        CKR(mhb_count_extract_range(st, &v, k, rg.first, rg.second, 1, d_per_read, d_a + n_round * WR, d_hist0, cw.hist_byte, nullptr));
+      n_round += n_view;
+      return MHB_OK;
+    }));
     if (n_round == 0) continue;
-    CKR(mhb_count_extract_range(st, &reads, k, rg.first, rg.second, 1, d_per_read, d_a, d_hist0, cw.hist_byte, nullptr));
     res->t_extract_ms += t.stop();
     // ---- sort / partition + solid edges ----
     t.start();
@@ -527,17 +621,24 @@ static int count_host_rounds(const mhb_count_args *args, mhb_count_result *res, 
         rc = mhb_set_error(MHB_ERR_CUDA, "tip edge upload failed");
     }
     if (!rc) rc = mhb_tipset_build(st, d_tip_edges, d_tip_aux, n_tip, k, d_tips, ts_bytes, n_tip);
-    if (!rc) rc = mhb_count_mark_mercy(st, &reads, k, d_tips, ts_bytes, n_tip, d_first, d_last);
     h_first.resize(n_reads);
     h_last.resize(n_reads);
-    if (!rc) {
-      cudaMemcpyAsync(h_first.data(), d_first, n_reads * 4, cudaMemcpyDeviceToHost, st);
-      cudaMemcpyAsync(h_last.data(), d_last, n_reads * 4, cudaMemcpyDeviceToHost, st);
-      if (cudaStreamSynchronize(st) != cudaSuccess) rc = mhb_set_error(MHB_ERR_CUDA, "mercy marking failed: %s", cudaGetErrorString(cudaGetLastError()));
-    }
+    // per view: marks into the view-sized first/last arrays, copied to the host arrays at the view's first read
+    if (!rc) rc = over_reads([&](const mhb_dev_reads &v, uint64_t r0) {
+      CKR(mhb_count_mark_mercy(st, &v, k, d_tips, ts_bytes, n_tip, d_first, d_last));
+      cudaMemcpyAsync(h_first.data() + r0, d_first, v.n_reads * 4, cudaMemcpyDeviceToHost, st);
+      cudaMemcpyAsync(h_last.data() + r0, d_last, v.n_reads * 4, cudaMemcpyDeviceToHost, st);
+      if (cudaStreamSynchronize(st) != cudaSuccess) return mhb_set_error(MHB_ERR_CUDA, "mercy marking failed: %s", cudaGetErrorString(cudaGetLastError()));
+      return MHB_OK;
+    });
     if (own) cudaFree(d_tmp);
     if (rc) return rc;
     res->t_mercy_ms = t.stop();
+  }
+  if (stream) {
+    double h2d_ms = 0;
+    mhb_read_stream_times(&h2d_ms, nullptr, nullptr, nullptr);
+    res->t_h2d_ms = h2d_ms;
   }
 
   res->edges = (uint32_t *)malloc(std::max<size_t>(1, h_edges.size() * 4));
@@ -573,6 +674,7 @@ extern "C" int mhb_count_host(const mhb_count_args *args, mhb_count_result *res)
   if (k < 1 || k > MHB_MAX_K) return mhb_set_error(MHB_ERR_ARG, "kmer size %u out of range", k);
   if (mhb_device_count() == 0) return mhb_set_error(MHB_ERR_CUDA, "no CUDA device: libmhb has no CPU path");
   res->words_per_edge = words_per_edge(k);
+  read_stream_stats_reset();
 
   BinIndex ix;
   CKR(index_bin(args->bin, args->bin_words, args->n_reads, k, &ix));
@@ -598,8 +700,8 @@ extern "C" int mhb_count_host(const mhb_count_args *args, mhb_count_result *res)
   if (args->want_mercy) need += 2 * Arena::pad((size_t)(n_reads + 1) * 4);
   {
     // A13: when one pass over all records does not fit the device (or the caller capped the round size), run the
-    // stage in rounds over ranges of the leading record byte
-    bool rounds = g_round_limit && n > g_round_limit;
+    // stage in rounds over ranges of the leading record byte; a chunk cap streams the library through those rounds
+    bool rounds = (g_round_limit && n > g_round_limit) || read_chunk_limit();
     if (!rounds && need > g_arena.cap) {
       size_t free_b = 0, total_b = 0;
       CK(cudaMemGetInfo(&free_b, &total_b));
@@ -1098,7 +1200,9 @@ static int build_host_rounds(const mhb_build_args *args, mhb_build_result *res) 
 
 extern "C" int mhb_build_host(const mhb_build_args *args, mhb_build_result *res) {
   if (!args || !res) return mhb_set_error(MHB_ERR_ARG, "null args");
-  if (g_round_limit || g_s2s_round_limit) return build_host_rounds(args, res);  // explicit caps (tests, small devices)
+  // explicit caps (tests, small devices); the staged route uploads the whole library nowhere (count streams it, the
+  // mercy edges use the `.cand` reads only)
+  if (g_round_limit || g_s2s_round_limit || read_chunk_limit()) return build_host_rounds(args, res);
   const int rc = build_host_impl(args, res, false);
   if (rc == MHB_ERR_NOMEM) {  // everything resident does not fit: the staged build, whose stages plan their own rounds
     mhb_free(res->bytes == args->sdbg_out ? nullptr : res->bytes);

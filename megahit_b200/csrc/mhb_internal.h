@@ -3,6 +3,7 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include <functional>
 #include <vector>
 
 int mhb_set_error(int code, const char *fmt, ...);
@@ -21,6 +22,56 @@ int mhb_sort_records_untraced(void *stream, uint32_t *a, uint32_t *b, uint64_t n
 
 // bytes held by the arena the host-level calls keep between calls (mhb_release frees it)
 size_t mhb_arena_bytes(void);
+
+// A read library kept in host memory and streamed through the device in chunks that end on read boundaries
+// (mhb_stream.cu).  Two pinned staging buffers and two device chunk slots: while host threads fill the staging buffer
+// of chunk i+1, chunk i uploads on a copy stream and the compute stream works on chunk i-1.  Every chunk is handed to
+// the caller as an ordinary view: image at offset 0 of its 16-byte aligned slot, and for variable-length libraries the
+// per-read offsets (record words, and the caller's second array: edge or base offsets) rebased to the chunk.
+struct ReadChunkView {
+  uint64_t index, first_read, n_reads;
+  const uint32_t *bin;  // device
+  uint64_t bin_words;
+  const uint64_t *rec_off, *aux_off;  // device, n_reads + 1 each; NULL for fixed-length libraries
+};
+class ReadStream {
+ public:
+  ReadStream() = default;
+  ReadStream(const ReadStream &) = delete;
+  ReadStream &operator=(const ReadStream &) = delete;
+  ~ReadStream();
+  // host library (rec_off / aux_off: n_reads + 1 entries each, or NULL when fixed_len > 0); plans the chunks
+  int init(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, uint32_t fixed_len, const uint64_t *rec_off,
+           const uint64_t *aux_off, uint64_t max_chunk_bytes);
+  size_t device_bytes() const { return 2 * slot_bytes_; }  // both chunk slots
+  void bind(void *device_slots);                            // device_bytes() bytes, 256-byte aligned
+  uint64_t n_chunks() const { return first_.empty() ? 0 : first_.size() - 1; }
+  uint64_t max_chunk_reads() const { return max_reads_; }
+  const std::vector<uint64_t> &first_reads() const { return first_; }
+  // one pass: fn runs once per chunk, in order, on the compute stream `stream`, while the chunk is on the device
+  int pass(void *stream, const std::function<int(const ReadChunkView &)> &fn);
+
+ private:
+  int stage(uint64_t i);
+  const uint32_t *bin_ = nullptr;
+  uint64_t n_reads_ = 0, stride_ = 0;
+  uint32_t fixed_len_ = 0;
+  const uint64_t *rec_off_ = nullptr, *aux_off_ = nullptr;
+  std::vector<uint64_t> first_;
+  uint64_t max_reads_ = 0;
+  size_t off_at_ = 0, slot_bytes_ = 0;
+  char *dev_ = nullptr;
+  char *host_[2] = {nullptr, nullptr};
+  void *copy_ = nullptr;       // cudaStream_t
+  std::vector<void *> ev_;     // cudaEvent_t: 4 per chunk (copy begin/end, compute begin/end)
+  uint64_t word_of(uint64_t r) const { return fixed_len_ ? r * stride_ : rec_off_[r]; }
+};
+// streaming statistics of the current host-level call (mhb_read_stream_stats)
+void read_stream_stats_reset();
+// the chunk cap: mhb_set_read_chunk_limit, or 0
+uint64_t read_chunk_limit();
+// the chunk size of a library that is streamed because it does not fit (no cap set)
+uint64_t read_chunk_auto_bytes();
 
 // The SdBG output of a build that runs its stage-2 sort in rounds over ascending bucket ranges: every round's emitter
 // output (mhb_s2s_emit / mhb_s2s_emit_fmt) is appended to one byte stream, its non-empty rows of the bucket table are

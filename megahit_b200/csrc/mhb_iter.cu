@@ -95,6 +95,11 @@ int index_reads(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, ReadI
   return MHB_OK;
 }
 
+int iter_reads_resident(const mhb_iterate_args *a, mhb_iterate_result *res, const ReadIndex &ix, const FlankTable &tab, int WCc,
+                        uint32_t w2, uint32_t KN, unsigned long long *cnt, uint64_t *n_cand_out, uint64_t *n_edges_out);
+int iter_reads_streamed(const mhb_iterate_args *a, mhb_iterate_result *res, const ReadIndex &ix, const FlankTable &tab, int WCc,
+                        uint32_t w2, uint32_t KN, unsigned long long *cnt, uint64_t *n_cand_out, uint64_t *n_edges_out);
+
 }  // namespace
 
 extern "C" int mhb_iterate_host(const mhb_iterate_args *a, mhb_iterate_result *res) {
@@ -107,6 +112,7 @@ extern "C" int mhb_iterate_host(const mhb_iterate_args *a, mhb_iterate_result *r
   if (wk + 2 > 17 || w2 > 17) return mhb_set_error(MHB_ERR_ARG, "iterate: k + step + 1 = %u is beyond the 17-word records of the device sort", KN);
   if (mhb_device_count() <= 0) return mhb_set_error(MHB_ERR_CUDA, "no CUDA device: libmhb has no CPU path");
   res->words_per_edge = w2;
+  read_stream_stats_reset();
   cudaStream_t st = 0;
   struct Events {
     cudaEvent_t a, b;
@@ -190,9 +196,39 @@ extern "C" int mhb_iterate_host(const mhb_iterate_args *a, mhb_iterate_result *r
   // ---- reads (FindNextKmersFromReads) ----
   ReadIndex ix;
   CKR(index_reads(a->bin, a->bin_words, a->n_reads, &ix));
-  IBuf d_bin, d_ro, d_bo, d_exist, d_out, d_out2, d_uniq;
   uint64_t n_cand = 0, n_edges = 0;
   if (a->n_reads && n_tab) {
+    // resident as before; streamed in chunks when a chunk cap is set or when the resident buffers do not fit
+    int rc = read_chunk_limit() ? MHB_ERR_NOMEM : iter_reads_resident(a, res, ix, tab, WCc, w2, KN, cnt, &n_cand, &n_edges);
+    if (rc == MHB_ERR_NOMEM) {
+      free(res->edges);
+      res->edges = nullptr;
+      res->n_aligned_reads = 0;
+      n_cand = n_edges = 0;
+      rc = iter_reads_streamed(a, res, ix, tab, WCc, w2, KN, cnt, &n_cand, &n_edges);
+    }
+    CKR(rc);
+  }
+  if (!res->edges) res->edges = (uint32_t *)malloc(4);
+  res->n_candidates = n_cand;
+  res->n_edges = n_edges;
+  cudaEventRecord(e1, st);
+  cudaEventSynchronize(e1);
+  float ms = 0;
+  cudaEventElapsedTime(&ms, e0, e1);
+  res->t_total_ms = ms;
+  return MHB_OK;
+}
+
+namespace {
+// the reads of a library resident in device memory: image, offsets, one mark bit per base, candidate buffers
+int iter_reads_resident(const mhb_iterate_args *a, mhb_iterate_result *res, const ReadIndex &ix, const FlankTable &tab, int WCc,
+                        uint32_t w2, uint32_t KN, unsigned long long *cnt, uint64_t *n_cand_out, uint64_t *n_edges_out) {
+  const uint32_t k = a->k, step = a->step;
+  cudaStream_t st = 0;
+  IBuf d_bin, d_ro, d_bo, d_exist, d_out, d_out2, d_ws, d_flag, d_off, d_bsum;
+  uint64_t n_cand = 0, n_edges = 0;
+  {
     CKR(d_bin.alloc(a->bin_words * 4 + 64, ".bin image"));
     CK(cudaMemcpyAsync(d_bin.p, a->bin, a->bin_words * 4, cudaMemcpyHostToDevice, st));
     IterReads rd{d_bin.as<u32>(), a->n_reads, ix.fixed_len, nullptr, nullptr};
@@ -260,16 +296,132 @@ extern "C" int mhb_iterate_host(const mhb_iterate_args *a, mhb_iterate_result *r
       CK(cudaStreamSynchronize(st));
     }
   }
-  if (!res->edges) res->edges = (uint32_t *)malloc(4);
-  res->n_candidates = n_cand;
-  res->n_edges = n_edges;
-  cudaEventRecord(e1, st);
-  cudaEventSynchronize(e1);
-  float ms = 0;
-  cudaEventElapsedTime(&ms, e0, e1);
-  res->t_total_ms = ms;
+  *n_cand_out = n_cand;
+  *n_edges_out = n_edges;
   return MHB_OK;
 }
+
+// a device buffer that only grows (its contents do not survive growth)
+struct Grow {
+  IBuf b;
+  size_t cap = 0;
+  int need(size_t bytes, const char *what) {
+    if (bytes <= cap) return MHB_OK;
+    CKR(b.alloc(bytes, what));
+    cap = bytes;
+    return MHB_OK;
+  }
+};
+
+// KmerCollector's set semantics on n records in a (b: same-sized buffer): relaxed sort on the key bytes, then the first
+// record of every run of equal records; *out points at the n_out unique records (in a or b)
+int sort_unique(cudaStream_t st, u32 *a, u32 *b, uint64_t n, uint32_t w2, uint32_t KN, Grow &ws, Grow &flag, Grow &off,
+                Grow &bsum, unsigned long long *cnt_slot, u32 **out, uint64_t *n_out) {
+  uint8_t bytes[72];
+  const uint32_t nb = top_bytes(w2, 2 * KN, bytes);
+  const size_t wsb = mhb_sort_workspace_bytes(n, w2);
+  CKR(ws.need(wsb, "sort workspace"));
+  int in_b = 0;
+  CKR(mhb_sort_records_relaxed(st, a, b, n, w2, bytes, nb, nullptr, ws.b.p, wsb, &in_b));
+  const u32 *sorted = in_b ? b : a;
+  u32 *uniq = in_b ? a : b;
+  CKR(flag.need(n * 4 + 16, "flags"));
+  CKR(off.need(n * 8 + 16, "offsets"));
+  CKR(bsum.need((n / 4096 + 4) * 8, "scan sums"));
+  k_iter_heads<<<igrid(n, 256), 256, 0, st>>>(sorted, n, w2, w2, flag.b.as<u32>());
+  CK_LAUNCH();
+  CKR(scan32(st, flag.b.as<u32>(), n, off.b.as<u64>(), (uint64_t *)cnt_slot, bsum.b.as<u64>()));
+  unsigned long long nu = 0;
+  CK(cudaMemcpyAsync(&nu, cnt_slot, 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  k_iter_compact<<<igrid(n, 256), 256, 0, st>>>(sorted, n, w2, flag.b.as<u32>(), off.b.as<u64>(), uniq);
+  CK_LAUNCH();
+  *out = uniq;
+  *n_out = nu;
+  return MHB_OK;
+}
+
+// The reads streamed from host memory in chunks (ReadStream), the flank index resident: per chunk mark + emit into a
+// mark array of the chunk's bases, make the chunk's candidates unique and merge them into the running set by the same
+// sort + unique over the union.  KmerCollector is a set, so the result is that of the resident pass.
+int iter_reads_streamed(const mhb_iterate_args *a, mhb_iterate_result *res, const ReadIndex &ix, const FlankTable &tab, int WCc,
+                        uint32_t w2, uint32_t KN, unsigned long long *cnt, uint64_t *n_cand_out, uint64_t *n_edges_out) {
+  const uint32_t k = a->k, step = a->step;
+  cudaStream_t st = 0;
+  ReadStream rs;
+  const uint64_t cap = read_chunk_limit() ? read_chunk_limit() : read_chunk_auto_bytes();
+  CKR(rs.init(a->bin, a->bin_words, a->n_reads, ix.fixed_len, ix.rec_off.data(), ix.base_off.data(), cap));
+  const std::vector<uint64_t> &first = rs.first_reads();
+  auto bases_of = [&](uint64_t b, uint64_t e) { return ix.fixed_len ? (e - b) * ix.fixed_len : ix.base_off[e] - ix.base_off[b]; };
+  uint64_t max_bases = 0;
+  for (uint64_t i = 0; i < rs.n_chunks(); ++i) max_bases = std::max(max_bases, bases_of(first[i], first[i + 1]));
+  IBuf d_slots, d_exist;
+  CKR(d_slots.alloc(rs.device_bytes(), "read chunk buffers"));
+  rs.bind(d_slots.p);
+  CKR(d_exist.alloc((max_bases / 32 + 2) * 4, "position marks"));
+  Grow c, c2, u, u2, ws, flag, off, bsum;
+  uint64_t n_cand = 0, n_set = 0;
+  auto chunk = [&](const ReadChunkView &v) -> int {
+    IterReads rd{v.bin, v.n_reads, ix.fixed_len, v.rec_off, v.aux_off};
+    const uint64_t bw = bases_of(v.first_read, v.first_read + v.n_reads) / 32 + 2;
+    CK(cudaMemsetAsync(d_exist.p, 0, bw * 4, st));
+    CK(cudaMemsetAsync(cnt + 4, 0, 16, st));
+#define M(WW)                                                                                                         \
+  if (WCc == WW) {                                                                                                    \
+    k_iter_mark<WW><<<igrid(v.n_reads, 128, 32), 128, 0, st>>>(rd, k, step, tab, d_exist.as<u32>());                   \
+    k_iter_emit<WW, false><<<igrid(v.n_reads, 128, 32), 128, 0, st>>>(rd, k, step, d_exist.as<u32>(), w2, nullptr,     \
+                                                                       cnt + 4, 0);                                   \
+  }
+    IT_FOR_WC(M)
+#undef M
+    CK_LAUNCH();
+    unsigned long long hc[2] = {0, 0};
+    CK(cudaMemcpyAsync(hc, cnt + 4, 16, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    n_cand += hc[0];
+    res->n_aligned_reads += hc[1];
+    if (!hc[0]) return MHB_OK;
+    const uint64_t nc = hc[0];
+    CKR(c.need((size_t)nc * w2 * 4 + 16, "edges"));
+    CKR(c2.need((size_t)nc * w2 * 4 + 16, "edges (sort buffer)"));
+    CK(cudaMemsetAsync(cnt + 6, 0, 8, st));
+#define M(WW)                                                                                                        \
+  if (WCc == WW)                                                                                                     \
+    k_iter_emit<WW, true><<<igrid(v.n_reads, 128, 32), 128, 0, st>>>(rd, k, step, d_exist.as<u32>(), w2, c.b.as<u32>(), \
+                                                                     cnt + 6, nc);
+    IT_FOR_WC(M)
+#undef M
+    CK_LAUNCH();
+    u32 *cu = nullptr;
+    uint64_t ncu = 0;
+    CKR(sort_unique(st, c.b.as<u32>(), c2.b.as<u32>(), nc, w2, KN, ws, flag, off, bsum, cnt + 7, &cu, &ncu));
+    // union = running set followed by this chunk's unique candidates
+    const size_t need = (size_t)(n_set + ncu) * w2 * 4 + 16;
+    if (need > u.cap) {
+      Grow g;
+      CKR(g.need(std::max(need, 2 * u.cap), "edge set"));
+      if (n_set) CK(cudaMemcpyAsync(g.b.p, u.b.p, (size_t)n_set * w2 * 4, cudaMemcpyDeviceToDevice, st));
+      CK(cudaStreamSynchronize(st));
+      std::swap(u.b.p, g.b.p);
+      std::swap(u.cap, g.cap);
+      CKR(u2.need(u.cap, "edge set (sort buffer)"));
+    }
+    CK(cudaMemcpyAsync(u.b.as<u32>() + (size_t)n_set * w2, cu, (size_t)ncu * w2 * 4, cudaMemcpyDeviceToDevice, st));
+    u32 *su = nullptr;
+    CKR(sort_unique(st, u.b.as<u32>(), u2.b.as<u32>(), n_set + ncu, w2, KN, ws, flag, off, bsum, cnt + 7, &su, &n_set));
+    if (su != u.b.as<u32>()) std::swap(u.b.p, u2.b.p);
+    return MHB_OK;
+  };
+  CKR(rs.pass(st, chunk));
+  res->edges = (uint32_t *)malloc(std::max<size_t>(1, (size_t)n_set * w2 * 4));
+  if (!res->edges) return mhb_set_error(MHB_ERR_NOMEM, "host malloc failed");
+  if (n_set) CK(cudaMemcpyAsync(res->edges, u.b.p, (size_t)n_set * w2 * 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  *n_cand_out = n_cand;
+  *n_edges_out = n_set;
+  return MHB_OK;
+}
+}  // namespace
 
 // ------------------------------------------------------------------------------------------------
 // Host mirror for the CPU tests: the same __host__ __device__ building blocks (flank records, flank search, read

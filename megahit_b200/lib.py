@@ -150,6 +150,8 @@ SYMBOLS = [
     "mhb_buildlib_host", "mhb_buildlib_free", "mhb_set_buildlib_chunk", "mhb_buildlib_run", "mhb_selftest_fastx",
     "mhb_s2s_sort", "mhb_s2s_sort_workspace_bytes", "mhb_s2s_sort_hist_byte", "mhb_s2s_sort_stats",
     "mhb_selftest_s2s_local_key",
+    "mhb_plan_read_chunks", "mhb_read_stream_decide", "mhb_set_read_chunk_limit", "mhb_read_stream_stats",
+    "mhb_read_stream_times",
 ]
 
 
@@ -347,6 +349,51 @@ def set_r2s_round_limit(s1: int = 0, s2: int = 0):
     L = load()
     L.mhb_set_r2s_round_limit.argtypes = [C.c_uint64, C.c_uint64]
     _check(L.mhb_set_r2s_round_limit(int(s1), int(s2)))
+
+
+def plan_read_chunks(bin_words: np.ndarray, n_reads: int, max_chunk_bytes: int) -> list[int]:
+    """Read chunks of the streamed path (host logic only): the first read of every chunk, then n_reads."""
+    L = load()
+    b = np.ascontiguousarray(bin_words, np.uint32).reshape(-1)
+    L.mhb_plan_read_chunks.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p, C.c_uint32]
+    n = L.mhb_plan_read_chunks(b.ctypes.data if len(b) else None, len(b), int(n_reads), int(max_chunk_bytes), None, 0)
+    if n < 0:
+        raise MhbError(L.mhb_last_error().decode())
+    first = np.zeros(n + 1, np.uint64)
+    n = L.mhb_plan_read_chunks(b.ctypes.data if len(b) else None, len(b), int(n_reads), int(max_chunk_bytes),
+                               first.ctypes.data, n + 1)
+    if n < 0:
+        raise MhbError(L.mhb_last_error().decode())
+    return [int(x) for x in first]
+
+
+def read_stream_decide(resident_bytes: int, avail_bytes: int, plan_failed: bool = False, chunk_limit: int = 0) -> bool:
+    """True when a library whose resident part takes resident_bytes is streamed, given avail_bytes of device memory."""
+    L = load()
+    L.mhb_read_stream_decide.argtypes = [C.c_uint64, C.c_uint64, C.c_int, C.c_uint64]
+    return bool(L.mhb_read_stream_decide(int(resident_bytes), int(avail_bytes), int(plan_failed), int(chunk_limit)))
+
+
+def set_read_chunk_limit(n_bytes: int = 0) -> None:
+    """Stream the read library of count / iterate in chunks of at most n_bytes (0 = only when it does not fit).  The
+    result does not depend on it."""
+    L = load()
+    L.mhb_set_read_chunk_limit.argtypes = [C.c_uint64]
+    _check(L.mhb_set_read_chunk_limit(int(n_bytes)))
+
+
+def read_stream_stats() -> dict:
+    """Streaming of the last count_host / iterate_host call: chunks (0 = resident), passes, bytes host to device, and
+    the copy-engine / compute-stream busy time, host fill time and wall time of those passes (ms)."""
+    L = load()
+    nc, npass, nb = C.c_uint64(), C.c_uint64(), C.c_uint64()
+    L.mhb_read_stream_stats.argtypes = [C.POINTER(C.c_uint64)] * 3
+    _check(L.mhb_read_stream_stats(C.byref(nc), C.byref(npass), C.byref(nb)))
+    h2d, kern, fill, wall = C.c_double(), C.c_double(), C.c_double(), C.c_double()
+    L.mhb_read_stream_times.argtypes = [C.POINTER(C.c_double)] * 4
+    _check(L.mhb_read_stream_times(C.byref(h2d), C.byref(kern), C.byref(fill), C.byref(wall)))
+    return {"n_chunks": nc.value, "n_passes": npass.value, "h2d_bytes": nb.value, "h2d_ms": h2d.value,
+            "kernel_ms": kern.value, "fill_ms": fill.value, "pass_ms": wall.value}
 
 
 def mercy_host(k: int, edges: np.ndarray, cand_bin: np.ndarray) -> np.ndarray:
