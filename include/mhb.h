@@ -391,7 +391,8 @@ int mhb_plan_rounds16(const uint64_t *hist256, const uint64_t *sub_hist, uint64_
  * resident part alone does not fit, when the plan next to it fails (count: one bucket exceeds the room left; iterate:
  * a cudaMalloc of the resident path fails), or when a chunk cap is set.  The output does not depend on it.
  * mhb_plan_read_chunks (host only, no GPU needed): cuts the reads into contiguous chunks [first[i], first[i+1]) whose
- * image is at most max_chunk_bytes each, except that a read larger than the cap gets a chunk of its own.  first_read_out
+ * image is at most max_chunk_bytes each, except that a read larger than the cap gets a chunk of its own - the plan a
+ * streamed mhb_count_host / mhb_iterate_host call uses, fixed-length libraries included.  first_read_out
  * (may be NULL) needs room for n_chunks + 1 entries (cap_out).  Returns n_chunks (0 for an empty library), or -1
  * (mhb_last_error).
  * mhb_read_stream_decide (host only): 1 when the library is streamed, given the bytes of its resident part, the device

@@ -23,16 +23,33 @@ int mhb_sort_records_untraced(void *stream, uint32_t *a, uint32_t *b, uint64_t n
 // bytes held by the arena the host-level calls keep between calls (mhb_release frees it)
 size_t mhb_arena_bytes(void);
 
-// A read library kept in host memory and streamed through the device in chunks that end on read boundaries
-// (mhb_stream.cu).  Two pinned staging buffers and two device chunk slots: while host threads fill the staging buffer
-// of chunk i+1, chunk i uploads on a copy stream and the compute stream works on chunk i-1.  Every chunk is handed to
-// the caller as an ordinary view: image at offset 0 of its 16-byte aligned slot, and for variable-length libraries the
-// per-read offsets (record words, and the caller's second array: edge or base offsets) rebased to the chunk.
+// The host-side index of a `.bin` image (sequence_package.h:224-240), mhb_stream.cu.  A fixed-length library needs no
+// side arrays; otherwise rec_off[r] = first word of read r and unit_off[r] = sum over the reads before r of
+// max(0, L - k): edge offsets for the count stage's k, base offsets for k = 0.  Both have n_reads + 1 entries.
+struct ReadLibIndex {
+  uint32_t fixed_len = 0;
+  std::vector<uint64_t> rec_off, unit_off;
+  uint64_t n_units = 0;  // sum of max(0, L - k) over all reads
+};
+// sampled = true: a library whose size matches n_reads x (1 + ceil(L0/16)) is taken as fixed-length after looking at
+// ~2048 of its length words only; the caller must then verify ALL of them on the device (mhb_check_fixed_len) and come
+// back with sampled = false when that fails.  (The full host scan touches every cache line of the image: ~10 ms for
+// 10 M reads, all of it inside the end-to-end time of the fused build.)
+int index_read_lib(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, uint32_t k, ReadLibIndex *ix,
+                   bool sampled = false);
+
+// Every pass over a read library (mhb_stream.cu), in one of two forms:
+// - resident: the library is uploaded once into the device memory the caller binds, and a pass hands it over whole;
+// - streamed: the `.bin` image stays in host memory and goes through the device in chunks that end on read boundaries.
+//   Two pinned staging buffers and two device chunk slots: while host threads fill the staging buffer of chunk i+1,
+//   chunk i uploads on a copy stream and the compute stream works on chunk i-1.
+// Either way a chunk is handed to the caller as an ordinary view: image at offset 0 of its 16-byte aligned slot, and
+// for variable-length libraries the index's two offset arrays rebased to the chunk.
 struct ReadChunkView {
   uint64_t index, first_read, n_reads;
   const uint32_t *bin;  // device
   uint64_t bin_words;
-  const uint64_t *rec_off, *aux_off;  // device, n_reads + 1 each; NULL for fixed-length libraries
+  const uint64_t *rec_off, *aux_off;  // device, n_reads + 1 each (rec_off / unit_off); NULL for fixed-length libraries
 };
 class ReadStream {
  public:
@@ -40,21 +57,24 @@ class ReadStream {
   ReadStream(const ReadStream &) = delete;
   ReadStream &operator=(const ReadStream &) = delete;
   ~ReadStream();
-  // host library (rec_off / aux_off: n_reads + 1 entries each, or NULL when fixed_len > 0); plans the chunks
-  int init(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, uint32_t fixed_len, const uint64_t *rec_off,
-           const uint64_t *aux_off, uint64_t max_chunk_bytes);
-  size_t device_bytes() const { return 2 * slot_bytes_; }  // both chunk slots
-  void bind(void *device_slots);                            // device_bytes() bytes, 256-byte aligned
-  uint64_t n_chunks() const { return first_.empty() ? 0 : first_.size() - 1; }
+  // host library and its index; max_chunk_bytes = 0: resident, otherwise streamed in chunks planned here
+  int init(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, const ReadLibIndex &ix, uint64_t max_chunk_bytes);
+  size_t device_bytes() const { return (resident_ ? 1 : 2) * slot_bytes_; }  // the library, or both chunk slots
+  // device_bytes() bytes, 256-byte aligned; the resident form uploads the library there on `stream`
+  int bind(void *device, void *stream);
+  uint64_t n_chunks() const { return resident_ ? 0 : first_.size() - 1; }  // chunks of the stream, 0 when resident
   uint64_t max_chunk_reads() const { return max_reads_; }
-  const std::vector<uint64_t> &first_reads() const { return first_; }
-  // one pass: fn runs once per chunk, in order, on the compute stream `stream`, while the chunk is on the device
+  const std::vector<uint64_t> &first_reads() const { return first_; }  // read bounds of the views, {0, n_reads} resident
+  // one pass: fn runs once per chunk, in order, on the compute stream `stream`, while the chunk is on the device; the
+  // resident form calls it once, with the whole library as chunk 0, and counts nothing in the stream statistics
   int pass(void *stream, const std::function<int(const ReadChunkView &)> &fn);
 
  private:
   int stage(uint64_t i);
+  ReadChunkView view(uint64_t i, const char *slot) const;
+  bool resident_ = false;
   const uint32_t *bin_ = nullptr;
-  uint64_t n_reads_ = 0, stride_ = 0;
+  uint64_t bin_words_ = 0, stride_ = 0;
   uint32_t fixed_len_ = 0;
   const uint64_t *rec_off_ = nullptr, *aux_off_ = nullptr;
   std::vector<uint64_t> first_;

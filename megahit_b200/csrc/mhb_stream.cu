@@ -1,6 +1,7 @@
-// mhb_stream.cu -- read libraries larger than device memory: the `.bin` image stays in host memory and every pass over
-// the reads streams it through the device in chunks that end on read boundaries (ReadStream, mhb_internal.h).  The
-// count and iterate stages hand each chunk to the same extraction / marking / emission kernels as a resident library.
+// mhb_stream.cu -- the host-side `.bin` index and every pass over a read library (ReadStream, mhb_internal.h): resident
+// in device memory, or, for libraries larger than device memory, kept in host memory and streamed through the device in
+// chunks that end on read boundaries.  The count and iterate stages hand each chunk to the same extraction / marking /
+// emission kernels whichever form the library takes.
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -30,26 +31,69 @@ struct {
 
 inline size_t pad256(size_t b) { return (b + 255) & ~(size_t)255; }
 
-// Greedy cut into chunks of at most max_bytes of image; a read larger than the cap gets a chunk of its own.
-// words_of(r) = image words of read r.  first gets n_chunks + 1 entries.
-template <class F>
-void plan_chunks(uint64_t n_reads, uint64_t max_bytes, F words_of, std::vector<uint64_t> *first) {
-  first->clear();
-  first->push_back(0);
-  uint64_t acc = 0, in = 0;
-  for (uint64_t r = 0; r < n_reads; ++r) {
-    const uint64_t b = 4 * words_of(r);
-    if (in && acc + b > max_bytes) {
-      first->push_back(r);
-      acc = 0;
-      in = 0;
+// Greedy cut into chunks of at most max_bytes of image; a read larger than the cap gets a chunk of its own.  For a
+// fixed-length library the same cut in closed form: floor(cap / record) reads per chunk.  first gets n_chunks + 1
+// entries.
+void plan_chunks(const ReadLibIndex &ix, uint64_t n_reads, uint64_t max_bytes, std::vector<uint64_t> *first) {
+  first->assign(1, 0);
+  if (ix.fixed_len) {
+    const uint64_t per = std::max<uint64_t>(1, max_bytes / (4 * (1 + div_ceil(ix.fixed_len, 16))));
+    for (uint64_t r = per; r < n_reads; r += per) first->push_back(r);
+  } else {
+    uint64_t acc = 0;
+    for (uint64_t r = 0; r < n_reads; ++r) {
+      const uint64_t b = 4 * (ix.rec_off[r + 1] - ix.rec_off[r]);
+      if (r > first->back() && acc + b > max_bytes) {
+        first->push_back(r);
+        acc = 0;
+      }
+      acc += b;
     }
-    acc += b;
-    ++in;
   }
   if (n_reads) first->push_back(n_reads);
 }
 }  // namespace
+
+int index_read_lib(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, uint32_t k, ReadLibIndex *ix, bool sampled) {
+  *ix = ReadLibIndex();
+  if (n_reads == 0) return MHB_OK;
+  if (bin_words == 0) return mhb_set_error(MHB_ERR_ARG, "empty .bin image for %llu reads", (unsigned long long)n_reads);
+  const uint32_t L0 = bin[0];
+  const uint64_t stride = 1 + div_ceil(L0, 16);
+  bool fixed = L0 > 0 && bin_words == n_reads * stride;
+  if (fixed && sampled) {
+    const uint64_t step = std::max<uint64_t>(1, n_reads / 1024);
+    for (uint64_t r = 0; r < n_reads && fixed; r += step) fixed = bin[r * stride] == L0;
+    for (uint64_t r = 0; r < std::min<uint64_t>(n_reads, 1024) && fixed; ++r) fixed = bin[r * stride] == L0;
+    fixed = fixed && bin[(n_reads - 1) * stride] == L0;
+  } else if (fixed) {
+    int bad = 0;
+#pragma omp parallel for reduction(| : bad) schedule(static)
+    for (long long r = 0; r < (long long)n_reads; ++r) bad |= bin[(uint64_t)r * stride] != L0;
+    fixed = !bad;
+  }
+  if (fixed) {
+    ix->fixed_len = L0;
+    ix->n_units = L0 > k ? n_reads * (uint64_t)(L0 - k) : 0;
+    return MHB_OK;
+  }
+  ix->rec_off.resize(n_reads + 1);
+  ix->unit_off.resize(n_reads + 1);
+  uint64_t pos = 0, u = 0;
+  for (uint64_t r = 0; r < n_reads; ++r) {
+    if (pos >= bin_words) return mhb_set_error(MHB_ERR_ARG, ".bin image truncated at read %llu", (unsigned long long)r);
+    const uint32_t L = bin[pos];
+    ix->rec_off[r] = pos;
+    ix->unit_off[r] = u;
+    if (L > k) u += L - k;
+    pos += 1 + div_ceil(L, 16);
+  }
+  if (pos > bin_words) return mhb_set_error(MHB_ERR_ARG, ".bin image truncated");
+  ix->rec_off[n_reads] = pos;
+  ix->unit_off[n_reads] = u;
+  ix->n_units = u;
+  return MHB_OK;
+}
 
 void read_stream_stats_reset() { memset(&g_st, 0, sizeof(g_st)); }
 uint64_t read_chunk_limit() { return g_chunk_limit; }
@@ -86,22 +130,10 @@ extern "C" int mhb_plan_read_chunks(const uint32_t *bin, uint64_t bin_words, uin
     mhb_set_error(MHB_ERR_ARG, "bad chunk plan arguments");
     return -1;
   }
-  std::vector<uint64_t> words(n_reads);
-  uint64_t pos = 0;
-  for (uint64_t r = 0; r < n_reads; ++r) {
-    if (pos >= bin_words) {
-      mhb_set_error(MHB_ERR_ARG, ".bin image truncated at read %llu", (unsigned long long)r);
-      return -1;
-    }
-    words[r] = 1 + div_ceil(bin[pos], 16);
-    pos += words[r];
-  }
-  if (pos > bin_words) {
-    mhb_set_error(MHB_ERR_ARG, ".bin image truncated");
-    return -1;
-  }
+  ReadLibIndex ix;
+  if (index_read_lib(bin, bin_words, n_reads, 0, &ix)) return -1;
   std::vector<uint64_t> first;
-  plan_chunks(n_reads, max_chunk_bytes, [&](uint64_t r) { return words[r]; }, &first);
+  plan_chunks(ix, n_reads, max_chunk_bytes, &first);
   const uint64_t n = first.size() - 1;
   if (first_read_out) {
     if (first.size() > cap_out) {
@@ -124,33 +156,29 @@ ReadStream::~ReadStream() {
   if (copy_) cudaStreamDestroy((cudaStream_t)copy_);
 }
 
-int ReadStream::init(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, uint32_t fixed_len, const uint64_t *rec_off,
-                     const uint64_t *aux_off, uint64_t max_chunk_bytes) {
+int ReadStream::init(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, const ReadLibIndex &ix, uint64_t max_chunk_bytes) {
+  resident_ = max_chunk_bytes == 0;
   bin_ = bin;
-  n_reads_ = n_reads;
-  fixed_len_ = fixed_len;
-  stride_ = fixed_len ? 1 + div_ceil(fixed_len, 16) : 0;
-  rec_off_ = rec_off;
-  aux_off_ = aux_off;
-  if (n_reads && !fixed_len && (!rec_off || !aux_off)) return mhb_set_error(MHB_ERR_ARG, "internal: stream of a variable-length library without offsets");
-  (void)bin_words;
-  if (fixed_len) {  // the greedy plan in closed form: floor(cap / record) reads per chunk
-    const uint64_t per = std::max<uint64_t>(1, max_chunk_bytes / (4 * stride_));
-    first_.clear();
-    for (uint64_t r = 0; r < n_reads; r += per) first_.push_back(r);
-    if (n_reads) first_.push_back(n_reads);
-    else first_.push_back(0);
+  bin_words_ = bin_words;
+  fixed_len_ = ix.fixed_len;
+  stride_ = fixed_len_ ? 1 + div_ceil(fixed_len_, 16) : 0;
+  rec_off_ = ix.rec_off.data();
+  aux_off_ = ix.unit_off.data();
+  uint64_t max_words = bin_words;
+  if (resident_) {
+    first_ = {0, n_reads};
+    max_reads_ = n_reads;
   } else {
-    plan_chunks(n_reads, max_chunk_bytes, [&](uint64_t r) { return rec_off[r + 1] - rec_off[r]; }, &first_);
+    plan_chunks(ix, n_reads, max_chunk_bytes, &first_);
+    max_words = max_reads_ = 0;
+    for (uint64_t i = 0; i < n_chunks(); ++i) {
+      max_reads_ = std::max(max_reads_, first_[i + 1] - first_[i]);
+      max_words = std::max(max_words, word_of(first_[i + 1]) - word_of(first_[i]));
+    }
   }
-  uint64_t max_words = 0;
-  max_reads_ = 0;
-  for (uint64_t i = 0; i < n_chunks(); ++i) {
-    max_reads_ = std::max(max_reads_, first_[i + 1] - first_[i]);
-    max_words = std::max(max_words, word_of(first_[i + 1]) - word_of(first_[i]));
-  }
-  off_at_ = pad256(max_words * 4 + 64);
-  slot_bytes_ = off_at_ + (fixed_len ? 0 : 2 * pad256((max_reads_ + 1) * 8));
+  // the image 16-byte aligned + 16 bytes: the extraction's bulk copies end on a 16-byte boundary
+  off_at_ = pad256(((max_words * 4 + 15) & ~(size_t)15) + 16);
+  slot_bytes_ = off_at_ + (fixed_len_ ? 0 : 2 * pad256((max_reads_ + 1) * 8));
   g_st.chunks = n_chunks();
   if (!n_chunks()) return MHB_OK;
   for (int s = 0; s < 2; ++s) CK(cudaHostAlloc((void **)&host_[s], slot_bytes_, cudaHostAllocDefault));
@@ -162,7 +190,30 @@ int ReadStream::init(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, 
   return MHB_OK;
 }
 
-void ReadStream::bind(void *device_slots) { dev_ = (char *)device_slots; }
+int ReadStream::bind(void *device, void *stream) {
+  dev_ = (char *)device;
+  if (!resident_) return MHB_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  const uint64_t n_reads = first_[1];
+  if (bin_words_) CK(cudaMemcpyAsync(dev_, bin_, bin_words_ * 4, cudaMemcpyHostToDevice, st));
+  if (!fixed_len_ && n_reads) {
+    CK(cudaMemcpyAsync(dev_ + off_at_, rec_off_, (n_reads + 1) * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(dev_ + off_at_ + pad256((n_reads + 1) * 8), aux_off_, (n_reads + 1) * 8, cudaMemcpyHostToDevice, st));
+  }
+  return MHB_OK;
+}
+
+ReadChunkView ReadStream::view(uint64_t i, const char *slot) const {
+  ReadChunkView v;
+  v.index = i;
+  v.first_read = first_[i];
+  v.n_reads = first_[i + 1] - first_[i];
+  v.bin = (const uint32_t *)slot;
+  v.bin_words = resident_ ? bin_words_ : word_of(first_[i + 1]) - word_of(first_[i]);
+  v.rec_off = fixed_len_ ? nullptr : (const uint64_t *)(slot + off_at_);
+  v.aux_off = fixed_len_ ? nullptr : (const uint64_t *)(slot + off_at_ + pad256((max_reads_ + 1) * 8));
+  return v;
+}
 
 // fill the staging buffer of chunk i (host threads) and queue its upload on the copy stream
 int ReadStream::stage(uint64_t i) {
@@ -206,9 +257,10 @@ int ReadStream::stage(uint64_t i) {
 }
 
 int ReadStream::pass(void *stream, const std::function<int(const ReadChunkView &)> &fn) {
+  if (!dev_) return mhb_set_error(MHB_ERR_ARG, "internal: read library without device memory");
+  if (resident_) return fn(view(0, dev_));
   const uint64_t nc = n_chunks();
   if (!nc) return MHB_OK;
-  if (!dev_) return mhb_set_error(MHB_ERR_ARG, "internal: read stream without device slots");
   cudaStream_t st = (cudaStream_t)stream;
   ++g_st.passes;
   const auto t0 = std::chrono::steady_clock::now();
@@ -218,16 +270,7 @@ int ReadStream::pass(void *stream, const std::function<int(const ReadChunkView &
     if (i + 1 < nc) CKR(stage(i + 1));
     CK(cudaStreamWaitEvent(st, (cudaEvent_t)ev_[4 * i + 1], 0));
     CK(cudaEventRecord((cudaEvent_t)ev_[4 * i + 2], st));
-    const char *d = dev_ + (i & 1) * slot_bytes_;
-    ReadChunkView v;
-    v.index = i;
-    v.first_read = first_[i];
-    v.n_reads = first_[i + 1] - first_[i];
-    v.bin = (const uint32_t *)d;
-    v.bin_words = word_of(first_[i + 1]) - word_of(first_[i]);
-    v.rec_off = fixed_len_ ? nullptr : (const uint64_t *)(d + off_at_);
-    v.aux_off = fixed_len_ ? nullptr : (const uint64_t *)(d + off_at_ + pad256((max_reads_ + 1) * 8));
-    CKR(fn(v));
+    CKR(fn(view(i, dev_ + (i & 1) * slot_bytes_)));
     CK(cudaEventRecord((cudaEvent_t)ev_[4 * i + 3], st));
   }
   CK(cudaEventSynchronize((cudaEvent_t)ev_[4 * (nc - 1) + 3]));
