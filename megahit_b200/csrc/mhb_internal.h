@@ -44,12 +44,13 @@ int index_read_lib(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, ui
 //   Two pinned staging buffers and two device chunk slots: while host threads fill the staging buffer of chunk i+1,
 //   chunk i uploads on a copy stream and the compute stream works on chunk i-1.
 // Either way a chunk is handed to the caller as an ordinary view: image at offset 0 of its 16-byte aligned slot, and
-// for variable-length libraries the index's two offset arrays rebased to the chunk.
+// for variable-length libraries the index's two offset arrays rebased to the chunk (unit_off only when the index has it).
 struct ReadChunkView {
   uint64_t index, first_read, n_reads;
   const uint32_t *bin;  // device
   uint64_t bin_words;
   const uint64_t *rec_off, *aux_off;  // device, n_reads + 1 each (rec_off / unit_off); NULL for fixed-length libraries
+                                      // (aux_off also when the index has no unit_off)
 };
 class ReadStream {
  public:

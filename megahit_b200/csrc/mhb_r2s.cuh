@@ -25,6 +25,8 @@ MHB_HD u32 r2s_s2_words(u32 k) { return div_ceil(2 * k + 4, 32); }            //
 static constexpr int kKmInsertThreshold = 64;                                 // kmsort.h:16
 
 // Reads in PACKAGE orientation (reversed, not complemented: read_to_sdbg_s1.cpp:89,100), one word-aligned run per read.
+// A view covers the whole library or one streamed chunk of it: read indices, words and the offset arrays are relative
+// to the view, base(r) - every bit-plane index and stage-1 payload - is global.
 struct PkgView {
   const u32 *words;
   u64 n_reads;
@@ -32,12 +34,13 @@ struct PkgView {
   u32 fixed_words;
   const u64 *word_off;  // variable-length libraries: n_reads + 1
   const u32 *len;       // n_reads (a zero-length read counts as one base, sequence_package.h:276-281)
-  const u64 *base_off;  // n_reads + 1: full_offset_in_pkg of each read
-  const u64 *s1_off;    // n_reads + 1: stage-1 records before read r
-  const u64 *edge_off;  // n_reads + 1: (k+1)-mer positions before read r
+  const u64 *base_off;  // n_reads + 1: bases before read r in the view
+  const u64 *s1_off;    // n_reads + 1: stage-1 records before read r in the view
+  const u64 *edge_off;  // n_reads + 1: (k+1)-mer positions before read r in the view
+  u64 base0;            // full_offset_in_pkg of the view's read 0 (0 for the whole library)
   MHB_HD u32 L(u64 r) const { return fixed_len ? fixed_len : len[r]; }
   MHB_HD const u32 *ptr(u64 r) const { return words + (fixed_len ? r * (u64)fixed_words : word_off[r]); }
-  MHB_HD u64 base(u64 r) const { return fixed_len ? r * (u64)fixed_len : base_off[r]; }
+  MHB_HD u64 base(u64 r) const { return base0 + (fixed_len ? r * (u64)fixed_len : base_off[r]); }
   // last r with off_array[r] <= x
   static MHB_HD u64 find(const u64 *off, u64 n, u64 x) {
     u64 lo = 0, hi = n;
@@ -47,8 +50,20 @@ struct PkgView {
     }
     return lo;
   }
-  MHB_HD u64 read_of_base(u64 off) const { return fixed_len ? off / fixed_len : find(base_off, n_reads, off); }
+  MHB_HD u64 read_of_base(u64 off) const {
+    return fixed_len ? (off - base0) / fixed_len : find(base_off, n_reads, off - base0);
+  }
 };
+
+// Package geometry of one read of file length L_file (the `.bin` length word), as index_pkg counts it: bases (a
+// zero-length read counts as one, sequence_package.h:276-281), package words, stage-1 records, (k+1)-mer positions.
+// Exclusive scans of these over a chunk give the chunk's base_off / word_off / s1_off / edge_off.
+MHB_HD void r2s_read_geom(u32 L_file, u32 k, u32 &len, u32 &words, u32 &s1, u32 &edges) {
+  len = L_file == 0 ? 1u : L_file;
+  words = div_ceil(len, 16);
+  s1 = len >= k + 1 ? len - k + 4 : 0u;
+  edges = len >= k + 1 ? len - k : 0u;
+}
 
 MHB_HD u32 comp_or_sentinel(u32 c) { return c == kSentinel ? kSentinel : 3u - c; }
 
@@ -511,6 +526,20 @@ __global__ void __launch_bounds__(256) k_r2s_reverse(const u32 *__restrict__ bin
       if (i < L) w |= base_at(src + 1, L - 1 - i) << (30 - 2 * c);
     }
     out[t] = w;
+  }
+}
+
+// per-read geometry (r2s_read_geom) of a variable-length `.bin` chunk, rec_off rebased to the chunk
+__global__ void __launch_bounds__(256) k_r2s_chunk_geom(const u32 *__restrict__ bin, const u64 *__restrict__ rec_off, u64 n_reads,
+                                                       u32 k, u32 *__restrict__ len, u32 *__restrict__ words,
+                                                       u32 *__restrict__ s1, u32 *__restrict__ edges) {
+  for (u64 r = (u64)blockIdx.x * 256 + threadIdx.x; r < n_reads; r += (u64)gridDim.x * 256) {
+    u32 l, w, s, e;
+    r2s_read_geom(bin[rec_off[r]], k, l, w, s, e);
+    len[r] = l;
+    words[r] = w;
+    s1[r] = s;
+    edges[r] = e;
   }
 }
 

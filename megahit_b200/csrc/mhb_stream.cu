@@ -163,7 +163,7 @@ int ReadStream::init(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, 
   fixed_len_ = ix.fixed_len;
   stride_ = fixed_len_ ? 1 + div_ceil(fixed_len_, 16) : 0;
   rec_off_ = ix.rec_off.data();
-  aux_off_ = ix.unit_off.data();
+  aux_off_ = ix.unit_off.empty() ? nullptr : ix.unit_off.data();  // an index without unit offsets streams none
   uint64_t max_words = bin_words;
   if (resident_) {
     first_ = {0, n_reads};
@@ -178,7 +178,7 @@ int ReadStream::init(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, 
   }
   // the image 16-byte aligned + 16 bytes: the extraction's bulk copies end on a 16-byte boundary
   off_at_ = pad256(((max_words * 4 + 15) & ~(size_t)15) + 16);
-  slot_bytes_ = off_at_ + (fixed_len_ ? 0 : 2 * pad256((max_reads_ + 1) * 8));
+  slot_bytes_ = off_at_ + (fixed_len_ ? 0 : (aux_off_ ? 2 : 1) * pad256((max_reads_ + 1) * 8));
   g_st.chunks = n_chunks();
   if (!n_chunks()) return MHB_OK;
   for (int s = 0; s < 2; ++s) CK(cudaHostAlloc((void **)&host_[s], slot_bytes_, cudaHostAllocDefault));
@@ -198,7 +198,8 @@ int ReadStream::bind(void *device, void *stream) {
   if (bin_words_) CK(cudaMemcpyAsync(dev_, bin_, bin_words_ * 4, cudaMemcpyHostToDevice, st));
   if (!fixed_len_ && n_reads) {
     CK(cudaMemcpyAsync(dev_ + off_at_, rec_off_, (n_reads + 1) * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(dev_ + off_at_ + pad256((n_reads + 1) * 8), aux_off_, (n_reads + 1) * 8, cudaMemcpyHostToDevice, st));
+    if (aux_off_)
+      CK(cudaMemcpyAsync(dev_ + off_at_ + pad256((n_reads + 1) * 8), aux_off_, (n_reads + 1) * 8, cudaMemcpyHostToDevice, st));
   }
   return MHB_OK;
 }
@@ -211,7 +212,7 @@ ReadChunkView ReadStream::view(uint64_t i, const char *slot) const {
   v.bin = (const uint32_t *)slot;
   v.bin_words = resident_ ? bin_words_ : word_of(first_[i + 1]) - word_of(first_[i]);
   v.rec_off = fixed_len_ ? nullptr : (const uint64_t *)(slot + off_at_);
-  v.aux_off = fixed_len_ ? nullptr : (const uint64_t *)(slot + off_at_ + pad256((max_reads_ + 1) * 8));
+  v.aux_off = fixed_len_ || !aux_off_ ? nullptr : (const uint64_t *)(slot + off_at_ + pad256((max_reads_ + 1) * 8));
   return v;
 }
 
@@ -234,11 +235,11 @@ int ReadStream::stage(uint64_t i) {
   const uint64_t nr = e - b;
   uint64_t *ro = (uint64_t *)(h + off_at_), *ao = (uint64_t *)(h + off_at_ + pad256((max_reads_ + 1) * 8));
   if (!fixed_len_) {
-    const uint64_t r0 = rec_off_[b], a0 = aux_off_[b];
+    const uint64_t r0 = rec_off_[b], a0 = aux_off_ ? aux_off_[b] : 0;
 #pragma omp parallel for schedule(static)
     for (long long r = 0; r <= (long long)nr; ++r) {
       ro[r] = rec_off_[b + r] - r0;
-      ao[r] = aux_off_[b + r] - a0;
+      if (aux_off_) ao[r] = aux_off_[b + r] - a0;
     }
   }
   g_st.fill_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
@@ -249,8 +250,9 @@ int ReadStream::stage(uint64_t i) {
   g_st.h2d_bytes += nw * 4;
   if (!fixed_len_) {
     CK(cudaMemcpyAsync(d + off_at_, ro, (nr + 1) * 8, cudaMemcpyHostToDevice, cs));
-    CK(cudaMemcpyAsync(d + off_at_ + pad256((max_reads_ + 1) * 8), ao, (nr + 1) * 8, cudaMemcpyHostToDevice, cs));
-    g_st.h2d_bytes += 2 * (nr + 1) * 8;
+    if (aux_off_)
+      CK(cudaMemcpyAsync(d + off_at_ + pad256((max_reads_ + 1) * 8), ao, (nr + 1) * 8, cudaMemcpyHostToDevice, cs));
+    g_st.h2d_bytes += (aux_off_ ? 2 : 1) * (nr + 1) * 8;
   }
   CK(cudaEventRecord((cudaEvent_t)ev_[4 * i + 1], cs));
   return MHB_OK;

@@ -147,6 +147,7 @@ SYMBOLS = [
     "mhb_release", "mhb_count_run", "mhb_count_run_multi", "mhb_seq2sdbg_run", "mhb_selftest_count_record", "mhb_selftest_count_records_roll", "mhb_selftest_s2s_record",
     "mhb_iterate_host", "mhb_iterate_run", "mhb_selftest_iterate", "mhb_s2s_extract_edges_pruned", "mhb_s2s_emit_fmt", "mhb_read2sdbg_host", "mhb_read2sdbg_run", "mhb_selftest_r2s_s1_record", "mhb_selftest_r2s_item",
     "mhb_selftest_kmsort", "mhb_selftest_kmsort_smem", "mhb_selftest_r2s_s1_group", "mhb_selftest_r2s_mercy_read",
+    "mhb_selftest_r2s_chunk_index", "mhb_selftest_r2s_stream_decide",
     "mhb_buildlib_host", "mhb_buildlib_free", "mhb_set_buildlib_chunk", "mhb_buildlib_run", "mhb_selftest_fastx",
     "mhb_s2s_sort", "mhb_s2s_sort_workspace_bytes", "mhb_s2s_sort_hist_byte", "mhb_s2s_sort_stats",
     "mhb_selftest_s2s_local_key",
@@ -375,15 +376,15 @@ def read_stream_decide(resident_bytes: int, avail_bytes: int, plan_failed: bool 
 
 
 def set_read_chunk_limit(n_bytes: int = 0) -> None:
-    """Stream the read library of count / iterate in chunks of at most n_bytes (0 = only when it does not fit).  The
-    result does not depend on it."""
+    """Stream the read library of count / iterate / read2sdbg in chunks of at most n_bytes (0 = only when it does not
+    fit).  The result does not depend on it."""
     L = load()
     L.mhb_set_read_chunk_limit.argtypes = [C.c_uint64]
     _check(L.mhb_set_read_chunk_limit(int(n_bytes)))
 
 
 def read_stream_stats() -> dict:
-    """Streaming of the last count_host / iterate_host call: chunks (0 = resident), passes, bytes host to device, and
+    """Streaming of the last count_host / iterate_host / read2sdbg_host call: chunks (0 = resident), passes, bytes host to device, and
     the copy-engine / compute-stream busy time, host fill time and wall time of those passes (ms)."""
     L = load()
     nc, npass, nb = C.c_uint64(), C.c_uint64(), C.c_uint64()
@@ -710,6 +711,40 @@ def selftest_kmsort(recs: np.ndarray, nw: int, smem: bool = False, cap: int = 65
     else:
         _check(load().mhb_selftest_kmsort(recs.ctypes.data, len(recs), nw))
     return recs
+
+
+def selftest_r2s_chunk_index(bin_words: np.ndarray, n_reads: int, k: int, first: int, count: int, derive: bool) -> dict:
+    """Offsets of the reads [first, first + count) of a read2sdbg package: as a streamed chunk derives them from its own
+    records (derive), or index_pkg's arrays of the whole library sliced and rebased.  Host code only."""
+    L = load()
+    b = np.ascontiguousarray(bin_words, np.uint32).reshape(-1)
+    out = {"len": np.zeros(max(count, 1), np.uint32)}
+    for name in ("word_off", "base_off", "s1_off", "edge_off"):
+        out[name] = np.zeros(count + 1, np.uint64)
+    base0 = C.c_uint64()
+    L.mhb_selftest_r2s_chunk_index.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_uint64, C.c_uint64,
+                                               C.c_int] + [C.c_void_p] * 5 + [C.POINTER(C.c_uint64)]
+    _check(L.mhb_selftest_r2s_chunk_index(b.ctypes.data if len(b) else None, len(b), n_reads, k, first, count, int(derive),
+                                          out["len"].ctypes.data, out["word_off"].ctypes.data, out["base_off"].ctypes.data,
+                                          out["s1_off"].ctypes.data, out["edge_off"].ctypes.data, C.byref(base0)))
+    out["len"] = out["len"][:count]
+    out["base0"] = base0.value
+    return out
+
+
+def r2s_stream_decide(n_reads: int, bin_words: int, fixed_len: int, n_words: int, n_bases: int, n_s1: int, n_edges: int,
+                      k: int, m: int, need_mercy: bool, free_bytes: int, chunk_limit: int = 0) -> dict:
+    """read2sdbg's residency rule on given library sizes: whether the library is streamed, and the bytes of its
+    resident form and of its upload.  Host code only."""
+    L = load()
+    res, up, stream = C.c_uint64(), C.c_uint64(), C.c_int()
+    L.mhb_selftest_r2s_stream_decide.argtypes = [C.c_uint64, C.c_uint64, C.c_uint32, C.c_uint64, C.c_uint64, C.c_uint64,
+                                                 C.c_uint64, C.c_uint32, C.c_int32, C.c_int, C.c_uint64, C.c_uint64,
+                                                 C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_int)]
+    _check(L.mhb_selftest_r2s_stream_decide(n_reads, bin_words, fixed_len, n_words, n_bases, n_s1, n_edges, k, m,
+                                            int(need_mercy), free_bytes, chunk_limit, C.byref(res), C.byref(up),
+                                            C.byref(stream)))
+    return {"stream": bool(stream.value), "resident": res.value, "upload": up.value}
 
 
 def set_buildlib_chunk(n_bytes: int) -> None:
