@@ -430,6 +430,48 @@ typedef struct {
 } mhb_s2s_result;
 
 int mhb_s2s_host(const mhb_s2s_args *args, mhb_s2s_result *res);
+/* Sequence sets and edge arrays larger than device memory (mhb_s2s_host, mhb_mercy_host, and so `seq2sdbg` and the
+ * staged mhb_build_host).  mhb_s2s_host keeps the sequences resident whenever they and a one-item round fit in 92 % of
+ * the free device memory (a cached arena counts as free) and no chunk cap is set (mhb_read_stream_decide); otherwise
+ * they stay in host memory and every pass streams them through the device in chunks that end on sequence boundaries
+ * (a sequence larger than the cap gets a chunk of its own): a top-byte histogram pass, one more pass for the
+ * second-byte histograms of leading bytes that alone exceed a round, and one pass per non-empty round.  A chunk of the
+ * fixed-length edge layout carries words + multiplicities, any other chunk also word_off, item_off and len.
+ * mhb_mercy_host streams the sorted edges when they do not fit next to the candidate reads and the scratch, or when the
+ * cap is set: the edge array is cut into contiguous leading-byte segments, each uploaded and searched in turn, their
+ * answers OR-ed into one set of answer planes.  Without a cap the segments are packed to about 1 GiB of edges, and a
+ * leading byte above that is a segment of its own, with device slots (two) and pinned staging sized to it; only a byte
+ * whose edges exceed half of what the candidate reads, scratch and planes leave of the device returns MHB_ERR_NOMEM
+ * naming the byte.  With a cap, a segment holds at most the cap and a byte above it is refused the same way.  The candidate reads stay resident.  The output depends on neither.
+ * mhb_set_s2s_chunk_limit: 0 = automatic; otherwise both calls stream, in chunks / segments of at most that many bytes
+ *   (independent of mhb_set_read_chunk_limit).
+ * mhb_plan_seq_chunks (host only): the chunks [first[i], first[i+1]) a streamed mhb_s2s_host uses; a sequence takes
+ *   4 bytes per word plus 2 (fixed-length edge layout, cut in closed form) or 22 (any other layout).  first_seq_out (may
+ *   be NULL) needs room for n_chunks + 1 entries.  Returns n_chunks (0 for no sequences) or -1.
+ * mhb_plan_mercy_segments (host only): the segments [first[i], first[i+1]) of leading bytes a streamed mhb_mercy_host
+ *   searches, first[0] = 0 and first[n] = 256; returns n or -1 (a byte above the cap: MHB_ERR_NOMEM).
+ * mhb_s2s_stream_stats / _times: mercy = 0, the last mhb_s2s_host call - chunks (0 = resident), passes over the
+ *   streamed sequences, rounds run (1 = one pass), bytes host to device; mercy = 1, the last mhb_mercy_host call -
+ *   segments (0 = resident) in n_chunks, passes, n_rounds = 0, bytes host to device.  Times as mhb_read_stream_times. */
+int mhb_set_s2s_chunk_limit(uint64_t bytes);
+int mhb_plan_seq_chunks(const uint64_t *word_off, const uint32_t *len, uint64_t n_seqs, uint32_t k, uint64_t max_chunk_bytes,
+                        uint64_t *first_seq_out, uint32_t cap_out);
+int mhb_plan_mercy_segments(const uint32_t *edges, uint64_t n_edges, uint32_t k, uint64_t max_segment_bytes,
+                            uint32_t *first_byte_out, uint32_t cap_out);
+int mhb_s2s_stream_stats(int mercy, uint64_t *n_chunks, uint64_t *n_passes, uint64_t *n_rounds, uint64_t *h2d_bytes);
+int mhb_s2s_stream_times(int mercy, double *h2d_ms, double *kernel_ms, double *fill_ms, double *pass_ms);
+/* The residency rules of mhb_s2s_host (rounds) and mhb_mercy_host on given sizes: the device bytes of the resident
+ * form and whether it is streamed with free_bytes of free device memory (host only, for tests). */
+int mhb_selftest_s2s_stream_decide(uint64_t n_seqs, uint64_t n_words, uint32_t k, uint64_t free_bytes, uint64_t chunk_limit,
+                                   uint64_t *resident_bytes, int *stream);
+/* mhb_mercy_host's segment plan without a cap on a leading-byte histogram (byte_edges[256] edges per byte) with free_bytes
+ * of free device memory: returns the number of segments (first_byte_out gets n + 1 entries, room for 257) and the bytes
+ * of one device slot, or -1 (MHB_ERR_NOMEM naming a byte that does not fit).  Host only, for tests. */
+int mhb_selftest_mercy_auto_plan(const uint64_t *byte_edges, uint32_t k, uint64_t n_cand_reads, uint64_t cand_words,
+                                 uint32_t max_read_len, uint64_t free_bytes, uint32_t *first_byte_out, uint64_t *slot_bytes);
+int mhb_selftest_mercy_stream_decide(uint64_t n_edges, uint32_t k, uint64_t n_cand_reads, uint64_t cand_words,
+                                     uint32_t max_read_len, uint64_t free_bytes, uint64_t chunk_limit,
+                                     uint64_t *resident_bytes, int *stream);
 
 /* Fused k_min build (SURVEY.md 8f N1): reads in, SdBG out, everything between stays in HBM.
  * count (extract + sort + solid edges + mercy bookkeeping) -> mercy edges (device, need_mercy) -> seq2sdbg

@@ -406,6 +406,9 @@ extern "C" int mhb_seq2sdbg_run(const mhb_seq2sdbg_opts *o) {
       uint32_t *mercy = nullptr;
       uint64_t nm = 0, nr = 0;
       if (int rc = mhb_mercy_host(k, edges.data(), n, cand.data(), cand.size(), &mercy, &nm, &nr)) return rc;
+      uint64_t n_seg = 0;
+      mhb_s2s_stream_stats(1, &n_seg, nullptr, nullptr, nullptr);
+      if (n_seg) XINFO("Mercy search: edges streamed in %llu leading-byte segments\n", (unsigned long long)n_seg);
       for (uint64_t i = 0; i < nm; ++i) seqs.append_packed(mercy + i * W, k + 1, 1);
       mhb_free(mercy);
       XINFO("Number of reads: %lld, Number of mercy edges: %lld\n", (long long)nr, (long long)nm);
@@ -442,6 +445,13 @@ extern "C" int mhb_seq2sdbg_run(const mhb_seq2sdbg_opts *o) {
   if (int rc = mhb_s2s_host(&a, res)) return rc;
   XINFO("GPU seq2sdbg: %llu sort items, extract %.2f ms, sort %.2f ms, emit %.2f ms\n", (unsigned long long)res->n_records,
         res->t_extract_ms, res->t_sort_ms, res->t_emit_ms);
+  {
+    uint64_t nc = 0, np = 0, nrd = 0, nb = 0;
+    mhb_s2s_stream_stats(0, &nc, &np, &nrd, &nb);
+    if (nc) XINFO("GPU seq2sdbg: sequences streamed in %llu chunks, %llu passes, %llu rounds, %.1f MB host to device\n",
+                  (unsigned long long)nc, (unsigned long long)np, (unsigned long long)nrd, nb / 1e6);
+    else XINFO("GPU seq2sdbg: sequences resident, %llu round(s)\n", (unsigned long long)nrd);
+  }
 
   const int rc = write_sdbg_single(prefix, k, res->words_per_tip_label, res->n_items, res->n_bytes, res->bytes, res->bucket_table);
   XINFO("Number of $ A C G T A- C- G- T-:\n");

@@ -622,55 +622,213 @@ extern "C" int mhb_count_host(const mhb_count_args *args, mhb_count_result *res)
 }
 
 // ================================================================================================
-// seq2sdbg, out of core (A13): rounds over ranges of the leading record byte
+// seq2sdbg, out of core (A13): rounds over ranges of the leading record byte, sequences resident or streamed
 // ================================================================================================
 namespace {
+uint64_t g_s2s_chunk_limit = 0;  // sequence chunk / mercy segment cap in bytes; 0 = stream only what does not fit
+StreamStats g_s2s_st, g_mercy_st;
+uint64_t g_s2s_rounds = 0;
+
 size_t s2s_round_bytes(uint64_t n, uint32_t W, uint32_t k) {
   return 2 * Arena::pad((size_t)n * W * 4 + 16) + Arena::pad(mhb_s2s_sort_workspace_bytes(n, k)) +
          Arena::pad(mhb_s2s_emit_scratch_bytes(n, k)) + Arena::pad((size_t)n * (4ull + 4ull * words_per_tip_label(k)) + 16);
+}
+// what the rounds keep next to the sequences: bucket table, histograms (+ the second-byte rows of oversized bytes),
+// totals, cursor
+size_t s2s_table_bytes() {
+  return Arena::pad((size_t)MHB_NUM_BUCKETS * 4 * 8) + 2 * Arena::pad(256 * 8) + Arena::pad(256 * 256 * 8) +
+         Arena::pad(16 * 8) + Arena::pad(64) + 8192;
+}
+double device_avail_bytes() {
+  size_t free_b = 0, total_b = 0;
+  if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) {
+    cudaGetLastError();
+    return 0;
+  }
+  return 0.92 * (double)(free_b + g_arena.cap);
+}
+
+// The layout of mhb_s2s_args: item offsets (exclusive prefix of 2 * (len - k + 2) over sequences of len >= k + 1) and
+// whether it is the fixed-length, gap-free layout of edges (every sequence L0 >= k + 1 bases at stride ceil(L0 / 16)).
+struct SeqLayout {
+  std::vector<uint64_t> item_off;
+  uint64_t n_items = 0, n_words = 0;
+  bool fixed = false;
+  uint32_t L0 = 0;
+};
+void seq_layout(const uint64_t *word_off, const uint32_t *len, uint64_t ns, uint32_t k, SeqLayout *ly) {
+  ly->item_off.resize(ns + 1);
+  ly->n_items = 0;
+  ly->fixed = ns > 0;
+  ly->L0 = ns ? len[0] : 0;
+  for (uint64_t s = 0; s < ns; ++s) {
+    ly->item_off[s] = ly->n_items;
+    const uint32_t L = len[s];
+    if (L >= k + 1) ly->n_items += 2ull * (L - k + 2);
+    if (L != ly->L0 || word_off[s] != s * (uint64_t)div_ceil(ly->L0, 16)) ly->fixed = false;
+  }
+  ly->item_off[ns] = ly->n_items;
+  if (ly->L0 < k + 1) ly->fixed = false;
+  ly->n_words = ns ? word_off[ns] : 0;
+}
+// upload bytes of one sequence in a chunk: its words, its multiplicity and, unless fixed-length, word_off + item_off +
+// len
+uint64_t seq_extra_bytes(bool fixed) { return fixed ? 2 : 8 + 8 + 4 + 2; }
+void plan_seq_chunks(const uint64_t *word_off, const SeqLayout &ly, uint64_t ns, uint64_t max_bytes, std::vector<uint64_t> *first) {
+  plan_chunks(ly.fixed ? nullptr : word_off, div_ceil(ly.L0, 16), seq_extra_bytes(ly.fixed), ns, max_bytes, first);
+}
+
+// The sequences of one mhb_s2s_host call as its round loop sees them, one pass at a time: resident (uploaded once and
+// handed over whole as one chunk, the arrays every call had), or kept in host memory and streamed through two device
+// slots in chunks that end on sequence boundaries.  A fixed-length chunk carries its words and multiplicities and is
+// viewed with fixed_len set; a variable-length one also carries word_off and item_off rebased to the chunk, and len.
+class SeqSource {
+ public:
+  SeqSource(const mhb_s2s_args *a, const SeqLayout &ly) : a_(a), ly_(ly) {}
+  // max_chunk_bytes = 0: resident
+  int init(uint64_t max_chunk_bytes) {
+    const uint64_t ns = a_->n_seqs;
+    resident_ = max_chunk_bytes == 0;
+    uint64_t max_words = ly_.n_words, max_n = ns;
+    if (resident_) {
+      first_ = {0, ns};
+    } else {
+      plan_seq_chunks(a_->word_off, ly_, ns, max_chunk_bytes, &first_);
+      max_words = max_n = 0;
+      for (uint64_t i = 0; i < n_chunks(); ++i) {
+        max_n = std::max(max_n, first_[i + 1] - first_[i]);
+        max_words = std::max(max_words, a_->word_off[first_[i + 1]] - a_->word_off[first_[i]]);
+      }
+    }
+    const bool arrays = resident_ || !ly_.fixed;  // the resident form keeps all four arrays, as it always did
+    o_wo_ = Arena::pad(max_words * 4 + 64);
+    o_io_ = o_wo_ + (arrays ? Arena::pad((max_n + 1) * 8) : 0);
+    o_len_ = o_io_ + (arrays ? Arena::pad((max_n + 1) * 8) : 0);
+    o_mult_ = o_len_ + (arrays ? Arena::pad((max_n + 1) * 4) : 0);
+    slot_bytes_ = o_mult_ + Arena::pad((max_n + 1) * 2);
+    g_s2s_st.chunks = n_chunks();
+    return resident_ ? MHB_OK : stager_.init(slot_bytes_, n_chunks(), &g_s2s_st);
+  }
+  static size_t resident_bytes(uint64_t ns, uint64_t n_words) {
+    return Arena::pad(n_words * 4 + 64) + 2 * Arena::pad((ns + 1) * 8) + Arena::pad((ns + 1) * 4) + Arena::pad((ns + 1) * 2);
+  }
+  size_t device_bytes() const { return (resident_ ? 1 : 2) * slot_bytes_; }
+  uint64_t n_chunks() const { return resident_ ? 0 : first_.size() - 1; }
+  // device_bytes() bytes; the resident form uploads the sequences there on st
+  int bind(char *dev, cudaStream_t st) {
+    dev_ = dev;
+    stager_.bind(dev);
+    const uint64_t ns = a_->n_seqs;
+    if (!resident_ || !ns) return MHB_OK;
+    CK(cudaMemcpyAsync(dev_, a_->words, ly_.n_words * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(dev_ + o_wo_, a_->word_off, (ns + 1) * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(dev_ + o_io_, ly_.item_off.data(), (ns + 1) * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(dev_ + o_len_, a_->len, ns * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(dev_ + o_mult_, a_->mult, ns * 2, cudaMemcpyHostToDevice, st));
+    return MHB_OK;
+  }
+  // fn(view, items of the chunk) once per chunk, in order, on st
+  int pass(cudaStream_t st, const std::function<int(const mhb_dev_seqs &, uint64_t)> &fn) {
+    if (resident_) return fn(view(0, dev_), ly_.n_items);
+    return stager_.pass(
+        st, [this](uint64_t i, char *h, ChunkStager::Copies *up) { return fill(i, h, up); },
+        [&](uint64_t i, const char *slot) { return fn(view(i, slot), ly_.item_off[first_[i + 1]] - ly_.item_off[first_[i]]); });
+  }
+
+ private:
+  mhb_dev_seqs view(uint64_t i, const char *slot) const {
+    const uint64_t b = first_[i], e = first_[i + 1];
+    const bool arrays = resident_ || !ly_.fixed;
+    mhb_dev_seqs v;
+    v.words = (const uint32_t *)slot;
+    v.n_words = a_->word_off[e] - a_->word_off[b];
+    v.n_seqs = e - b;
+    v.fixed_len = ly_.fixed ? ly_.L0 : 0;
+    v.word_off = arrays ? (const uint64_t *)(slot + o_wo_) : nullptr;
+    v.item_off = arrays ? (const uint64_t *)(slot + o_io_) : nullptr;
+    v.len = arrays ? (const uint32_t *)(slot + o_len_) : nullptr;
+    v.mult = (const uint16_t *)(slot + o_mult_);
+    v.fixed_stride = 0;
+    return v;
+  }
+  int fill(uint64_t i, char *h, ChunkStager::Copies *up) const {
+    const uint64_t b = first_[i], e = first_[i + 1], n = e - b, w0 = a_->word_off[b], nw = a_->word_off[e] - w0;
+    {
+      const uint64_t bytes = nw * 4, blk = 4ull << 20, nblk = (bytes + blk - 1) / blk;
+#pragma omp parallel for schedule(static)
+      for (long long j = 0; j < (long long)nblk; ++j) {
+        const uint64_t o = (uint64_t)j * blk;
+        memcpy(h + o, (const char *)(a_->words + w0) + o, std::min(blk, bytes - o));
+      }
+    }
+    up->add(0, nw * 4);
+    if (!ly_.fixed) {
+      uint64_t *wo = (uint64_t *)(h + o_wo_), *io = (uint64_t *)(h + o_io_);
+      const uint64_t i0 = ly_.item_off[b];
+#pragma omp parallel for schedule(static)
+      for (long long s = 0; s <= (long long)n; ++s) {
+        wo[s] = a_->word_off[b + s] - w0;
+        io[s] = ly_.item_off[b + s] - i0;
+      }
+      memcpy(h + o_len_, a_->len + b, n * 4);
+      up->add(o_wo_, (n + 1) * 8);
+      up->add(o_io_, (n + 1) * 8);
+      up->add(o_len_, n * 4);
+    }
+    memcpy(h + o_mult_, a_->mult + b, n * 2);
+    up->add(o_mult_, n * 2);
+    return MHB_OK;
+  }
+  const mhb_s2s_args *a_;
+  const SeqLayout &ly_;
+  bool resident_ = true;
+  std::vector<uint64_t> first_;
+  size_t o_wo_ = 0, o_io_ = 0, o_len_ = 0, o_mult_ = 0, slot_bytes_ = 0;
+  char *dev_ = nullptr;
+  ChunkStager stager_;
+};
+
+// the smallest device footprint of the rounds over resident sequences: the sequences, the tables and a one-item round
+size_t s2s_resident_round_bytes(uint64_t ns, uint64_t n_words, uint32_t k) {
+  return SeqSource::resident_bytes(ns, n_words) + s2s_table_bytes() + s2s_round_bytes(1, s2s_record_words(k), k);
 }
 }  // namespace
 
 // Same idea as count_host_rounds: the sort items of all sequences do not fit in HBM next to the sequences, so the
 // stage runs once per contiguous range of leading record bytes (a (k-1)-mer group, and a bucket, never spans two
 // ranges): extract the range -> sort -> emit -> append the item bytes and that range's rows of the bucket table to the
-// host result.  Ranges ascend, so the concatenated stream is in bucket order.
-static int s2s_host_rounds(const mhb_s2s_args *args, mhb_s2s_result *res, const std::vector<uint64_t> &item_off,
-                           uint64_t n_items, bool fixed, uint32_t L0, uint64_t n_words, uint64_t max_items) {
+// host result.  Ranges ascend, so the concatenated stream is in bucket order.  Every extraction is one pass over the
+// sequences (SeqSource): the top-byte histogram, the second-byte histograms of the leading bytes that alone exceed a
+// round, and each non-empty round, whose chunks append their in-range items at the round's cursor.
+static int s2s_host_rounds(const mhb_s2s_args *args, mhb_s2s_result *res, SeqSource &src, uint64_t n_items, uint64_t max_items) {
   const uint32_t k = args->k;
-  const uint64_t ns = args->n_seqs;
   const uint32_t W = s2s_record_words(k), WPT = words_per_tip_label(k);
   const int top_byte = (int)(4 * W - 1);
   cudaStream_t st = 0;
   Timer t_all(st), t(st);
   t_all.start();
 
-  const size_t fixed_b = Arena::pad(n_words * 4 + 64) + Arena::pad((ns + 1) * 8) * 2 + Arena::pad((ns + 1) * 4) +
-                         Arena::pad((ns + 1) * 2) + Arena::pad((size_t)MHB_NUM_BUCKETS * 4 * 8) + 2 * Arena::pad(256 * 8) +
-                         Arena::pad(16 * 8) + Arena::pad(64) + 8192;
+  const size_t fixed_b = src.device_bytes() + s2s_table_bytes();
   if (!max_items) {
-    size_t free_b = 0, total_b = 0;
-    CK(cudaMemGetInfo(&free_b, &total_b));
-    const size_t avail = (size_t)((double)(free_b + g_arena.cap) * 0.92);
-    if (avail <= fixed_b) return mhb_set_error(MHB_ERR_NOMEM, "the sequences alone (%zu bytes) do not fit the device", fixed_b);
+    const double avail = device_avail_bytes();
+    if (avail <= (double)fixed_b)
+      return mhb_set_error(MHB_ERR_NOMEM, "the sequences%s alone (%zu bytes) do not fit the device",
+                           src.n_chunks() ? "' chunk buffers" : "", fixed_b);
     uint64_t lo = 1, hi = n_items;
     while (lo < hi) {
       const uint64_t mid = lo + (hi - lo + 1) / 2;
-      if (fixed_b + s2s_round_bytes(mid, W, k) <= avail) lo = mid;
+      if ((double)(fixed_b + s2s_round_bytes(mid, W, k)) <= avail) lo = mid;
       else hi = mid - 1;
     }
     max_items = lo;
   }
   max_items = std::min<uint64_t>(std::max<uint64_t>(max_items, 1), std::max<uint64_t>(n_items, 1));
   CKR(g_arena.reserve(fixed_b + s2s_round_bytes(max_items, W, k)));
-  uint32_t *d_words = g_arena.take<uint32_t>(n_words + 16);
-  uint64_t *d_word_off = g_arena.take<uint64_t>(ns + 1);
-  uint64_t *d_item_off = g_arena.take<uint64_t>(ns + 1);
-  uint32_t *d_len = g_arena.take<uint32_t>(ns + 1);
-  uint16_t *d_mult = g_arena.take<uint16_t>(ns + 1);
+  char *d_seqs = g_arena.take<char>(src.device_bytes());
   uint64_t *d_table = g_arena.take<uint64_t>((size_t)MHB_NUM_BUCKETS * 4);
   uint64_t *d_hist0 = g_arena.take<uint64_t>(256);
   uint64_t *d_hist_top = g_arena.take<uint64_t>(256);
+  uint64_t *d_sub = g_arena.take<uint64_t>(256 * 256);
   uint64_t *d_totals = g_arena.take<uint64_t>(16);
   uint64_t *d_cursor = g_arena.take<uint64_t>(8);
   uint32_t *d_a = g_arena.take<uint32_t>((size_t)max_items * W + 4);
@@ -681,39 +839,30 @@ static int s2s_host_rounds(const mhb_s2s_args *args, mhb_s2s_result *res, const 
   char *d_ws = g_arena.take<char>(ws_bytes);
   char *d_scratch = g_arena.take<char>(scratch_bytes);
   uint8_t *d_bytes = g_arena.take<uint8_t>(cap_bytes);
-
-  if (ns) {
-    CK(cudaMemcpyAsync(d_words, args->words, n_words * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_word_off, args->word_off, (ns + 1) * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_item_off, item_off.data(), (ns + 1) * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_len, args->len, ns * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_mult, args->mult, ns * 2, cudaMemcpyHostToDevice, st));
-  }
+  CKR(src.bind(d_seqs, st));
   CK(cudaMemsetAsync(d_hist_top, 0, 256 * 8, st));
-  mhb_dev_seqs seqs;
-  seqs.words = d_words;
-  seqs.n_words = n_words;
-  seqs.n_seqs = ns;
-  seqs.fixed_len = fixed ? L0 : 0;
-  seqs.word_off = d_word_off;
-  seqs.len = d_len;
-  seqs.item_off = d_item_off;
-  seqs.mult = d_mult;
-  seqs.fixed_stride = 0;
 
   // ---- plan (two-level, as in count_host_rounds) ----
   t.start();
   uint64_t h_top[256];
-  CKR(mhb_s2s_extract_range(st, &seqs, k, nullptr, n_items, 0, 65535, nullptr, 0, d_hist_top, top_byte));
+  CKR(src.pass(st, [&](const mhb_dev_seqs &s, uint64_t n) {
+    return mhb_s2s_extract_range(st, &s, k, nullptr, n, 0, 65535, nullptr, 0, d_hist_top, top_byte);
+  }));
   CK(cudaMemcpyAsync(h_top, d_hist_top, sizeof(h_top), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
+  std::vector<uint32_t> over;
+  for (uint32_t b = 0; b < 256; ++b)
+    if (h_top[b] > max_items) over.push_back(b);
   std::vector<uint64_t> h_sub;
-  for (uint32_t b = 0; b < 256; ++b) {
-    if (h_top[b] <= max_items) continue;
-    if (h_sub.empty()) h_sub.assign(256 * 256, 0);
-    CK(cudaMemsetAsync(d_hist0, 0, 256 * 8, st));
-    CKR(mhb_s2s_extract_range(st, &seqs, k, nullptr, n_items, b << 8, (b << 8) | 255u, nullptr, 0, d_hist0, top_byte - 1));
-    CK(cudaMemcpyAsync(h_sub.data() + (size_t)b * 256, d_hist0, 256 * 8, cudaMemcpyDeviceToHost, st));
+  if (!over.empty()) {
+    h_sub.assign(256 * 256, 0);
+    CK(cudaMemsetAsync(d_sub, 0, 256 * 256 * 8, st));
+    CKR(src.pass(st, [&](const mhb_dev_seqs &s, uint64_t n) {
+      for (uint32_t b : over)
+        CKR(mhb_s2s_extract_range(st, &s, k, nullptr, n, b << 8, (b << 8) | 255u, nullptr, 0, d_sub + (size_t)b * 256, top_byte - 1));
+      return MHB_OK;
+    }));
+    CK(cudaMemcpyAsync(h_sub.data(), d_sub, 256 * 256 * 8, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
   }
   std::vector<uint32_t> r_lo(65536), r_hi(65536);
@@ -723,16 +872,29 @@ static int s2s_host_rounds(const mhb_s2s_args *args, mhb_s2s_result *res, const 
 
   SdbgStitch out;
   for (int ri = 0; ri < n_ranges; ++ri) {
+    uint64_t planned = 0;  // the range's items, from the histograms
+    for (uint32_t b = r_lo[ri] >> 8; b <= r_hi[ri] >> 8; ++b) {
+      const uint32_t c0 = b == r_lo[ri] >> 8 ? r_lo[ri] & 255 : 0, c1 = b == r_hi[ri] >> 8 ? r_hi[ri] & 255 : 255;
+      if (c0 == 0 && c1 == 255) planned += h_top[b];
+      else
+        for (uint32_t c = c0; c <= c1; ++c) planned += h_sub[(size_t)b * 256 + c];
+    }
+    if (planned == 0) continue;
+    ++g_s2s_rounds;
     t.start();
     CK(cudaMemsetAsync(d_hist0, 0, 256 * 8, st));
     CK(cudaMemsetAsync(d_cursor, 0, 64, st));
-    CKR(mhb_s2s_extract_range(st, &seqs, k, d_a, n_items, r_lo[ri], r_hi[ri], d_cursor, max_items, d_hist0, mhb_s2s_sort_hist_byte(max_items, k)));
+    CKR(src.pass(st, [&](const mhb_dev_seqs &s, uint64_t n) {
+      return mhb_s2s_extract_range(st, &s, k, d_a, n, r_lo[ri], r_hi[ri], d_cursor, max_items, d_hist0,
+                                   mhb_s2s_sort_hist_byte(max_items, k));
+    }));
     uint64_t n_round = 0;
     CK(cudaMemcpyAsync(&n_round, d_cursor, 8, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     res->t_extract_ms += t.stop();
-    if (n_round > max_items) return mhb_set_error(MHB_ERR_NOMEM, "internal: round of %llu items exceeds its plan", (unsigned long long)n_round);
-    if (n_round == 0) continue;
+    if (n_round != planned)
+      return mhb_set_error(MHB_ERR_NOMEM, "internal: round of %llu items, %llu planned", (unsigned long long)n_round,
+                           (unsigned long long)planned);
     t.start();
     int in_b = 0;
     // the histogram is of the byte a sort of max_items items starts with: pass it only if this round's sort does too
@@ -758,6 +920,56 @@ static int s2s_host_rounds(const mhb_s2s_args *args, mhb_s2s_result *res, const 
   return MHB_OK;
 }
 
+extern "C" int mhb_set_s2s_chunk_limit(uint64_t bytes) {
+  g_s2s_chunk_limit = bytes;
+  return MHB_OK;
+}
+
+extern "C" int mhb_s2s_stream_stats(int mercy, uint64_t *n_chunks, uint64_t *n_passes, uint64_t *n_rounds, uint64_t *h2d_bytes) {
+  const StreamStats &s = mercy ? g_mercy_st : g_s2s_st;
+  if (n_chunks) *n_chunks = s.chunks;
+  if (n_passes) *n_passes = s.passes;
+  if (n_rounds) *n_rounds = mercy ? 0 : g_s2s_rounds;
+  if (h2d_bytes) *h2d_bytes = s.h2d_bytes;
+  return MHB_OK;
+}
+
+extern "C" int mhb_s2s_stream_times(int mercy, double *h2d_ms, double *kernel_ms, double *fill_ms, double *pass_ms) {
+  const StreamStats &s = mercy ? g_mercy_st : g_s2s_st;
+  if (h2d_ms) *h2d_ms = s.copy_ms;
+  if (kernel_ms) *kernel_ms = s.kernel_ms;
+  if (fill_ms) *fill_ms = s.fill_ms;
+  if (pass_ms) *pass_ms = s.pass_ms;
+  return MHB_OK;
+}
+
+extern "C" int mhb_plan_seq_chunks(const uint64_t *word_off, const uint32_t *len, uint64_t n_seqs, uint32_t k,
+                                   uint64_t max_chunk_bytes, uint64_t *first_seq_out, uint32_t cap_out) {
+  if ((n_seqs && (!word_off || !len)) || max_chunk_bytes == 0) {
+    mhb_set_error(MHB_ERR_ARG, "bad chunk plan arguments");
+    return -1;
+  }
+  SeqLayout ly;
+  seq_layout(word_off, len, n_seqs, k, &ly);
+  std::vector<uint64_t> first;
+  plan_seq_chunks(word_off, ly, n_seqs, max_chunk_bytes, &first);
+  if (first_seq_out) {
+    if (first.size() > cap_out) {
+      mhb_set_error(MHB_ERR_ARG, "chunk plan needs %llu entries, room for %u", (unsigned long long)first.size(), cap_out);
+      return -1;
+    }
+    memcpy(first_seq_out, first.data(), first.size() * 8);
+  }
+  return (int)(first.size() - 1);
+}
+
+extern "C" int mhb_selftest_s2s_stream_decide(uint64_t n_seqs, uint64_t n_words, uint32_t k, uint64_t free_bytes,
+                                              uint64_t chunk_limit, uint64_t *resident_bytes, int *stream) {
+  *resident_bytes = s2s_resident_round_bytes(n_seqs, n_words, k);
+  *stream = mhb_read_stream_decide(*resident_bytes, (uint64_t)(0.92 * (double)free_bytes), 0, chunk_limit);
+  return MHB_OK;
+}
+
 // ================================================================================================
 // seq2sdbg
 // ================================================================================================
@@ -769,21 +981,13 @@ extern "C" int mhb_s2s_host(const mhb_s2s_args *args, mhb_s2s_result *res) {
   if (mhb_device_count() == 0) return mhb_set_error(MHB_ERR_CUDA, "no CUDA device: libmhb has no CPU path");
   res->words_per_tip_label = words_per_tip_label(k);
   const uint64_t ns = args->n_seqs;
+  g_s2s_st = StreamStats();
+  g_s2s_rounds = 0;
 
-  // item offsets; detect the fixed-length, gap-free layout (edges only)
-  std::vector<uint64_t> item_off(ns + 1);
-  uint64_t n_items = 0;
-  bool fixed = ns > 0;
-  const uint32_t L0 = ns ? args->len[0] : 0;
-  for (uint64_t s = 0; s < ns; ++s) {
-    item_off[s] = n_items;
-    const uint32_t L = args->len[s];
-    if (L >= k + 1) n_items += 2ull * (L - k + 2);
-    if (L != L0 || args->word_off[s] != s * (uint64_t)div_ceil(L0, 16)) fixed = false;
-  }
-  item_off[ns] = n_items;
-  if (L0 < k + 1) fixed = false;
-  const uint64_t n_words = ns ? args->word_off[ns] : 0;
+  SeqLayout ly;
+  seq_layout(args->word_off, args->len, ns, k, &ly);
+  const std::vector<uint64_t> &item_off = ly.item_off;
+  const uint64_t n_items = ly.n_items, n_words = ly.n_words;
   res->n_records = n_items;
 
   cudaStream_t st = 0;
@@ -799,15 +1003,23 @@ extern "C" int mhb_s2s_host(const mhb_s2s_args *args, mhb_s2s_result *res) {
                 Arena::pad(scratch_bytes) + Arena::pad(cap_bytes) + Arena::pad((size_t)MHB_NUM_BUCKETS * 4 * 8) +
                 Arena::pad(256 * 8) + Arena::pad(16 * 8) + 4096;
   {
-    // A13: items that do not fit the device at once (or a caller-imposed cap) -> rounds over leading-byte ranges
+    // A13: items that do not fit the device at once (or a caller-imposed cap) -> rounds over leading-byte ranges; the
+    // sequences are streamed when a chunk cap is set or when they leave no room for even a one-item round
     bool rounds = g_s2s_round_limit && n_items > g_s2s_round_limit;
     if (!rounds && need > g_arena.cap) {
       size_t free_b = 0, total_b = 0;
       CK(cudaMemGetInfo(&free_b, &total_b));
       rounds = (double)need > 0.92 * (double)(free_b + g_arena.cap);
     }
-    if (rounds) return s2s_host_rounds(args, res, item_off, n_items, fixed, L0, n_words, g_s2s_round_limit);
+    const bool stream = g_s2s_chunk_limit != 0 ||
+                        (rounds && mhb_read_stream_decide(s2s_resident_round_bytes(ns, n_words, k), (uint64_t)device_avail_bytes(), 0, 0));
+    if (rounds || stream) {
+      SeqSource src(args, ly);
+      CKR(src.init(stream ? (g_s2s_chunk_limit ? g_s2s_chunk_limit : read_chunk_auto_bytes()) : 0));
+      return s2s_host_rounds(args, res, src, n_items, g_s2s_round_limit);
+    }
   }
+  g_s2s_rounds = 1;
   CKR(g_arena.reserve(need));
   uint32_t *d_words = g_arena.take<uint32_t>(n_words + 16);
   uint64_t *d_word_off = g_arena.take<uint64_t>(ns + 1);
@@ -836,7 +1048,7 @@ extern "C" int mhb_s2s_host(const mhb_s2s_args *args, mhb_s2s_result *res) {
   seqs.words = d_words;
   seqs.n_words = n_words;
   seqs.n_seqs = ns;
-  seqs.fixed_len = fixed ? L0 : 0;
+  seqs.fixed_len = ly.fixed ? ly.L0 : 0;
   seqs.word_off = d_word_off;
   seqs.len = d_len;
   seqs.item_off = d_item_off;
@@ -1298,8 +1510,111 @@ static int build_host_impl(const mhb_build_args *args, mhb_build_result *res, bo
 }
 
 // ================================================================================================
-// mercy edges from host buffers (what `seq2sdbg --need_mercy` needs between reading `.edges`/`.cand` and SeqToSdbg::Run)
+// mercy edges from host buffers, the sorted edges resident or streamed in leading-byte segments
 // ================================================================================================
+namespace {
+// first edge of every leading byte in a sorted edge array (start[256] = n_edges)
+void edge_byte_starts(const uint32_t *edges, uint64_t n_edges, uint32_t WE, uint64_t start[257]) {
+  uint64_t lo = 0;
+  for (uint32_t b = 0; b < 256; ++b) {
+    uint64_t l = lo, r = n_edges;  // first edge with leading byte >= b
+    while (l < r) {
+      const uint64_t mid = l + (r - l) / 2;
+      if ((edges[mid * WE] >> 24) < b) l = mid + 1;
+      else r = mid;
+    }
+    start[b] = lo = l;
+  }
+  start[256] = n_edges;
+}
+// Greedy packing of the 256 leading bytes into contiguous ranges [first[i], first[i+1]): a range closes before the byte
+// that would take its edges past target bytes.  A byte above target is a segment of its own; a byte above limit (what
+// one device slot can hold) cannot be searched in one segment and is reported.
+int plan_mercy_segments(const uint64_t start[257], uint32_t WE, uint64_t target, uint64_t limit, std::vector<uint32_t> *first) {
+  first->assign(1, 0);
+  uint64_t acc = 0;
+  for (uint32_t b = 0; b < 256; ++b) {
+    const uint64_t bytes = (start[b + 1] - start[b]) * WE * 4ull;
+    if (bytes > limit)
+      return mhb_set_error(MHB_ERR_NOMEM, "leading byte 0x%02x alone holds %llu edges (%llu bytes), more than one mercy segment can take (%llu bytes)",
+                           b, (unsigned long long)(start[b + 1] - start[b]), (unsigned long long)bytes, (unsigned long long)limit);
+    if (acc && acc + bytes > target) {
+      first->push_back(b);
+      acc = 0;
+    }
+    acc += bytes;
+  }
+  first->push_back(256);
+  return MHB_OK;
+}
+// device bytes of a streamed search besides its two segment slots: candidate reads, scratch and the answer planes
+size_t mercy_stream_fixed_bytes(uint64_t n_reads, uint64_t cand_words, uint32_t max_len) {
+  const size_t bin_bytes = (cand_words * 4 + 15) & ~(size_t)15;
+  return Arena::pad(bin_bytes + 16) + 3 * Arena::pad((n_reads + 1) * 8) + Arena::pad(mhb_mercy_edges_scratch_bytes(n_reads, max_len)) +
+         4096 + Arena::pad(mhb_mercy_planes_words(n_reads, max_len) * 4);
+}
+// Segment sizes of a search streamed because its edges do not fit (no cap set): segments are packed to 1 GiB, which
+// keeps the pinned staging small and the uploads overlapping, but a leading byte may take a slot of up to half the room
+// the reads, scratch and planes leave.
+constexpr uint64_t kMercySegmentTarget = 1ull << 30;
+void mercy_auto_segment_bytes(double avail, size_t fixed, uint64_t *target, uint64_t *limit) {
+  const double room = avail - (double)fixed;
+  *limit = room > 2.0 * 4096 ? (uint64_t)(room / 2) - 4096 : 0;
+  *target = std::min(*limit, kMercySegmentTarget);
+}
+// the resident search: candidate reads (image, record and edge offsets, ids), the sorted edges and the scratch
+size_t mercy_resident_bytes(uint64_t n_edges, uint32_t k, uint64_t n_reads, uint64_t cand_words, uint32_t max_len) {
+  const size_t bin_bytes = (cand_words * 4 + 15) & ~(size_t)15;
+  return Arena::pad(bin_bytes + 16) + 3 * Arena::pad((n_reads + 1) * 8) + Arena::pad((size_t)n_edges * words_per_edge(k) * 4 + 16) +
+         Arena::pad(mhb_mercy_edges_scratch_bytes(n_reads, max_len)) + 4096;
+}
+}  // namespace
+
+extern "C" int mhb_plan_mercy_segments(const uint32_t *edges, uint64_t n_edges, uint32_t k, uint64_t max_segment_bytes,
+                                       uint32_t *first_byte_out, uint32_t cap_out) {
+  if ((n_edges && !edges) || max_segment_bytes == 0 || k < 12 || k > MHB_MAX_K) {
+    mhb_set_error(MHB_ERR_ARG, "bad segment plan arguments");
+    return -1;
+  }
+  uint64_t start[257];
+  edge_byte_starts(edges, n_edges, words_per_edge(k), start);
+  std::vector<uint32_t> first;
+  if (plan_mercy_segments(start, words_per_edge(k), max_segment_bytes, max_segment_bytes, &first)) return -1;
+  if (first_byte_out) {
+    if (first.size() > cap_out) {
+      mhb_set_error(MHB_ERR_ARG, "segment plan needs %llu entries, room for %u", (unsigned long long)first.size(), cap_out);
+      return -1;
+    }
+    memcpy(first_byte_out, first.data(), first.size() * 4);
+  }
+  return (int)(first.size() - 1);
+}
+
+extern "C" int mhb_selftest_mercy_stream_decide(uint64_t n_edges, uint32_t k, uint64_t n_cand_reads, uint64_t cand_words,
+                                                uint32_t max_read_len, uint64_t free_bytes, uint64_t chunk_limit,
+                                                uint64_t *resident_bytes, int *stream) {
+  *resident_bytes = mercy_resident_bytes(n_edges, k, n_cand_reads, cand_words, max_read_len);
+  *stream = mhb_read_stream_decide(*resident_bytes, (uint64_t)(0.92 * (double)free_bytes), 0, chunk_limit);
+  return MHB_OK;
+}
+
+extern "C" int mhb_selftest_mercy_auto_plan(const uint64_t *byte_edges, uint32_t k, uint64_t n_cand_reads, uint64_t cand_words,
+                                            uint32_t max_read_len, uint64_t free_bytes, uint32_t *first_byte_out,
+                                            uint64_t *slot_bytes) {
+  uint64_t start[257] = {0};
+  for (int b = 0; b < 256; ++b) start[b + 1] = start[b] + byte_edges[b];
+  uint64_t target = 0, limit = 0;
+  mercy_auto_segment_bytes(0.92 * (double)free_bytes, mercy_stream_fixed_bytes(n_cand_reads, cand_words, max_read_len), &target,
+                           &limit);
+  std::vector<uint32_t> first;
+  if (plan_mercy_segments(start, words_per_edge(k), target, limit, &first)) return -1;
+  memcpy(first_byte_out, first.data(), first.size() * 4);
+  uint64_t max_seg = 0;
+  for (size_t i = 0; i + 1 < first.size(); ++i) max_seg = std::max(max_seg, start[first[i + 1]] - start[first[i]]);
+  *slot_bytes = Arena::pad(max_seg * words_per_edge(k) * 4 + 16);
+  return (int)(first.size() - 1);
+}
+
 extern "C" int mhb_mercy_host(uint32_t k, const uint32_t *edges, uint64_t n_edges, const uint32_t *cand_bin,
                               uint64_t cand_words, uint32_t **mercy_out, uint64_t *n_mercy_out, uint64_t *n_cand_reads_out) {
   if (!mercy_out || !n_mercy_out) return mhb_set_error(MHB_ERR_ARG, "null output");
@@ -1309,6 +1624,7 @@ extern "C" int mhb_mercy_host(uint32_t k, const uint32_t *edges, uint64_t n_edge
   if (k < 12 || k > MHB_MAX_K) return mhb_set_error(MHB_ERR_ARG, "mercy edges need 12 <= k <= 255");
   if (mhb_device_count() == 0) return mhb_set_error(MHB_ERR_CUDA, "no CUDA device: libmhb has no CPU path");
   const uint32_t WE = words_per_edge(k);
+  g_mercy_st = StreamStats();
   // `.cand` holds the reads as KmerCounter held them: REVERSED (kmer_counter.cpp:387-401; read back with reverse=false,
   // seq_to_sdbg.cpp:175-176).  The device kernels take a library in file orientation and apply the reversal themselves,
   // so every candidate read is turned around once here (they are ~0.2 % of a library).
@@ -1341,15 +1657,32 @@ extern "C" int mhb_mercy_host(uint32_t k, const uint32_t *edges, uint64_t n_edge
   }
   const size_t bin_bytes = (bin.size() * 4 + 15) & ~(size_t)15;
   const size_t ms_bytes = mhb_mercy_edges_scratch_bytes(n_reads, max_len);
-  const size_t need = Arena::pad(bin_bytes + 16) + 3 * Arena::pad((n_reads + 1) * 8) + Arena::pad((size_t)n_edges * WE * 4 + 16) +
-                      Arena::pad(ms_bytes) + 4096;
-  CKR(g_arena.reserve(need));
+  const size_t need = mercy_resident_bytes(n_edges, k, n_reads, bin.size(), max_len);
+  // The edges are streamed in leading-byte segments when they do not fit next to the candidate reads and the scratch,
+  // or when a chunk cap is set: every search stays inside one 12-base prefix, so inside one leading byte and one segment
+  const bool stream = g_s2s_chunk_limit != 0 ||
+                      (need > g_arena.cap && mhb_read_stream_decide(need, (uint64_t)device_avail_bytes(), 0, 0));
+  const size_t pw = stream ? mhb_mercy_planes_words(n_reads, max_len) : 0;
+  const size_t fixed_b = mercy_stream_fixed_bytes(n_reads, bin.size(), max_len);
+  uint64_t start[257];
+  std::vector<uint32_t> seg_first;
+  size_t slot_bytes = 0;
+  if (stream) {
+    uint64_t target = g_s2s_chunk_limit, limit = g_s2s_chunk_limit;
+    if (!target) mercy_auto_segment_bytes(device_avail_bytes(), fixed_b, &target, &limit);
+    edge_byte_starts(edges, n_edges, WE, start);
+    CKR(plan_mercy_segments(start, WE, target, limit, &seg_first));
+    uint64_t max_seg = 0;
+    for (size_t i = 0; i + 1 < seg_first.size(); ++i) max_seg = std::max(max_seg, start[seg_first[i + 1]] - start[seg_first[i]]);
+    slot_bytes = Arena::pad(max_seg * WE * 4 + 16);
+  }
+  CKR(g_arena.reserve(stream ? fixed_b + 2 * slot_bytes : need));
   cudaStream_t st = 0;
   uint32_t *d_bin = g_arena.take<uint32_t>(bin_bytes / 4 + 4);
   uint64_t *d_rec_off = g_arena.take<uint64_t>(n_reads + 1);
   uint64_t *d_edge_off = g_arena.take<uint64_t>(n_reads + 1);
   uint64_t *d_ids = g_arena.take<uint64_t>(n_reads + 1);
-  uint32_t *d_edges = g_arena.take<uint32_t>((size_t)n_edges * WE + 4);
+  uint32_t *d_edges = stream ? nullptr : g_arena.take<uint32_t>((size_t)n_edges * WE + 4);
   char *d_ms = g_arena.take<char>(ms_bytes);
   std::vector<uint64_t> ids(n_reads);
   for (uint64_t r = 0; r < n_reads; ++r) ids[r] = r;
@@ -1357,7 +1690,7 @@ extern "C" int mhb_mercy_host(uint32_t k, const uint32_t *edges, uint64_t n_edge
   CK(cudaMemcpyAsync(d_rec_off, rec_off.data(), (n_reads + 1) * 8, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d_edge_off, edge_off.data(), (n_reads + 1) * 8, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d_ids, ids.data(), n_reads * 8, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d_edges, edges, (size_t)n_edges * WE * 4, cudaMemcpyHostToDevice, st));
+  if (!stream) CK(cudaMemcpyAsync(d_edges, edges, (size_t)n_edges * WE * 4, cudaMemcpyHostToDevice, st));
   mhb_dev_reads reads;
   reads.bin = d_bin;
   reads.bin_words = bin.size();
@@ -1367,12 +1700,48 @@ extern "C" int mhb_mercy_host(uint32_t k, const uint32_t *edges, uint64_t n_edge
   reads.edge_off = d_edge_off;
   const size_t core = ms_bytes - mhb_edge_lut_bytes();
   void *lut = d_ms + core;
-  CKR(mhb_edge_lut_build(st, d_edges, n_edges, k, lut));
-  const uint32_t *seg_e[1] = {d_edges};
-  const uint64_t seg_n[1] = {n_edges};
-  const void *seg_l[1] = {lut};
   uint64_t n_mercy = 0;
-  CKR(mhb_mercy_edges_count(st, &reads, d_ids, n_reads, max_len, k, 1, seg_e, seg_n, seg_l, nullptr, &n_mercy, d_ms, core));
+  if (!stream) {
+    CKR(mhb_edge_lut_build(st, d_edges, n_edges, k, lut));
+    const uint32_t *seg_e[1] = {d_edges};
+    const uint64_t seg_n[1] = {n_edges};
+    const void *seg_l[1] = {lut};
+    CKR(mhb_mercy_edges_count(st, &reads, d_ids, n_reads, max_len, k, 1, seg_e, seg_n, seg_l, nullptr, &n_mercy, d_ms, core));
+  } else {
+    // segment i answers the searches whose leading byte it holds; the answers of all segments are OR-ed into one set
+    // of planes, which then stands for the single-segment search
+    uint32_t *d_planes = g_arena.take<uint32_t>(pw);
+    char *d_slots = g_arena.take<char>(2 * slot_bytes);
+    const uint64_t n_seg = seg_first.size() - 1;
+    uint8_t owner[256];
+    for (uint64_t i = 0; i < n_seg; ++i)
+      for (uint32_t b = seg_first[i]; b < seg_first[i + 1]; ++b) owner[b] = (uint8_t)i;
+    CK(cudaMemsetAsync(d_planes, 0, pw * 4, st));
+    ChunkStager stager;
+    g_mercy_st.chunks = n_seg;
+    CKR(stager.init(slot_bytes, n_seg, &g_mercy_st));
+    stager.bind(d_slots);
+    auto seg_edges = [&](uint64_t i) { return start[seg_first[i + 1]] - start[seg_first[i]]; };
+    const ChunkStager::Fill fill = [&](uint64_t i, char *h, ChunkStager::Copies *up) {
+      const uint64_t bytes = seg_edges(i) * WE * 4, blk = 4ull << 20, nblk = (bytes + blk - 1) / blk;
+      const char *src = (const char *)(edges + start[seg_first[i]] * WE);
+#pragma omp parallel for schedule(static)
+      for (long long j = 0; j < (long long)nblk; ++j) {
+        const uint64_t o = (uint64_t)j * blk;
+        memcpy(h + o, src + o, std::min(blk, bytes - o));
+      }
+      up->add(0, bytes);
+      return MHB_OK;
+    };
+    const ChunkStager::Run run = [&](uint64_t i, const char *slot) {
+      const uint32_t *d_seg = (const uint32_t *)slot;
+      CKR(mhb_edge_lut_build(st, d_seg, seg_edges(i), k, lut));
+      return mercy_probe_owned(st, &reads, d_ids, n_reads, max_len, k, d_seg, seg_edges(i), lut, owner, (uint32_t)i, d_planes,
+                               true);
+    };
+    CKR(stager.pass(st, fill, run));
+    CKR(mhb_mercy_count_planes(st, &reads, d_ids, n_reads, max_len, k, d_planes, 1, pw, &n_mercy, d_ms, core));
+  }
   *mercy_out = (uint32_t *)malloc(std::max<size_t>(4, (size_t)n_mercy * WE * 4));
   if (!*mercy_out) return mhb_set_error(MHB_ERR_NOMEM, "host malloc failed");
   if (n_mercy) {

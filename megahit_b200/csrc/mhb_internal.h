@@ -6,6 +6,8 @@
 #include <functional>
 #include <vector>
 
+#include "mhb.h"
+
 int mhb_set_error(int code, const char *fmt, ...);
 
 // mhb_sort_records + optional per-pass timings (host array of n_bytes doubles, ms; forces a stream sync)
@@ -38,6 +40,59 @@ struct ReadLibIndex {
 int index_read_lib(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, uint32_t k, ReadLibIndex *ix,
                    bool sampled = false);
 
+// Streaming statistics of one host-level call: chunks (0 = resident), passes, bytes host to device, and the copy-engine
+// and compute-stream busy time, host fill time and wall time of the passes (ms).
+struct StreamStats {
+  uint64_t chunks = 0, passes = 0, h2d_bytes = 0;
+  double copy_ms = 0, kernel_ms = 0, fill_ms = 0, pass_ms = 0;
+};
+
+// Greedy cut of n items into contiguous chunks [first[i], first[i+1]) of at most max_bytes each; a larger item gets a
+// chunk of its own.  Item r takes 4 * (word_off[r+1] - word_off[r]) + extra_bytes, or with word_off == NULL
+// 4 * stride_words + extra_bytes, cut in closed form.  first gets n_chunks + 1 entries ({0} when n == 0).
+void plan_chunks(const uint64_t *word_off, uint64_t stride_words, uint64_t extra_bytes, uint64_t n, uint64_t max_bytes,
+                 std::vector<uint64_t> *first);
+
+// The uploads of data kept in host memory, chunk by chunk, through two device slots (mhb_stream.cu): two pinned staging
+// buffers, a non-blocking copy stream and four events per chunk.  While host threads fill the staging buffer of chunk
+// i+1, chunk i uploads on the copy stream and the compute stream works on chunk i-1.  Each chunk's bytes land at the
+// same offsets of its device slot as fill put them in the staging buffer.
+class ChunkStager {
+ public:
+  struct Copies {  // the ranges of the staging buffer fill wrote, uploaded in this order
+    size_t off[6], bytes[6];
+    int n = 0;
+    void add(size_t o, size_t b) {
+      if (b) {
+        off[n] = o;
+        bytes[n++] = b;
+      }
+    }
+  };
+  using Fill = std::function<int(uint64_t chunk, char *host, Copies *up)>;  // host threads, off the compute stream
+  using Run = std::function<int(uint64_t chunk, const char *slot)>;       // on the compute stream
+  ChunkStager() = default;
+  ChunkStager(const ChunkStager &) = delete;
+  ChunkStager &operator=(const ChunkStager &) = delete;
+  ~ChunkStager();
+  // n_chunks chunks of at most slot_bytes; the passes are counted into *stats
+  int init(size_t slot_bytes, uint64_t n_chunks, StreamStats *stats);
+  size_t device_bytes() const { return 2 * slot_bytes_; }
+  void bind(char *device) { dev_ = device; }  // device_bytes() bytes, 256-byte aligned
+  // one pass: every chunk filled, uploaded and handed to run, in order
+  int pass(void *stream, const Fill &fill, const Run &run);
+
+ private:
+  int stage(uint64_t i, const Fill &fill);
+  size_t slot_bytes_ = 0;
+  uint64_t n_chunks_ = 0;
+  StreamStats *st_ = nullptr;
+  char *dev_ = nullptr;
+  char *host_[2] = {nullptr, nullptr};
+  void *copy_ = nullptr;    // cudaStream_t
+  std::vector<void *> ev_;  // cudaEvent_t: 4 per chunk (copy begin/end, compute begin/end)
+};
+
 // Every pass over a read library (mhb_stream.cu), in one of two forms:
 // - resident: the library is uploaded once into the device memory the caller binds, and a pass hands it over whole;
 // - streamed: the `.bin` image stays in host memory and goes through the device in chunks that end on read boundaries.
@@ -57,7 +112,6 @@ class ReadStream {
   ReadStream() = default;
   ReadStream(const ReadStream &) = delete;
   ReadStream &operator=(const ReadStream &) = delete;
-  ~ReadStream();
   // host library and its index; max_chunk_bytes = 0: resident, otherwise streamed in chunks planned here
   int init(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, const ReadLibIndex &ix, uint64_t max_chunk_bytes);
   size_t device_bytes() const { return (resident_ ? 1 : 2) * slot_bytes_; }  // the library, or both chunk slots
@@ -71,7 +125,7 @@ class ReadStream {
   int pass(void *stream, const std::function<int(const ReadChunkView &)> &fn);
 
  private:
-  int stage(uint64_t i);
+  int fill(uint64_t i, char *h, ChunkStager::Copies *up) const;
   ReadChunkView view(uint64_t i, const char *slot) const;
   bool resident_ = false;
   const uint32_t *bin_ = nullptr;
@@ -82,9 +136,7 @@ class ReadStream {
   uint64_t max_reads_ = 0;
   size_t off_at_ = 0, slot_bytes_ = 0;
   char *dev_ = nullptr;
-  char *host_[2] = {nullptr, nullptr};
-  void *copy_ = nullptr;       // cudaStream_t
-  std::vector<void *> ev_;     // cudaEvent_t: 4 per chunk (copy begin/end, compute begin/end)
+  ChunkStager stager_;
   uint64_t word_of(uint64_t r) const { return fixed_len_ ? r * stride_ : rec_off_[r]; }
 };
 // streaming statistics of the current host-level call (mhb_read_stream_stats)
@@ -93,6 +145,11 @@ void read_stream_stats_reset();
 uint64_t read_chunk_limit();
 // the chunk size of a library that is streamed because it does not fit (no cap set)
 uint64_t read_chunk_auto_bytes();
+
+// mhb_mercy_probe_owned, with accumulate = true OR-ing the answers into planes_out instead of storing them (mhb_multi.cu)
+int mercy_probe_owned(void *stream, const mhb_dev_reads *reads, const uint64_t *cand_ids, uint64_t n_cand,
+                      uint32_t max_read_len, uint32_t k, const uint32_t *edges, uint64_t n_edges, const void *lut,
+                      const uint8_t *owner_of_byte, uint32_t me, uint32_t *planes_out, bool accumulate);
 
 // The SdBG output of a build that runs its stage-2 sort in rounds over ascending bucket ranges: every round's emitter
 // output (mhb_s2s_emit / mhb_s2s_emit_fmt) is appended to one byte stream, its non-empty rows of the bucket table are

@@ -12,6 +12,8 @@
 //                             bucket range from local HBM and the per-position answer bits are exchanged instead of
 //                             the edges (instead of bisecting the peers' edge arrays over NVLink)
 //   mhb_mercy_count_planes    OR the answer planes of all ranks into (A, O, N) and count the mercy edges
+// The single-GPU mercy search of an edge array larger than device memory (mhb_mercy_host) runs the same probe once per
+// leading-byte segment, OR-ing each segment's answers into one set of planes (mercy_probe_owned, accumulate = true).
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <string.h>
@@ -173,7 +175,9 @@ struct OwnerTab {
 //         G3 = OR_{ch != next'} S(ch + rvk, k+1) while <= km + 'T'
 // With hits OR-ed over the owners:  A = F1|F2,  O = G1|G2|G3,  N = G1 ? G1n : G2  - identical to the reference's
 // nested ifs because the else-branches only matter when the earlier search missed everywhere.
-template <int WM>
+// Accumulate: OR the answers into planes already holding those of other segments (one edge array streamed through the
+// device in leading-byte segments), instead of storing them.
+template <int WM, bool Accumulate>
 __global__ void __launch_bounds__(256)
     k_mercy_probe_owned(ReadsView rv, const u64 *__restrict__ cand_ids, u64 n_cand, u32 k, const u32 *__restrict__ edges,
                         long long n_edges, const uint2 *__restrict__ lut, OwnerTab ot, u32 me, u32 we, u32 *__restrict__ planes,
@@ -244,11 +248,19 @@ __global__ void __launch_bounds__(256)
                 m3 = __ballot_sync(0xffffffffu, G1n), m4 = __ballot_sync(0xffffffffu, G2);
       if (lane == 0) {
         const u32 w = i0 >> 5;
-        pl[w] = m0;
-        pl[words_per_read + w] = m1;
-        pl[2 * words_per_read + w] = m2;
-        pl[3 * words_per_read + w] = m3;
-        pl[4 * words_per_read + w] = m4;
+        if (Accumulate) {
+          pl[w] |= m0;
+          pl[words_per_read + w] |= m1;
+          pl[2 * words_per_read + w] |= m2;
+          pl[3 * words_per_read + w] |= m3;
+          pl[4 * words_per_read + w] |= m4;
+        } else {
+          pl[w] = m0;
+          pl[words_per_read + w] = m1;
+          pl[2 * words_per_read + w] = m2;
+          pl[3 * words_per_read + w] = m3;
+          pl[4 * words_per_read + w] = m4;
+        }
       }
     }
   }
@@ -282,9 +294,9 @@ extern "C" size_t mhb_mercy_planes_words(uint64_t n_cand, uint32_t max_read_len)
   return (size_t)n_cand * kOwnedPlanes * ((max_read_len + 31) / 32 + 1);
 }
 
-extern "C" int mhb_mercy_probe_owned(void *stream, const mhb_dev_reads *reads, const uint64_t *cand_ids, uint64_t n_cand,
-                                     uint32_t max_read_len, uint32_t k, const uint32_t *edges, uint64_t n_edges, const void *lut,
-                                     const uint8_t *owner_of_byte, uint32_t me, uint32_t *planes_out) {
+int mercy_probe_owned(void *stream, const mhb_dev_reads *reads, const uint64_t *cand_ids, uint64_t n_cand,
+                      uint32_t max_read_len, uint32_t k, const uint32_t *edges, uint64_t n_edges, const void *lut,
+                      const uint8_t *owner_of_byte, uint32_t me, uint32_t *planes_out, bool accumulate) {
   if (int rc = check_reads(reads, k)) return rc;
   if (n_cand == 0) return MHB_OK;
   if (k < 12) return mhb_set_error(MHB_ERR_ARG, "mercy edges need k >= 12 (12-mer look-up prefix)");
@@ -297,13 +309,25 @@ extern "C" int mhb_mercy_probe_owned(void *stream, const mhb_dev_reads *reads, c
   if (g64 > (u64)sm_count() * 16) g64 = (u64)sm_count() * 16;
   cudaStream_t st = (cudaStream_t)stream;
 #define M(WW)                                                                                                               \
-  if (WM == WW)                                                                                                             \
-    k_mercy_probe_owned<WW><<<(unsigned)g64, 256, 0, st>>>(rv, cand_ids, n_cand, k, edges, (long long)n_edges, (const uint2 *)lut, \
-                                                           ot, me, WE, planes_out, wpr);
+  if (WM == WW) {                                                                                                           \
+    if (accumulate)                                                                                                         \
+      k_mercy_probe_owned<WW, true><<<(unsigned)g64, 256, 0, st>>>(rv, cand_ids, n_cand, k, edges, (long long)n_edges,       \
+                                                                   (const uint2 *)lut, ot, me, WE, planes_out, wpr);         \
+    else                                                                                                                    \
+      k_mercy_probe_owned<WW, false><<<(unsigned)g64, 256, 0, st>>>(rv, cand_ids, n_cand, k, edges, (long long)n_edges,      \
+                                                                    (const uint2 *)lut, ot, me, WE, planes_out, wpr);        \
+  }
   MHB_FOR_W(M)
 #undef M
   CK_LAUNCH();
   return MHB_OK;
+}
+
+extern "C" int mhb_mercy_probe_owned(void *stream, const mhb_dev_reads *reads, const uint64_t *cand_ids, uint64_t n_cand,
+                                     uint32_t max_read_len, uint32_t k, const uint32_t *edges, uint64_t n_edges, const void *lut,
+                                     const uint8_t *owner_of_byte, uint32_t me, uint32_t *planes_out) {
+  return mercy_probe_owned(stream, reads, cand_ids, n_cand, max_read_len, k, edges, n_edges, lut, owner_of_byte, me,
+                           planes_out, false);
 }
 
 extern "C" int mhb_mercy_count_planes(void *stream, const mhb_dev_reads *reads, const uint64_t *cand_ids, uint64_t n_cand,

@@ -24,25 +24,22 @@ using namespace mhb;
 
 namespace {
 uint64_t g_chunk_limit = 0;
-struct {
-  uint64_t chunks, passes, h2d_bytes;
-  double copy_ms, kernel_ms, fill_ms, pass_ms;
-} g_st = {0, 0, 0, 0, 0, 0, 0};
+StreamStats g_st;
 
 inline size_t pad256(size_t b) { return (b + 255) & ~(size_t)255; }
 
-// Greedy cut into chunks of at most max_bytes of image; a read larger than the cap gets a chunk of its own.  For a
-// fixed-length library the same cut in closed form: floor(cap / record) reads per chunk.  first gets n_chunks + 1
-// entries.
-void plan_chunks(const ReadLibIndex &ix, uint64_t n_reads, uint64_t max_bytes, std::vector<uint64_t> *first) {
+}  // namespace
+
+void plan_chunks(const uint64_t *word_off, uint64_t stride_words, uint64_t extra_bytes, uint64_t n, uint64_t max_bytes,
+                 std::vector<uint64_t> *first) {
   first->assign(1, 0);
-  if (ix.fixed_len) {
-    const uint64_t per = std::max<uint64_t>(1, max_bytes / (4 * (1 + div_ceil(ix.fixed_len, 16))));
-    for (uint64_t r = per; r < n_reads; r += per) first->push_back(r);
+  if (!word_off) {
+    const uint64_t per = std::max<uint64_t>(1, max_bytes / (4 * stride_words + extra_bytes));
+    for (uint64_t r = per; r < n; r += per) first->push_back(r);
   } else {
     uint64_t acc = 0;
-    for (uint64_t r = 0; r < n_reads; ++r) {
-      const uint64_t b = 4 * (ix.rec_off[r + 1] - ix.rec_off[r]);
+    for (uint64_t r = 0; r < n; ++r) {
+      const uint64_t b = 4 * (word_off[r + 1] - word_off[r]) + extra_bytes;
       if (r > first->back() && acc + b > max_bytes) {
         first->push_back(r);
         acc = 0;
@@ -50,9 +47,13 @@ void plan_chunks(const ReadLibIndex &ix, uint64_t n_reads, uint64_t max_bytes, s
       acc += b;
     }
   }
-  if (n_reads) first->push_back(n_reads);
+  if (n) first->push_back(n);
 }
-}  // namespace
+
+// a library's read chunks: the image only, a fixed-length library cut in closed form
+static void plan_read_chunks(const ReadLibIndex &ix, uint64_t n_reads, uint64_t max_bytes, std::vector<uint64_t> *first) {
+  plan_chunks(ix.fixed_len ? nullptr : ix.rec_off.data(), 1 + div_ceil(ix.fixed_len, 16), 0, n_reads, max_bytes, first);
+}
 
 int index_read_lib(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, uint32_t k, ReadLibIndex *ix, bool sampled) {
   *ix = ReadLibIndex();
@@ -95,7 +96,7 @@ int index_read_lib(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, ui
   return MHB_OK;
 }
 
-void read_stream_stats_reset() { memset(&g_st, 0, sizeof(g_st)); }
+void read_stream_stats_reset() { g_st = StreamStats(); }
 uint64_t read_chunk_limit() { return g_chunk_limit; }
 // 64 MiB: the shortest passes of scripts/read_stream_time.py (DESIGN.md A13); larger chunks overlap less
 uint64_t read_chunk_auto_bytes() { return 64ull << 20; }
@@ -133,7 +134,7 @@ extern "C" int mhb_plan_read_chunks(const uint32_t *bin, uint64_t bin_words, uin
   ReadLibIndex ix;
   if (index_read_lib(bin, bin_words, n_reads, 0, &ix)) return -1;
   std::vector<uint64_t> first;
-  plan_chunks(ix, n_reads, max_chunk_bytes, &first);
+  plan_read_chunks(ix, n_reads, max_chunk_bytes, &first);
   const uint64_t n = first.size() - 1;
   if (first_read_out) {
     if (first.size() > cap_out) {
@@ -146,9 +147,9 @@ extern "C" int mhb_plan_read_chunks(const uint32_t *bin, uint64_t bin_words, uin
 }
 
 // ------------------------------------------------------------------------------------------------
-// ReadStream
+// ChunkStager
 // ------------------------------------------------------------------------------------------------
-ReadStream::~ReadStream() {
+ChunkStager::~ChunkStager() {
   if (copy_) cudaStreamSynchronize((cudaStream_t)copy_);
   for (void *e : ev_) cudaEventDestroy((cudaEvent_t)e);
   for (char *h : host_)
@@ -156,6 +157,72 @@ ReadStream::~ReadStream() {
   if (copy_) cudaStreamDestroy((cudaStream_t)copy_);
 }
 
+int ChunkStager::init(size_t slot_bytes, uint64_t n_chunks, StreamStats *stats) {
+  slot_bytes_ = slot_bytes;
+  n_chunks_ = n_chunks;
+  st_ = stats;
+  if (!n_chunks) return MHB_OK;
+  for (int s = 0; s < 2; ++s) CK(cudaHostAlloc((void **)&host_[s], slot_bytes_, cudaHostAllocDefault));
+  cudaStream_t cs;
+  CK(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
+  copy_ = cs;
+  ev_.assign(4 * n_chunks, nullptr);
+  for (auto &e : ev_) CK(cudaEventCreate((cudaEvent_t *)&e));
+  return MHB_OK;
+}
+
+// fill the staging buffer of chunk i (host threads) and queue its upload on the copy stream
+int ChunkStager::stage(uint64_t i, const Fill &fill) {
+  const int s = (int)(i & 1);
+  cudaStream_t cs = (cudaStream_t)copy_;
+  if (i >= 2) CK(cudaEventSynchronize((cudaEvent_t)ev_[4 * (i - 2) + 1]));  // upload of chunk i-2 has left staging s
+  const auto t0 = std::chrono::steady_clock::now();
+  Copies up;
+  CKR(fill(i, host_[s], &up));
+  st_->fill_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  char *d = dev_ + s * slot_bytes_;
+  if (i >= 2) CK(cudaStreamWaitEvent(cs, (cudaEvent_t)ev_[4 * (i - 2) + 3], 0));  // kernels of chunk i-2 are done with slot s
+  CK(cudaEventRecord((cudaEvent_t)ev_[4 * i], cs));
+  for (int j = 0; j < up.n; ++j) {
+    CK(cudaMemcpyAsync(d + up.off[j], host_[s] + up.off[j], up.bytes[j], cudaMemcpyHostToDevice, cs));
+    st_->h2d_bytes += up.bytes[j];
+  }
+  CK(cudaEventRecord((cudaEvent_t)ev_[4 * i + 1], cs));
+  return MHB_OK;
+}
+
+int ChunkStager::pass(void *stream, const Fill &fill, const Run &run) {
+  const uint64_t nc = n_chunks_;
+  if (!nc) return MHB_OK;
+  if (!dev_) return mhb_set_error(MHB_ERR_ARG, "internal: chunk stager without device memory");
+  cudaStream_t st = (cudaStream_t)stream;
+  ++st_->passes;
+  const auto t0 = std::chrono::steady_clock::now();
+  CKR(stage(0, fill));
+  for (uint64_t i = 0; i < nc; ++i) {
+    // the next upload is queued before the kernels of this chunk, so a host read inside run does not stall the copy
+    if (i + 1 < nc) CKR(stage(i + 1, fill));
+    CK(cudaStreamWaitEvent(st, (cudaEvent_t)ev_[4 * i + 1], 0));
+    CK(cudaEventRecord((cudaEvent_t)ev_[4 * i + 2], st));
+    CKR(run(i, dev_ + (i & 1) * slot_bytes_));
+    CK(cudaEventRecord((cudaEvent_t)ev_[4 * i + 3], st));
+  }
+  CK(cudaEventSynchronize((cudaEvent_t)ev_[4 * (nc - 1) + 3]));
+  CK(cudaStreamSynchronize((cudaStream_t)copy_));
+  st_->pass_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  for (uint64_t i = 0; i < nc; ++i) {
+    float a = 0, b = 0;
+    CK(cudaEventElapsedTime(&a, (cudaEvent_t)ev_[4 * i], (cudaEvent_t)ev_[4 * i + 1]));
+    CK(cudaEventElapsedTime(&b, (cudaEvent_t)ev_[4 * i + 2], (cudaEvent_t)ev_[4 * i + 3]));
+    st_->copy_ms += a;
+    st_->kernel_ms += b;
+  }
+  return MHB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// ReadStream
+// ------------------------------------------------------------------------------------------------
 int ReadStream::init(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, const ReadLibIndex &ix, uint64_t max_chunk_bytes) {
   resident_ = max_chunk_bytes == 0;
   bin_ = bin;
@@ -169,7 +236,7 @@ int ReadStream::init(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, 
     first_ = {0, n_reads};
     max_reads_ = n_reads;
   } else {
-    plan_chunks(ix, n_reads, max_chunk_bytes, &first_);
+    plan_read_chunks(ix, n_reads, max_chunk_bytes, &first_);
     max_words = max_reads_ = 0;
     for (uint64_t i = 0; i < n_chunks(); ++i) {
       max_reads_ = std::max(max_reads_, first_[i + 1] - first_[i]);
@@ -180,18 +247,12 @@ int ReadStream::init(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, 
   off_at_ = pad256(((max_words * 4 + 15) & ~(size_t)15) + 16);
   slot_bytes_ = off_at_ + (fixed_len_ ? 0 : (aux_off_ ? 2 : 1) * pad256((max_reads_ + 1) * 8));
   g_st.chunks = n_chunks();
-  if (!n_chunks()) return MHB_OK;
-  for (int s = 0; s < 2; ++s) CK(cudaHostAlloc((void **)&host_[s], slot_bytes_, cudaHostAllocDefault));
-  cudaStream_t cs;
-  CK(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-  copy_ = cs;
-  ev_.assign(4 * n_chunks(), nullptr);
-  for (auto &e : ev_) CK(cudaEventCreate((cudaEvent_t *)&e));
-  return MHB_OK;
+  return stager_.init(slot_bytes_, n_chunks(), &g_st);
 }
 
 int ReadStream::bind(void *device, void *stream) {
   dev_ = (char *)device;
+  stager_.bind(dev_);
   if (!resident_) return MHB_OK;
   cudaStream_t st = (cudaStream_t)stream;
   const uint64_t n_reads = first_[1];
@@ -216,14 +277,9 @@ ReadChunkView ReadStream::view(uint64_t i, const char *slot) const {
   return v;
 }
 
-// fill the staging buffer of chunk i (host threads) and queue its upload on the copy stream
-int ReadStream::stage(uint64_t i) {
-  const int s = (int)(i & 1);
-  cudaStream_t cs = (cudaStream_t)copy_;
-  if (i >= 2) CK(cudaEventSynchronize((cudaEvent_t)ev_[4 * (i - 2) + 1]));  // upload of chunk i-2 has left staging s
-  const auto t0 = std::chrono::steady_clock::now();
+// chunk i into a staging buffer: its image, and for a variable-length library its offsets rebased to the chunk
+int ReadStream::fill(uint64_t i, char *h, ChunkStager::Copies *up) const {
   const uint64_t b = first_[i], e = first_[i + 1], w0 = word_of(b), nw = word_of(e) - w0;
-  char *h = host_[s];
   {
     const uint64_t bytes = nw * 4, blk = 4ull << 20, nblk = (bytes + blk - 1) / blk;
 #pragma omp parallel for schedule(static)
@@ -232,58 +288,25 @@ int ReadStream::stage(uint64_t i) {
       memcpy(h + o, (const char *)(bin_ + w0) + o, std::min(blk, bytes - o));
     }
   }
-  const uint64_t nr = e - b;
-  uint64_t *ro = (uint64_t *)(h + off_at_), *ao = (uint64_t *)(h + off_at_ + pad256((max_reads_ + 1) * 8));
-  if (!fixed_len_) {
-    const uint64_t r0 = rec_off_[b], a0 = aux_off_ ? aux_off_[b] : 0;
+  up->add(0, nw * 4);
+  if (fixed_len_) return MHB_OK;
+  const uint64_t nr = e - b, ao_at = off_at_ + pad256((max_reads_ + 1) * 8);
+  uint64_t *ro = (uint64_t *)(h + off_at_), *ao = (uint64_t *)(h + ao_at);
+  const uint64_t r0 = rec_off_[b], a0 = aux_off_ ? aux_off_[b] : 0;
 #pragma omp parallel for schedule(static)
-    for (long long r = 0; r <= (long long)nr; ++r) {
-      ro[r] = rec_off_[b + r] - r0;
-      if (aux_off_) ao[r] = aux_off_[b + r] - a0;
-    }
+  for (long long r = 0; r <= (long long)nr; ++r) {
+    ro[r] = rec_off_[b + r] - r0;
+    if (aux_off_) ao[r] = aux_off_[b + r] - a0;
   }
-  g_st.fill_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-  char *d = dev_ + s * slot_bytes_;
-  if (i >= 2) CK(cudaStreamWaitEvent(cs, (cudaEvent_t)ev_[4 * (i - 2) + 3], 0));  // kernels of chunk i-2 are done with slot s
-  CK(cudaEventRecord((cudaEvent_t)ev_[4 * i], cs));
-  if (nw) CK(cudaMemcpyAsync(d, h, nw * 4, cudaMemcpyHostToDevice, cs));
-  g_st.h2d_bytes += nw * 4;
-  if (!fixed_len_) {
-    CK(cudaMemcpyAsync(d + off_at_, ro, (nr + 1) * 8, cudaMemcpyHostToDevice, cs));
-    if (aux_off_)
-      CK(cudaMemcpyAsync(d + off_at_ + pad256((max_reads_ + 1) * 8), ao, (nr + 1) * 8, cudaMemcpyHostToDevice, cs));
-    g_st.h2d_bytes += (aux_off_ ? 2 : 1) * (nr + 1) * 8;
-  }
-  CK(cudaEventRecord((cudaEvent_t)ev_[4 * i + 1], cs));
+  up->add(off_at_, (nr + 1) * 8);
+  if (aux_off_) up->add(ao_at, (nr + 1) * 8);
   return MHB_OK;
 }
 
 int ReadStream::pass(void *stream, const std::function<int(const ReadChunkView &)> &fn) {
   if (!dev_) return mhb_set_error(MHB_ERR_ARG, "internal: read library without device memory");
   if (resident_) return fn(view(0, dev_));
-  const uint64_t nc = n_chunks();
-  if (!nc) return MHB_OK;
-  cudaStream_t st = (cudaStream_t)stream;
-  ++g_st.passes;
-  const auto t0 = std::chrono::steady_clock::now();
-  CKR(stage(0));
-  for (uint64_t i = 0; i < nc; ++i) {
-    // the next upload is queued before the kernels of this chunk, so a host read inside fn does not stall the copy
-    if (i + 1 < nc) CKR(stage(i + 1));
-    CK(cudaStreamWaitEvent(st, (cudaEvent_t)ev_[4 * i + 1], 0));
-    CK(cudaEventRecord((cudaEvent_t)ev_[4 * i + 2], st));
-    CKR(fn(view(i, dev_ + (i & 1) * slot_bytes_)));
-    CK(cudaEventRecord((cudaEvent_t)ev_[4 * i + 3], st));
-  }
-  CK(cudaEventSynchronize((cudaEvent_t)ev_[4 * (nc - 1) + 3]));
-  CK(cudaStreamSynchronize((cudaStream_t)copy_));
-  g_st.pass_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-  for (uint64_t i = 0; i < nc; ++i) {
-    float a = 0, b = 0;
-    CK(cudaEventElapsedTime(&a, (cudaEvent_t)ev_[4 * i], (cudaEvent_t)ev_[4 * i + 1]));
-    CK(cudaEventElapsedTime(&b, (cudaEvent_t)ev_[4 * i + 2], (cudaEvent_t)ev_[4 * i + 3]));
-    g_st.copy_ms += a;
-    g_st.kernel_ms += b;
-  }
-  return MHB_OK;
+  return stager_.pass(
+      stream, [this](uint64_t i, char *h, ChunkStager::Copies *up) { return fill(i, h, up); },
+      [&](uint64_t i, const char *slot) { return fn(view(i, slot)); });
 }

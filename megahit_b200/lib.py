@@ -153,6 +153,9 @@ SYMBOLS = [
     "mhb_selftest_s2s_local_key",
     "mhb_plan_read_chunks", "mhb_read_stream_decide", "mhb_set_read_chunk_limit", "mhb_read_stream_stats",
     "mhb_read_stream_times",
+    "mhb_set_s2s_chunk_limit", "mhb_plan_seq_chunks", "mhb_plan_mercy_segments", "mhb_s2s_stream_stats",
+    "mhb_s2s_stream_times", "mhb_selftest_s2s_stream_decide", "mhb_selftest_mercy_stream_decide",
+    "mhb_selftest_mercy_auto_plan",
 ]
 
 
@@ -395,6 +398,98 @@ def read_stream_stats() -> dict:
     _check(L.mhb_read_stream_times(C.byref(h2d), C.byref(kern), C.byref(fill), C.byref(wall)))
     return {"n_chunks": nc.value, "n_passes": npass.value, "h2d_bytes": nb.value, "h2d_ms": h2d.value,
             "kernel_ms": kern.value, "fill_ms": fill.value, "pass_ms": wall.value}
+
+
+def set_s2s_chunk_limit(n_bytes: int = 0) -> None:
+    """Stream the sequences of s2s_host in chunks, and the edges of mercy_host in leading-byte segments, of at most
+    n_bytes (0 = only when they do not fit).  Independent of set_read_chunk_limit; the result does not depend on it."""
+    L = load()
+    L.mhb_set_s2s_chunk_limit.argtypes = [C.c_uint64]
+    _check(L.mhb_set_s2s_chunk_limit(int(n_bytes)))
+
+
+def plan_seq_chunks(word_off: np.ndarray, length: np.ndarray, k: int, max_chunk_bytes: int) -> list[int]:
+    """Sequence chunks of a streamed s2s_host (host logic only): the first sequence of every chunk, then n_seqs."""
+    L = load()
+    wo = np.ascontiguousarray(word_off, np.uint64)
+    ln = np.ascontiguousarray(length, np.uint32)
+    n = len(wo) - 1
+    L.mhb_plan_seq_chunks.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint64, C.c_void_p, C.c_uint32]
+    args = (wo.ctypes.data if n else None, ln.ctypes.data if n else None, n, k, int(max_chunk_bytes))
+    nc = L.mhb_plan_seq_chunks(*args, None, 0)
+    if nc < 0:
+        raise MhbError(L.mhb_last_error().decode())
+    first = np.zeros(nc + 1, np.uint64)
+    if L.mhb_plan_seq_chunks(*args, first.ctypes.data, nc + 1) < 0:
+        raise MhbError(L.mhb_last_error().decode())
+    return [int(x) for x in first]
+
+
+def plan_mercy_segments(edges: np.ndarray, k: int, max_segment_bytes: int) -> list[int]:
+    """Leading-byte segments of a streamed mercy_host (host logic only): the first byte of every segment, then 256."""
+    L = load()
+    e = np.ascontiguousarray(edges, np.uint32).reshape(-1)
+    n = len(e) // words_per_edge(k)
+    L.mhb_plan_mercy_segments.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint64, C.c_void_p, C.c_uint32]
+    first = np.zeros(257, np.uint32)
+    ns = L.mhb_plan_mercy_segments(e.ctypes.data if n else None, n, k, int(max_segment_bytes), first.ctypes.data, 257)
+    if ns < 0:
+        raise MhbError(L.mhb_last_error().decode())
+    return [int(x) for x in first[: ns + 1]]
+
+
+def s2s_stream_stats(mercy: bool = False) -> dict:
+    """Streaming of the last s2s_host call (mercy=False: chunks, 0 = resident; passes; rounds run) or mercy_host call
+    (mercy=True: segments in n_chunks, 0 = resident), with the bytes host to device and the copy-engine / compute-stream
+    busy time, host fill time and wall time of the passes (ms)."""
+    L = load()
+    nc, npass, nr, nb = C.c_uint64(), C.c_uint64(), C.c_uint64(), C.c_uint64()
+    L.mhb_s2s_stream_stats.argtypes = [C.c_int] + [C.POINTER(C.c_uint64)] * 4
+    _check(L.mhb_s2s_stream_stats(int(mercy), C.byref(nc), C.byref(npass), C.byref(nr), C.byref(nb)))
+    h2d, kern, fill, wall = C.c_double(), C.c_double(), C.c_double(), C.c_double()
+    L.mhb_s2s_stream_times.argtypes = [C.c_int] + [C.POINTER(C.c_double)] * 4
+    _check(L.mhb_s2s_stream_times(int(mercy), C.byref(h2d), C.byref(kern), C.byref(fill), C.byref(wall)))
+    return {"n_chunks": nc.value, "n_passes": npass.value, "n_rounds": nr.value, "h2d_bytes": nb.value, "h2d_ms": h2d.value,
+            "kernel_ms": kern.value, "fill_ms": fill.value, "pass_ms": wall.value}
+
+
+def s2s_stream_decide(n_seqs: int, n_words: int, k: int, free_bytes: int, chunk_limit: int = 0) -> dict:
+    """mhb_s2s_host's residency rule for its rounds on given sizes (host code only)."""
+    L = load()
+    res, stream = C.c_uint64(), C.c_int()
+    L.mhb_selftest_s2s_stream_decide.argtypes = [C.c_uint64, C.c_uint64, C.c_uint32, C.c_uint64, C.c_uint64,
+                                                 C.POINTER(C.c_uint64), C.POINTER(C.c_int)]
+    _check(L.mhb_selftest_s2s_stream_decide(n_seqs, n_words, k, free_bytes, chunk_limit, C.byref(res), C.byref(stream)))
+    return {"stream": bool(stream.value), "resident": res.value}
+
+
+def mercy_stream_decide(n_edges: int, k: int, n_cand_reads: int, cand_words: int, max_read_len: int, free_bytes: int,
+                        chunk_limit: int = 0) -> dict:
+    """mhb_mercy_host's residency rule on given sizes (host code only)."""
+    L = load()
+    res, stream = C.c_uint64(), C.c_int()
+    L.mhb_selftest_mercy_stream_decide.argtypes = [C.c_uint64, C.c_uint32, C.c_uint64, C.c_uint64, C.c_uint32, C.c_uint64,
+                                                   C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_int)]
+    _check(L.mhb_selftest_mercy_stream_decide(n_edges, k, n_cand_reads, cand_words, max_read_len, free_bytes, chunk_limit,
+                                              C.byref(res), C.byref(stream)))
+    return {"stream": bool(stream.value), "resident": res.value}
+
+
+def mercy_auto_plan(byte_edges, k: int, n_cand_reads: int, cand_words: int, max_read_len: int, free_bytes: int) -> dict:
+    """mhb_mercy_host's segment plan without a cap, on a histogram of edges per leading byte (host code only): the first
+    byte of every segment, then 256, and the bytes of one device slot."""
+    L = load()
+    h = np.ascontiguousarray(byte_edges, np.uint64)
+    assert h.shape == (256,)
+    first = np.zeros(257, np.uint32)
+    slot = C.c_uint64()
+    L.mhb_selftest_mercy_auto_plan.argtypes = [C.c_void_p, C.c_uint32, C.c_uint64, C.c_uint64, C.c_uint32, C.c_uint64,
+                                               C.c_void_p, C.POINTER(C.c_uint64)]
+    n = L.mhb_selftest_mercy_auto_plan(h.ctypes.data, k, n_cand_reads, cand_words, max_read_len, free_bytes,
+                                       first.ctypes.data, C.byref(slot))
+    if n < 0:
+        raise MhbError(L.mhb_last_error().decode())
+    return {"first": [int(x) for x in first[: n + 1]], "slot_bytes": slot.value}
 
 
 def mercy_host(k: int, edges: np.ndarray, cand_bin: np.ndarray) -> np.ndarray:
