@@ -351,16 +351,10 @@ static int count_host_rounds(const mhb_count_args *args, mhb_count_result *res, 
       CK(cudaMemGetInfo(&free_b, &total_b));
       const size_t avail = (size_t)((double)(free_b + g_arena.cap) * 0.92);
       if (!stream && mhb_read_stream_decide(fixed, avail, 0, read_chunk_limit())) return restart_streamed();
-      if (avail <= fixed)
+      max_records = largest_round(n, fixed, avail, [&](uint64_t r) { return round_bytes(r, WR, WE, m, k); });
+      if (!max_records)
         return mhb_set_error(MHB_ERR_NOMEM, "the read library's %s (%zu bytes) does not fit the device",
                              stream ? "chunk buffers" : "image", fixed);
-      uint64_t lo = 1, hi = n;  // largest round that fits (round_bytes is monotone)
-      while (lo < hi) {
-        const uint64_t mid = lo + (hi - lo + 1) / 2;
-        if (fixed + round_bytes(mid, WR, WE, m, k) <= avail) lo = mid;
-        else hi = mid - 1;
-      }
-      max_records = lo;
     }
     max_records = std::min<uint64_t>(std::max<uint64_t>(max_records, 1), std::max<uint64_t>(n, 1));
   }
@@ -633,11 +627,11 @@ size_t s2s_round_bytes(uint64_t n, uint32_t W, uint32_t k) {
   return 2 * Arena::pad((size_t)n * W * 4 + 16) + Arena::pad(mhb_s2s_sort_workspace_bytes(n, k)) +
          Arena::pad(mhb_s2s_emit_scratch_bytes(n, k)) + Arena::pad((size_t)n * (4ull + 4ull * words_per_tip_label(k)) + 16);
 }
-// what the rounds keep next to the sequences: bucket table, histograms (+ the second-byte rows of oversized bytes),
-// totals, cursor
-size_t s2s_table_bytes() {
-  return Arena::pad((size_t)MHB_NUM_BUCKETS * 4 * 8) + 2 * Arena::pad(256 * 8) + Arena::pad(256 * 256 * 8) +
-         Arena::pad(16 * 8) + Arena::pad(64) + 8192;
+// what the rounds keep next to the sequences: bucket table, the histogram of the sort's first byte, totals and, to plan
+// rounds, the top-byte histogram, the second-byte rows of oversized bytes and the cursor
+size_t s2s_table_bytes(bool plan) {
+  return Arena::pad((size_t)MHB_NUM_BUCKETS * 4 * 8) + Arena::pad(256 * 8) + Arena::pad(16 * 8) +
+         (plan ? Arena::pad(256 * 8) + Arena::pad(256 * 256 * 8) + Arena::pad(64) + 8192 : 4096);
 }
 double device_avail_bytes() {
   size_t free_b = 0, total_b = 0;
@@ -741,7 +735,7 @@ class SeqSource {
     const bool arrays = resident_ || !ly_.fixed;
     mhb_dev_seqs v;
     v.words = (const uint32_t *)slot;
-    v.n_words = a_->word_off[e] - a_->word_off[b];
+    v.n_words = e > b ? a_->word_off[e] - a_->word_off[b] : 0;  // no word_off read for an empty set
     v.n_seqs = e - b;
     v.fixed_len = ly_.fixed ? ly_.L0 : 0;
     v.word_off = arrays ? (const uint64_t *)(slot + o_wo_) : nullptr;
@@ -790,17 +784,19 @@ class SeqSource {
 
 // the smallest device footprint of the rounds over resident sequences: the sequences, the tables and a one-item round
 size_t s2s_resident_round_bytes(uint64_t ns, uint64_t n_words, uint32_t k) {
-  return SeqSource::resident_bytes(ns, n_words) + s2s_table_bytes() + s2s_round_bytes(1, s2s_record_words(k), k);
+  return SeqSource::resident_bytes(ns, n_words) + s2s_table_bytes(true) + s2s_round_bytes(1, s2s_record_words(k), k);
 }
 }  // namespace
 
-// Same idea as count_host_rounds: the sort items of all sequences do not fit in HBM next to the sequences, so the
-// stage runs once per contiguous range of leading record bytes (a (k-1)-mer group, and a bucket, never spans two
-// ranges): extract the range -> sort -> emit -> append the item bytes and that range's rows of the bucket table to the
-// host result.  Ranges ascend, so the concatenated stream is in bucket order.  Every extraction is one pass over the
-// sequences (SeqSource): the top-byte histogram, the second-byte histograms of the leading bytes that alone exceed a
-// round, and each non-empty round, whose chunks append their in-range items at the round's cursor.
-static int s2s_host_rounds(const mhb_s2s_args *args, mhb_s2s_result *res, SeqSource &src, uint64_t n_items, uint64_t max_items) {
+// Same idea as count_host_rounds: the stage runs once per contiguous range of leading record bytes (a (k-1)-mer group,
+// and a bucket, never spans two ranges): extract the range -> sort -> emit -> append the item bytes and that range's
+// rows of the bucket table to the host result.  Ranges ascend, so the concatenated stream is in bucket order.  Every
+// extraction is one pass over the sequences (SeqSource).  one_pass (resident sequences whose items all fit next to
+// them): the one range over all bucket ids, known without a pass, extracted by mhb_s2s_extract, its output straight
+// into the result.  Otherwise the top-byte histogram and the second-byte histograms of the leading bytes that alone
+// exceed a round plan the ranges, and each non-empty round's chunks append their in-range items at its cursor.
+static int s2s_host_rounds(const mhb_s2s_args *args, mhb_s2s_result *res, SeqSource &src, uint64_t n_items, uint64_t max_items,
+                           bool one_pass) {
   const uint32_t k = args->k;
   const uint32_t W = s2s_record_words(k), WPT = words_per_tip_label(k);
   const int top_byte = (int)(4 * W - 1);
@@ -808,89 +804,106 @@ static int s2s_host_rounds(const mhb_s2s_args *args, mhb_s2s_result *res, SeqSou
   Timer t_all(st), t(st);
   t_all.start();
 
-  const size_t fixed_b = src.device_bytes() + s2s_table_bytes();
-  if (!max_items) {
-    const double avail = device_avail_bytes();
-    if (avail <= (double)fixed_b)
-      return mhb_set_error(MHB_ERR_NOMEM, "the sequences%s alone (%zu bytes) do not fit the device",
-                           src.n_chunks() ? "' chunk buffers" : "", fixed_b);
-    uint64_t lo = 1, hi = n_items;
-    while (lo < hi) {
-      const uint64_t mid = lo + (hi - lo + 1) / 2;
-      if ((double)(fixed_b + s2s_round_bytes(mid, W, k)) <= avail) lo = mid;
-      else hi = mid - 1;
+  const size_t fixed_b = src.device_bytes() + s2s_table_bytes(!one_pass);
+  if (one_pass) {
+    max_items = n_items;
+  } else {
+    if (!max_items) {
+      const size_t avail = (size_t)device_avail_bytes();
+      max_items = largest_round(n_items, fixed_b, avail, [&](uint64_t n) { return s2s_round_bytes(n, W, k); });
+      if (!max_items)
+        return mhb_set_error(MHB_ERR_NOMEM, "the sequences%s alone (%zu bytes) do not fit the device",
+                             src.n_chunks() ? "' chunk buffers" : "", fixed_b);
     }
-    max_items = lo;
+    max_items = std::min<uint64_t>(max_items, std::max<uint64_t>(n_items, 1));
   }
-  max_items = std::min<uint64_t>(std::max<uint64_t>(max_items, 1), std::max<uint64_t>(n_items, 1));
   CKR(g_arena.reserve(fixed_b + s2s_round_bytes(max_items, W, k)));
   char *d_seqs = g_arena.take<char>(src.device_bytes());
   uint64_t *d_table = g_arena.take<uint64_t>((size_t)MHB_NUM_BUCKETS * 4);
   uint64_t *d_hist0 = g_arena.take<uint64_t>(256);
-  uint64_t *d_hist_top = g_arena.take<uint64_t>(256);
-  uint64_t *d_sub = g_arena.take<uint64_t>(256 * 256);
   uint64_t *d_totals = g_arena.take<uint64_t>(16);
-  uint64_t *d_cursor = g_arena.take<uint64_t>(8);
+  uint64_t *d_hist_top = nullptr, *d_sub = nullptr, *d_cursor = nullptr;  // to plan rounds
+  if (!one_pass) {
+    d_hist_top = g_arena.take<uint64_t>(256);
+    d_sub = g_arena.take<uint64_t>(256 * 256);
+    d_cursor = g_arena.take<uint64_t>(8);
+  }
   uint32_t *d_a = g_arena.take<uint32_t>((size_t)max_items * W + 4);
   uint32_t *d_b = g_arena.take<uint32_t>((size_t)max_items * W + 4);
   const size_t ws_bytes = mhb_s2s_sort_workspace_bytes(max_items, k);
   const size_t scratch_bytes = mhb_s2s_emit_scratch_bytes(max_items, k);
+  // worst case bytes per sort item: 2 + 2 + 4*WPT (every item a large-multiplicity tip)
   const uint64_t cap_bytes = max_items * (4ull + 4ull * WPT) + 16;
   char *d_ws = g_arena.take<char>(ws_bytes);
   char *d_scratch = g_arena.take<char>(scratch_bytes);
   uint8_t *d_bytes = g_arena.take<uint8_t>(cap_bytes);
   CKR(src.bind(d_seqs, st));
-  CK(cudaMemsetAsync(d_hist_top, 0, 256 * 8, st));
 
-  // ---- plan (two-level, as in count_host_rounds) ----
-  t.start();
+  // ---- plan: one range over all bucket ids, or two-level, as in count_host_rounds ----
+  std::vector<std::pair<uint32_t, uint32_t>> ranges = {{0u, 65535u}};
   uint64_t h_top[256];
-  CKR(src.pass(st, [&](const mhb_dev_seqs &s, uint64_t n) {
-    return mhb_s2s_extract_range(st, &s, k, nullptr, n, 0, 65535, nullptr, 0, d_hist_top, top_byte);
-  }));
-  CK(cudaMemcpyAsync(h_top, d_hist_top, sizeof(h_top), cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  std::vector<uint32_t> over;
-  for (uint32_t b = 0; b < 256; ++b)
-    if (h_top[b] > max_items) over.push_back(b);
   std::vector<uint64_t> h_sub;
-  if (!over.empty()) {
-    h_sub.assign(256 * 256, 0);
-    CK(cudaMemsetAsync(d_sub, 0, 256 * 256 * 8, st));
+  if (!one_pass) {
+    t.start();
+    CK(cudaMemsetAsync(d_hist_top, 0, 256 * 8, st));
     CKR(src.pass(st, [&](const mhb_dev_seqs &s, uint64_t n) {
-      for (uint32_t b : over)
-        CKR(mhb_s2s_extract_range(st, &s, k, nullptr, n, b << 8, (b << 8) | 255u, nullptr, 0, d_sub + (size_t)b * 256, top_byte - 1));
-      return MHB_OK;
+      return mhb_s2s_extract_range(st, &s, k, nullptr, n, 0, 65535, nullptr, 0, d_hist_top, top_byte);
     }));
-    CK(cudaMemcpyAsync(h_sub.data(), d_sub, 256 * 256 * 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(h_top, d_hist_top, sizeof(h_top), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
+    std::vector<uint32_t> over;
+    for (uint32_t b = 0; b < 256; ++b)
+      if (h_top[b] > max_items) over.push_back(b);
+    if (!over.empty()) {
+      h_sub.assign(256 * 256, 0);
+      CK(cudaMemsetAsync(d_sub, 0, 256 * 256 * 8, st));
+      CKR(src.pass(st, [&](const mhb_dev_seqs &s, uint64_t n) {
+        for (uint32_t b : over)
+          CKR(mhb_s2s_extract_range(st, &s, k, nullptr, n, b << 8, (b << 8) | 255u, nullptr, 0, d_sub + (size_t)b * 256, top_byte - 1));
+        return MHB_OK;
+      }));
+      CK(cudaMemcpyAsync(h_sub.data(), d_sub, 256 * 256 * 8, cudaMemcpyDeviceToHost, st));
+      CK(cudaStreamSynchronize(st));
+    }
+    std::vector<uint32_t> r_lo(65536), r_hi(65536);
+    const int n_ranges = mhb_plan_rounds16(h_top, h_sub.empty() ? nullptr : h_sub.data(), max_items, r_lo.data(), r_hi.data(), 65536);
+    if (n_ranges < 0) return MHB_ERR_NOMEM;
+    ranges.clear();
+    for (int i = 0; i < n_ranges; ++i) ranges.push_back({r_lo[i], r_hi[i]});
+    res->t_extract_ms = t.stop();
   }
-  std::vector<uint32_t> r_lo(65536), r_hi(65536);
-  const int n_ranges = mhb_plan_rounds16(h_top, h_sub.empty() ? nullptr : h_sub.data(), max_items, r_lo.data(), r_hi.data(), 65536);
-  if (n_ranges < 0) return MHB_ERR_NOMEM;
-  res->t_extract_ms = t.stop();
 
   SdbgStitch out;
-  for (int ri = 0; ri < n_ranges; ++ri) {
-    uint64_t planned = 0;  // the range's items, from the histograms
-    for (uint32_t b = r_lo[ri] >> 8; b <= r_hi[ri] >> 8; ++b) {
-      const uint32_t c0 = b == r_lo[ri] >> 8 ? r_lo[ri] & 255 : 0, c1 = b == r_hi[ri] >> 8 ? r_hi[ri] & 255 : 255;
-      if (c0 == 0 && c1 == 255) planned += h_top[b];
-      else
-        for (uint32_t c = c0; c <= c1; ++c) planned += h_sub[(size_t)b * 256 + c];
+  uint64_t tot[16] = {0};  // one pass: the emitter's totals
+  for (const auto &rg : ranges) {
+    uint64_t planned = n_items;  // the range's items, from the histograms
+    if (!one_pass) {
+      planned = 0;
+      for (uint32_t b = rg.first >> 8; b <= rg.second >> 8; ++b) {
+        const uint32_t c0 = b == rg.first >> 8 ? rg.first & 255 : 0, c1 = b == rg.second >> 8 ? rg.second & 255 : 255;
+        if (c0 == 0 && c1 == 255) planned += h_top[b];
+        else
+          for (uint32_t c = c0; c <= c1; ++c) planned += h_sub[(size_t)b * 256 + c];
+      }
+      if (planned == 0) continue;
     }
-    if (planned == 0) continue;
     ++g_s2s_rounds;
     t.start();
     CK(cudaMemsetAsync(d_hist0, 0, 256 * 8, st));
-    CK(cudaMemsetAsync(d_cursor, 0, 64, st));
-    CKR(src.pass(st, [&](const mhb_dev_seqs &s, uint64_t n) {
-      return mhb_s2s_extract_range(st, &s, k, d_a, n, r_lo[ri], r_hi[ri], d_cursor, max_items, d_hist0,
-                                   mhb_s2s_sort_hist_byte(max_items, k));
-    }));
-    uint64_t n_round = 0;
-    CK(cudaMemcpyAsync(&n_round, d_cursor, 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    uint64_t n_round = n_items;
+    if (one_pass) {
+      CKR(src.pass(st, [&](const mhb_dev_seqs &s, uint64_t n) {
+        return mhb_s2s_extract(st, &s, k, d_a, n, d_hist0, mhb_s2s_sort_hist_byte(max_items, k));
+      }));
+    } else {
+      CK(cudaMemsetAsync(d_cursor, 0, 64, st));
+      CKR(src.pass(st, [&](const mhb_dev_seqs &s, uint64_t n) {
+        return mhb_s2s_extract_range(st, &s, k, d_a, n, rg.first, rg.second, d_cursor, max_items, d_hist0,
+                                     mhb_s2s_sort_hist_byte(max_items, k));
+      }));
+      CK(cudaMemcpyAsync(&n_round, d_cursor, 8, cudaMemcpyDeviceToHost, st));
+      CK(cudaStreamSynchronize(st));
+    }
     res->t_extract_ms += t.stop();
     if (n_round != planned)
       return mhb_set_error(MHB_ERR_NOMEM, "internal: round of %llu items, %llu planned", (unsigned long long)n_round,
@@ -903,19 +916,22 @@ static int s2s_host_rounds(const mhb_s2s_args *args, mhb_s2s_result *res, SeqSou
     res->t_sort_ms += t.stop();
     t.start();
     CKR(mhb_s2s_emit(st, in_b ? d_b : d_a, n_round, k, d_bytes, cap_bytes, d_table, d_totals, d_scratch, scratch_bytes));
-    CKR(out.append(st, d_bytes, cap_bytes, d_table, d_totals));
+    if (one_pass) {
+      CK(cudaMemcpyAsync(tot, d_totals, sizeof(tot), cudaMemcpyDeviceToHost, st));
+      CK(cudaMemcpyAsync(res->bucket_table, d_table, sizeof(res->bucket_table), cudaMemcpyDeviceToHost, st));
+      CK(cudaStreamSynchronize(st));
+      if (tot[0] > cap_bytes) return mhb_set_error(MHB_ERR_NOMEM, "internal: SdBG byte stream exceeds capacity");
+    } else {
+      CKR(out.append(st, d_bytes, cap_bytes, d_table, d_totals));
+    }
     res->t_emit_ms += t.stop();
   }
-  res->n_bytes = out.tot[0];
-  res->n_items = out.tot[1];
-  res->n_tips = out.tot[2];
-  res->n_large_mul = out.tot[3];
-  for (int i = 0; i < 9; ++i) res->w_count[i] = out.tot[4 + i];
-  res->ones_in_last = out.tot[13];
-  memcpy(res->bucket_table, out.table.data(), sizeof(res->bucket_table));
-  res->bytes = (uint8_t *)malloc(std::max<size_t>(1, out.bytes.size()));
+  set_sdbg_totals(res, one_pass ? tot : out.tot);
+  if (!one_pass) memcpy(res->bucket_table, out.table.data(), sizeof(res->bucket_table));
+  res->bytes = (uint8_t *)malloc(std::max<size_t>(1, res->n_bytes));
   if (!res->bytes) return mhb_set_error(MHB_ERR_NOMEM, "host malloc failed");
-  if (!out.bytes.empty()) memcpy(res->bytes, out.bytes.data(), out.bytes.size());
+  if (res->n_bytes && one_pass) CK(cudaMemcpy(res->bytes, d_bytes, res->n_bytes, cudaMemcpyDeviceToHost));
+  else if (res->n_bytes) memcpy(res->bytes, out.bytes.data(), res->n_bytes);
   res->t_total_ms = t_all.stop();
   return MHB_OK;
 }
@@ -986,101 +1002,24 @@ extern "C" int mhb_s2s_host(const mhb_s2s_args *args, mhb_s2s_result *res) {
 
   SeqLayout ly;
   seq_layout(args->word_off, args->len, ns, k, &ly);
-  const std::vector<uint64_t> &item_off = ly.item_off;
   const uint64_t n_items = ly.n_items, n_words = ly.n_words;
   res->n_records = n_items;
 
-  cudaStream_t st = 0;
-  Timer t_all(st), t(st);
-  t_all.start();
-  const uint32_t W = s2s_record_words(k);
-  const size_t ws_bytes = mhb_s2s_sort_workspace_bytes(n_items, k);
-  const size_t scratch_bytes = mhb_s2s_emit_scratch_bytes(n_items, k);
-  // worst case bytes per sort item: 2 + 2 + 4*WPT (every item a large-multiplicity tip)
-  const uint64_t cap_bytes = n_items * (4ull + 4ull * res->words_per_tip_label) + 16;
-  size_t need = Arena::pad(n_words * 4 + 64) + Arena::pad((ns + 1) * 8) * 2 + Arena::pad((ns + 1) * 4) +
-                Arena::pad((ns + 1) * 2) + 2 * Arena::pad((size_t)n_items * W * 4 + 16) + Arena::pad(ws_bytes) +
-                Arena::pad(scratch_bytes) + Arena::pad(cap_bytes) + Arena::pad((size_t)MHB_NUM_BUCKETS * 4 * 8) +
-                Arena::pad(256 * 8) + Arena::pad(16 * 8) + 4096;
-  {
-    // A13: items that do not fit the device at once (or a caller-imposed cap) -> rounds over leading-byte ranges; the
-    // sequences are streamed when a chunk cap is set or when they leave no room for even a one-item round
-    bool rounds = g_s2s_round_limit && n_items > g_s2s_round_limit;
-    if (!rounds && need > g_arena.cap) {
-      size_t free_b = 0, total_b = 0;
-      CK(cudaMemGetInfo(&free_b, &total_b));
-      rounds = (double)need > 0.92 * (double)(free_b + g_arena.cap);
-    }
-    const bool stream = g_s2s_chunk_limit != 0 ||
-                        (rounds && mhb_read_stream_decide(s2s_resident_round_bytes(ns, n_words, k), (uint64_t)device_avail_bytes(), 0, 0));
-    if (rounds || stream) {
-      SeqSource src(args, ly);
-      CKR(src.init(stream ? (g_s2s_chunk_limit ? g_s2s_chunk_limit : read_chunk_auto_bytes()) : 0));
-      return s2s_host_rounds(args, res, src, n_items, g_s2s_round_limit);
-    }
+  // A13: items that do not fit the device at once (or a caller-imposed cap) -> rounds over leading-byte ranges; the
+  // sequences are streamed when a chunk cap is set or when they leave no room for even a one-item round
+  const size_t need = SeqSource::resident_bytes(ns, n_words) + s2s_table_bytes(false) +
+                      s2s_round_bytes(n_items, s2s_record_words(k), k);
+  bool rounds = g_s2s_round_limit && n_items > g_s2s_round_limit;
+  if (!rounds && need > g_arena.cap) {
+    size_t free_b = 0, total_b = 0;
+    CK(cudaMemGetInfo(&free_b, &total_b));
+    rounds = (double)need > 0.92 * (double)(free_b + g_arena.cap);
   }
-  g_s2s_rounds = 1;
-  CKR(g_arena.reserve(need));
-  uint32_t *d_words = g_arena.take<uint32_t>(n_words + 16);
-  uint64_t *d_word_off = g_arena.take<uint64_t>(ns + 1);
-  uint64_t *d_item_off = g_arena.take<uint64_t>(ns + 1);
-  uint32_t *d_len = g_arena.take<uint32_t>(ns + 1);
-  uint16_t *d_mult = g_arena.take<uint16_t>(ns + 1);
-  uint32_t *d_a = g_arena.take<uint32_t>((size_t)n_items * W + 4);
-  uint32_t *d_b = g_arena.take<uint32_t>((size_t)n_items * W + 4);
-  char *d_ws = g_arena.take<char>(ws_bytes);
-  char *d_scratch = g_arena.take<char>(scratch_bytes);
-  uint8_t *d_bytes = g_arena.take<uint8_t>(cap_bytes);
-  uint64_t *d_table = g_arena.take<uint64_t>((size_t)MHB_NUM_BUCKETS * 4);
-  uint64_t *d_hist0 = g_arena.take<uint64_t>(256);
-  uint64_t *d_totals = g_arena.take<uint64_t>(16);
-
-  if (ns) {
-    CK(cudaMemcpyAsync(d_words, args->words, n_words * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_word_off, args->word_off, (ns + 1) * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_item_off, item_off.data(), (ns + 1) * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_len, args->len, ns * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_mult, args->mult, ns * 2, cudaMemcpyHostToDevice, st));
-  }
-  CK(cudaMemsetAsync(d_hist0, 0, 256 * 8, st));
-
-  mhb_dev_seqs seqs;
-  seqs.words = d_words;
-  seqs.n_words = n_words;
-  seqs.n_seqs = ns;
-  seqs.fixed_len = ly.fixed ? ly.L0 : 0;
-  seqs.word_off = d_word_off;
-  seqs.len = d_len;
-  seqs.item_off = d_item_off;
-  seqs.mult = d_mult;
-  seqs.fixed_stride = 0;
-
-  t.start();
-  CKR(mhb_s2s_extract(st, &seqs, k, d_a, n_items, d_hist0, mhb_s2s_sort_hist_byte(n_items, k)));
-  res->t_extract_ms = t.stop();
-  t.start();
-  int in_b = 0;
-  CKR(mhb_s2s_sort(st, d_a, d_b, n_items, k, d_hist0, d_ws, ws_bytes, &in_b));
-  res->t_sort_ms = t.stop();
-  t.start();
-  CKR(mhb_s2s_emit(st, in_b ? d_b : d_a, n_items, k, d_bytes, cap_bytes, d_table, d_totals, d_scratch, scratch_bytes));
-  uint64_t totals[16];
-  CK(cudaMemcpyAsync(totals, d_totals, sizeof(totals), cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(res->bucket_table, d_table, sizeof(res->bucket_table), cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  res->t_emit_ms = t.stop();
-  res->n_bytes = totals[0];
-  res->n_items = totals[1];
-  res->n_tips = totals[2];
-  res->n_large_mul = totals[3];
-  for (int i = 0; i < 9; ++i) res->w_count[i] = totals[4 + i];
-  res->ones_in_last = totals[13];
-  if (res->n_bytes > cap_bytes) return mhb_set_error(MHB_ERR_NOMEM, "internal: SdBG byte stream exceeds capacity");
-  res->bytes = (uint8_t *)malloc(std::max<size_t>(1, res->n_bytes));
-  if (!res->bytes) return mhb_set_error(MHB_ERR_NOMEM, "host malloc failed");
-  if (res->n_bytes) CK(cudaMemcpy(res->bytes, d_bytes, res->n_bytes, cudaMemcpyDeviceToHost));
-  res->t_total_ms = t_all.stop();
-  return MHB_OK;
+  const bool stream = g_s2s_chunk_limit != 0 ||
+                      (rounds && mhb_read_stream_decide(s2s_resident_round_bytes(ns, n_words, k), (uint64_t)device_avail_bytes(), 0, 0));
+  SeqSource src(args, ly);
+  CKR(src.init(stream ? (g_s2s_chunk_limit ? g_s2s_chunk_limit : read_chunk_auto_bytes()) : 0));
+  return s2s_host_rounds(args, res, src, n_items, g_s2s_round_limit, !rounds && !stream);
 }
 
 // ================================================================================================
@@ -1478,12 +1417,7 @@ static int build_host_impl(const mhb_build_args *args, mhb_build_result *res, bo
   CK(cudaMemcpyAsync(totals, d_totals, sizeof(totals), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   res->t_s2s_ms = t.stop();
-  res->n_bytes = totals[0];
-  res->n_items = totals[1];
-  res->n_tips = totals[2];
-  res->n_large_mul = totals[3];
-  for (int i = 0; i < 9; ++i) res->w_count[i] = totals[4 + i];
-  res->ones_in_last = totals[13];
+  set_sdbg_totals(res, totals);
   if (res->n_bytes > cap_bytes) return mhb_set_error(MHB_ERR_NOMEM, "internal: SdBG byte stream exceeds capacity");
 
   // ---- D2H ----

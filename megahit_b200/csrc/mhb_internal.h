@@ -3,12 +3,26 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include <algorithm>
 #include <functional>
 #include <vector>
 
 #include "mhb.h"
 
 int mhb_set_error(int code, const char *fmt, ...);
+
+// largest n <= n_max with fixed + bytes(n) <= avail (bytes(n) grows with n); 0 when not even one fits
+template <class F>
+uint64_t largest_round(uint64_t n_max, size_t fixed, size_t avail, F bytes) {
+  if (fixed + bytes(1) > avail) return 0;
+  uint64_t lo = 1, hi = std::max<uint64_t>(n_max, 1);
+  while (lo < hi) {
+    const uint64_t mid = lo + (hi - lo + 1) / 2;
+    if (fixed + bytes(mid) <= avail) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
 
 // mhb_sort_records + optional per-pass timings (host array of n_bytes doubles, ms; forces a stream sync)
 int mhb_sort_records_impl(void *stream, uint32_t *a, uint32_t *b, uint64_t n, uint32_t words, const uint8_t *bytes,
@@ -163,3 +177,14 @@ struct SdbgStitch {
  private:
   std::vector<uint64_t> round_table = std::vector<uint64_t>((size_t)65536 * 4);
 };
+
+// the emitter's totals (SdbgStitch::tot layout) into the counts of a result (mhb_build_result, mhb_s2s_result)
+template <class R>
+void set_sdbg_totals(R *res, const uint64_t tot[16]) {
+  res->n_bytes = tot[0];
+  res->n_items = tot[1];
+  res->n_tips = tot[2];
+  res->n_large_mul = tot[3];
+  for (int i = 0; i < 9; ++i) res->w_count[i] = tot[4 + i];
+  res->ones_in_last = tot[13];
+}
