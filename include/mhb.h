@@ -132,9 +132,24 @@ int mhb_s2s_sort(void *stream, uint32_t *a, uint32_t *b, uint64_t n, uint32_t k,
                  size_t ws_bytes, int *result_in_b);
 size_t mhb_s2s_sort_workspace_bytes(uint64_t n, uint32_t k);
 int mhb_s2s_sort_hist_byte(uint64_t n, uint32_t k);
-/* buckets the last mhb_s2s_sort of this process left to the radix engine and their items; buckets it sorted with the
- * large shared-memory geometry after the small one (any pointer may be NULL) */
+/* buckets the last mhb_s2s_sort (or mhb_s2s_sort_emit) of this process left to the radix engine and their items;
+ * buckets it sorted with the large shared-memory geometry after the small one (any pointer may be NULL) */
 void mhb_s2s_sort_stats(uint64_t *n_oversized, uint64_t *oversized_items, uint64_t *n_large);
+
+/* mhb_s2s_sort of the n items in a (b: the other buffer, same size) followed by mhb_s2s_emit of the sorted items into
+ * bytes_out / bucket_table / totals: the same bytes[0 .. totals[0]), the same table and the same 16 totals, and the same
+ * capacity contract (nothing is written past capacity_bytes; the totals report the whole stream, so the caller checks
+ * totals[0]).  On the bucket path (9 <= k <= 38, up to 403 M items) the bucket kernel emits every bucket it sorts
+ * straight out of shared memory (the sorted items are never written back): each bucket's bytes go to a staging slot
+ * known in advance, one small scan over the 65 536 bucket rows gives the table and one gather copies the bytes to their
+ * offsets.  Off that path it is exactly those two calls.  a and b are both overwritten (neither holds the sorted
+ * items afterwards); they must be 16-byte aligned.  ws: mhb_s2s_sort_emit_workspace_bytes(n, k) bytes, at most
+ * mhb_s2s_sort_workspace_bytes + mhb_s2s_emit_scratch_bytes (each rounded up to 256).  May synchronise the stream once
+ * (twice with buckets for the large geometry).  Leaves ONE entry in the mhb_sort_pass_ms ring, as mhb_s2s_sort. */
+int mhb_s2s_sort_emit(void *stream, uint32_t *a, uint32_t *b, uint64_t n, uint32_t k, const uint64_t *first_hist,
+                      uint8_t *bytes_out, uint64_t capacity_bytes, uint64_t *bucket_table, uint64_t *totals, void *ws,
+                      size_t ws_bytes);
+size_t mhb_s2s_sort_emit_workspace_bytes(uint64_t n, uint32_t k);
 
 /* Fused partition + exchange for the multi-GPU path: ONE stable radix pass whose per-digit destinations are arbitrary
  * device byte addresses (bin_addr_dev[256], device memory) = where the first record of digit d coming from THIS call

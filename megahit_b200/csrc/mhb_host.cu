@@ -830,12 +830,11 @@ static int s2s_host_rounds(const mhb_s2s_args *args, mhb_s2s_result *res, SeqSou
   }
   uint32_t *d_a = g_arena.take<uint32_t>((size_t)max_items * W + 4);
   uint32_t *d_b = g_arena.take<uint32_t>((size_t)max_items * W + 4);
-  const size_t ws_bytes = mhb_s2s_sort_workspace_bytes(max_items, k);
-  const size_t scratch_bytes = mhb_s2s_emit_scratch_bytes(max_items, k);
+  // sort + emit workspace (at most the sort workspace plus the emit scratch s2s_round_bytes reserves)
+  const size_t ws_bytes = mhb_s2s_sort_emit_workspace_bytes(max_items, k);
   // worst case bytes per sort item: 2 + 2 + 4*WPT (every item a large-multiplicity tip)
   const uint64_t cap_bytes = max_items * (4ull + 4ull * WPT) + 16;
   char *d_ws = g_arena.take<char>(ws_bytes);
-  char *d_scratch = g_arena.take<char>(scratch_bytes);
   uint8_t *d_bytes = g_arena.take<uint8_t>(cap_bytes);
   CKR(src.bind(d_seqs, st));
 
@@ -909,13 +908,13 @@ static int s2s_host_rounds(const mhb_s2s_args *args, mhb_s2s_result *res, SeqSou
       return mhb_set_error(MHB_ERR_NOMEM, "internal: round of %llu items, %llu planned", (unsigned long long)n_round,
                            (unsigned long long)planned);
     t.start();
-    int in_b = 0;
     // the histogram is of the byte a sort of max_items items starts with: pass it only if this round's sort does too
     const bool hist_ok = mhb_s2s_sort_hist_byte(n_round, k) == mhb_s2s_sort_hist_byte(max_items, k);
-    CKR(mhb_s2s_sort(st, d_a, d_b, n_round, k, hist_ok ? d_hist0 : nullptr, d_ws, ws_bytes, &in_b));
+    // sort and emit in one call (the bucket kernel emits every bucket it sorts): t_sort_ms carries both
+    CKR(mhb_s2s_sort_emit(st, d_a, d_b, n_round, k, hist_ok ? d_hist0 : nullptr, d_bytes, cap_bytes, d_table, d_totals, d_ws,
+                          ws_bytes));
     res->t_sort_ms += t.stop();
     t.start();
-    CKR(mhb_s2s_emit(st, in_b ? d_b : d_a, n_round, k, d_bytes, cap_bytes, d_table, d_totals, d_scratch, scratch_bytes));
     if (one_pass) {
       CK(cudaMemcpyAsync(tot, d_totals, sizeof(tot), cudaMemcpyDeviceToHost, st));
       CK(cudaMemcpyAsync(res->bucket_table, d_table, sizeof(res->bucket_table), cudaMemcpyDeviceToHost, st));
@@ -1367,9 +1366,9 @@ static int build_host_impl(const mhb_build_args *args, mhb_build_result *res, bo
   const uint64_t n_seqs = n_solid + n_mercy;
   const uint64_t n_items = n_seqs * 6;  // 2 strands x (k+1 - k + 2)
   res->n_sort_items = n_items;
-  const size_t s_ws = mhb_s2s_sort_workspace_bytes(n_items, k), s_scr = mhb_s2s_emit_scratch_bytes(n_items, k);
+  const size_t s_ws = mhb_s2s_sort_emit_workspace_bytes(n_items, k);
   const uint64_t cap_bytes = n_items * (4ull + 4ull * WPT) + 16;
-  const size_t s2s_work = 2 * Arena::pad((size_t)n_items * W2 * 4 + 16) + Arena::pad(s_ws) + Arena::pad(s_scr) + Arena::pad(cap_bytes);
+  const size_t s2s_work = 2 * Arena::pad((size_t)n_items * W2 * 4 + 16) + Arena::pad(s_ws) + Arena::pad(cap_bytes);
   char *sw = work;
   if (s2s_work > work_bytes) {
     CK(cudaStreamSynchronize(st));
@@ -1385,8 +1384,7 @@ static int build_host_impl(const mhb_build_args *args, mhb_build_result *res, bo
   uint32_t *s_a = (uint32_t *)sw;
   uint32_t *s_b = (uint32_t *)(sw + Arena::pad((size_t)n_items * W2 * 4 + 16));
   char *s_wsp = sw + 2 * Arena::pad((size_t)n_items * W2 * 4 + 16);
-  char *s_scrp = s_wsp + Arena::pad(s_ws);
-  uint8_t *d_bytes = (uint8_t *)(s_scrp + Arena::pad(s_scr));
+  uint8_t *d_bytes = (uint8_t *)(s_wsp + Arena::pad(s_ws));
   mhb_dev_seqs seqs;
   memset(&seqs, 0, sizeof(seqs));
   seqs.words = d_all_edges;
@@ -1408,11 +1406,9 @@ static int build_host_impl(const mhb_build_args *args, mhb_build_result *res, bo
   } else {
     CKR(mhb_s2s_extract(st, &seqs, k, s_a, n_items, d_hist1, mhb_s2s_sort_hist_byte(n_items, k)));
   }
-  int s_in_b = 0;
   // the extraction histogrammed the byte a sort of n_items (the bound) starts with; the pruned count may start with another
   const bool hist_ok = mhb_s2s_sort_hist_byte(n_sorted, k) == mhb_s2s_sort_hist_byte(n_items, k);
-  CKR(mhb_s2s_sort(st, s_a, s_b, n_sorted, k, hist_ok ? d_hist1 : nullptr, s_wsp, s_ws, &s_in_b));
-  CKR(mhb_s2s_emit(st, s_in_b ? s_b : s_a, n_sorted, k, d_bytes, cap_bytes, d_table, d_totals, s_scrp, s_scr));
+  CKR(mhb_s2s_sort_emit(st, s_a, s_b, n_sorted, k, hist_ok ? d_hist1 : nullptr, d_bytes, cap_bytes, d_table, d_totals, s_wsp, s_ws));
   uint64_t totals[16];
   CK(cudaMemcpyAsync(totals, d_totals, sizeof(totals), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));

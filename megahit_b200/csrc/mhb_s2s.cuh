@@ -470,7 +470,7 @@ __global__ void __launch_bounds__(kEmitThreads)
 // behind each range, then the thread walks its range backwards.  (The first version let every bucket scan forward for
 // its successor: fine while all buckets are populated, but a rank of a multi-GPU build owns one contiguous range, and
 // its last bucket then walked tens of thousands of empty buckets in one thread.)
-__global__ void __launch_bounds__(1024) k_bucket_finalize(const u64 *bucket_start, const u64 *totals, u64 *bucket_table) {
+static __global__ void __launch_bounds__(1024) k_bucket_finalize(const u64 *bucket_start, const u64 *totals, u64 *bucket_table) {
   constexpr u32 PER = MHB_NUM_BUCKETS / 1024;
   __shared__ u32 s_first[1024];
   const u32 t = threadIdx.x, b0 = t * PER;
@@ -542,16 +542,19 @@ struct StagedRecs {
   }
 };
 
-// walk the group starting at record i; returns its end.  WRITE: append item bytes at out + acc.bytes.
-template <int W, bool WRITE>
-__device__ __forceinline__ u64 s2s_group2(const StagedRecs<W> &sr, u64 n, u64 i, u32 k, EmitAcc &acc, uint8_t *out,
-                                          u32 *w_count, u32 &ones, u32 fmt) {
+// walk the group starting at record i; returns its end.  WRITE: append item bytes at out + acc.bytes (an item that
+// would end past `cap` bytes of out is counted but not written) and count w and `last`.  Recs: any source with
+// get(index, record) over records 0 .. n-1 (StagedRecs, or the bucket kernel's shared-memory bucket); I: the index type
+// (u32 inside one bucket saves the registers of 64-bit indices).
+template <int W, bool WRITE, class Recs, class I>
+__device__ __forceinline__ I s2s_group2(const Recs &sr, I n, I i, u32 k, EmitAcc &acc, uint8_t *out,
+                                          u32 *w_count, u32 &ones, u32 fmt, u32 cap = 0xFFFFFFFFu) {
   const u32 WPT = words_per_tip_label(k);
   u32 r0[W], x[W];
   sr.get(i, r0);
   u32 hsa = 0, hsb = 0;
-  u64 e = i;
-  for (u64 j = i; j < n; ++j) {  // :724-738
+  I e = i;
+  for (I j = i; j < n; ++j) {  // :724-738
     sr.get(j, x);
     if (j > i && diff_km1<W>(r0, x, k)) break;
     const u32 a = s2s_a<W>(x, k), b = s2s_b<W>(x);
@@ -562,13 +565,13 @@ __device__ __forceinline__ u64 s2s_group2(const StagedRecs<W> &sr, u64 n, u64 i,
     e = j + 1;
   }
   u32 outputed_b = 0;
-  u64 j = i;
+  I j = i;
   u32 cur[W];
 #pragma unroll
   for (int q = 0; q < W; ++q) cur[q] = r0[q];
   while (j < e) {  // :740-786
     const u32 a = s2s_a<W>(cur, k), b = s2s_b<W>(cur);
-    u64 t = j + 1;
+    I t = j + 1;
     u32 na = 0xFF, nb = 0xFF;
     u32 nx[W];
     u32 best = cur[W - 1] & 0xFFFFu;
@@ -591,17 +594,19 @@ __device__ __forceinline__ u64 s2s_group2(const StagedRecs<W> &sr, u64 n, u64 i,
       const u32 tip = a == kSentinel ? 1u : 0u;
       const u32 sz = 2u + (mul > 254u ? 2u : 0u) + (tip ? 4u * WPT : 0u);
       if (WRITE) {
-        uint16_t *o = reinterpret_cast<uint16_t *>(out + acc.bytes);
-        o[0] = (uint16_t)((w | (last << 4) | (tip << 5)) | ((mul > 255u ? 255u : mul) << 8));
-        u32 p = 1;
-        if (mul > 254u) o[p++] = (uint16_t)mul;
-        if (tip) {
-          for (u32 q = 0; q < WPT; ++q) {
-            u32 lw = pick<W>(cur, q);
-            if (fmt) lw = r2s_label_word(lw, q, (u32)W, k, b);
-            else if (q == (u32)W - 1) lw = (lw & 0xFFFF0000u) | best;  // label = raw words of the run's first sorted record
-            o[p++] = (uint16_t)(lw & 0xFFFFu);
-            o[p++] = (uint16_t)(lw >> 16);
+        if (acc.bytes + sz <= cap) {
+          uint16_t *o = reinterpret_cast<uint16_t *>(out + acc.bytes);
+          o[0] = (uint16_t)((w | (last << 4) | (tip << 5)) | ((mul > 255u ? 255u : mul) << 8));
+          u32 p = 1;
+          if (mul > 254u) o[p++] = (uint16_t)mul;
+          if (tip) {
+            for (u32 q = 0; q < WPT; ++q) {
+              u32 lw = pick<W>(cur, q);
+              if (fmt) lw = r2s_label_word(lw, q, (u32)W, k, b);
+              else if (q == (u32)W - 1) lw = (lw & 0xFFFF0000u) | best;  // label = raw words of the run's first sorted record
+              o[p++] = (uint16_t)(lw & 0xFFFFu);
+              o[p++] = (uint16_t)(lw >> 16);
+            }
           }
         }
         atomicAdd(&w_count[w], 1u);
@@ -719,7 +724,7 @@ __global__ void __launch_bounds__(kEmit2Warps * 32)
 }
 
 // copy every chunk's compact bytes to their final position (all sizes and offsets are even)
-__global__ void __launch_bounds__(256)
+static __global__ void __launch_bounds__(256)
     k_s2s_gather(const uint8_t *__restrict__ tmp, u32 chunk_records, u32 maxb, u32 n_chunks,
                  const u32 *__restrict__ chunk_bytes, const u64 *__restrict__ chunk_off, uint8_t *__restrict__ out,
                  u64 capacity) {
@@ -735,7 +740,7 @@ __global__ void __launch_bounds__(256)
 }
 
 // bucket_local {chunk, bytes, items, tips, large within the chunk} + the chunks' global offsets -> bucket_start
-__global__ void k_bucket_starts(const u32 *bucket_local, const u64 *chunk_off /*4 planes*/, u64 n_chunks, u64 *bucket_start) {
+static __global__ void k_bucket_starts(const u32 *bucket_local, const u64 *chunk_off /*4 planes*/, u64 n_chunks, u64 *bucket_start) {
   for (u32 b = blockIdx.x * blockDim.x + threadIdx.x; b < MHB_NUM_BUCKETS; b += gridDim.x * blockDim.x) {
     const u32 *bl = bucket_local + 5ull * b;
     u64 *o = bucket_start + 4ull * b;

@@ -50,6 +50,21 @@ def s2s_sort(a: torch.Tensor, b: torch.Tensor, n: int, k: int, first_hist=None, 
     return b if in_b.value else a
 
 
+def s2s_sort_emit(a: torch.Tensor, b: torch.Tensor, n: int, k: int, first_hist, bytes_out: torch.Tensor, table: torch.Tensor,
+                  totals: torch.Tensor, ws=None, cap_bytes: int | None = None):
+    """The seq2sdbg item sort and the SdBG emitter in one call (mhb_s2s_sort_emit) over the n items in a (b: the other
+    buffer; both are overwritten): the item stream goes to bytes_out (cap_bytes, default its size), the bucket table to
+    table (int64[65536 * 4]) and the totals to totals (int64[16])."""
+    L = lib.load()
+    need = L.mhb_s2s_sort_emit_workspace_bytes(n, k)
+    if ws is None or ws.numel() < need:
+        ws = torch.empty(need, dtype=torch.uint8, device=a.device)
+    cap = bytes_out.numel() if cap_bytes is None else cap_bytes
+    lib._check(L.mhb_s2s_sort_emit(_stream(), _ptr(a), _ptr(b), n, k, _ptr(first_hist), _ptr(bytes_out), cap, _ptr(table),
+                                   _ptr(totals), _ptr(ws), ws.numel()))
+    return totals
+
+
 class CountPlan:
     """`count` (extract -> sort -> solid edges [-> mercy bookkeeping]) for a fixed-length read library
     resident on the device."""
@@ -195,8 +210,8 @@ class S2sPlan:
         i32 = dict(dtype=torch.int32, device=device)
         self.a = torch.empty(n * self.W + 4, **i32)
         self.b = torch.empty(n * self.W + 4, **i32)
-        self.ws = torch.empty(L.mhb_s2s_sort_workspace_bytes(n, k), dtype=torch.uint8, device=device)
-        self.scratch = torch.empty(L.mhb_s2s_emit_scratch_bytes(n, k), dtype=torch.uint8, device=device)
+        # sort + emit workspace (mhb_s2s_sort_emit)
+        self.ws = torch.empty(L.mhb_s2s_sort_emit_workspace_bytes(n, k), dtype=torch.uint8, device=device)
         wpt = (k + 15) // 16
         self.cap_bytes = n * (4 + 4 * wpt) + 16
         self.bytes = torch.empty(self.cap_bytes, dtype=torch.uint8, device=device)
@@ -226,15 +241,15 @@ class S2sPlan:
                                           lib.s2s_sort_hist_byte(self.n_items, self.k)))
         if timed:
             ev[1].record()
-        srt = s2s_sort(self.a, self.b, self.n_items, self.k, self.hist0, self.ws)
-        if timed:
+        self._sort_emit(self.hist0)
+        if timed:  # sort and emit are one call: ev[1] -> ev[2] is both, ev[2] -> ev[3] is empty
             ev[2].record()
-        lib._check(self.L.mhb_s2s_emit(_stream(), _ptr(srt), self.n_items, self.k, _ptr(self.bytes), self.cap_bytes,
-                                       _ptr(self.table), _ptr(self.totals), _ptr(self.scratch), self.scratch.numel()))
-        if timed:
             ev[3].record()
             self.events.append(ev)
         return self.totals
+
+    def _sort_emit(self, hist):
+        s2s_sort_emit(self.a, self.b, self.n_items, self.k, hist, self.bytes, self.table, self.totals, self.ws, self.cap_bytes)
 
     def _run_pruned(self, edges: torch.Tensor, n_edges: int, aux: torch.Tensor, n_aux: int, timed: bool):
         cap = self.n_items
@@ -252,12 +267,9 @@ class S2sPlan:
             ev[1].record()
         # the histogram is of the byte a sort of `cap` items starts with; pass it only if this sort starts there too
         same = lib.s2s_sort_hist_byte(self.n_items, self.k) == lib.s2s_sort_hist_byte(cap, self.k)
-        srt = s2s_sort(self.a, self.b, self.n_items, self.k, self.hist0 if same else None, self.ws)
-        if timed:
+        self._sort_emit(self.hist0 if same else None)
+        if timed:  # sort and emit are one call: ev[1] -> ev[2] is both, ev[2] -> ev[3] is empty
             ev[2].record()
-        lib._check(self.L.mhb_s2s_emit(_stream(), _ptr(srt), self.n_items, self.k, _ptr(self.bytes), self.cap_bytes,
-                                       _ptr(self.table), _ptr(self.totals), _ptr(self.scratch), self.scratch.numel()))
-        if timed:
             ev[3].record()
             self.events.append(ev)
         return self.totals

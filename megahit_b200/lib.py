@@ -150,6 +150,7 @@ SYMBOLS = [
     "mhb_selftest_r2s_chunk_index", "mhb_selftest_r2s_stream_decide",
     "mhb_buildlib_host", "mhb_buildlib_free", "mhb_set_buildlib_chunk", "mhb_buildlib_run", "mhb_selftest_fastx",
     "mhb_s2s_sort", "mhb_s2s_sort_workspace_bytes", "mhb_s2s_sort_hist_byte", "mhb_s2s_sort_stats",
+    "mhb_s2s_sort_emit", "mhb_s2s_sort_emit_workspace_bytes",
     "mhb_selftest_s2s_local_key",
     "mhb_plan_read_chunks", "mhb_read_stream_decide", "mhb_set_read_chunk_limit", "mhb_read_stream_stats",
     "mhb_read_stream_times",
@@ -192,6 +193,10 @@ def load():
     L.mhb_s2s_sort_hist_byte.argtypes = [C.c_uint64, C.c_uint32]
     L.mhb_s2s_sort_stats.argtypes = [C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
     L.mhb_s2s_sort_stats.restype = None
+    L.mhb_s2s_sort_emit.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p,
+                                    C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
+    L.mhb_s2s_sort_emit_workspace_bytes.argtypes = [C.c_uint64, C.c_uint32]
+    L.mhb_s2s_sort_emit_workspace_bytes.restype = C.c_size_t
     L.mhb_selftest_s2s_local_key.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p]
     L.mhb_count_solid.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p,
                                   C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
