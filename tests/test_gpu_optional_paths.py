@@ -43,10 +43,6 @@ def test_fused_build_with_chunked_upload_matches_reference(name, k, m, gold):
         assert r["sdbg"] == gold["sdbg_sha256"] and r["edges"] == gold["edges_sha256"]
 
 
-# The new radix-pass variants (compact look-back descriptors, two-stream ranking) are deliberately NOT exercised here:
-# they contain spin-waits, and an unverified spin-wait does not belong in an unattended test run.  scripts/sort_sweep.py
-# checks and times them one process each, with a timeout (scripts/gpu_r2_first.sh).
-
 
 _CHILD_ROLL = r"""
 import json, os, sys
