@@ -64,6 +64,9 @@ int cap_class(uint32_t words) { return words <= 2 ? 2 : words <= 4 ? 4 : words <
 int iter_reads(const mhb_iterate_args *a, mhb_iterate_result *res, const ReadLibIndex &ix, const FlankTable &tab, int WCc,
                uint32_t w2, uint32_t KN, unsigned long long *cnt, bool stream, uint64_t *n_cand_out, uint64_t *n_edges_out);
 
+// mhb_selftest_iterate_narrow: the narrow flank index at a k whose wide records fit, to compare the two layouts
+bool g_iter_force_narrow = false;
+
 }  // namespace
 
 extern "C" int mhb_iterate_host(const mhb_iterate_args *a, mhb_iterate_result *res) {
@@ -73,7 +76,7 @@ extern "C" int mhb_iterate_host(const mhb_iterate_args *a, mhb_iterate_result *r
   // main_iterate.cpp:73-93: step even, 0 < step <= 28
   if (k < 9 || step == 0 || step > 28 || (step & 1)) return mhb_set_error(MHB_ERR_ARG, "iterate: invalid k / step");
   const uint32_t wk = div_ceil(K1, 16), w2 = words_per_edge(k + step), wn = div_ceil(KN, 16);
-  if (wk + 2 > 17 || w2 > 17) return mhb_set_error(MHB_ERR_ARG, "iterate: k + step + 1 = %u is beyond the 17-word records of the device sort", KN);
+  if (w2 > 17) return mhb_set_error(MHB_ERR_ARG, "iterate: k + step + 1 = %u is beyond the 17-word edge records of the device sort", KN);
   if (mhb_device_count() <= 0) return mhb_set_error(MHB_ERR_CUDA, "no CUDA device: libmhb has no CPU path");
   res->words_per_edge = w2;
   read_stream_stats_reset();
@@ -94,7 +97,7 @@ extern "C" int mhb_iterate_host(const mhb_iterate_args *a, mhb_iterate_result *r
   const int WCc = cap_class(std::max(wn, wk));
 
   // ---- flank index (FeedBatchContigs) ----
-  IBuf d_cw, d_co, d_cl, d_fl, d_fl2, d_ws, d_flag, d_off, d_bsum, d_cnt, d_tab, d_lut;
+  IBuf d_cw, d_co, d_cl, d_fl, d_fl2, d_val, d_ws, d_flag, d_off, d_bsum, d_cnt, d_tab, d_lut;
   CKR(d_cnt.alloc(64, "counters"));
   CK(cudaMemsetAsync(d_cnt.p, 0, 64, st));
   unsigned long long *cnt = d_cnt.as<unsigned long long>();
@@ -109,11 +112,19 @@ extern "C" int mhb_iterate_host(const mhb_iterate_args *a, mhb_iterate_result *r
     CK(cudaMemcpyAsync(d_co.p, a->contig_word_off, (a->n_contigs + 1) * 8, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_cl.p, a->contig_len, a->n_contigs * 4, cudaMemcpyHostToDevice, st));
     const uint64_t cap = 2 * a->n_contigs;
-    CKR(d_fl.alloc(cap * frw * 4 + 16, "flank records"));
-    CKR(d_fl2.alloc(cap * frw * 4 + 16, "flank records (sort buffer)"));
+    // wide: {key, ~val} records of frw words.  Narrow (frw beyond the 17-word records of the device sort): key + row
+    // index records of wk + 1 words, ~val in a side array.
+    const bool narrow = frw > 17 || g_iter_force_narrow;
+    const uint32_t srw = narrow ? wk + 1 : frw;
+    if (cap >= (1ull << 32) && narrow) return mhb_set_error(MHB_ERR_ARG, "iterate: too many contigs for 32-bit flank rows");
+    CKR(d_fl.alloc(cap * srw * 4 + 16, "flank records"));
+    CKR(d_fl2.alloc(cap * srw * 4 + 16, "flank records (sort buffer)"));
+    if (narrow) CKR(d_val.alloc(cap * 8 + 16, "flank values"));
     IterContigs cs{d_cw.as<u32>(), d_co.as<u64>(), d_cl.as<u32>(), a->n_contigs};
-#define M(WW) \
-  if (WCc == WW) k_iter_flanks<WW><<<igrid(cap, 256), 256, 0, st>>>(cs, k, step, wk, d_fl.as<u32>(), cnt);
+#define M(WW)                                                                                                    \
+  if (WCc == WW)                                                                                                 \
+    k_iter_flanks<WW><<<igrid(cap, 256), 256, 0, st>>>(cs, k, step, wk, d_fl.as<u32>(), narrow ? d_val.as<u64>() : nullptr, \
+                                                       cnt);
     IT_FOR_WC(M)
 #undef M
     CK_LAUNCH();
@@ -121,29 +132,40 @@ extern "C" int mhb_iterate_host(const mhb_iterate_args *a, mhb_iterate_result *r
     CK(cudaMemcpyAsync(&nf, cnt, 8, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     if (nf) {
-      // ascending on key, then on ~val: within a key the largest (ext_len, ext_seq) comes first and survives
       uint8_t bytes[72];
       uint32_t nb = 0;
-      for (uint32_t b = 0; b < 8; ++b) bytes[nb++] = (uint8_t)b;  // the two ~val words
       uint8_t kb[72];
-      const uint32_t nkb = top_bytes(wk, 2 * K1, kb);             // key bytes inside the key words ...
-      for (uint32_t i = 0; i < nkb; ++i) bytes[nb++] = (uint8_t)(kb[i] + 8);  // ... sit above the 8 val bytes
-      const size_t wsb = mhb_sort_workspace_bytes(nf, frw);
+      const uint32_t nkb = top_bytes(wk, 2 * K1, kb);  // key bytes inside the key words
+      if (narrow) {  // the key alone: the best value of each key is picked from its run afterwards
+        for (uint32_t i = 0; i < nkb; ++i) bytes[nb++] = (uint8_t)(kb[i] + 4);  // above the row-index word
+      } else {
+        // ascending on key, then on ~val: within a key the largest (ext_len, ext_seq) comes first and survives
+        for (uint32_t b = 0; b < 8; ++b) bytes[nb++] = (uint8_t)b;               // the two ~val words
+        for (uint32_t i = 0; i < nkb; ++i) bytes[nb++] = (uint8_t)(kb[i] + 8);  // the key bytes above them
+      }
+      const size_t wsb = mhb_sort_workspace_bytes(nf, srw);
       CKR(d_ws.alloc(wsb, "sort workspace"));
       int in_b = 0;
-      CKR(mhb_sort_records(st, d_fl.as<u32>(), d_fl2.as<u32>(), nf, frw, bytes, nb, nullptr, d_ws.p, wsb, &in_b));
+      if (narrow)
+        CKR(mhb_sort_records_relaxed(st, d_fl.as<u32>(), d_fl2.as<u32>(), nf, srw, bytes, nb, nullptr, d_ws.p, wsb, &in_b));
+      else
+        CKR(mhb_sort_records(st, d_fl.as<u32>(), d_fl2.as<u32>(), nf, srw, bytes, nb, nullptr, d_ws.p, wsb, &in_b));
       const u32 *sorted = in_b ? d_fl2.as<u32>() : d_fl.as<u32>();
       CKR(d_flag.alloc(nf * 4 + 16, "flags"));
       CKR(d_off.alloc(nf * 8 + 16, "offsets"));
       CKR(d_bsum.alloc((nf / 4096 + 4) * 8, "scan sums"));
-      k_iter_heads<<<igrid(nf, 256), 256, 0, st>>>(sorted, nf, frw, wk, d_flag.as<u32>());
+      k_iter_heads<<<igrid(nf, 256), 256, 0, st>>>(sorted, nf, srw, wk, d_flag.as<u32>());
       CK_LAUNCH();
       CKR(scan32(st, d_flag.as<u32>(), nf, d_off.as<u64>(), (uint64_t *)(cnt + 2), d_bsum.as<u64>()));
       unsigned long long nu = 0;
       CK(cudaMemcpyAsync(&nu, cnt + 2, 8, cudaMemcpyDeviceToHost, st));
       CK(cudaStreamSynchronize(st));
       CKR(d_tab.alloc((size_t)nu * frw * 4 + 16, "flank table"));
-      k_iter_compact<<<igrid(nf, 256), 256, 0, st>>>(sorted, nf, frw, d_flag.as<u32>(), d_off.as<u64>(), d_tab.as<u32>());
+      if (narrow)
+        k_iter_best<<<igrid(nf, 256), 256, 0, st>>>(sorted, nf, wk, d_val.as<u64>(), d_flag.as<u32>(), d_off.as<u64>(),
+                                                    d_tab.as<u32>());
+      else
+        k_iter_compact<<<igrid(nf, 256), 256, 0, st>>>(sorted, nf, frw, d_flag.as<u32>(), d_off.as<u64>(), d_tab.as<u32>());
       CK_LAUNCH();
       n_tab = nu;
     }
@@ -319,6 +341,15 @@ int iter_reads(const mhb_iterate_args *a, mhb_iterate_result *res, const ReadLib
 }
 }  // namespace
 
+// mhb_iterate_host with the narrow flank index (key + row index records, values in a side array) at any k: the layout
+// mhb_iterate_host takes only when k + 1 > 240, run where both fit so that the tests can compare the two
+extern "C" int mhb_selftest_iterate_narrow(const mhb_iterate_args *a, mhb_iterate_result *res) {
+  g_iter_force_narrow = true;
+  const int rc = mhb_iterate_host(a, res);
+  g_iter_force_narrow = false;
+  return rc;
+}
+
 // ------------------------------------------------------------------------------------------------
 // Host mirror for the CPU tests: the same __host__ __device__ building blocks (flank records, flank search, read
 // marking, edge emission) driven serially; std::sort stands in for the device radix sort.  Not a compute path of the
@@ -330,7 +361,7 @@ extern "C" int mhb_selftest_iterate(const mhb_iterate_args *a, mhb_iterate_resul
   const uint32_t k = a->k, step = a->step, K1 = k + 1, KN = k + step + 1;
   if (k < 9 || step == 0 || step > 28 || (step & 1)) return mhb_set_error(MHB_ERR_ARG, "iterate: invalid k / step");
   const uint32_t wk = div_ceil(K1, 16), w2 = words_per_edge(k + step), wn = div_ceil(KN, 16), frw = wk + 2;
-  if (frw > 17 || w2 > 17) return mhb_set_error(MHB_ERR_ARG, "iterate: record too wide");
+  if (w2 > 17) return mhb_set_error(MHB_ERR_ARG, "iterate: record too wide");
   res->words_per_edge = w2;
   const int WCc = cap_class(std::max(wn, wk));
   std::vector<std::vector<u32>> fl;

@@ -179,16 +179,44 @@ struct IterContigs {
   u64 n;
 };
 
+// vals == nullptr: records of wk + 2 words (key, ~val).  Otherwise the narrow layout for keys too wide for a
+// (wk + 2)-word sort record: wk key words + the 32-bit row index, and ~val of row i in vals[i].
 template <int WC>
 __global__ void __launch_bounds__(256) k_iter_flanks(IterContigs cs, u32 k, u32 step, u32 wk, u32 *__restrict__ recs,
-                                                    unsigned long long *__restrict__ cursor) {
+                                                    u64 *__restrict__ vals, unsigned long long *__restrict__ cursor) {
   for (u64 t = (u64)blockIdx.x * 256 + threadIdx.x; t < 2 * cs.n; t += (u64)gridDim.x * 256) {
     const u64 c = t >> 1;
     u32 rec[20];
     if (iter_flank_record<WC>(cs.words + cs.word_off[c], cs.len[c], k, step, (u32)(t & 1), wk, rec)) {
       const unsigned long long at = atomicAdd(cursor, 1ull);
-      for (u32 q = 0; q < wk + 2; ++q) recs[at * (wk + 2) + q] = rec[q];
+      if (vals) {
+        for (u32 q = 0; q < wk; ++q) recs[at * (wk + 1) + q] = rec[q];
+        recs[at * (wk + 1) + wk] = (u32)at;
+        vals[at] = ((u64)rec[wk] << 32) | rec[wk + 1];
+      } else {
+        for (u32 q = 0; q < wk + 2; ++q) recs[at * (wk + 2) + q] = rec[q];
+      }
     }
+  }
+}
+
+// Narrow flank records (wk key words + row index) sorted on the key, run heads flagged: per run of equal keys the
+// smallest ~val - the largest (ext_len, ext_seq), which the wide layout's sort on {key, ~val} puts first - goes with
+// the key into the (wk + 2)-word flank table at off[head].
+__global__ void __launch_bounds__(256) k_iter_best(const u32 *__restrict__ recs, u64 n, u32 wk, const u64 *__restrict__ vals,
+                                                  const u32 *__restrict__ flag, const u64 *__restrict__ off,
+                                                  u32 *__restrict__ out) {
+  for (u64 i = (u64)blockIdx.x * 256 + threadIdx.x; i < n; i += (u64)gridDim.x * 256) {
+    if (!flag[i]) continue;
+    u64 best = ~0ull;
+    for (u64 j = i; j < n && (j == i || !flag[j]); ++j) {
+      const u64 v = vals[recs[j * (wk + 1) + wk]];
+      best = v < best ? v : best;
+    }
+    u32 *o = out + off[i] * (wk + 2);
+    for (u32 q = 0; q < wk; ++q) o[q] = recs[i * (wk + 1) + q];
+    o[wk] = (u32)(best >> 32);
+    o[wk + 1] = (u32)best;
   }
 }
 

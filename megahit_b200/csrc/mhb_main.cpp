@@ -196,7 +196,7 @@ int main_iterate(int argc, char **argv, char **full_argv) {
   if (out.empty()) return fail_usage("No output prefix!", usage);
   o.k = (uint32_t)k;
   o.step = (uint32_t)step;
-  if (k < 9 || k + 1 > 240 || r == "-") {  // outside the device path (17-word records; stdin): the reference's CPU path
+  if (k < 9 || r == "-") {  // outside the device path (k < 9; stdin): the reference's CPU path
     fprintf(stderr, "megahit_b200: iterate with k = %d is forwarded to the reference\n", k);
     return forward_to_reference(full_argv);
   }
@@ -231,10 +231,6 @@ int main_read2sdbg(int argc, char **argv, char **full_argv) {
   o.output_prefix = out.c_str();
   if (lib.empty()) return fail_usage("No input file!", usage);
   if (o.host_mem == 0) return fail_usage("Please specify the host memory!", usage);
-  if (o.m > 1 && o.k > 237) {  // stage-1 records wider than the device sort handles: the reference's CPU path
-    fprintf(stderr, "megahit_b200: read2sdbg with k = %u and min count %d is forwarded to the reference\n", o.k, o.m);
-    return forward_to_reference(full_argv);
-  }
   if (int rc = mhb_read2sdbg_run(&o)) {
     fprintf(stderr, "FATAL megahit_b200: %s\n", mhb_last_error());
     (void)rc;

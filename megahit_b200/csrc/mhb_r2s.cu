@@ -16,7 +16,7 @@ using namespace mhb;
 
 // three-phase scan of mhb_device.cu
 int scan32(cudaStream_t st, const uint32_t *in, uint64_t n, uint64_t *out, uint64_t *total_dev, uint64_t *bsum);
-#define MHB_FOR_RW(M) M(3) M(4) M(5) M(6) M(7) M(8) M(9) M(10) M(11) M(12) M(13) M(14) M(15) M(16) M(17)
+#define MHB_FOR_RW(M) M(3) M(4) M(5) M(6) M(7) M(8) M(9) M(10) M(11) M(12) M(13) M(14) M(15) M(16) M(17) M(18)
 
 namespace {
 
@@ -196,11 +196,50 @@ size_t free_device_bytes() {
   return f;
 }
 
-// device bytes of one stage-1 pass over n records: records, sort buffer and workspace, kmsort scratch
-size_t s1_pass_bytes(uint64_t n, uint32_t RW) {
+// The stage-1 record layout of k (DESIGN.md §4.10).  Wide: NW key words + the 2 read_info words, sorted as whole
+// records.  Narrow, where that exceeds the 17-word records of mhb_sort_records (k > 237): NW key words + a 32-bit row
+// index into a side array of read_info; the bucket partition sorts (word 0, row) pairs and gathers the records.  Both
+// order records by the key bytes and the input order alone, so both give kmsort's permutation.
+bool g_r2s_force_narrow = false;  // mhb_selftest_read2sdbg_narrow: the narrow layout where the wide one fits
+struct S1Layout {
+  uint32_t NW, RW;
+  bool narrow;
+};
+S1Layout s1_layout(uint32_t k) {
+  const uint32_t NW = r2s_s1_key_words(k);
+  const bool narrow = NW + 2 > 17 || g_r2s_force_narrow;
+  return {NW, narrow ? NW + 1 : NW + 2, narrow};
+}
+// most records of one stage-1 round: the narrow layout's row index is 32 bits
+uint64_t s1_round_cap(const S1Layout &l) { return l.narrow ? 0xFFFFFFFFull : (1ull << 40) - 1; }
+// workspace of the bucket partition: the records themselves, or the (word 0, row) pairs
+size_t s1_ws_bytes(uint64_t n, const S1Layout &l) { return mhb_sort_workspace_bytes(n, l.narrow ? 2 : l.RW); }
+
+// device bytes of one stage-1 pass over n records: records, sort buffer and workspace, kmsort scratch; narrow: the
+// read_info side array and the two pair buffers
+size_t s1_pass_bytes(uint64_t n, const S1Layout &l) {
   const uint64_t seg_cap = n / (kKmInsertThreshold + 1) + 2;
-  return 2 * pad((size_t)n * RW * 4 + 16) + pad(mhb_sort_workspace_bytes(n, RW)) + pad((MHB_NUM_BUCKETS + 1) * 8) +
-         2 * pad(seg_cap * sizeof(KmSeg)) + 2 * pad((n / 32 + 2) * 4) + pad((size_t)n * 2 + 64) + 256;
+  return 2 * pad((size_t)n * l.RW * 4 + 16) + pad(s1_ws_bytes(n, l)) + pad((MHB_NUM_BUCKETS + 1) * 8) +
+         2 * pad(seg_cap * sizeof(KmSeg)) + 2 * pad((n / 32 + 2) * 4) + pad((size_t)n * 2 + 64) + 256 +
+         (l.narrow ? 3 * pad((size_t)n * 8 + 16) : 0);
+}
+
+// The stage-1 round plan: *max_n = 0 for one pass over all n_s1 records, else the most records of one round - the
+// cap `limit` (mhb_set_r2s_round_limit) or what fits `avail` next to the per-chunk scratch of max_reads reads - and
+// never more than s1_round_cap.  Returns non-zero when not even a one-record round fits.
+int s1_plan_round(const S1Layout &l, uint64_t n_s1, uint64_t max_reads, size_t avail, uint64_t limit, uint64_t *max_n) {
+  *max_n = 0;
+  const uint64_t cap = s1_round_cap(l);
+  if (!((limit && n_s1 > limit) || s1_pass_bytes(n_s1, l) > avail || n_s1 > cap)) return 0;
+  uint64_t mx = limit;
+  if (!mx) {
+    const size_t fixed = pad(max_reads * 4) + pad((max_reads + 1) * 8) + pad((max_reads / 4096 + 4) * 8) +
+                         pad(MHB_NUM_BUCKETS * 8) + 256;
+    mx = largest_round(n_s1, fixed, avail, [&](uint64_t n) { return s1_pass_bytes(n, l); });
+    if (!mx) return 1;
+  }
+  *max_n = std::min({mx, n_s1, cap});
+  return 0;
 }
 
 // device bytes of one stage-2 pass over n items: items, sort buffer and workspace, run collapse, emitter scratch + stream
@@ -406,17 +445,20 @@ ResidentPlan resident_plan(const PkgIndex &ix, uint64_t bin_words, int32_t m, bo
 // chunk cap is set.
 bool stream_decide(const ResidentPlan &p, const PkgIndex &ix, uint32_t k, int32_t m, size_t free_b, uint64_t chunk_limit) {
   const double room = free_b > p.resident ? 0.92 * (double)(free_b - p.resident) : 0.0;
-  const uint32_t RW = r2s_s1_key_words(k) + 2, W = s2s_record_words(k);
+  const uint32_t W = s2s_record_words(k);
   const size_t s1_fixed = pad(ix.n_reads * 4) + pad((ix.n_reads + 1) * 8) + pad((ix.n_reads / 4096 + 4) * 8) +
                           pad(MHB_NUM_BUCKETS * 8) + 256;
-  const bool no_round = (m > 1 && ix.n_s1 && (double)(s1_fixed + s1_pass_bytes(1, RW)) > room) ||
+  const bool no_round = (m > 1 && ix.n_s1 && (double)(s1_fixed + s1_pass_bytes(1, s1_layout(k))) > room) ||
                         (ix.n_edges && (double)s2_pass_bytes(1, W, k) > room);
   return mhb_read_stream_decide(p.resident + p.upload, free_b, no_round ? 1 : 0, chunk_limit) != 0;
 }
 
 // ---- stage 1 on the device: is_solid bits, mercy planes, multiplicity histogram ----
+struct S1Side {  // the narrow layout's read_info side array and the pair buffers of its bucket partition
+  DevBuf info, pa, pb;
+};
 int s1_sort_post(cudaStream_t st, const PkgView &pv, uint32_t k, int32_t m, bool need_mercy, const S1Out &out,
-                 unsigned long long *d_mul_hist, PhaseTrace &tr, BigBufs &big, uint64_t n);
+                 unsigned long long *d_mul_hist, PhaseTrace &tr, BigBufs &big, S1Side &side, uint64_t n);
 
 // Stage 1 in rounds over contiguous ranges of bucket ids, each of at most max_n records; *n_rounds counts the
 // non-empty ones.  max_n == 0: one pass, the one range over all bucket ids, known without a pass: each chunk's records
@@ -429,15 +471,21 @@ int s1_sort_post(cudaStream_t st, const PkgView &pv, uint32_t k, int32_t m, bool
 int run_stage1(cudaStream_t st, const EachChunk &each, const PkgView &shape, const PkgIndex &ix, uint64_t chunk_reads,
                uint32_t k, int32_t m, bool need_mercy, const S1Out &out, unsigned long long *d_mul_hist, PhaseTrace &tr,
                BigBufs &big, uint64_t max_n, size_t min_rec_bytes, size_t min_ws_bytes, uint32_t *n_rounds) {
-  const uint32_t NW = r2s_s1_key_words(k), RW = NW + 2;
+  const S1Layout l = s1_layout(k);
+  const uint32_t NW = l.NW, RW = l.RW;
   const bool one_pass = max_n == 0;
   if (one_pass) max_n = ix.n_s1;
-  if (RW > 17)
-    return mhb_set_error(MHB_ERR_ARG, "read2sdbg: stage 1 supports k <= 237 (record of %u words > 17)", RW);
-  if (max_n >= (1ull << 40)) return mhb_set_error(MHB_ERR_ARG, "read2sdbg: too many stage-1 records for one round");
+  if (max_n > s1_round_cap(l)) return mhb_set_error(MHB_ERR_ARG, "read2sdbg: too many stage-1 records for one round");
   CKR(big.a.ensure(std::max((size_t)max_n * RW * 4 + 16, min_rec_bytes), "records"));
   CKR(big.b.ensure(std::max((size_t)max_n * RW * 4 + 16, min_rec_bytes), "records (sort buffer)"));
-  CKR(big.ws.ensure(std::max(mhb_sort_workspace_bytes(max_n, RW), min_ws_bytes), "sort workspace"));
+  CKR(big.ws.ensure(std::max(s1_ws_bytes(max_n, l), min_ws_bytes), "sort workspace"));
+  S1Side side;
+  if (l.narrow) {
+    CKR(side.info.alloc((size_t)max_n * 8 + 16, "stage-1 read_info"));
+    CKR(side.pa.alloc((size_t)max_n * 8 + 16, "bucket partition pairs"));
+    CKR(side.pb.alloc((size_t)max_n * 8 + 16, "bucket partition pairs (sort buffer)"));
+  }
+  u64 *d_info = l.narrow ? side.info.as<u64>() : nullptr;
   std::vector<std::pair<uint32_t, uint32_t>> ranges = {{0u, 65535u}};
   DevBuf per_read, off, bsum, total;
   if (!one_pass) {
@@ -453,7 +501,7 @@ int run_stage1(cudaStream_t st, const EachChunk &each, const PkgView &shape, con
 #define M(WW)   \
   if (NW == WW) \
     k_r2s_s1_range<WW, kS1Hist><<<grid, 256, 0, st>>>(c.pv, k, 0, 65535, h16.as<unsigned long long>(), nullptr, nullptr, nullptr);
-      MHB_FOR_W(M)
+      MHB_FOR_WR(M)
 #undef M
       CK_LAUNCH();
       return MHB_OK;
@@ -471,10 +519,10 @@ int run_stage1(cudaStream_t st, const EachChunk &each, const PkgView &shape, con
     if (int rc_ = each([&](const PkgChunk &c) -> int {
       if (one_pass) {
         if (c.n_s1) {
-          u32 *dst = big.a.as<u32>() + c.s1_0 * RW;
-#define M(WW) \
-  if (NW == WW) k_r2s_s1_extract<WW><<<grid_for(c.n_s1, 256), 256, 0, st>>>(c.pv, k, dst, c.n_s1);
-          MHB_FOR_W(M)
+#define M(WW)                                                                                                      \
+  if (NW == WW)                                                                                                    \
+    k_r2s_s1_extract<WW><<<grid_for(c.n_s1, 256), 256, 0, st>>>(c.pv, k, big.a.as<u32>(), d_info, c.s1_0, c.n_s1);
+          MHB_FOR_WR(M)
 #undef M
           CK_LAUNCH();
         }
@@ -486,7 +534,7 @@ int run_stage1(cudaStream_t st, const EachChunk &each, const PkgView &shape, con
   if (NW == WW)                                                                                                        \
     k_r2s_s1_range<WW, kS1Count><<<grid, 256, 0, st>>>(c.pv, k, rg.first, rg.second, nullptr, per_read.as<u32>(), nullptr, \
                                                        nullptr);
-      MHB_FOR_W(M)
+      MHB_FOR_WR(M)
 #undef M
       CK_LAUNCH();
       CKR(scan32(st, per_read.as<u32>(), c.pv.n_reads, off.as<u64>(), total.as<u64>(), bsum.as<u64>()));
@@ -496,12 +544,12 @@ int run_stage1(cudaStream_t st, const EachChunk &each, const PkgView &shape, con
       if (n + t > max_n)
         return mhb_set_error(MHB_ERR_CUDA, "read2sdbg: internal: round of %llu stage-1 records exceeds its plan (%llu)",
                              (unsigned long long)(n + t), (unsigned long long)max_n);
-      if (t) {
-        u32 *dst = big.a.as<u32>() + n * RW;  // after the records of the chunks before: read order
+      if (t) {  // rows n on: after the records of the chunks before, read order
 #define M(WW)                                                                                                          \
   if (NW == WW)                                                                                                        \
-    k_r2s_s1_range<WW, kS1Write><<<grid, 256, 0, st>>>(c.pv, k, rg.first, rg.second, nullptr, nullptr, off.as<u64>(), dst);
-        MHB_FOR_W(M)
+    k_r2s_s1_range<WW, kS1Write><<<grid, 256, 0, st>>>(c.pv, k, rg.first, rg.second, nullptr, nullptr, off.as<u64>(), \
+                                                       big.a.as<u32>(), d_info, n);
+        MHB_FOR_WR(M)
 #undef M
         CK_LAUNCH();
       }
@@ -512,7 +560,7 @@ int run_stage1(cudaStream_t st, const EachChunk &each, const PkgView &shape, con
     seen += n;
     if (n == 0) continue;
     tr.mark("s1.extract");
-    CKR(s1_sort_post(st, shape, k, m, need_mercy, out, d_mul_hist, tr, big, n));
+    CKR(s1_sort_post(st, shape, k, m, need_mercy, out, d_mul_hist, tr, big, side, n));
     ++*n_rounds;
   }
   if (seen != ix.n_s1)
@@ -523,11 +571,12 @@ int run_stage1(cudaStream_t st, const EachChunk &each, const PkgView &shape, con
 
 // stable bucket partition, kmsort emulation and Lv2Postprocess of the n records in big.a
 int s1_sort_post(cudaStream_t st, const PkgView &pv, uint32_t k, int32_t m, bool need_mercy, const S1Out &out,
-                 unsigned long long *d_mul_hist, PhaseTrace &tr, BigBufs &big, uint64_t n) {
-  const uint32_t NW = r2s_s1_key_words(k), RW = NW + 2;
+                 unsigned long long *d_mul_hist, PhaseTrace &tr, BigBufs &big, S1Side &side, uint64_t n) {
+  const S1Layout l = s1_layout(k);
+  const uint32_t NW = l.NW, RW = l.RW;
   DevBuf bstart, segs0, segs1, counter, bnd;
   DevBuf &a = big.a, &b = big.b, &ws = big.ws;
-  const size_t ws_bytes = mhb_sort_workspace_bytes(n, RW);
+  const size_t ws_bytes = s1_ws_bytes(n, l);
   CKR(bstart.alloc((MHB_NUM_BUCKETS + 1) * 8, "bucket bounds"));
   const uint64_t seg_cap = n / (kKmInsertThreshold + 1) + 2;
   CKR(segs0.alloc(seg_cap * sizeof(KmSeg), "kmsort ranges"));
@@ -537,9 +586,21 @@ int s1_sort_post(cudaStream_t st, const PkgView &pv, uint32_t k, int32_t m, bool
   CK(cudaMemsetAsync(bnd.p, 0, (n / 32 + 2) * 4, st));
   // the reference's bucket input order: records of one 16-bit bucket in global read order = a STABLE sort on the two
   // leading key bytes (base_engine.cpp:323-348 fills every bucket thread by thread, i.e. in read order)
-  const uint8_t bytes[2] = {(uint8_t)(4 * RW - 2), (uint8_t)(4 * RW - 1)};
   int in_b = 0;
-  CKR(mhb_sort_records(st, a.as<u32>(), b.as<u32>(), n, RW, bytes, 2, nullptr, ws.p, ws_bytes, &in_b));
+  if (l.narrow) {
+    const uint8_t bytes[2] = {6, 7};  // the two leading bytes of a (word 0, row) pair
+    k_r2s_s1_pairs<<<grid_for(n, 256), 256, 0, st>>>(a.as<u32>(), n, RW, side.pa.as<u32>());
+    CK_LAUNCH();
+    int in_pb = 0;
+    CKR(mhb_sort_records(st, side.pa.as<u32>(), side.pb.as<u32>(), n, 2, bytes, 2, nullptr, ws.p, ws_bytes, &in_pb));
+    k_r2s_s1_gather<<<grid_for(n * RW, 256), 256, 0, st>>>(a.as<u32>(), in_pb ? side.pb.as<u32>() : side.pa.as<u32>(), n,
+                                                           RW, b.as<u32>());
+    CK_LAUNCH();
+    in_b = 1;
+  } else {
+    const uint8_t bytes[2] = {(uint8_t)(4 * RW - 2), (uint8_t)(4 * RW - 1)};
+    CKR(mhb_sort_records(st, a.as<u32>(), b.as<u32>(), n, RW, bytes, 2, nullptr, ws.p, ws_bytes, &in_b));
+  }
   u32 *recs = in_b ? b.as<u32>() : a.as<u32>();
   tr.mark("s1.partition");
   k_r2s_bucket_bounds<<<(MHB_NUM_BUCKETS + 1 + 255) / 256, 256, 0, st>>>(recs, n, RW, bstart.as<u64>());
@@ -634,7 +695,8 @@ int s1_sort_post(cudaStream_t st, const PkgView &pv, uint32_t k, int32_t m, bool
   tr.mark("s1.kmsort.finish");
 #define M(WW)                                                                                                          \
   if (RW == WW)                                                                                                        \
-    k_r2s_s1_post<WW><<<grid_for(n, 256, 32), 256, 0, st>>>(recs, n, NW, k, m, pv, out, need_mercy ? 1 : 0, d_mul_hist);
+    k_r2s_s1_post<WW><<<grid_for(n, 256, 32), 256, 0, st>>>(recs, l.narrow ? side.info.as<u64>() : nullptr, n, NW, k, m, \
+                                                            pv, out, need_mercy ? 1 : 0, d_mul_hist);
   MHB_FOR_RW(M)
 #undef M
   CK_LAUNCH();
@@ -909,13 +971,13 @@ extern "C" int mhb_read2sdbg_host(const mhb_build_args *args, mhb_build_result *
   if (!res->bucket_table || !res->counting) return mhb_set_error(MHB_ERR_NOMEM, "host malloc failed");
 
   // ---- device memory: the package resident, or streamed from host memory in chunks (DESIGN.md §4.9) ----
-  const uint32_t RW = r2s_s1_key_words(k) + 2;
+  const S1Layout l1 = s1_layout(k);
   const bool s1_runs = m > 1 && ix.n_s1 > 0;
   const bool mercy = args->need_mercy && m > 1;
   const uint64_t bit_words = ix.n_bases / 32 + 2;
   const ResidentPlan rp = resident_plan(ix, args->bin_words, m, mercy);
   const uint64_t est_items = (uint64_t)(2.2 * (double)ix.n_edges) + 1024;
-  const size_t s1_one = s1_runs ? s1_pass_bytes(ix.n_s1, RW) : 0;
+  const size_t s1_one = s1_runs ? s1_pass_bytes(ix.n_s1, l1) : 0;
   const size_t s2_est = ix.n_edges ? s2_pass_bytes(est_items, W, k) : 0;
   // the arena earlier host-level calls keep is reclaimable: free it when it stands in the way of this call
   if (mhb_arena_bytes() &&
@@ -976,20 +1038,12 @@ extern "C" int mhb_read2sdbg_host(const mhb_build_args *args, mhb_build_result *
     const size_t avail = (size_t)(0.92 * (double)free_device_bytes());
     uint64_t max_n = 0;  // one pass
     size_t min_rec = 0, min_ws = 0;
-    if ((g_r2s_s1_limit && ix.n_s1 > g_r2s_s1_limit) || s1_one > avail) {
-      max_n = g_r2s_s1_limit;
-      if (!max_n) {
-        const size_t fixed = pad(src.max_reads * 4) + pad((src.max_reads + 1) * 8) + pad((src.max_reads / 4096 + 4) * 8) +
-                             pad(MHB_NUM_BUCKETS * 8) + 256;
-        max_n = largest_round(ix.n_s1, fixed, avail, [&](uint64_t n) { return s1_pass_bytes(n, RW); });
-        if (!max_n)
-          return mhb_set_error(MHB_ERR_NOMEM, "read2sdbg: %s no room for a stage-1 round (%zu bytes free)", held, avail);
-      }
-      max_n = std::min(max_n, ix.n_s1);
-    } else {
+    if (s1_plan_round(l1, ix.n_s1, src.max_reads, avail, g_r2s_s1_limit, &max_n))
+      return mhb_set_error(MHB_ERR_NOMEM, "read2sdbg: %s no room for a stage-1 round (%zu bytes free)", held, avail);
+    if (max_n == 0) {
       // size the shared buffers for stage 2 as well when that fits: ~1.6 items per edge position on a 30x library, 2.2
       // to be safe (stage 2 reallocates when its count launch says more)
-      const size_t rec1 = pad((size_t)ix.n_s1 * RW * 4 + 16), ws1 = pad(mhb_sort_workspace_bytes(ix.n_s1, RW));
+      const size_t rec1 = pad((size_t)ix.n_s1 * l1.RW * 4 + 16), ws1 = pad(s1_ws_bytes(ix.n_s1, l1));
       const size_t rec2 = pad((size_t)est_items * W * 4 + 16), ws2 = pad(mhb_s2s_sort_workspace_bytes(est_items, k));
       if (s1_one - 2 * rec1 - ws1 + 2 * std::max(rec1, rec2) + std::max(ws1, ws2) <= avail) {
         min_rec = (size_t)est_items * W * 4 + 16;
@@ -1050,7 +1104,7 @@ extern "C" int mhb_selftest_r2s_s1_record(const uint32_t *pkg_words, uint32_t nw
     make_s1_record<WW>(pkg_words, nwords, L, k, p, want, base_off, rec); \
     memcpy(rec_out, rec, sizeof(rec));                              \
   }
-  MHB_FOR_W(M)
+  MHB_FOR_WR(M)
 #undef M
   return MHB_OK;
 }
@@ -1073,9 +1127,8 @@ extern "C" int mhb_selftest_r2s_item(const uint32_t *pkg_words, uint32_t nwords,
 
 // kmsort emulation of ONE bucket on the host, exactly as the kernels do it (records of nw + 2 words): radix levels that
 // mark the range starts, then the insertion sorts of all marked small ranges
-extern "C" int mhb_selftest_kmsort(uint32_t *recs, uint64_t n, uint32_t nw) {
-  const uint32_t RW = nw + 2;
-  if (nw < 1 || RW > 17 || n >= (1ull << 32)) return mhb_set_error(MHB_ERR_ARG, "bad args");
+namespace {
+int kmsort_host(uint32_t *recs, uint64_t n, uint32_t nw, uint32_t RW) {
   if (n <= 1) return MHB_OK;
   std::vector<KmSeg> cur, nxt;
   std::vector<u32> count(256), last(256), bnd(n / 32 + 2, 0u);
@@ -1114,9 +1167,7 @@ extern "C" int mhb_selftest_kmsort(uint32_t *recs, uint64_t n, uint32_t nw) {
 // km_insertion_idx on the index array of a staged range): level 0 gathers the bucket into a second buffer, later levels
 // stage ranges of at most `wcap` records (0 = km_wcap of the record width, as on the device), larger ones and buckets
 // above `cap` tags take the in-place walk; what is left unsorted is marked and finished by insertion.
-extern "C" int mhb_selftest_kmsort_smem(uint32_t *recs, uint64_t n, uint32_t nw, uint32_t cap, uint32_t wcap) {
-  const uint32_t RW = nw + 2;
-  if (nw < 1 || RW > 17 || n >= (1ull << 32)) return mhb_set_error(MHB_ERR_ARG, "bad args");
+int kmsort_smem_host(uint32_t *recs, uint64_t n, uint32_t nw, uint32_t RW, uint32_t cap, uint32_t wcap) {
   if (n <= 1) return MHB_OK;
   std::vector<KmSeg> cur, nxt;
   std::vector<u32> cnt(256), last(256), beg(256), bnd(n / 32 + 2, 0u), todo(n / 32 + 2, 0u);
@@ -1200,6 +1251,23 @@ extern "C" int mhb_selftest_kmsort_smem(uint32_t *recs, uint64_t n, uint32_t nw,
 #undef M
   return MHB_OK;
 }
+}  // namespace
+
+extern "C" int mhb_selftest_kmsort(uint32_t *recs, uint64_t n, uint32_t nw) {
+  if (nw < 1 || nw + 2 > 17 || n >= (1ull << 32)) return mhb_set_error(MHB_ERR_ARG, "bad args");
+  return kmsort_host(recs, n, nw, nw + 2);
+}
+
+extern "C" int mhb_selftest_kmsort_smem(uint32_t *recs, uint64_t n, uint32_t nw, uint32_t cap, uint32_t wcap) {
+  if (nw < 1 || nw + 2 > 17 || n >= (1ull << 32)) return mhb_set_error(MHB_ERR_ARG, "bad args");
+  return kmsort_smem_host(recs, n, nw, nw + 2, cap, wcap);
+}
+
+// The same two forms on the narrow stage-1 layout: records of nw key words + one row-index word (nw <= 17)
+extern "C" int mhb_selftest_kmsort_narrow(uint32_t *recs, uint64_t n, uint32_t nw, int smem, uint32_t cap, uint32_t wcap) {
+  if (nw < 2 || nw > 17 || n >= (1ull << 32)) return mhb_set_error(MHB_ERR_ARG, "bad args");
+  return smem ? kmsort_smem_host(recs, n, nw, nw + 1, cap, wcap) : kmsort_host(recs, n, nw, nw + 1);
+}
 
 // stage-1 Lv2Postprocess + the mercy step on host arrays (one sorted bucket / one read), same code as the kernels
 extern "C" int mhb_selftest_r2s_s1_group(const uint32_t *recs, uint64_t n, uint32_t k, int32_t m, uint32_t fixed_len,
@@ -1213,7 +1281,7 @@ extern "C" int mhb_selftest_r2s_s1_group(const uint32_t *recs, uint64_t n, uint3
   S1Out o{is_solid, no_in, no_out, any};
   for (u64 g = 0; g < n;) {
     u32 hv[16], nh;
-    g = s1_group(recs, n, g, rw, nw, k, m, pv, o, need_mercy != 0, hv, nh);
+    g = s1_group(recs, nullptr, n, g, rw, nw, k, m, pv, o, need_mercy != 0, hv, nh);
     for (u32 q = 0; q < nh; ++q) counting[hv[q] > MHB_MAX_MUL ? MHB_MAX_MUL : hv[q]]++;
   }
   return MHB_OK;
@@ -1298,5 +1366,27 @@ extern "C" int mhb_selftest_r2s_stream_decide(uint64_t n_reads, uint64_t bin_wor
   *resident_out = p.resident;
   *upload_out = p.upload;
   *stream_out = stream_decide(p, ix, k, m, free_bytes, chunk_limit) ? 1 : 0;
+  return MHB_OK;
+}
+
+// mhb_read2sdbg_host with the narrow stage-1 layout (key + row index records, read_info in a side array) at any k: the
+// layout mhb_read2sdbg_host takes only for k > 237, run where both fit so that the tests can compare the two
+extern "C" int mhb_selftest_read2sdbg_narrow(const mhb_build_args *args, mhb_build_result *res) {
+  g_r2s_force_narrow = true;
+  const int rc = mhb_read2sdbg_host(args, res);
+  g_r2s_force_narrow = false;
+  return rc;
+}
+
+// The stage-1 round plan of mhb_read2sdbg_host for n_s1 records of k, chunks of at most max_reads reads, avail free
+// device bytes and the round cap `limit` (0 = none): *max_n_out = 0 for one pass, else the most records of a round;
+// *rec_words_out = words per stage-1 sort record.
+extern "C" int mhb_selftest_r2s_s1_plan(uint32_t k, uint64_t n_s1, uint64_t max_reads, uint64_t avail, uint64_t limit,
+                                        uint64_t *max_n_out, uint32_t *rec_words_out) {
+  if (k < 9 || k > MHB_MAX_K) return mhb_set_error(MHB_ERR_ARG, "bad args");
+  const S1Layout l = s1_layout(k);
+  *rec_words_out = l.RW;
+  if (s1_plan_round(l, n_s1, max_reads, (size_t)avail, limit, max_n_out))
+    return mhb_set_error(MHB_ERR_NOMEM, "read2sdbg: no room for a stage-1 round");
   return MHB_OK;
 }

@@ -369,10 +369,16 @@ struct S1Out {
   u32 *any;
 };
 
+// read_info (full_offset<<6 | prev<<3 | next) of a stage-1 record: its two payload words, or - narrow layout, info !=
+// nullptr - the side-array entry its row index (the word after the nw key words) points at
+MHB_HD u64 s1_info(const u32 *r, u32 nw, const u64 *info) {
+  return info ? info[r[nw]] : ((u64)r[nw] << 32) | r[nw + 1];
+}
+
 // walks the group [g0, end) twice: tallies, then per-record outputs.  Returns the group's end.  hist_vals[0..n_hist)
 // (room for 16) receives the occurrence count of every distinct (k+1)-mer of the group (edge_counter_.Add, :430-432).
-MHB_HD u64 s1_group(const u32 *recs, u64 n, u64 g0, u32 rw, u32 nw, u32 k, int m, const PkgView &pv, const S1Out &o,
-                    bool need_mercy, u32 *hist_vals, u32 &n_hist) {
+MHB_HD u64 s1_group(const u32 *recs, const u64 *info, u64 n, u64 g0, u32 rw, u32 nw, u32 k, int m, const PkgView &pv,
+                    const S1Out &o, bool need_mercy, u32 *hist_vals, u32 &n_hist) {
   n_hist = 0;
   const u32 *first = recs + g0 * rw;
   u32 cht[40];  // count_head_tail, index head<<3|tail <= 36
@@ -384,7 +390,7 @@ MHB_HD u64 s1_group(const u32 *recs, u64 n, u64 g0, u32 rw, u32 nw, u32 k, int m
   }
   // :393-401: prev/next of the FIRST record stand in for every member, so has_in / has_out exist only when the first
   // record has a prev / next at all, and then count heads / tails over the whole group
-  const u32 pn_first = first[nw + 1] & 63u;
+  const u32 pn_first = (u32)s1_info(first, nw, info) & 63u;
   u32 has_in = 0, has_out = 0, l_has_out = 0, r_has_in = 0;
   for (u32 j = 0; j < 4; ++j) {
     u32 heads = 0, tails = 0;
@@ -411,9 +417,9 @@ MHB_HD u64 s1_group(const u32 *recs, u64 n, u64 g0, u32 rw, u32 nw, u32 k, int m
       if (both) hist_vals[n_hist++] = cht[ht];
     }
     if (!both && !need_mercy) continue;
-    const u64 info = (((u64)r[nw] << 32) | r[nw + 1]) >> 6;
-    const u32 strand = (u32)(info & 1);
-    const u64 pos = info >> 1;  // full offset of the (k-1)-mer; the (k+1)-mer head S tail starts one base earlier
+    const u64 full = s1_info(r, nw, info) >> 6;
+    const u32 strand = (u32)(full & 1);
+    const u64 pos = full >> 1;  // full offset of the (k-1)-mer; the (k+1)-mer head S tail starts one base earlier
     const bool solid = both && cht[ht] >= (u32)m;
     if (solid) bit_or(o.is_solid, pos - 1);  // :441
     if (!need_mercy) continue;
@@ -543,9 +549,25 @@ __global__ void __launch_bounds__(256) k_r2s_chunk_geom(const u32 *__restrict__ 
   }
 }
 
-// stage-1 records in the reference's bucket input order: record s1_off[r] + e
+// row i of a stage-1 buffer: the whole record (info == nullptr), or the narrow layout - the NW key words and the row
+// index i, read_info in info[i]
 template <int NW>
-__global__ void __launch_bounds__(256) k_r2s_s1_extract(PkgView pv, u32 k, u32 *__restrict__ recs, u64 n_recs) {
+__device__ __forceinline__ void s1_store(u32 *recs, u64 *info, u64 i, const u32 (&rec)[NW + 2]) {
+  if (!info) {
+    st_rec<NW + 2>(recs, i, rec);
+    return;
+  }
+  u32 *o = recs + i * (NW + 1);
+#pragma unroll
+  for (int j = 0; j < NW; ++j) o[j] = rec[j];
+  o[NW] = (u32)i;
+  info[i] = ((u64)rec[NW] << 32) | rec[NW + 1];
+}
+
+// stage-1 records in the reference's bucket input order: record s1_off[r] + e at row at0 + s1_off[r] + e
+template <int NW>
+__global__ void __launch_bounds__(256) k_r2s_s1_extract(PkgView pv, u32 k, u32 *__restrict__ recs, u64 *__restrict__ info,
+                                                       u64 at0, u64 n_recs) {
   for (u64 t = (u64)blockIdx.x * 256 + threadIdx.x; t < n_recs; t += (u64)gridDim.x * 256) {
     u64 r;
     u32 e;
@@ -562,7 +584,7 @@ __global__ void __launch_bounds__(256) k_r2s_s1_extract(PkgView pv, u32 k, u32 *
     s1_emission(L, k, e, p, want);
     u32 rec[NW + 2];
     make_s1_record<NW>(pv.ptr(r), div_ceil(L, 16), L, k, p, want, pv.base(r), rec);
-    st_rec<NW + 2>(recs, t, rec);
+    s1_store<NW>(recs, info, at0 + t, rec);
   }
 }
 
@@ -572,16 +594,17 @@ __global__ void __launch_bounds__(256) k_r2s_s1_extract(PkgView pv, u32 k, u32 *
 // k_r2s_s1_extract gives them, so the stable bucket partition and kmsort see the reference's bucket input order.
 //   kS1Hist : hist[bucket id] += 1 over the whole library (the round planner's input)
 //   kS1Count: per_read[r] = number of records of read r with bucket id in [lo, hi]
-//   kS1Write: those records, stored from off[r] on (off = exclusive scan of the counts)
+//   kS1Write: those records, stored at rows at0 + off[r] on (off = exclusive scan of the counts)
 enum { kS1Hist = 0, kS1Count = 1, kS1Write = 2 };
 template <int NW, int MODE>
 __global__ void __launch_bounds__(256) k_r2s_s1_range(PkgView pv, u32 k, u32 lo, u32 hi, unsigned long long *__restrict__ hist,
-                                                     u32 *__restrict__ per_read, const u64 *__restrict__ off, u32 *__restrict__ recs) {
+                                                     u32 *__restrict__ per_read, const u64 *__restrict__ off, u32 *__restrict__ recs,
+                                                     u64 *__restrict__ info = nullptr, u64 at0 = 0) {
   const u32 lane = lane_id(), lt = lanemask_lt();
   const u64 n_warps = (u64)gridDim.x * 8;
   for (u64 r = ((u64)blockIdx.x * 256 + threadIdx.x) >> 5; r < pv.n_reads; r += n_warps) {
     const u32 L = pv.L(r);
-    u64 run = MODE == kS1Write ? off[r] : 0;
+    u64 run = MODE == kS1Write ? at0 + off[r] : 0;
     if (L >= k + 1) {
       const u32 n_e = L - k + 4, nwords = div_ceil(L, 16);
       const u32 *s = pv.ptr(r);
@@ -600,11 +623,28 @@ __global__ void __launch_bounds__(256) k_r2s_s1_range(PkgView pv, u32 k, u32 lo,
         }
         if (MODE == kS1Hist) continue;
         const u32 mask = __ballot_sync(0xffffffffu, in);
-        if (MODE == kS1Write && in) st_rec<NW + 2>(recs, run + __popc(mask & lt), rec);
+        if (MODE == kS1Write && in) s1_store<NW>(recs, info, run + __popc(mask & lt), rec);
         run += __popc(mask);
       }
     }
     if (MODE == kS1Count && lane == 0) per_read[r] = (u32)run;
+  }
+}
+
+// The bucket partition of the narrow layout, whose records may be wider than mhb_sort_records takes: (word 0, row)
+// pairs are sorted stably on the bucket id, then the records gathered in that order.  Row r sits at position r and its
+// index word says r, so the gathered records keep their side-array rows.
+__global__ void __launch_bounds__(256) k_r2s_s1_pairs(const u32 *__restrict__ recs, u64 n, u32 rw, u32 *__restrict__ pairs) {
+  for (u64 i = (u64)blockIdx.x * 256 + threadIdx.x; i < n; i += (u64)gridDim.x * 256) {
+    pairs[2 * i] = recs[i * rw];
+    pairs[2 * i + 1] = (u32)i;
+  }
+}
+__global__ void __launch_bounds__(256) k_r2s_s1_gather(const u32 *__restrict__ recs, const u32 *__restrict__ pairs, u64 n,
+                                                      u32 rw, u32 *__restrict__ out) {
+  for (u64 t = (u64)blockIdx.x * 256 + threadIdx.x; t < n * rw; t += (u64)gridDim.x * 256) {
+    const u64 i = t / rw;
+    out[t] = recs[(u64)pairs[2 * i + 1] * rw + (t - i * rw)];
   }
 }
 
@@ -766,7 +806,10 @@ __global__ void __launch_bounds__(128) k_r2s_km_bucket(const u32 *__restrict__ i
 static constexpr int kKmWarps = 8;
 template <int RW>
 __host__ __device__ constexpr size_t km_warp_smem() {  // per warp: staged records, index array, tags, 3 x 256 counters
-  return (size_t)km_wcap(RW) * RW * 4 + (size_t)km_wcap(RW) * 2 + (size_t)((km_wcap(RW) + 3) & ~3u) + 3 * 256 * 4;
+  // rounded up to 16 bytes: the next warp's staged records and counters start there (an odd km_wcap would leave them
+  // 2 bytes off a word boundary)
+  return ((size_t)km_wcap(RW) * RW * 4 + (size_t)km_wcap(RW) * 2 + (size_t)((km_wcap(RW) + 3) & ~3u) + 3 * 256 * 4 + 15) &
+         ~(size_t)15;
 }
 
 template <int RW>
@@ -858,10 +901,12 @@ __global__ void __launch_bounds__(kKmWarps * 32) k_r2s_km_warp(u32 *__restrict__
 
 static constexpr int kS1HistSmem = 2048;
 
-// Lv2Postprocess of stage 1: the thread whose record opens a (k-1)-mer group walks it
+// Lv2Postprocess of stage 1: the thread whose record opens a (k-1)-mer group walks it (info: the narrow layout's
+// read_info side array, nullptr for the wide layout)
 template <int RW>
-__global__ void __launch_bounds__(256) k_r2s_s1_post(const u32 *__restrict__ recs, u64 n, u32 nw, u32 k, int m, PkgView pv, S1Out o,
-                                                    int need_mercy, unsigned long long *__restrict__ mul_hist) {
+__global__ void __launch_bounds__(256) k_r2s_s1_post(const u32 *__restrict__ recs, const u64 *__restrict__ info, u64 n, u32 nw,
+                                                    u32 k, int m, PkgView pv, S1Out o, int need_mercy,
+                                                    unsigned long long *__restrict__ mul_hist) {
   __shared__ u32 s_hist[kS1HistSmem];
   for (int i = threadIdx.x; i < kS1HistSmem; i += 256) s_hist[i] = 0;
   __syncthreads();
@@ -869,7 +914,7 @@ __global__ void __launch_bounds__(256) k_r2s_s1_post(const u32 *__restrict__ rec
     const bool head = i == 0 || s1_diff_km1(recs + (i - 1) * RW, recs + i * RW, k);
     if (head) {
       u32 hv[16], nh;
-      s1_group(recs, n, i, RW, nw, k, m, pv, o, need_mercy != 0, hv, nh);
+      s1_group(recs, info, n, i, RW, nw, k, m, pv, o, need_mercy != 0, hv, nh);
       for (u32 q = 0; q < nh; ++q) {
         const u32 c = hv[q];
         if (c < (u32)kS1HistSmem) atomicAdd(&s_hist[c], 1u);

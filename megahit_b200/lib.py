@@ -148,6 +148,7 @@ SYMBOLS = [
     "mhb_iterate_host", "mhb_iterate_run", "mhb_selftest_iterate", "mhb_s2s_extract_edges_pruned", "mhb_s2s_emit_fmt", "mhb_read2sdbg_host", "mhb_read2sdbg_run", "mhb_selftest_r2s_s1_record", "mhb_selftest_r2s_item",
     "mhb_selftest_kmsort", "mhb_selftest_kmsort_smem", "mhb_selftest_r2s_s1_group", "mhb_selftest_r2s_mercy_read",
     "mhb_selftest_r2s_chunk_index", "mhb_selftest_r2s_stream_decide",
+    "mhb_selftest_kmsort_narrow", "mhb_selftest_r2s_s1_plan", "mhb_selftest_read2sdbg_narrow", "mhb_selftest_iterate_narrow",
     "mhb_buildlib_host", "mhb_buildlib_free", "mhb_set_buildlib_chunk", "mhb_buildlib_run", "mhb_selftest_fastx",
     "mhb_s2s_sort", "mhb_s2s_sort_workspace_bytes", "mhb_s2s_sort_hist_byte", "mhb_s2s_sort_stats",
     "mhb_s2s_sort_emit", "mhb_s2s_sort_emit_workspace_bytes",
@@ -278,6 +279,9 @@ def load():
                                         C.c_void_p, C.POINTER(C.c_uint32)]
     L.mhb_selftest_kmsort.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32]
     L.mhb_selftest_kmsort_smem.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32]
+    L.mhb_selftest_kmsort_narrow.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_int, C.c_uint32, C.c_uint32]
+    L.mhb_selftest_read2sdbg_narrow.argtypes = [C.POINTER(BuildArgs), C.POINTER(BuildResult)]
+    L.mhb_selftest_iterate_narrow.argtypes = [C.POINTER(IterateArgs), C.POINTER(IterateResult)]
     L.mhb_selftest_r2s_s1_group.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_int32, C.c_uint32, C.c_uint64, C.c_int,
                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.mhb_selftest_r2s_mercy_read.argtypes = [C.c_uint32, C.c_uint64, C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p,
@@ -654,14 +658,15 @@ def build_host(bin_words: np.ndarray, n_reads: int, k: int, m: int, need_mercy: 
     return out
 
 
-def read2sdbg_host(bin_words: np.ndarray, n_reads: int, k: int, m: int, need_mercy: bool = True) -> dict:
+def read2sdbg_host(bin_words: np.ndarray, n_reads: int, k: int, m: int, need_mercy: bool = True,
+                   narrow: bool = False) -> dict:
     """The 1-pass build (`megahit_core read2sdbg`, main_sdbg_build.cpp:88-156): `.bin` image in, SdBG item stream out,
-    plus what stage 1 writes to P.counting."""
+    plus what stage 1 writes to P.counting.  narrow: the stage-1 layout of k > 237 at any k (tests)."""
     L = load()
     bin_words = np.ascontiguousarray(bin_words, dtype=np.uint32).reshape(-1)
     a = BuildArgs(k, m, bin_words.ctypes.data if len(bin_words) else None, len(bin_words), n_reads, int(need_mercy), 0, None, 0)
     r = BuildResult()
-    _check(L.mhb_read2sdbg_host(C.byref(a), C.byref(r)))
+    _check((L.mhb_selftest_read2sdbg_narrow if narrow else L.mhb_read2sdbg_host)(C.byref(a), C.byref(r)))
     out = {
         "n_edge_records": r.n_edge_records, "n_distinct_items": r.n_solid, "n_mercy": r.n_mercy,
         "n_sort_items": r.n_sort_items, "n_items": r.n_items, "n_tips": r.n_tips, "n_large_mul": r.n_large_mul,
@@ -711,10 +716,10 @@ def seq2sdbg_run(output_prefix: str, k: int, k_from: int = 0, input_prefix: str 
 
 
 def iterate_host(contig_words: np.ndarray, contig_word_off: np.ndarray, contig_len: np.ndarray, bin_words: np.ndarray,
-                 n_reads: int, k: int, step: int, selftest: bool = False) -> dict:
+                 n_reads: int, k: int, step: int, selftest: bool = False, narrow: bool = False) -> dict:
     """`megahit_core iterate` (main_iterate.cpp): contigs (file orientation, flag-filtered) + read library in, the set of
     iterative edges for k + step out (ascending `.edges` records, multiplicity 0).  selftest: the host mirror of the
-    device code (CPU tests), not a compute path."""
+    device code (CPU tests), not a compute path.  narrow: the flank-index layout of k + 1 > 240 at any k (tests)."""
     L = load()
     cw = np.ascontiguousarray(contig_words, np.uint32)
     if len(cw) == 0:
@@ -728,7 +733,8 @@ def iterate_host(contig_words: np.ndarray, contig_word_off: np.ndarray, contig_l
     a = IterateArgs(k, step, cw.ctypes.data, co.ctypes.data, cl.ctypes.data, n_contigs, b.ctypes.data if len(b) else None,
                     len(b), n_reads)
     r = IterateResult()
-    _check((L.mhb_selftest_iterate if selftest else L.mhb_iterate_host)(C.byref(a), C.byref(r)))
+    fn = L.mhb_selftest_iterate if selftest else L.mhb_selftest_iterate_narrow if narrow else L.mhb_iterate_host
+    _check(fn(C.byref(a), C.byref(r)))
     W = r.words_per_edge
     out = {"n_flanks": r.n_flanks, "n_aligned_reads": r.n_aligned_reads, "n_candidates": r.n_candidates, "n_edges": r.n_edges,
            "edges": np.ctypeslib.as_array(r.edges, (max(r.n_edges, 1) * W,))[: r.n_edges * W].reshape(-1, W).copy(),
@@ -811,6 +817,23 @@ def selftest_kmsort(recs: np.ndarray, nw: int, smem: bool = False, cap: int = 65
     else:
         _check(load().mhb_selftest_kmsort(recs.ctypes.data, len(recs), nw))
     return recs
+
+
+def selftest_kmsort_narrow(recs: np.ndarray, nw: int, smem: bool = False, cap: int = 65535, wcap: int = 0) -> np.ndarray:
+    """selftest_kmsort on the narrow stage-1 layout (k > 237): records of nw key words + one row-index word"""
+    recs = np.ascontiguousarray(recs, np.uint32).copy()
+    _check(load().mhb_selftest_kmsort_narrow(recs.ctypes.data, len(recs), nw, int(smem), cap, wcap))
+    return recs
+
+
+def r2s_s1_plan(k: int, n_s1: int, max_reads: int, avail: int, limit: int = 0) -> dict:
+    """read2sdbg's stage-1 round plan (host code): max_n = 0 for one pass, else the most records of one round;
+    rec_words = words per stage-1 sort record"""
+    L = load()
+    mx, rw = C.c_uint64(), C.c_uint32()
+    L.mhb_selftest_r2s_s1_plan.argtypes = [C.c_uint32] + [C.c_uint64] * 4 + [C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]
+    _check(L.mhb_selftest_r2s_s1_plan(k, n_s1, max_reads, avail, limit, C.byref(mx), C.byref(rw)))
+    return {"max_n": mx.value, "rec_words": rw.value}
 
 
 def selftest_r2s_chunk_index(bin_words: np.ndarray, n_reads: int, k: int, first: int, count: int, derive: bool) -> dict:
