@@ -328,6 +328,15 @@ int mhb_s2s_extract_range(void *stream, const mhb_dev_seqs *seqs, uint32_t k, ui
                           uint32_t lo, uint32_t hi, uint64_t *cursor_dev, uint64_t capacity, uint64_t *hist256,
                           int hist_byte);
 
+/* All sort items, each stored straight into the buffer of the rank that owns its leading record byte (the exchange of
+ * a multi-GPU seq2sdbg, with no local item array in between).  Device arrays: owner_of_byte[256] -> owner o;
+ * owner_base[o] = the address where this rank's items for o begin (a segment of o's receive buffer, possibly opened
+ * through CUDA IPC); cursor_dev[o] (caller-zeroed) ends at the number of items sent to o; items beyond capacity_dev[o]
+ * are counted but not stored.  The order of the items inside a segment is unspecified. */
+int mhb_s2s_extract_owners(void *stream, const mhb_dev_seqs *seqs, uint32_t k, uint64_t n_items,
+                           const uint8_t *owner_of_byte, const uint64_t *owner_base, uint64_t *cursor_dev,
+                           const uint64_t *capacity_dev);
+
 /* A10 (seq_to_sdbg.cpp:702-789 + sdbg_writer.cpp:25-58): SdBG item stream from sorted records.
  *   bytes_out     capacity_bytes; the variable-length item stream in sorted (= bucket) order
  *   bucket_table  uint64[65536*4] device: per bucket {byte offset, #items, #tips, #large_mul};
@@ -707,8 +716,23 @@ int mhb_buildlib_run(const char *lib_file, const char *out_prefix);
  * P.sdbg.<r>, rank 0 the merged P.edges.info (num_files = n_gpus, edge_io_meta.h:25-44), P.sdbg_info
  * (sdbg_meta.cpp:44-61), P.cand, P.counting, and the marker P.sdbg_fused ("k need_mercy n_gpus") that lets a following
  * `seq2sdbg --need_mercy --input_prefix P -o P` return at once instead of rebuilding the same graph.  The caller must not
- * have initialised CUDA in this process (the workers are forked). */
+ * have initialised CUDA in this process (the workers are forked).  Rank r runs on device r % device_count: with more
+ * ranks than devices, ranks share a device (its compute mode must admit several processes). */
 int mhb_count_run_multi(const mhb_count_opts *opts, int n_gpus);
+
+/* `seq2sdbg` on n_gpus GPUs of this node: the same options and inputs as mhb_seq2sdbg_run.  n_gpus <= 1 runs
+ * mhb_seq2sdbg_run; so does --need_mercy (the mercy search over edge files stays on one GPU), except where the multi-GPU
+ * count left its P.sdbg_fused marker, which means there is nothing to do.  Otherwise the sequences are loaded on the
+ * host and dealt in contiguous shares balanced on their item count (mhb_plan_seq_shares) to one forked worker per GPU
+ * (devices shared as in mhb_count_run_multi); each worker extracts its items straight into the owners' receive buffers
+ * (mhb_s2s_extract_owners), sorts and emits its bucket range and writes P.sdbg.<r>; rank 0 writes the merged P.sdbg_info
+ * (num_files = n_gpus, sdbg_meta.cpp:44-61).  Resident only: a rank whose share does not fit returns MHB_ERR_NOMEM.
+ * The caller must not have initialised CUDA in this process. */
+int mhb_seq2sdbg_run_multi(const mhb_seq2sdbg_opts *opts, int n_gpus);
+/* The shares of mhb_seq2sdbg_run_multi (host only): n_ranks contiguous runs [first[r], first[r+1]) of the n_seqs
+ * sequences (lengths len), every cut at the sequence boundary whose item count (2 * (len - k + 2) per sequence of length
+ * >= k + 1) before it is closest to r / n_ranks of the total.  first_out gets n_ranks + 1 entries. */
+int mhb_plan_seq_shares(const uint32_t *len, uint64_t n_seqs, uint32_t k, uint32_t n_ranks, uint64_t *first_out);
 
 /* ---------------------------------------------------------------------------------------------
  * Self-test hooks (host): build ONE sort record with the same __host__ __device__ code the kernels

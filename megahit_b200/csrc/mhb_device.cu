@@ -472,6 +472,27 @@ extern "C" int mhb_s2s_extract_edges_pruned(void *stream, const uint32_t *edges,
 // histogram of record byte hist_byte over the in-range items); otherwise the in-range records are appended at
 // records[*cursor_dev ...) (cursor_dev: device uint64, caller-zeroed; ends at the number of in-range items even when
 // that exceeds `capacity`, in which case the surplus was not stored).
+// k_s2s_extract_range over the items [lo, hi] of the sequences, into any sink (checks done by the callers)
+template <class Sink>
+static int launch_extract_range(cudaStream_t st, const mhb_dev_seqs *seqs, uint32_t k, uint64_t n_items, uint32_t lo,
+                                uint32_t hi, const Sink &sink, uint64_t *hist256, int hist_byte) {
+  if (!seqs->mult && !(seqs->fixed_len && seqs->fixed_stride))
+    return mhb_set_error(MHB_ERR_ARG, "seqs->mult is NULL (only allowed for fixed-stride edge records)");
+  if (!seqs->fixed_len && (!seqs->word_off || !seqs->len || !seqs->item_off))
+    return mhb_set_error(MHB_ERR_ARG, "variable-length sequences need word_off, len and item_off");
+  if (seqs->fixed_len && seqs->fixed_len < k + 1) return mhb_set_error(MHB_ERR_ARG, "fixed_len < k+1");
+  const SeqsView sv = make_seqs_view(seqs);
+  const u32 W = s2s_record_words(k);
+  u64 g = (n_items + 255) / 256;
+  if (g > (u64)sm_count() * 32) g = (u64)sm_count() * 32;
+#define M(WW) \
+  if (W == WW) k_s2s_extract_range<WW, Sink><<<(unsigned)g, 256, 0, st>>>(sv, k, n_items, lo, hi, sink, hist256, hist_byte);
+  MHB_FOR_WR(M)
+#undef M
+  CK_LAUNCH();
+  return MHB_OK;
+}
+
 extern "C" int mhb_s2s_extract_range(void *stream, const mhb_dev_seqs *seqs, uint32_t k, uint32_t *records, uint64_t n_items,
                                      uint32_t lo, uint32_t hi, uint64_t *cursor_dev, uint64_t capacity, uint64_t *hist256,
                                      int hist_byte) {
@@ -479,24 +500,18 @@ extern "C" int mhb_s2s_extract_range(void *stream, const mhb_dev_seqs *seqs, uin
   if (lo > hi || hi > 65535) return mhb_set_error(MHB_ERR_ARG, "bad bucket range [%u, %u]", lo, hi);
   if (records && !cursor_dev) return mhb_set_error(MHB_ERR_ARG, "cursor is NULL");
   if (n_items == 0) return MHB_OK;
-  if (!seqs->mult && !(seqs->fixed_len && seqs->fixed_stride))
-    return mhb_set_error(MHB_ERR_ARG, "seqs->mult is NULL (only allowed for fixed-stride edge records)");
-  if (!seqs->fixed_len && (!seqs->word_off || !seqs->len || !seqs->item_off))
-    return mhb_set_error(MHB_ERR_ARG, "variable-length sequences need word_off, len and item_off");
-  if (seqs->fixed_len && seqs->fixed_len < k + 1) return mhb_set_error(MHB_ERR_ARG, "fixed_len < k+1");
-  cudaStream_t st = (cudaStream_t)stream;
-  const SeqsView sv = make_seqs_view(seqs);
-  const u32 W = s2s_record_words(k);
-  u64 g = (n_items + 255) / 256;
-  if (g > (u64)sm_count() * 32) g = (u64)sm_count() * 32;
-#define M(WW)                                                                                                        \
-  if (W == WW)                                                                                                       \
-    k_s2s_extract_range<WW><<<(unsigned)g, 256, 0, st>>>(sv, k, records, n_items, lo, hi, (unsigned long long *)cursor_dev, \
-                                                         capacity, hist256, hist_byte);
-  MHB_FOR_WR(M)
-#undef M
-  CK_LAUNCH();
-  return MHB_OK;
+  const RangeSink sink{records, (unsigned long long *)cursor_dev, capacity};
+  return launch_extract_range((cudaStream_t)stream, seqs, k, n_items, lo, hi, sink, hist256, hist_byte);
+}
+
+extern "C" int mhb_s2s_extract_owners(void *stream, const mhb_dev_seqs *seqs, uint32_t k, uint64_t n_items,
+                                      const uint8_t *owner_of_byte, const uint64_t *owner_base, uint64_t *cursor_dev,
+                                      const uint64_t *capacity_dev) {
+  if (!seqs || k < 9 || k > MHB_MAX_K) return mhb_set_error(MHB_ERR_ARG, "kmer size must be >= 9 and <= 255");
+  if (!owner_of_byte || !owner_base || !cursor_dev || !capacity_dev) return mhb_set_error(MHB_ERR_ARG, "bad args");
+  if (n_items == 0) return MHB_OK;
+  const OwnerSink sink{owner_of_byte, owner_base, (unsigned long long *)cursor_dev, capacity_dev};
+  return launch_extract_range((cudaStream_t)stream, seqs, k, n_items, 0, 65535, sink, nullptr, 0);
 }
 
 // in-place exclusive scan of n u64 values (three phases, no serial chain); total -> *total_dev

@@ -160,6 +160,24 @@ uint64_t read_chunk_limit();
 // the chunk size of a library that is streamed because it does not fit (no cap set)
 uint64_t read_chunk_auto_bytes();
 
+// host container mirroring what SeqPackage holds for seq2sdbg: word-aligned package-orientation sequences (mhb_files.cpp)
+struct HostSeqs {
+  std::vector<uint32_t> words;
+  std::vector<uint64_t> word_off{0};
+  std::vector<uint32_t> len;
+  std::vector<uint16_t> mult;
+  size_t size() const { return len.size(); }
+  void append_packed(const uint32_t *w, uint32_t L, uint16_t m);  // already left-aligned, tail bits may be dirty
+  void append_ascii(const char *s, uint32_t L, bool reverse, uint16_t m);  // sequence_package.h:245-273
+};
+
+// The parts of mhb_seq2sdbg_run that mhb_seq2sdbg_run_multi shares (mhb_files.cpp): the argument checks; whether a
+// multi-GPU count has already built this graph (logs so, with the time since t0); and the loader of every input
+// (edges, mercy edges with --need_mercy, contig / bubble / addi / local FASTA) into one sequence set.
+int seq2sdbg_check_opts(const mhb_seq2sdbg_opts *o);
+bool seq2sdbg_prebuilt(const mhb_seq2sdbg_opts *o, double t0);
+int seq2sdbg_load(const mhb_seq2sdbg_opts *o, HostSeqs *seqs);
+
 // mhb_mercy_probe_owned, with accumulate = true OR-ing the answers into planes_out instead of storing them (mhb_multi.cu)
 int mercy_probe_owned(void *stream, const mhb_dev_reads *reads, const uint64_t *cand_ids, uint64_t n_cand,
                       uint32_t max_read_len, uint32_t k, const uint32_t *edges, uint64_t n_edges, const void *lut,

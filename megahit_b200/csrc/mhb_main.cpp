@@ -134,7 +134,8 @@ int main_seq2sdbg(int argc, char **argv) {
   const std::vector<Opt> opts = {{"host_mem", "", false},     {"kmer_size", "k", false},    {"kmer_from", "", false},
                                  {"num_cpu_threads", "t", false}, {"contig", "", false},    {"bubble", "", false},
                                  {"addi_contig", "", false},  {"local_contig", "", false},  {"input_prefix", "", false},
-                                 {"output_prefix", "o", false}, {"need_mercy", "", true},   {"mem_flag", "", false}};
+                                 {"output_prefix", "o", false}, {"need_mercy", "", true},   {"mem_flag", "", false},
+                                 {"gpus", "", false}};
   const char *usage =
       "Usage: sdbg_builder seq2sdbg -k kmer_size --contig contigs.fa [--addi_contig add.fa] [--input_prefix input] -o out";
   std::map<std::string, std::string> v;
@@ -159,7 +160,9 @@ int main_seq2sdbg(int argc, char **argv) {
   if (in.empty() && contig.empty() && addi.empty()) return fail_usage("No input files!", usage);
   if (o.k < 9) return fail_usage("kmer size must be >= 9!", usage);
   if (o.host_mem == 0) return fail_usage("Please specify the host memory!", usage);
-  if (int rc = mhb_seq2sdbg_run(&o)) {
+  // --gpus N / MHB_GPUS=N (not an option of the reference, which the Python driver never passes): one worker per GPU
+  const int gpus = v.count("gpus") ? atoi(v["gpus"].c_str()) : (getenv("MHB_GPUS") ? atoi(getenv("MHB_GPUS")) : 1);
+  if (int rc = gpus > 1 ? mhb_seq2sdbg_run_multi(&o, gpus) : mhb_seq2sdbg_run(&o)) {
     fprintf(stderr, "FATAL megahit_b200: %s\n", mhb_last_error());
     (void)rc;
     exit(1);

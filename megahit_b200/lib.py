@@ -144,7 +144,8 @@ SYMBOLS = [
     "mhb_tipset_build", "mhb_count_mark_mercy", "mhb_count_tip_edges", "mhb_s2s_extract", "mhb_s2s_extract_range",
     "mhb_s2s_emit_scratch_bytes", "mhb_s2s_emit", "mhb_set_device", "mhb_count_host", "mhb_s2s_host", "mhb_build_host", "mhb_free",
     "mhb_mercy_candidates_scratch_bytes", "mhb_mercy_candidates", "mhb_mercy_edges_scratch_bytes", "mhb_mercy_edges", "mhb_mercy_edges_count", "mhb_mercy_edges_write", "mhb_mercy_edges_segs", "mhb_mercy_host", "mhb_mercy_planes_words", "mhb_mercy_probe_owned", "mhb_mercy_count_planes", "mhb_edge_lut_bytes", "mhb_edge_lut_build",
-    "mhb_release", "mhb_count_run", "mhb_count_run_multi", "mhb_seq2sdbg_run", "mhb_selftest_count_record", "mhb_selftest_count_records_roll", "mhb_selftest_s2s_record",
+    "mhb_release", "mhb_count_run", "mhb_count_run_multi", "mhb_seq2sdbg_run", "mhb_seq2sdbg_run_multi",
+    "mhb_plan_seq_shares", "mhb_s2s_extract_owners","mhb_selftest_count_record", "mhb_selftest_count_records_roll", "mhb_selftest_s2s_record",
     "mhb_iterate_host", "mhb_iterate_run", "mhb_selftest_iterate", "mhb_s2s_extract_edges_pruned", "mhb_s2s_emit_fmt", "mhb_read2sdbg_host", "mhb_read2sdbg_run", "mhb_selftest_r2s_s1_record", "mhb_selftest_r2s_item",
     "mhb_selftest_kmsort", "mhb_selftest_kmsort_smem", "mhb_selftest_r2s_s1_group", "mhb_selftest_r2s_mercy_read",
     "mhb_selftest_r2s_chunk_index", "mhb_selftest_r2s_stream_decide",
@@ -260,6 +261,12 @@ def load():
     L.mhb_free.argtypes = [C.c_void_p]
     L.mhb_count_run.argtypes = [C.POINTER(CountOpts)]
     L.mhb_seq2sdbg_run.argtypes = [C.POINTER(Seq2SdbgOpts)]
+    L.mhb_seq2sdbg_run_multi.argtypes = [C.POINTER(Seq2SdbgOpts), C.c_int]
+    L.mhb_plan_seq_shares.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_void_p]
+    L.mhb_s2s_extract_range.argtypes = [C.c_void_p, C.POINTER(DevSeqs), C.c_uint32, C.c_void_p, C.c_uint64, C.c_uint32,
+                                        C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_int]
+    L.mhb_s2s_extract_owners.argtypes = [C.c_void_p, C.POINTER(DevSeqs), C.c_uint32, C.c_uint64, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p]
     L.mhb_selftest_count_record.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p,
                                             C.POINTER(C.c_uint32)]
     L.mhb_selftest_count_records_roll.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p,
@@ -709,10 +716,22 @@ def count_run(read_lib_file: str, output_prefix: str, k: int = 21, m: int = 2, h
 
 def seq2sdbg_run(output_prefix: str, k: int, k_from: int = 0, input_prefix: str = "", contig: str = "",
                  bubble: str = "", addi_contig: str = "", local_contig: str = "", need_mercy: bool = False,
-                 host_mem: float = 1e9, num_cpu_threads: int = 0, mem_flag: int = 1) -> None:
+                 host_mem: float = 1e9, num_cpu_threads: int = 0, mem_flag: int = 1, gpus: int = 1) -> None:
+    """gpus > 1: mhb_seq2sdbg_run_multi, which forks one worker per GPU and so must be called from a process that has
+    not initialised CUDA (torch included); it writes one P.sdbg.<r> per rank."""
     o = Seq2SdbgOpts(host_mem, k, k_from, num_cpu_threads, contig.encode(), bubble.encode(), addi_contig.encode(),
                      local_contig.encode(), input_prefix.encode(), output_prefix.encode(), int(need_mercy), mem_flag)
-    _check(load().mhb_seq2sdbg_run(C.byref(o)))
+    L = load()
+    _check(L.mhb_seq2sdbg_run_multi(C.byref(o), int(gpus)) if gpus > 1 else L.mhb_seq2sdbg_run(C.byref(o)))
+
+
+def plan_seq_shares(length: np.ndarray, k: int, n_ranks: int) -> list[int]:
+    """The shares of a multi-GPU seq2sdbg (host logic only): the first sequence of every rank's share, then n_seqs."""
+    L = load()
+    ln = np.ascontiguousarray(length, np.uint32)
+    first = np.zeros(n_ranks + 1, np.uint64)
+    _check(L.mhb_plan_seq_shares(ln.ctypes.data if len(ln) else None, len(ln), k, n_ranks, first.ctypes.data))
+    return [int(x) for x in first]
 
 
 def iterate_host(contig_words: np.ndarray, contig_word_off: np.ndarray, contig_len: np.ndarray, bin_words: np.ndarray,
