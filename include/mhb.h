@@ -733,6 +733,19 @@ int mhb_seq2sdbg_run_multi(const mhb_seq2sdbg_opts *opts, int n_gpus);
  * sequences (lengths len), every cut at the sequence boundary whose item count (2 * (len - k + 2) per sequence of length
  * >= k + 1) before it is closest to r / n_ranks of the total.  first_out gets n_ranks + 1 entries. */
 int mhb_plan_seq_shares(const uint32_t *len, uint64_t n_seqs, uint32_t k, uint32_t n_ranks, uint64_t *first_out);
+/* `iterate` on n_gpus GPUs of this node: the same options, checks and output files as mhb_iterate_run, byte for byte.
+ * n_gpus <= 1 runs mhb_iterate_run.  Otherwise the contigs, bubbles and `.bin` image are loaded on the host and the
+ * reads dealt in contiguous shares balanced on their bases (mhb_plan_read_shares) to one forked worker per GPU (devices
+ * shared as in mhb_count_run_multi).  Every worker builds the flank index of all contigs and runs the read pass over its
+ * share, streamed in chunks when the share does not fit, as mhb_iterate_host does with a whole library; its unique
+ * candidate edges go to the rank owning their leading byte (mhb_partition_scatter), which sorts and dedups them.  The
+ * owners' ascending runs follow each other in rank order in the one P.edges.0; rank 0 writes P.edges.info.  A rank
+ * whose received edges do not fit returns MHB_ERR_NOMEM.  The caller must not have initialised CUDA in this process. */
+int mhb_iterate_run_multi(const mhb_iterate_opts *opts, int n_gpus);
+/* The shares of mhb_iterate_run_multi (host only): n_ranks contiguous runs [first[r], first[r+1]) of the n_reads reads of
+ * the `.bin` image bin (bin_words words, fixed or variable read length), every cut at the read boundary whose base count
+ * before it is closest to r / n_ranks of the total.  first_out gets n_ranks + 1 entries. */
+int mhb_plan_read_shares(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, uint32_t n_ranks, uint64_t *first_out);
 
 /* ---------------------------------------------------------------------------------------------
  * Self-test hooks (host): build ONE sort record with the same __host__ __device__ code the kernels

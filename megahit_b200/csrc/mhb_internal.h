@@ -5,6 +5,7 @@
 
 #include <algorithm>
 #include <functional>
+#include <string>
 #include <vector>
 
 #include "mhb.h"
@@ -177,6 +178,63 @@ struct HostSeqs {
 int seq2sdbg_check_opts(const mhb_seq2sdbg_opts *o);
 bool seq2sdbg_prebuilt(const mhb_seq2sdbg_opts *o, double t0);
 int seq2sdbg_load(const mhb_seq2sdbg_opts *o, HostSeqs *seqs);
+
+// The parts of mhb_iterate_run that mhb_iterate_run_multi shares (mhb_files.cpp): the option checks; the loader, checks
+// included, of the contigs and bubbles (file orientation, standalone and loop contigs discarded) and of the `.bin`
+// image (n_reads counted from its length words); and P.edges.info of n unordered edges of k_out = k + step.
+int iterate_check_opts(const mhb_iterate_opts *o);
+int iterate_load(const mhb_iterate_opts *o, HostSeqs *contigs, std::vector<uint32_t> *bin, uint64_t *n_reads);
+int iterate_write_info(const std::string &prefix, uint32_t k_out, uint32_t words_per_edge, uint64_t n);
+// n_ranks contiguous shares of n items, cut r at the item boundary whose weight before it is closest to r / n_ranks of
+// the total (so a share is off its ideal weight by at most one item's); first gets n_ranks + 1 entries
+template <class Weight>
+void plan_shares(uint64_t n, uint32_t n_ranks, Weight weight, uint64_t *first) {
+  uint64_t total = 0;
+  for (uint64_t i = 0; i < n; ++i) total += weight(i);
+  first[0] = 0;
+  uint64_t b = 0, cum = 0;  // cum = weight of the items before b
+  for (uint32_t r = 1; r < n_ranks; ++r) {
+    const uint64_t target = (uint64_t)((unsigned __int128)total * r / n_ranks);
+    while (b < n && cum + weight(b) <= target) cum += weight(b++);
+    // the previous cut may already lie beyond this target (cum > target): then the cut stays where it is
+    if (b < n && cum < target && cum + weight(b) - target < target - cum) cum += weight(b++);
+    first[r] = b;
+  }
+  first[n_ranks] = n;
+}
+
+// ---- iterate's device pieces (mhb_iter.cu), shared by mhb_iterate_host and the multi-GPU worker ----
+// a device allocation released with the object; a failed cudaMalloc is MHB_ERR_NOMEM naming the bytes
+struct IterBuf {
+  void *p = nullptr;
+  IterBuf() = default;
+  IterBuf(const IterBuf &) = delete;
+  IterBuf &operator=(const IterBuf &) = delete;
+  ~IterBuf();
+  int alloc(size_t bytes, const char *what);
+  void release();
+  template <class T>
+  T *as() const { return reinterpret_cast<T *>(p); }
+};
+// the checks of mhb_iterate_host on k and step (main_iterate.cpp:73-93, and the 17-word records of the device sort)
+int iterate_check_args(uint32_t k, uint32_t step);
+// The flank index (FeedBatchContigs) of a's contigs on the current device: n unique records of ceil((k+1)/16) + 2
+// words in tab, and its 65537-entry prefix table in lut.  Every caller gets the same table from the same contigs.
+struct IterFlanks {
+  IterBuf tab, lut;
+  uint64_t n = 0;
+};
+int iter_build_flanks(const mhb_iterate_args *a, IterFlanks *f);
+// The read pass (FindNextKmersFromReads) over a's reads against the flank index: resident, or streamed in chunks when a
+// chunk cap is set or when the resident buffers do not fit.  *set = the n_set unique candidate edges, ascending, on the
+// device (nothing allocated when there are none); n_cand = candidates before the dedup; n_aligned = reads with one.
+int iter_collect(const mhb_iterate_args *a, const IterFlanks &f, IterBuf *set, uint64_t *n_set, uint64_t *n_cand,
+                 uint64_t *n_aligned);
+// KmerCollector's set semantics on n edge records of k + step in a (b: a buffer of the same size): sort, then the first
+// record of every run of equal ones; *out = where the n_out unique records are (a or b)
+int iter_sort_unique(uint32_t *a, uint32_t *b, uint64_t n, uint32_t k, uint32_t step, uint32_t **out, uint64_t *n_out);
+// hist[v] += records among the n of `words` words whose byte `byte` (the sort's numbering) is v (mhb_sortdisp.cu)
+int hist_byte(void *stream, const uint32_t *recs, uint64_t n, uint32_t words, int byte, uint64_t *hist);
 
 // mhb_mercy_probe_owned, with accumulate = true OR-ing the answers into planes_out instead of storing them (mhb_multi.cu)
 int mercy_probe_owned(void *stream, const mhb_dev_reads *reads, const uint64_t *cand_ids, uint64_t n_cand,

@@ -14,27 +14,23 @@ using namespace mhb;
 
 int scan32(cudaStream_t st, const uint32_t *in, uint64_t n, uint64_t *out, uint64_t *total_dev, uint64_t *bsum);
 
-namespace {
-
-struct IBuf {
-  void *p = nullptr;
-  ~IBuf() {
-    if (p) cudaFree(p);
-  }
-  int alloc(size_t b, const char *what) {
-    if (p) cudaFree(p);
+IterBuf::~IterBuf() { release(); }
+void IterBuf::release() {
+  if (p) cudaFree(p);
+  p = nullptr;
+}
+int IterBuf::alloc(size_t b, const char *what) {
+  release();
+  b = ((b ? b : 1) + 255) & ~(size_t)255;
+  if (cudaMalloc(&p, b) != cudaSuccess) {
+    cudaGetLastError();
     p = nullptr;
-    b = ((b ? b : 1) + 255) & ~(size_t)255;
-    if (cudaMalloc(&p, b) != cudaSuccess) {
-      cudaGetLastError();
-      p = nullptr;
-      return mhb_set_error(MHB_ERR_NOMEM, "iterate: cudaMalloc of %zu bytes for %s failed", b, what);
-    }
-    return MHB_OK;
+    return mhb_set_error(MHB_ERR_NOMEM, "iterate: cudaMalloc of %zu bytes for %s failed", b, what);
   }
-  template <class T>
-  T *as() const { return reinterpret_cast<T *>(p); }
-};
+  return MHB_OK;
+}
+
+namespace {
 
 #define CKR(call)        \
   do {                   \
@@ -61,48 +57,36 @@ uint32_t top_bytes(uint32_t words, uint32_t bits, uint8_t *out) {
 int cap_class(uint32_t words) { return words <= 2 ? 2 : words <= 4 ? 4 : words <= 8 ? 8 : 17; }
 #define IT_FOR_WC(M) M(2) M(4) M(8) M(17)
 
-int iter_reads(const mhb_iterate_args *a, mhb_iterate_result *res, const ReadLibIndex &ix, const FlankTable &tab, int WCc,
-               uint32_t w2, uint32_t KN, unsigned long long *cnt, bool stream, uint64_t *n_cand_out, uint64_t *n_edges_out);
+// the kernels' capacity class of (k, step): the wider of the (k+1)-mer keys and the (k+step+1)-mers
+int iter_class(uint32_t k, uint32_t step) { return cap_class(std::max(div_ceil(k + step + 1, 16), div_ceil(k + 1, 16))); }
+
+int iter_reads(const mhb_iterate_args *a, const ReadLibIndex &ix, const FlankTable &tab, bool stream, IterBuf *set,
+               uint64_t *n_set_out, uint64_t *n_cand_out, uint64_t *n_aligned_out);
 
 // mhb_selftest_iterate_narrow: the narrow flank index at a k whose wide records fit, to compare the two layouts
 bool g_iter_force_narrow = false;
 
 }  // namespace
 
-extern "C" int mhb_iterate_host(const mhb_iterate_args *a, mhb_iterate_result *res) {
-  if (!a || !res) return mhb_set_error(MHB_ERR_ARG, "null argument");
-  memset(res, 0, sizeof(*res));
-  const uint32_t k = a->k, step = a->step, K1 = k + 1, KN = k + step + 1;
+int iterate_check_args(uint32_t k, uint32_t step) {
   // main_iterate.cpp:73-93: step even, 0 < step <= 28
   if (k < 9 || step == 0 || step > 28 || (step & 1)) return mhb_set_error(MHB_ERR_ARG, "iterate: invalid k / step");
-  const uint32_t wk = div_ceil(K1, 16), w2 = words_per_edge(k + step), wn = div_ceil(KN, 16);
-  if (w2 > 17) return mhb_set_error(MHB_ERR_ARG, "iterate: k + step + 1 = %u is beyond the 17-word edge records of the device sort", KN);
-  if (mhb_device_count() <= 0) return mhb_set_error(MHB_ERR_CUDA, "no CUDA device: libmhb has no CPU path");
-  res->words_per_edge = w2;
-  read_stream_stats_reset();
-  cudaStream_t st = 0;
-  struct Events {
-    cudaEvent_t a, b;
-    Events() {
-      cudaEventCreate(&a);
-      cudaEventCreate(&b);
-    }
-    ~Events() {
-      cudaEventDestroy(a);
-      cudaEventDestroy(b);
-    }
-  } ev;
-  cudaEvent_t e0 = ev.a, e1 = ev.b;
-  cudaEventRecord(e0, st);
-  const int WCc = cap_class(std::max(wn, wk));
+  if (words_per_edge(k + step) > 17)
+    return mhb_set_error(MHB_ERR_ARG, "iterate: k + step + 1 = %u is beyond the 17-word edge records of the device sort",
+                         k + step + 1);
+  return MHB_OK;
+}
 
-  // ---- flank index (FeedBatchContigs) ----
-  IBuf d_cw, d_co, d_cl, d_fl, d_fl2, d_val, d_ws, d_flag, d_off, d_bsum, d_cnt, d_tab, d_lut;
+int iter_build_flanks(const mhb_iterate_args *a, IterFlanks *f) {
+  const uint32_t k = a->k, step = a->step, K1 = k + 1, wk = div_ceil(K1, 16), frw = wk + 2;
+  const int WCc = iter_class(k, step);
+  cudaStream_t st = 0;
+  IterBuf d_cw, d_co, d_cl, d_fl, d_fl2, d_val, d_ws, d_flag, d_off, d_bsum, d_cnt;
   CKR(d_cnt.alloc(64, "counters"));
   CK(cudaMemsetAsync(d_cnt.p, 0, 64, st));
   unsigned long long *cnt = d_cnt.as<unsigned long long>();
-  const uint32_t frw = wk + 2;
-  uint64_t n_tab = 0;
+  f->n = 0;
+  f->tab.release();
   if (a->n_contigs) {
     const uint64_t cw = a->contig_word_off[a->n_contigs];
     CKR(d_cw.alloc(cw * 4 + 64, "contigs"));
@@ -160,44 +144,74 @@ extern "C" int mhb_iterate_host(const mhb_iterate_args *a, mhb_iterate_result *r
       unsigned long long nu = 0;
       CK(cudaMemcpyAsync(&nu, cnt + 2, 8, cudaMemcpyDeviceToHost, st));
       CK(cudaStreamSynchronize(st));
-      CKR(d_tab.alloc((size_t)nu * frw * 4 + 16, "flank table"));
+      CKR(f->tab.alloc((size_t)nu * frw * 4 + 16, "flank table"));
       if (narrow)
         k_iter_best<<<igrid(nf, 256), 256, 0, st>>>(sorted, nf, wk, d_val.as<u64>(), d_flag.as<u32>(), d_off.as<u64>(),
-                                                    d_tab.as<u32>());
+                                                    f->tab.as<u32>());
       else
-        k_iter_compact<<<igrid(nf, 256), 256, 0, st>>>(sorted, nf, frw, d_flag.as<u32>(), d_off.as<u64>(), d_tab.as<u32>());
+        k_iter_compact<<<igrid(nf, 256), 256, 0, st>>>(sorted, nf, frw, d_flag.as<u32>(), d_off.as<u64>(), f->tab.as<u32>());
       CK_LAUNCH();
-      n_tab = nu;
+      f->n = nu;
     }
   }
-  res->n_flanks = n_tab;
-  CKR(d_lut.alloc(65537 * 4, "flank prefix table"));
-  CK(cudaMemsetAsync(d_lut.p, 0, 65537 * 4, st));
-  if (n_tab) {
-    k_iter_lut<<<(65537 + 255) / 256, 256, 0, st>>>(d_tab.as<u32>(), n_tab, frw, d_lut.as<u32>());
+  CKR(f->lut.alloc(65537 * 4, "flank prefix table"));
+  CK(cudaMemsetAsync(f->lut.p, 0, 65537 * 4, st));
+  if (f->n) {
+    k_iter_lut<<<(65537 + 255) / 256, 256, 0, st>>>(f->tab.as<u32>(), f->n, frw, f->lut.as<u32>());
     CK_LAUNCH();
   }
-  FlankTable tab{d_tab.as<u32>(), n_tab, wk, d_lut.as<u32>()};
+  CK(cudaStreamSynchronize(st));  // the scratch buffers above are freed on return
+  return MHB_OK;
+}
 
-  // ---- reads (FindNextKmersFromReads) ----
+int iter_collect(const mhb_iterate_args *a, const IterFlanks &f, IterBuf *set, uint64_t *n_set, uint64_t *n_cand,
+                 uint64_t *n_aligned) {
+  *n_set = *n_cand = *n_aligned = 0;
+  set->release();
   ReadLibIndex ix;
   CKR(index_read_lib(a->bin, a->bin_words, a->n_reads, 0, &ix));
-  uint64_t n_cand = 0, n_edges = 0;
-  if (a->n_reads && n_tab) {
-    // resident; streamed in chunks when a chunk cap is set or when the resident buffers do not fit
-    int rc = iter_reads(a, res, ix, tab, WCc, w2, KN, cnt, read_chunk_limit() != 0, &n_cand, &n_edges);
-    if (rc == MHB_ERR_NOMEM && !read_chunk_limit()) {
-      free(res->edges);
-      res->edges = nullptr;
-      res->n_aligned_reads = 0;
-      n_cand = n_edges = 0;
-      rc = iter_reads(a, res, ix, tab, WCc, w2, KN, cnt, true, &n_cand, &n_edges);
+  if (!a->n_reads || !f.n) return MHB_OK;
+  const FlankTable tab{f.tab.as<u32>(), f.n, div_ceil(a->k + 1, 16), f.lut.as<u32>()};
+  // resident; streamed in chunks when a chunk cap is set or when the resident buffers do not fit
+  int rc = iter_reads(a, ix, tab, read_chunk_limit() != 0, set, n_set, n_cand, n_aligned);
+  if (rc == MHB_ERR_NOMEM && !read_chunk_limit()) rc = iter_reads(a, ix, tab, true, set, n_set, n_cand, n_aligned);
+  return rc;
+}
+
+extern "C" int mhb_iterate_host(const mhb_iterate_args *a, mhb_iterate_result *res) {
+  if (!a || !res) return mhb_set_error(MHB_ERR_ARG, "null argument");
+  memset(res, 0, sizeof(*res));
+  CKR(iterate_check_args(a->k, a->step));
+  if (mhb_device_count() <= 0) return mhb_set_error(MHB_ERR_CUDA, "no CUDA device: libmhb has no CPU path");
+  const uint32_t w2 = words_per_edge(a->k + a->step);
+  res->words_per_edge = w2;
+  read_stream_stats_reset();
+  cudaStream_t st = 0;
+  struct Events {
+    cudaEvent_t a, b;
+    Events() {
+      cudaEventCreate(&a);
+      cudaEventCreate(&b);
     }
-    CKR(rc);
-  }
-  if (!res->edges) res->edges = (uint32_t *)malloc(4);
+    ~Events() {
+      cudaEventDestroy(a);
+      cudaEventDestroy(b);
+    }
+  } ev;
+  cudaEvent_t e0 = ev.a, e1 = ev.b;
+  cudaEventRecord(e0, st);
+  IterFlanks flanks;
+  CKR(iter_build_flanks(a, &flanks));
+  res->n_flanks = flanks.n;
+  IterBuf set;
+  uint64_t n_set = 0, n_cand = 0, n_aligned = 0;
+  CKR(iter_collect(a, flanks, &set, &n_set, &n_cand, &n_aligned));
+  res->edges = (uint32_t *)malloc(std::max<size_t>(4, (size_t)n_set * w2 * 4));
+  if (!res->edges) return mhb_set_error(MHB_ERR_NOMEM, "host malloc failed");
+  if (n_set) CK(cudaMemcpyAsync(res->edges, set.p, (size_t)n_set * w2 * 4, cudaMemcpyDeviceToHost, st));
+  res->n_aligned_reads = n_aligned;
   res->n_candidates = n_cand;
-  res->n_edges = n_edges;
+  res->n_edges = n_set;
   cudaEventRecord(e1, st);
   cudaEventSynchronize(e1);
   float ms = 0;
@@ -209,7 +223,7 @@ extern "C" int mhb_iterate_host(const mhb_iterate_args *a, mhb_iterate_result *r
 namespace {
 // a device buffer that only grows (its contents do not survive growth)
 struct Grow {
-  IBuf b;
+  IterBuf b;
   size_t cap = 0;
   int need(size_t bytes, const char *what) {
     if (bytes <= cap) return MHB_OK;
@@ -255,9 +269,10 @@ void swap_bufs(Grow &x, Grow &y) {
 // The reads (ReadStream: resident, or streamed from host memory in chunks), the flank index resident: per chunk mark +
 // emit into a mark array of the chunk's bases, make the chunk's candidates unique and merge them into the running set by
 // the same sort + unique over the union.  KmerCollector is a set, so the result does not depend on the chunks.
-int iter_reads(const mhb_iterate_args *a, mhb_iterate_result *res, const ReadLibIndex &ix, const FlankTable &tab, int WCc,
-               uint32_t w2, uint32_t KN, unsigned long long *cnt, bool stream, uint64_t *n_cand_out, uint64_t *n_edges_out) {
-  const uint32_t k = a->k, step = a->step;
+int iter_reads(const mhb_iterate_args *a, const ReadLibIndex &ix, const FlankTable &tab, bool stream, IterBuf *set,
+               uint64_t *n_set_out, uint64_t *n_cand_out, uint64_t *n_aligned_out) {
+  const uint32_t k = a->k, step = a->step, KN = k + step + 1, w2 = words_per_edge(k + step);
+  const int WCc = iter_class(k, step);
   cudaStream_t st = 0;
   ReadStream rs;
   const uint64_t cap = read_chunk_limit() ? read_chunk_limit() : read_chunk_auto_bytes();
@@ -266,12 +281,14 @@ int iter_reads(const mhb_iterate_args *a, mhb_iterate_result *res, const ReadLib
   auto bases_of = [&](uint64_t b, uint64_t e) { return ix.fixed_len ? (e - b) * ix.fixed_len : ix.unit_off[e] - ix.unit_off[b]; };
   uint64_t max_bases = 0;
   for (uint64_t i = 0; i + 1 < first.size(); ++i) max_bases = std::max(max_bases, bases_of(first[i], first[i + 1]));
-  IBuf d_lib, d_exist;
+  IterBuf d_lib, d_exist, d_cnt;
+  CKR(d_cnt.alloc(64, "counters"));
+  unsigned long long *cnt = d_cnt.as<unsigned long long>();
   CKR(d_lib.alloc(rs.device_bytes(), stream ? "read chunk buffers" : ".bin image"));
   CKR(rs.bind(d_lib.p, st));
   CKR(d_exist.alloc((max_bases / 32 + 2) * 4, "position marks"));
   Grow c, c2, u, u2, ws, flag, off, bsum;
-  uint64_t n_cand = 0, n_set = 0;
+  uint64_t n_cand = 0, n_set = 0, n_aligned = 0;
   auto chunk = [&](const ReadChunkView &v) -> int {
     IterReads rd{v.bin, v.n_reads, ix.fixed_len, v.rec_off, v.aux_off};
     const uint64_t bw = bases_of(v.first_read, v.first_read + v.n_reads) / 32 + 2;
@@ -290,7 +307,7 @@ int iter_reads(const mhb_iterate_args *a, mhb_iterate_result *res, const ReadLib
     CK(cudaMemcpyAsync(hc, cnt + 4, 16, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     n_cand += hc[0];
-    res->n_aligned_reads += hc[1];
+    n_aligned += hc[1];
     if (!hc[0]) return MHB_OK;
     const uint64_t nc = hc[0];
     CKR(c.need((size_t)nc * w2 * 4 + 16, "edges"));
@@ -331,15 +348,27 @@ int iter_reads(const mhb_iterate_args *a, mhb_iterate_result *res, const ReadLib
     return MHB_OK;
   };
   CKR(rs.pass(st, chunk));
-  res->edges = (uint32_t *)malloc(std::max<size_t>(1, (size_t)n_set * w2 * 4));
-  if (!res->edges) return mhb_set_error(MHB_ERR_NOMEM, "host malloc failed");
-  if (n_set) CK(cudaMemcpyAsync(res->edges, u.b.p, (size_t)n_set * w2 * 4, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
+  std::swap(set->p, u.b.p);  // the set leaves with the caller; every other buffer is freed here
+  *n_set_out = n_set;
   *n_cand_out = n_cand;
-  *n_edges_out = n_set;
+  *n_aligned_out = n_aligned;
   return MHB_OK;
 }
 }  // namespace
+
+int iter_sort_unique(uint32_t *a, uint32_t *b, uint64_t n, uint32_t k, uint32_t step, uint32_t **out, uint64_t *n_out) {
+  *out = a;
+  *n_out = 0;
+  if (!n) return MHB_OK;
+  IterBuf cnt;
+  CKR(cnt.alloc(64, "counters"));
+  Grow ws, flag, off, bsum;
+  CKR(sort_unique(0, a, b, n, words_per_edge(k + step), k + step + 1, ws, flag, off, bsum, cnt.as<unsigned long long>(), out,
+                  n_out));
+  CK(cudaStreamSynchronize(0));
+  return MHB_OK;
+}
 
 // mhb_iterate_host with the narrow flank index (key + row index records, values in a side array) at any k: the layout
 // mhb_iterate_host takes only when k + 1 > 240, run where both fit so that the tests can compare the two

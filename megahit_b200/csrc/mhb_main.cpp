@@ -14,6 +14,7 @@
 #include <sys/time.h>
 #include <unistd.h>
 
+#include <algorithm>
 #include <fstream>
 #include <map>
 #include <string>
@@ -172,12 +173,39 @@ int main_seq2sdbg(int argc, char **argv) {
 
 int forward_to_reference(char **argv);
 
+// argv without the option `name` (in the "--name value" and "--name=value" forms `parse` takes), walked as `parse` walks
+// it so that an option's value is never mistaken for an option; argv[0] and argv[1] (the sub-command) are kept
+std::vector<char *> drop_option(int argc, char **argv, const std::vector<Opt> &opts, const std::string &name) {
+  std::vector<char *> out(argv, argv + std::min(argc, 2));
+  for (int i = 2; i < argc; ++i) {
+    const std::string a = argv[i];
+    if (a == "--" + name) {
+      ++i;  // and its value
+      continue;
+    }
+    if (a.rfind("--" + name + "=", 0) == 0) continue;
+    out.push_back(argv[i]);
+    bool takes_next = false;  // a value-taking option whose value is the next argument
+    if (a.rfind("--", 0) == 0) {
+      if (a.find('=') == std::string::npos)
+        for (const auto &o : opts)
+          if (a.substr(2) == o.long_name) takes_next = !o.is_flag;
+    } else if (a.size() == 2 && a[0] == '-') {
+      for (const auto &o : opts)
+        if (o.short_name[0] && a.substr(1) == o.short_name) takes_next = !o.is_flag;
+    }
+    if (takes_next && i + 1 < argc) out.push_back(argv[++i]);
+  }
+  out.push_back(nullptr);
+  return out;
+}
+
 // main_iterate (main_iterate.cpp:57-112, 196-221)
 int main_iterate(int argc, char **argv, char **full_argv) {
   RssRecorder rec;
   const std::vector<Opt> opts = {{"contig_file", "c", false}, {"bubble_file", "b", false},     {"read_file", "r", false},
                                  {"num_cpu_threads", "t", false}, {"kmer_k", "k", false},       {"step", "s", false},
-                                 {"output_prefix", "o", false}};
+                                 {"output_prefix", "o", false}, {"gpus", "", false}};
   const char *usage = "Usage: megahit_core iterate [opt]\nopt with (*) are must";
   std::map<std::string, std::string> v;
   std::string err;
@@ -201,9 +229,13 @@ int main_iterate(int argc, char **argv, char **full_argv) {
   o.step = (uint32_t)step;
   if (k < 9 || r == "-") {  // outside the device path (k < 9; stdin): the reference's CPU path
     fprintf(stderr, "megahit_b200: iterate with k = %d is forwarded to the reference\n", k);
-    return forward_to_reference(full_argv);
+    // the reference's iterate refuses options it does not know: --gpus stays here
+    std::vector<char *> fwd = drop_option(argc + 1, full_argv, opts, "gpus");
+    return forward_to_reference(fwd.data());
   }
-  if (int rc = mhb_iterate_run(&o)) {
+  // --gpus N / MHB_GPUS=N (not an option of the reference, which the Python driver never passes): one worker per GPU
+  const int gpus = v.count("gpus") ? atoi(v["gpus"].c_str()) : (getenv("MHB_GPUS") ? atoi(getenv("MHB_GPUS")) : 1);
+  if (int rc = gpus > 1 ? mhb_iterate_run_multi(&o, gpus) : mhb_iterate_run(&o)) {
     fprintf(stderr, "FATAL megahit_b200: %s\n", mhb_last_error());
     (void)rc;
     exit(1);

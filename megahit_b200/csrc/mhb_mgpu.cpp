@@ -19,6 +19,10 @@
 // contiguous shares, balanced on their item count; each rank histograms its items' leading bytes, and after the plan
 // extracts every item straight into its owner's receive buffer (mhb_s2s_extract_owners); the owners sort and emit as
 // the count worker's SdBG stage does (sdbg_owner_stage, sdbg_merge_info).
+//
+// `iterate` (mhb_iterate_run_multi) deals contiguous read shares, balanced on bases; each rank builds the whole flank
+// index, runs the single-GPU read pass over its share and sends its unique candidates to their owners, which sort and
+// dedup them; the owners' ascending runs, written in rank order, are the single-GPU P.edges.0.
 #include <cuda_runtime.h>
 #include <fcntl.h>
 #include <pthread.h>
@@ -70,6 +74,7 @@ struct Control {
   uint64_t n_solid[kMaxRanks], n_tip[kMaxRanks], n_cand[kMaxRanks], n_mercy[kMaxRanks], n_records[kMaxRanks];
   uint64_t sdbg_totals[kMaxRanks][16];
   uint64_t has_tips[kMaxRanks];
+  uint64_t n_edges[kMaxRanks], n_aligned[kMaxRanks];  // iterate
   int err_code[kMaxRanks];  // MHB_ERR_* of a failed rank
 };
 
@@ -746,21 +751,9 @@ void worker(const Job &J, Exchange &X) {
 // ================================================================================================
 uint64_t seq_items(uint32_t len, uint32_t k) { return len >= k + 1 ? 2ull * (len - k + 2) : 0; }
 
-// n_ranks contiguous shares of the sequences; cut r lies at the sequence boundary whose item count before it is
-// closest to r / n_ranks of the total (so a share is off its ideal size by at most one sequence's items)
+// n_ranks contiguous shares of the sequences, balanced on their items (plan_shares)
 void plan_seq_shares(const uint32_t *len, uint64_t n, uint32_t k, uint32_t n_ranks, uint64_t *first) {
-  uint64_t total = 0;
-  for (uint64_t i = 0; i < n; ++i) total += seq_items(len[i], k);
-  first[0] = 0;
-  uint64_t b = 0, cum = 0;  // cum = items of the sequences before b
-  for (uint32_t r = 1; r < n_ranks; ++r) {
-    const uint64_t target = (uint64_t)((unsigned __int128)total * r / n_ranks);
-    while (b < n && cum + seq_items(len[b], k) <= target) cum += seq_items(len[b++], k);
-    // the previous cut may already lie beyond this target (cum > target): then the cut stays where it is
-    if (b < n && cum < target && cum + seq_items(len[b], k) - target < target - cum) cum += seq_items(len[b++], k);
-    first[r] = b;
-  }
-  first[n_ranks] = n;
+  plan_shares(n, n_ranks, [&](uint64_t i) { return seq_items(len[i], k); }, first);
 }
 
 struct SeqJob {
@@ -835,6 +828,122 @@ void s2s_worker(const SeqJob &J, Exchange &X) {
   if (r == 0) sdbg_merge_info(X, k, J.prefix);
   X.barrier();
   X.cleanup("stab");
+}
+
+// ================================================================================================
+// iterate on several GPUs: the reads are dealt in contiguous shares, the candidate sets meet on their owners
+// ================================================================================================
+// rec_off[i] = first word of read i of the `.bin` image, n_reads + 1 entries; false when the image ends inside a read
+bool read_offsets(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, std::vector<uint64_t> *rec_off) {
+  rec_off->assign(n_reads + 1, 0);
+  uint64_t pos = 0;
+  for (uint64_t i = 0; i < n_reads; ++i) {
+    if (pos >= bin_words) return false;
+    (*rec_off)[i] = pos;
+    pos += 1 + div_ceil(bin[pos], 16);
+  }
+  (*rec_off)[n_reads] = pos;
+  return pos <= bin_words;
+}
+
+// n_ranks contiguous shares of the reads, balanced on their bases: the mark pass scans every base of every read
+void plan_read_shares(const uint32_t *bin, const std::vector<uint64_t> &rec_off, uint32_t n_ranks, uint64_t *first) {
+  plan_shares(rec_off.size() - 1, n_ranks, [&](uint64_t i) { return (uint64_t)bin[rec_off[i]]; }, first);
+}
+
+struct IterJob {
+  mhb_iterate_args a;          // every contig and the whole `.bin` image (host, inherited by the workers)
+  std::vector<uint64_t> first;  // read shares
+  std::vector<uint64_t> word;   // first word of every share, n_ranks + 1 entries
+  int fd;                       // P.edges.0, created empty by the parent
+  std::string prefix;
+};
+
+#define CKI(call)                                      \
+  do {                                                 \
+    if (int rc_ = (call)) throw Fail{mhb_last_error(), rc_}; \
+  } while (0)
+
+void iter_worker(const IterJob &J, Exchange &X) {
+  Control *C = X.C;
+  const int W = X.world, r = X.rank;
+  const uint32_t k = J.a.k, step = J.a.step, w2 = mhb_words_per_edge(k + step);
+  const int top = (int)(4 * w2 - 1);
+  bind_device(r, W);
+  DevPool pool;
+
+  // ---- the flank index of every contig, then the read pass over my share: my unique candidates, on the device ----
+  mhb_iterate_args a = J.a;
+  a.bin = J.a.bin + J.word[r];
+  a.bin_words = J.word[r + 1] - J.word[r];
+  a.n_reads = J.first[r + 1] - J.first[r];
+  IterBuf set;
+  uint64_t n_flanks = 0, n_set = 0, n_cand = 0, n_aligned = 0, n_chunks = 0;
+  read_stream_stats_reset();
+  {
+    IterFlanks flanks;
+    CKI(iter_build_flanks(&a, &flanks));
+    n_flanks = flanks.n;
+    CKI(iter_collect(&a, flanks, &set, &n_set, &n_cand, &n_aligned));
+    CKM(mhb_read_stream_stats(&n_chunks, nullptr, nullptr));
+  }  // the flank table and the buffers of the read pass are freed: only the set stays
+
+  // ---- every edge to the rank owning its leading byte ----
+  uint64_t *d_hist = pool.get<uint64_t>(256);
+  CKC(cudaMemset(d_hist, 0, 256 * 8));
+  CKI(hist_byte(nullptr, set.as<uint32_t>(), n_set, w2, top, d_hist));
+  const size_t ws_bytes = mhb_sort_workspace_bytes(std::max<uint64_t>(n_set, 1), w2);
+  void *d_ws = pool.get<char>(ws_bytes);
+  PeerBuf pb;
+  const Plan P = partition_and_exchange(X, 0, set.as<uint32_t>(), n_set, w2, top, d_hist, d_ws, ws_bytes, pool, &pb);
+  set.release();
+  pool.drop(d_ws);
+
+  // ---- the owner's sort + unique over what it received: an ascending run of the whole set ----
+  const uint64_t n_own = P.recv_tot[r];
+  uint64_t n_uniq = 0;
+  std::vector<uint32_t> edges;
+  {
+    uint32_t *d_tmp = pool.get<uint32_t>(n_own * w2 + 16), *uniq = nullptr;
+    CKI(iter_sort_unique((uint32_t *)pb.mine, d_tmp, n_own, k, step, &uniq, &n_uniq));
+    edges.resize(n_uniq * w2);
+    if (n_uniq) CKC(cudaMemcpy(edges.data(), uniq, n_uniq * w2 * 4, cudaMemcpyDeviceToHost));
+    pool.drop(d_tmp);
+  }
+  close_peers(X, &pb);
+  C->n_edges[r] = n_uniq;
+  C->n_cand[r] = n_cand;
+  C->n_aligned[r] = n_aligned;
+  XINFO("rank %d: %llu reads (%s), %llu candidates, %llu unique sent, %llu received, %llu owned\n", r,
+        (unsigned long long)a.n_reads, n_chunks ? (std::to_string(n_chunks) + " chunks").c_str() : "resident",
+        (unsigned long long)n_cand, (unsigned long long)n_set, (unsigned long long)n_own, (unsigned long long)n_uniq);
+  X.barrier();
+
+  // ---- the owners' runs follow each other in rank order: one P.edges.0, as the single-GPU iterate writes it ----
+  uint64_t before = 0;
+  for (int o = 0; o < r; ++o) before += C->n_edges[o];
+  const char *p = (const char *)edges.data();
+  size_t left = edges.size() * 4;
+  off_t at = (off_t)(before * w2 * 4);
+  while (left) {
+    const ssize_t got = pwrite(J.fd, p, left, at);
+    if (got <= 0) throw Fail{"write to " + J.prefix + ".edges.0 failed", MHB_ERR_IO};
+    p += got;
+    left -= (size_t)got;
+    at += got;
+  }
+  X.barrier();
+  if (r == 0) {
+    uint64_t n_edges = 0, aligned = 0;
+    for (int o = 0; o < W; ++o) {
+      n_edges += C->n_edges[o];
+      aligned += C->n_aligned[o];
+    }
+    CKI(iterate_write_info(J.prefix, k + step, w2, n_edges));
+    XINFO("Number of flank kmers: %llu\n", (unsigned long long)n_flanks);
+    XINFO("Total: %llu, aligned: %llu. Iterative edges: %llu\n", (unsigned long long)J.first[W],
+          (unsigned long long)aligned, (unsigned long long)n_edges);
+  }
 }
 
 // Forks one worker per rank around a fresh control block and waits for all of them.  A worker that dies would leave
@@ -973,6 +1082,54 @@ extern "C" int mhb_seq2sdbg_run_multi(const mhb_seq2sdbg_opts *o, int n_gpus) {
   const int rc = run_workers(n_gpus, "seq2sdbg", {"stab"}, [&](Exchange &X) { s2s_worker(J, X); });
   if (!rc) XINFO("seq2sdbg on %d GPUs done. Time elapsed: %.4f\n", n_gpus, now_s() - t0);
   return rc;
+}
+
+extern "C" int mhb_iterate_run_multi(const mhb_iterate_opts *o, int n_gpus) {
+  if (n_gpus <= 1) return mhb_iterate_run(o);
+  if (int rc = iterate_check_opts(o)) return rc;
+  if (n_gpus > kMaxRanks) return mhb_set_error(MHB_ERR_ARG, "at most %d GPUs of one node are supported", kMaxRanks);
+  if (int rc = iterate_check_args(o->k, o->step)) return rc;
+  const double t0 = now_s();
+  HostSeqs seqs;  // loaded before the fork: no CUDA in this process
+  std::vector<uint32_t> bin;
+  uint64_t n_reads = 0;
+  if (int rc = iterate_load(o, &seqs, &bin, &n_reads)) return rc;
+  std::vector<uint64_t> rec_off;
+  if (!read_offsets(bin.data(), bin.size(), n_reads, &rec_off))
+    return mhb_set_error(MHB_ERR_IO, "%s ends inside a read", o->read_file);
+  IterJob J;
+  memset(&J.a, 0, sizeof(J.a));
+  J.a.k = o->k;
+  J.a.step = o->step;
+  if (seqs.words.empty()) seqs.words.push_back(0);
+  J.a.contig_words = seqs.words.data();
+  J.a.contig_word_off = seqs.word_off.data();
+  J.a.contig_len = seqs.len.data();
+  J.a.n_contigs = seqs.size();
+  J.a.bin = bin.data();
+  J.a.bin_words = bin.size();
+  J.a.n_reads = n_reads;
+  J.first.resize(n_gpus + 1);
+  plan_read_shares(bin.data(), rec_off, (uint32_t)n_gpus, J.first.data());
+  for (uint64_t f : J.first) J.word.push_back(rec_off[f]);
+  J.prefix = o->output_prefix;
+  J.fd = open((J.prefix + ".edges.0").c_str(), O_WRONLY | O_CREAT | O_TRUNC, 0666);
+  if (J.fd < 0) return mhb_set_error(MHB_ERR_IO, "cannot open %s.edges.0 for writing", J.prefix.c_str());
+  XINFO("%llu reads, %zu contigs; k = %u, step = %u; %d GPUs\n", (unsigned long long)n_reads, seqs.size(), o->k, o->step,
+        n_gpus);
+  const int rc = run_workers(n_gpus, "iterate", {}, [&](Exchange &X) { iter_worker(J, X); });
+  close(J.fd);
+  if (!rc) XINFO("iterate on %d GPUs done. Time elapsed: %.4f\n", n_gpus, now_s() - t0);
+  return rc;
+}
+
+extern "C" int mhb_plan_read_shares(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, uint32_t n_ranks,
+                                    uint64_t *first_out) {
+  if ((!bin && bin_words) || !first_out || n_ranks < 1) return mhb_set_error(MHB_ERR_ARG, "bad args");
+  std::vector<uint64_t> rec_off;
+  if (!read_offsets(bin, bin_words, n_reads, &rec_off)) return mhb_set_error(MHB_ERR_ARG, "the image ends inside a read");
+  plan_read_shares(bin, rec_off, n_ranks, first_out);
+  return MHB_OK;
 }
 
 extern "C" int mhb_plan_seq_shares(const uint32_t *len, uint64_t n_seqs, uint32_t k, uint32_t n_ranks, uint64_t *first_out) {

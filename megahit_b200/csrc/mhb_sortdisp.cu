@@ -206,6 +206,18 @@ static int sort_records_core(void *stream, uint32_t *a, uint32_t *b, uint64_t n,
   return MHB_OK;
 }
 
+int hist_byte(void *stream, const uint32_t *recs, uint64_t n, uint32_t words, int byte, uint64_t *hist) {
+  if (words < 1 || words > 17 || byte < 0 || byte >= (int)(4 * words)) return mhb_set_error(MHB_ERR_ARG, "bad geometry");
+  if (n == 0) return MHB_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+#define M(WW) \
+  if (words == WW) k_hist_byte<WW><<<sm_count() * 4, 256, 0, st>>>(recs, n, byte, hist);
+  MHB_FOR_WR(M)
+#undef M
+  CK_LAUNCH();
+  return MHB_OK;
+}
+
 // ------------------------------------------------------------------------------------------------
 // fused partition + exchange: one unstable partition pass whose per-owner destinations are arbitrary device addresses,
 // e.g. slots inside OTHER GPUs' receive buffers opened through CUDA IPC.  The scatter stores travel over NVLink while

@@ -146,7 +146,7 @@ SYMBOLS = [
     "mhb_mercy_candidates_scratch_bytes", "mhb_mercy_candidates", "mhb_mercy_edges_scratch_bytes", "mhb_mercy_edges", "mhb_mercy_edges_count", "mhb_mercy_edges_write", "mhb_mercy_edges_segs", "mhb_mercy_host", "mhb_mercy_planes_words", "mhb_mercy_probe_owned", "mhb_mercy_count_planes", "mhb_edge_lut_bytes", "mhb_edge_lut_build",
     "mhb_release", "mhb_count_run", "mhb_count_run_multi", "mhb_seq2sdbg_run", "mhb_seq2sdbg_run_multi",
     "mhb_plan_seq_shares", "mhb_s2s_extract_owners","mhb_selftest_count_record", "mhb_selftest_count_records_roll", "mhb_selftest_s2s_record",
-    "mhb_iterate_host", "mhb_iterate_run", "mhb_selftest_iterate", "mhb_s2s_extract_edges_pruned", "mhb_s2s_emit_fmt", "mhb_read2sdbg_host", "mhb_read2sdbg_run", "mhb_selftest_r2s_s1_record", "mhb_selftest_r2s_item",
+    "mhb_iterate_host", "mhb_iterate_run", "mhb_iterate_run_multi", "mhb_plan_read_shares", "mhb_selftest_iterate", "mhb_s2s_extract_edges_pruned", "mhb_s2s_emit_fmt", "mhb_read2sdbg_host", "mhb_read2sdbg_run", "mhb_selftest_r2s_s1_record", "mhb_selftest_r2s_item",
     "mhb_selftest_kmsort", "mhb_selftest_kmsort_smem", "mhb_selftest_r2s_s1_group", "mhb_selftest_r2s_mercy_read",
     "mhb_selftest_r2s_chunk_index", "mhb_selftest_r2s_stream_decide",
     "mhb_selftest_kmsort_narrow", "mhb_selftest_r2s_s1_plan", "mhb_selftest_read2sdbg_narrow", "mhb_selftest_iterate_narrow",
@@ -277,6 +277,8 @@ def load():
     L.mhb_iterate_host.argtypes = [C.POINTER(IterateArgs), C.POINTER(IterateResult)]
     L.mhb_selftest_iterate.argtypes = [C.POINTER(IterateArgs), C.POINTER(IterateResult)]
     L.mhb_iterate_run.argtypes = [C.POINTER(IterateOpts)]
+    L.mhb_iterate_run_multi.argtypes = [C.POINTER(IterateOpts), C.c_int]
+    L.mhb_plan_read_shares.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_void_p]
     L.mhb_s2s_extract_edges_pruned.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint32,
                                                C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_int]
     L.mhb_read2sdbg_host.argtypes = [C.POINTER(BuildArgs), C.POINTER(BuildResult)]
@@ -763,10 +765,22 @@ def iterate_host(contig_words: np.ndarray, contig_word_off: np.ndarray, contig_l
 
 
 def iterate_run(contig_file: str, bubble_file: str, read_file: str, output_prefix: str, k: int, step: int,
-                num_cpu_threads: int = 0) -> None:
+                num_cpu_threads: int = 0, gpus: int = 1) -> None:
+    """gpus > 1: mhb_iterate_run_multi, which forks one worker per GPU and so must be called from a process that has
+    not initialised CUDA (torch included); it writes the same P.edges.0 and P.edges.info as one GPU."""
     o = IterateOpts(contig_file.encode(), bubble_file.encode(), read_file.encode(), num_cpu_threads, k, step,
                     output_prefix.encode())
-    _check(load().mhb_iterate_run(C.byref(o)))
+    L = load()
+    _check(L.mhb_iterate_run_multi(C.byref(o), int(gpus)) if gpus > 1 else L.mhb_iterate_run(C.byref(o)))
+
+
+def plan_read_shares(bin_words: np.ndarray, n_reads: int, n_ranks: int) -> list[int]:
+    """The shares of a multi-GPU iterate (host logic only): the first read of every rank's share, then n_reads."""
+    L = load()
+    b = np.ascontiguousarray(bin_words, np.uint32).reshape(-1)
+    first = np.zeros(n_ranks + 1, np.uint64)
+    _check(L.mhb_plan_read_shares(b.ctypes.data if len(b) else None, len(b), n_reads, n_ranks, first.ctypes.data))
+    return [int(x) for x in first]
 
 
 def read2sdbg_run(read_lib_file: str, output_prefix: str, k: int = 21, m: int = 2, need_mercy: bool = False,
