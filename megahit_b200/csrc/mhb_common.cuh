@@ -26,3 +26,33 @@ extern unsigned long long g_mhb_launches;
 // SM count of the device this process is bound to (mhb_device.cu)
 int mhb_sm_count();
 static inline int sm_count() { return mhb_sm_count(); }
+
+// blocks for n items of per_block items each, at most blocks_per_sm per SM, at least 1
+static inline unsigned grid_cap(uint64_t n, uint64_t per_block, unsigned blocks_per_sm) {
+  const uint64_t g = std::min((n + per_block - 1) / per_block, (uint64_t)sm_count() * blocks_per_sm);
+  return (unsigned)std::max<uint64_t>(g, 1);
+}
+
+// ms between start() and stop() on one stream, from two CUDA events (stop waits for the stream to reach it)
+struct EventTimer {
+  cudaEvent_t a, b;
+  cudaStream_t st;
+  explicit EventTimer(cudaStream_t s = 0) : st(s) {
+    cudaEventCreate(&a);
+    cudaEventCreate(&b);
+  }
+  EventTimer(const EventTimer &) = delete;
+  EventTimer &operator=(const EventTimer &) = delete;
+  ~EventTimer() {
+    cudaEventDestroy(a);
+    cudaEventDestroy(b);
+  }
+  void start() { cudaEventRecord(a, st); }
+  double stop() {
+    cudaEventRecord(b, st);
+    cudaEventSynchronize(b);
+    float ms = 0;
+    cudaEventElapsedTime(&ms, a, b);
+    return ms;
+  }
+};

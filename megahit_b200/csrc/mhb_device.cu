@@ -155,8 +155,7 @@ extern "C" int mhb_count_extract(void *stream, const mhb_dev_reads *reads, uint3
   cudaStream_t st = (cudaStream_t)stream;
   const ReadsView rv = make_reads_view(reads);
   const u32 W = count_key_words(k), WR = count_record_words(k);
-  const u64 n_batches = (rv.n_reads + kReadsPerBatch - 1) / kReadsPerBatch;
-  const int grid = (int)(n_batches < (u64)(sm_count() * 8) ? n_batches : (u64)(sm_count() * 8));
+  const int grid = (int)grid_cap(rv.n_reads, kReadsPerBatch, 8);
   static const bool roll = getenv("MHB_EXTRACT_ROLL") && !strcmp(getenv("MHB_EXTRACT_ROLL"), "1");  // opt-in (no gain measured)
   if (roll && W == 2 && WR == 2 && k + 1 >= 17) {
     k_count_extract_roll<<<grid, kExtractThreads, 0, st>>>(rv, k, records, hist256, hist_byte);
@@ -192,8 +191,7 @@ extern "C" int mhb_count_extract_range(void *stream, const mhb_dev_reads *reads,
   }
   const ReadsView rv = make_reads_view(reads);
   const u32 W = count_key_words(k), WR = count_record_words(k);
-  const u64 n_batches = (rv.n_reads + kReadsPerBatch - 1) / kReadsPerBatch;
-  const int grid = (int)(n_batches < (u64)(sm_count() * 8) ? n_batches : (u64)(sm_count() * 8));
+  const int grid = (int)grid_cap(rv.n_reads, kReadsPerBatch, 8);
 #define M2(WW, WRR)                                                                                                   \
   if (W == WW && WR == WRR) {                                                                                         \
     if (write)                                                                                                        \
@@ -241,11 +239,11 @@ extern "C" int mhb_count_solid(void *stream, const uint32_t *sorted_records, uin
     u32 *ticket = (u32 *)p;                                                                                            \
     p += 256;                                                                                                          \
     uint2 *solid_list = (uint2 *)p;                                                                                    \
-    p += ((size_t)n_chunks * CH * 8 + 255) & ~(size_t)255;                                                             \
+    p += pad256((size_t)n_chunks * CH * 8);                                                                            \
     u32 *chunk_count = (u32 *)p;                                                                                       \
-    p += ((size_t)n_chunks * 4 + 255) & ~(size_t)255;                                                                  \
+    p += pad256((size_t)n_chunks * 4);                                                                                 \
     u64 *chunk_off = (u64 *)p;                                                                                         \
-    p += ((size_t)n_chunks * 8 + 255) & ~(size_t)255;                                                                  \
+    p += pad256((size_t)n_chunks * 8);                                                                                 \
     u64 *bsum = (u64 *)p;                                                                                              \
     CK(cudaMemsetAsync(ticket, 0, 256, st));                                                                           \
     const size_t smem = (size_t)kCount3Warps * count3_warp_words(WW) * 4;                                              \
@@ -266,9 +264,7 @@ extern "C" int mhb_count_solid(void *stream, const uint32_t *sorted_records, uin
     CK_LAUNCH();                                                                                                       \
     k_scan32_apply<<<(unsigned)n_sblk, kScanThreads, 0, st>>>(chunk_count, n_chunks, bsum, chunk_off);                 \
     CK_LAUNCH();                                                                                                       \
-    u64 gw = (n_chunks + 7) / 8;                                                                                       \
-    if (gw > (u64)sm_count() * 16) gw = (u64)sm_count() * 16;                                                          \
-    k_count_write<WW><<<(unsigned)gw, 256, 0, st>>>(sorted_records, k, (u32)n_chunks, solid_list, chunk_count,         \
+    k_count_write<WW><<<grid_cap(n_chunks, 8, 16), 256, 0, st>>>(sorted_records, k, (u32)n_chunks, solid_list, chunk_count, \
                                                     chunk_off, edges_out, aux_out, capacity_edges);                   \
   }
     MHB_FOR_WR(M)
@@ -304,7 +300,7 @@ static int small_scratch(unsigned long long **out) {
   int dev = 0;
   CK(cudaGetDevice(&dev));
   if (dev < 0 || dev >= 64) return mhb_set_error(MHB_ERR_CUDA, "device index %d out of range", dev);
-  if (!buf[dev]) CK(cudaMalloc((void **)&buf[dev], 256));
+  if (!buf[dev]) CK(cudaMalloc((void **)&buf[dev], 256));  // per device, kept for the life of the process
   *out = buf[dev];
   return MHB_OK;
 }
@@ -430,18 +426,16 @@ extern "C" int mhb_s2s_extract(void *stream, const mhb_dev_seqs *seqs, uint32_t 
   if (seqs->fixed_len == k + 1 && seqs->fixed_stride && !seqs->mult && k + 1 <= 32 && k + 1 > 16 &&
       n_items == seqs->n_seqs * 6) {
     // `.edges` records of short (k+1)-mers: one thread per edge, 64-bit arithmetic
-    u64 ge = (seqs->n_seqs + 255) / 256;
-    if (ge > (u64)sm_count() * 32) ge = (u64)sm_count() * 32;
-    if (W == 2) k_s2s_extract_edges<2><<<(unsigned)ge, 256, 0, st>>>(seqs->words, seqs->n_seqs, seqs->fixed_stride, k, records, hist256, hist_byte);
-    else if (W == 3) k_s2s_extract_edges<3><<<(unsigned)ge, 256, 0, st>>>(seqs->words, seqs->n_seqs, seqs->fixed_stride, k, records, hist256, hist_byte);
+    const unsigned ge = grid_cap(seqs->n_seqs, 256, 32);
+    if (W == 2) k_s2s_extract_edges<2><<<ge, 256, 0, st>>>(seqs->words, seqs->n_seqs, seqs->fixed_stride, k, records, hist256, hist_byte);
+    else if (W == 3) k_s2s_extract_edges<3><<<ge, 256, 0, st>>>(seqs->words, seqs->n_seqs, seqs->fixed_stride, k, records, hist256, hist_byte);
     else return mhb_set_error(MHB_ERR_ARG, "internal: unexpected record width %u", W);
     CK_LAUNCH();
     return MHB_OK;
   }
-  u64 g = (n_items + 255) / 256;
-  if (g > (u64)sm_count() * 32) g = (u64)sm_count() * 32;
+  const unsigned g = grid_cap(n_items, 256, 32);
 #define M(WW) \
-  if (W == WW) k_s2s_extract<WW><<<(unsigned)g, 256, 0, st>>>(sv, k, records, n_items, hist256, hist_byte);
+  if (W == WW) k_s2s_extract<WW><<<g, 256, 0, st>>>(sv, k, records, n_items, hist256, hist_byte);
   MHB_FOR_WR(M)
 #undef M
   CK_LAUNCH();
@@ -456,11 +450,10 @@ extern "C" int mhb_s2s_extract_edges_pruned(void *stream, const uint32_t *edges,
   if (n_edges == 0) return MHB_OK;
   cudaStream_t st = (cudaStream_t)stream;
   const u32 W = s2s_record_words(k), WE = words_per_edge(k);
-  u64 g = (n_edges + 255) / 256;
-  if (g > (u64)sm_count() * 32) g = (u64)sm_count() * 32;
+  const unsigned g = grid_cap(n_edges, 256, 32);
 #define M(WW)                                                                                                        \
   if (W == WW)                                                                                                       \
-    k_s2s_extract_edges_pruned<WW><<<(unsigned)g, 256, 0, st>>>(edges, aux, n_edges, n_with_aux, WE, k, records,       \
+    k_s2s_extract_edges_pruned<WW><<<g, 256, 0, st>>>(edges, aux, n_edges, n_with_aux, WE, k, records,               \
                                                                (unsigned long long *)cursor_dev, capacity, hist256, hist_byte);
   MHB_FOR_WR(M)
 #undef M
@@ -483,10 +476,9 @@ static int launch_extract_range(cudaStream_t st, const mhb_dev_seqs *seqs, uint3
   if (seqs->fixed_len && seqs->fixed_len < k + 1) return mhb_set_error(MHB_ERR_ARG, "fixed_len < k+1");
   const SeqsView sv = make_seqs_view(seqs);
   const u32 W = s2s_record_words(k);
-  u64 g = (n_items + 255) / 256;
-  if (g > (u64)sm_count() * 32) g = (u64)sm_count() * 32;
+  const unsigned g = grid_cap(n_items, 256, 32);
 #define M(WW) \
-  if (W == WW) k_s2s_extract_range<WW, Sink><<<(unsigned)g, 256, 0, st>>>(sv, k, n_items, lo, hi, sink, hist256, hist_byte);
+  if (W == WW) k_s2s_extract_range<WW, Sink><<<g, 256, 0, st>>>(sv, k, n_items, lo, hi, sink, hist256, hist_byte);
   MHB_FOR_WR(M)
 #undef M
   CK_LAUNCH();
@@ -584,7 +576,7 @@ extern "C" int mhb_s2s_emit_fmt(void *stream, const uint32_t *sorted_records, ui
     u64 *bsum = (u64 *)p;
     p += (size_t)(nc / kScanTile + 2) * 8;
     u32 *chunk_tot = (u32 *)p;
-    p += ((size_t)nc * 4 * 4 + 255) & ~(size_t)255;
+    p += pad256((size_t)nc * 4 * 4);
     uint8_t *tmp = (uint8_t *)p;
     CK(cudaMemsetAsync(bucket_local, 0xFF, (size_t)MHB_NUM_BUCKETS * 5 * 4, st));
 #define M(WW)                                                                                                       \
@@ -606,9 +598,7 @@ extern "C" int mhb_s2s_emit_fmt(void *stream, const uint32_t *sorted_records, ui
     CK_LAUNCH();
     for (int q = 0; q < 4; ++q)
       if (int rc = scan32(st, chunk_tot + (u64)q * nc, nc, chunk_off + (u64)q * nc, totals + q, bsum)) return rc;
-    u64 gg = (nc + 7) / 8;
-    if (gg > (u64)sm_count() * 16) gg = (u64)sm_count() * 16;
-    k_s2s_gather<<<(unsigned)gg, 256, 0, st>>>(tmp, chrec, maxb, (u32)nc, chunk_tot, chunk_off, bytes_out, capacity_bytes);
+    k_s2s_gather<<<grid_cap(nc, 8, 16), 256, 0, st>>>(tmp, chrec, maxb, (u32)nc, chunk_tot, chunk_off, bytes_out, capacity_bytes);
     CK_LAUNCH();
     k_bucket_starts<<<64, 256, 0, st>>>(bucket_local, chunk_off, nc, bucket_start);
     CK_LAUNCH();
@@ -669,9 +659,9 @@ extern "C" int mhb_mercy_candidates(void *stream, const uint32_t *first_0_out, c
   u64 *total = (u64 *)p;
   p += 256;
   u32 *flag = (u32 *)p;
-  p += ((size_t)n_reads * 4 + 255) & ~(size_t)255;
+  p += pad256((size_t)n_reads * 4);
   u64 *off = (u64 *)p;
-  p += ((size_t)n_reads * 8 + 255) & ~(size_t)255;
+  p += pad256((size_t)n_reads * 8);
   u64 *bsum = (u64 *)p;
   const unsigned g = (unsigned)((n_reads + 255) / 256);
   k_cand_flags<<<g, 256, 0, st>>>(first_0_out, last_0_in, n_reads, flag);
@@ -692,7 +682,7 @@ size_t mercy_core_scratch(uint64_t n_cand, uint32_t max_read_len) {
 // scratch for mhb_mercy_edges (single segment: includes room for its look-up table); the segmented call needs
 // this minus mhb_edge_lut_bytes()
 extern "C" size_t mhb_mercy_edges_scratch_bytes(uint64_t n_cand, uint32_t max_read_len) {
-  return ((mercy_core_scratch(n_cand, max_read_len) + 255) & ~(size_t)255) + 512 + mhb_edge_lut_bytes();
+  return pad256(mercy_core_scratch(n_cand, max_read_len)) + 512 + mhb_edge_lut_bytes();
 }
 
 extern "C" size_t mhb_edge_lut_bytes(void) { return (size_t)kLutEntries * sizeof(uint2); }
@@ -702,9 +692,7 @@ extern "C" int mhb_edge_lut_build(void *stream, const uint32_t *edges, uint64_t 
   cudaStream_t st = (cudaStream_t)stream;
   CK(cudaMemsetAsync(lut, 0xFF, mhb_edge_lut_bytes(), st));
   if (n_edges == 0) return MHB_OK;
-  u64 g = (n_edges + 255) / 256;
-  if (g > (u64)sm_count() * 16) g = (u64)sm_count() * 16;
-  k_edge_lut<<<(unsigned)g, 256, 0, st>>>(edges, n_edges, words_per_edge(k), (uint2 *)lut);
+  k_edge_lut<<<grid_cap(n_edges, 256, 16), 256, 0, st>>>(edges, n_edges, words_per_edge(k), (uint2 *)lut);
   CK_LAUNCH();
   return MHB_OK;
 }
@@ -716,11 +704,11 @@ MercyScratch mercy_scratch_layout(void *scratch, uint64_t n_cand, uint32_t max_r
   m.total = (u64 *)p;
   p += 256;
   m.bits = (u32 *)p;
-  p += ((size_t)n_cand * 3 * m.wpr * 4 + 255) & ~(size_t)255;
+  p += pad256((size_t)n_cand * 3 * m.wpr * 4);
   m.count = (u32 *)p;
-  p += ((size_t)n_cand * 4 + 255) & ~(size_t)255;
+  p += pad256((size_t)n_cand * 4);
   m.off = (u64 *)p;
-  p += ((size_t)n_cand * 8 + 255) & ~(size_t)255;
+  p += pad256((size_t)n_cand * 8);
   m.bsum = (u64 *)p;
   return m;
 }
@@ -751,10 +739,9 @@ extern "C" int mhb_mercy_edges_count(void *stream, const mhb_dev_reads *reads, c
   }
   const u32 WE = words_per_edge(k), WM = div_ceil(k + 1, 16);
   const MercyScratch ms = mercy_scratch_layout(scratch, n_cand, max_read_len);
-  u64 g64 = (n_cand + 7) / 8;
-  if (g64 > (u64)sm_count() * 16) g64 = (u64)sm_count() * 16;
+  const unsigned g64 = grid_cap(n_cand, 8, 16);
 #define M(WW) \
-  if (WM == WW) k_mercy_probe<WW><<<(unsigned)g64, 256, 0, st>>>(rv, cand_ids, n_cand, k, sg, WE, ms.bits, ms.wpr);
+  if (WM == WW) k_mercy_probe<WW><<<g64, 256, 0, st>>>(rv, cand_ids, n_cand, k, sg, WE, ms.bits, ms.wpr);
   MHB_FOR_W(M)
 #undef M
   CK_LAUNCH();
@@ -803,7 +790,7 @@ extern "C" int mhb_mercy_edges(void *stream, const mhb_dev_reads *reads, const u
   *n_mercy_host = 0;
   if (n_cand == 0) return MHB_OK;
   // single segment: the look-up table lives behind the core scratch in the caller's buffer
-  const size_t core = (mercy_core_scratch(n_cand, max_read_len) + 255) & ~(size_t)255;
+  const size_t core = pad256(mercy_core_scratch(n_cand, max_read_len));
   if (scratch_bytes < core + mhb_edge_lut_bytes()) return mhb_set_error(MHB_ERR_ARG, "scratch too small");
   void *lut = (char *)scratch + core;
   if (int rc = mhb_edge_lut_build(stream, edges, n_edges, k, lut)) return rc;

@@ -251,53 +251,17 @@ __global__ void k_fx_zip(const u32 *pa, const u32 *pb, const u64 *oa, const u64 
   }
 }
 
-unsigned grid_for(u64 n, unsigned per_block) {
-  u64 g = (n + per_block - 1) / per_block;
-  const u64 cap = (u64)sm_count() * 32;
-  return (unsigned)std::max<u64>(1, std::min(g, cap));
-}
-
-struct DBuf {
-  void *p = nullptr;
-  size_t cap = 0;
-  ~DBuf() {
-    if (p) cudaFree(p);
-  }
-  int need(size_t b) {
-    b = (b + 255) & ~(size_t)255;
-    if (b <= cap && p) return MHB_OK;
-    if (p) cudaFree(p);
-    p = nullptr;
-    cap = 0;
-    b = std::max<size_t>(b, 256);
-    if (cudaMalloc(&p, b) != cudaSuccess) {
-      cudaGetLastError();
-      return mhb_set_error(MHB_ERR_NOMEM, "buildlib: cudaMalloc of %zu bytes failed", b);
-    }
-    cap = b;
-    return MHB_OK;
-  }
-  template <class T>
-  T *as() const { return reinterpret_cast<T *>(p); }
-};
-
-#define CKR(call)        \
-  do {                   \
-    int rc_ = (call);    \
-    if (rc_) return rc_; \
-  } while (0)
-
 // scan32 with its per-4096-input block sums in `bsum`, grown to fit n first (every scan of a chunk has its own n: tiles,
 // segments, records, pairs)
-int scan_n(cudaStream_t st, const u32 *in, u64 n, u64 *out, u64 *total_dev, DBuf &bsum) {
-  CKR(bsum.need((n / 4096 + 4) * 8));
+int scan_n(cudaStream_t st, const u32 *in, u64 n, u64 *out, u64 *total_dev, DevBuf &bsum) {
+  CKR(bsum.ensure((n / 4096 + 4) * 8, "buildlib"));
   return scan32(st, in, n, out, total_dev, bsum.as<u64>());
 }
 
 // One chunk of one stream parsed on the device.  The packed reads stay on the device (pack, at woff[r]); the host gets
 // per record its trimmed length (kErrLen = error) and where the stream resumes after it.
 struct FxChunk {
-  DBuf text, tcnt, toff, bsum, tot, nl, seg, entry, exit_st, count, dirty, ndirty, roff, rec, bpos, len, words, woff, pack;
+  DevBuf text, tcnt, toff, bsum, tot, nl, seg, entry, exit_st, count, dirty, ndirty, roff, rec, bpos, len, words, woff, pack;
   std::vector<FxRec> h_rec;
   std::vector<u32> h_len;
   u64 n_rec = 0, n_words = 0, n_lines = 0;
@@ -306,12 +270,12 @@ struct FxChunk {
 
   // text[0, n): complete lines (plus an unterminated last line when final); the carried state is SEEK or HDR
   int parse(cudaStream_t st, const uint8_t *h_text, u64 n, int final_chunk, u32 carry_mode) {
-    CKR(text.need(n + 16));
+    CKR(text.ensure(n + 16, "buildlib"));
     if (n) CK(cudaMemcpyAsync(text.p, h_text, n, cudaMemcpyHostToDevice, st));
     const u64 tiles = std::max<u64>(1, (n + kTile - 1) / kTile);
-    CKR(tcnt.need(tiles * 4));
-    CKR(toff.need(tiles * 8));
-    CKR(tot.need(64));
+    CKR(tcnt.ensure(tiles * 4, "buildlib"));
+    CKR(toff.ensure(tiles * 8, "buildlib"));
+    CKR(tot.ensure(64, "buildlib"));
     CK(cudaMemsetAsync(tcnt.p, 0, tiles * 4, st));
     if (n) {
       k_nl_count<<<(unsigned)tiles, 256, 0, st>>>(text.as<uint8_t>(), n, tcnt.as<u32>());
@@ -321,7 +285,7 @@ struct FxChunk {
     u64 n_nl = 0;
     CK(cudaMemcpyAsync(&n_nl, tot.p, 8, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
-    CKR(nl.need((n_nl + 1) * 8));
+    CKR(nl.ensure((n_nl + 1) * 8, "buildlib"));
     if (n) {
       k_nl_write<<<(unsigned)tiles, 256, 0, st>>>(text.as<uint8_t>(), n, toff.as<u64>(), nl.as<u64>());
       CK_LAUNCH();
@@ -331,13 +295,13 @@ struct FxChunk {
     if (n_lines >= 0xFFFFFFF0ull) return mhb_set_error(MHB_ERR_ARG, "buildlib: a chunk of more than 2^32 lines");
     FxLines L{text.as<uint8_t>(), nl.as<u64>(), (u32)n_lines, n, final_chunk};
     const u32 n_seg = (u32)std::max<u64>(1, (n_lines + kSegLines - 1) / kSegLines);
-    CKR(seg.need((n_seg + 1) * 4));
-    CKR(entry.need(n_seg * sizeof(FxState)));
-    CKR(exit_st.need(n_seg * sizeof(FxState)));
-    CKR(count.need(n_seg * 4));
-    CKR(dirty.need(n_seg * 4));
-    CKR(ndirty.need(8));
-    CKR(roff.need(n_seg * 8));
+    CKR(seg.ensure((n_seg + 1) * 4, "buildlib"));
+    CKR(entry.ensure(n_seg * sizeof(FxState), "buildlib"));
+    CKR(exit_st.ensure(n_seg * sizeof(FxState), "buildlib"));
+    CKR(count.ensure(n_seg * 4, "buildlib"));
+    CKR(dirty.ensure(n_seg * 4, "buildlib"));
+    CKR(ndirty.ensure(8, "buildlib"));
+    CKR(roff.ensure(n_seg * 8, "buildlib"));
     const unsigned gs = (n_seg + 1 + 255) / 256, gw = (n_seg + 127) / 128;
     k_fx_seg_start<<<gs, 256, 0, st>>>(L, n_seg, seg.as<u32>());
     CK_LAUNCH();
@@ -366,24 +330,24 @@ struct FxChunk {
     CK(cudaMemcpyAsync(&n_rec, tot.p, 8, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(&exit_last, exit_st.as<FxState>() + (n_seg - 1), sizeof(FxState), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
-    CKR(rec.need((n_rec + 1) * sizeof(FxRec)));
-    CKR(bpos.need((n_rec + 1) * 4));
-    CKR(len.need((n_rec + 1) * 4));
-    CKR(words.need((n_rec + 1) * 4));
-    CKR(woff.need((n_rec + 1) * 8));
+    CKR(rec.ensure((n_rec + 1) * sizeof(FxRec), "buildlib"));
+    CKR(bpos.ensure((n_rec + 1) * 4, "buildlib"));
+    CKR(len.ensure((n_rec + 1) * 4, "buildlib"));
+    CKR(words.ensure((n_rec + 1) * 4, "buildlib"));
+    CKR(woff.ensure((n_rec + 1) * 8, "buildlib"));
     n_words = 0;
     if (n_rec) {
       k_fx_walk<<<gw, 128, 0, st>>>(L, n_seg, seg.as<u32>(), entry.as<FxState>(), exit_st.as<FxState>(), count.as<u32>(),
                                     nullptr, 1, roff.as<u64>(), rec.as<FxRec>());
       CK_LAUNCH();
-      k_fx_trim<<<grid_for(n_rec * 32, 256), 256, 0, st>>>(L, rec.as<FxRec>(), n_rec, bpos.as<u32>(), len.as<u32>(),
+      k_fx_trim<<<grid_cap(n_rec * 32, 256, 32), 256, 0, st>>>(L, rec.as<FxRec>(), n_rec, bpos.as<u32>(), len.as<u32>(),
                                                              words.as<u32>());
       CK_LAUNCH();
       CKR(scan_n(st, words.as<u32>(), n_rec, woff.as<u64>(), tot.as<u64>(), bsum));
       CK(cudaMemcpyAsync(&n_words, tot.p, 8, cudaMemcpyDeviceToHost, st));
       CK(cudaStreamSynchronize(st));
-      CKR(pack.need(n_words * 4 + 16));
-      k_fx_pack<<<grid_for(n_rec * 32, 256), 256, 0, st>>>(L, rec.as<FxRec>(), n_rec, bpos.as<u32>(), len.as<u32>(),
+      CKR(pack.ensure(n_words * 4 + 16, "buildlib"));
+      k_fx_pack<<<grid_cap(n_rec * 32, 256, 32), 256, 0, st>>>(L, rec.as<FxRec>(), n_rec, bpos.as<u32>(), len.as<u32>(),
                                                              woff.as<u64>(), pack.as<u32>());
       CK_LAUNCH();
     }
@@ -569,7 +533,7 @@ int do_se(cudaStream_t st, FxInput &in, u64 chunk0, LibOut &out) {
 int do_pe(cudaStream_t st, FxInput &ia, FxInput &ib, u64 chunk0, LibOut &out) {
   FxChunk ca, cb;
   BatchState bs;
-  DBuf w, off, tot, bsum, zip;
+  DevBuf w, off, tot, bsum, zip;
   u64 chunk_a = chunk0, chunk_b = chunk0;
   for (;;) {
     u64 na, nb;
@@ -610,18 +574,18 @@ int do_pe(cudaStream_t st, FxInput &ia, FxInput &ib, u64 chunk0, LibOut &out) {
       if (bs.bases >= kBatchBases || bs.i >= kBatchReads) bs.i = bs.bases = 0;
     }
     if (m) {
-      CKR(w.need(m * 4));
-      CKR(off.need(m * 8));
-      CKR(tot.need(64));
-      k_fx_zip_words<<<grid_for(m, 256), 256, 0, st>>>(ca.len.as<u32>(), cb.len.as<u32>(), ca.words.as<u32>(),
+      CKR(w.ensure(m * 4, "buildlib"));
+      CKR(off.ensure(m * 8, "buildlib"));
+      CKR(tot.ensure(64, "buildlib"));
+      k_fx_zip_words<<<grid_cap(m, 256, 32), 256, 0, st>>>(ca.len.as<u32>(), cb.len.as<u32>(), ca.words.as<u32>(),
                                                        cb.words.as<u32>(), m, stop, w.as<u32>());
       CK_LAUNCH();
       CKR(scan_n(st, w.as<u32>(), m, off.as<u64>(), tot.as<u64>(), bsum));
       u64 words = 0;
       CK(cudaMemcpyAsync(&words, tot.p, 8, cudaMemcpyDeviceToHost, st));
       CK(cudaStreamSynchronize(st));
-      CKR(zip.need(words * 4 + 16));
-      k_fx_zip<<<grid_for(m * 32, 256), 256, 0, st>>>(ca.pack.as<u32>(), cb.pack.as<u32>(), ca.woff.as<u64>(),
+      CKR(zip.ensure(words * 4 + 16, "buildlib"));
+      k_fx_zip<<<grid_cap(m * 32, 256, 32), 256, 0, st>>>(ca.pack.as<u32>(), cb.pack.as<u32>(), ca.woff.as<u64>(),
                                                       cb.woff.as<u64>(), ca.words.as<u32>(), w.as<u32>(), off.as<u64>(), m,
                                                       zip.as<u32>());
       CK_LAUNCH();

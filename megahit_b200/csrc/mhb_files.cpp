@@ -278,6 +278,14 @@ int write_sdbg_single(const std::string &prefix, uint32_t k, uint32_t words_per_
 
 }  // namespace
 
+int load_read_lib(const std::string &prefix, std::vector<uint32_t> *bin, long long *n_reads, long long *total_bases) {
+  {
+    std::ifstream is(prefix + ".lib_info");
+    if (!(is >> *total_bases >> *n_reads)) return mhb_set_error(MHB_ERR_IO, "cannot read %s.lib_info", prefix.c_str());
+  }
+  return read_file(prefix + ".bin", bin) ? MHB_OK : MHB_ERR_IO;
+}
+
 // ================================================================================================
 // count
 // ================================================================================================
@@ -287,12 +295,8 @@ extern "C" int mhb_count_run(const mhb_count_opts *o) {
   const std::string lib = o->read_lib_file, prefix = o->output_prefix ? o->output_prefix : "out";
   const double t0 = now_s();
   long long total_bases = 0, n_reads = 0;
-  {
-    std::ifstream is(lib + ".lib_info");
-    if (!(is >> total_bases >> n_reads)) return mhb_set_error(MHB_ERR_IO, "cannot read %s.lib_info", lib.c_str());
-  }
   std::vector<uint32_t> bin;
-  if (!read_file(lib + ".bin", &bin)) return MHB_ERR_IO;
+  if (int rc = load_read_lib(lib, &bin, &n_reads, &total_bases)) return rc;
   XINFO("%lld reads, %lld bases; k = %u, m = %d\n", n_reads, total_bases, o->k, o->m);
 
   mhb_count_args a;
@@ -489,12 +493,8 @@ extern "C" int mhb_read2sdbg_run(const mhb_read2sdbg_opts *o) {
   const std::string lib = o->read_lib_file, prefix = o->output_prefix ? o->output_prefix : "out";
   const double t0 = now_s();
   long long total_bases = 0, n_reads = 0;
-  {
-    std::ifstream is(lib + ".lib_info");
-    if (!(is >> total_bases >> n_reads)) return mhb_set_error(MHB_ERR_IO, "cannot read %s.lib_info", lib.c_str());
-  }
   std::vector<uint32_t> bin;
-  if (!read_file(lib + ".bin", &bin)) return MHB_ERR_IO;
+  if (int rc = load_read_lib(lib, &bin, &n_reads, &total_bases)) return rc;
   XINFO("%lld reads, %lld total bases; k = %u, m = %d, need_mercy = %d\n", n_reads, total_bases, o->k, o->m, o->need_mercy);
   // the candidate files stage 1 hands to stage 2 inside the reference process (read_to_sdbg_s1.cpp:111-126: 1, 2, 4 .. 64
   // files by read count); here the candidates never leave the device (three bit planes), the files are created empty so

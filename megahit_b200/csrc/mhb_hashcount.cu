@@ -537,32 +537,31 @@ struct HcLayout {
 };
 HcLayout hc_layout(uint64_t n, int32_t m) {
   HcLayout L;
-  auto pad = [](size_t x) { return (x + 255) & ~(size_t)255; };
   L.max_slices = n / HcGeomB::SLICE + 65536 + 2;  // sum over the buckets of ceil(n_b / SLICE) <= n / SLICE + 65536
-  L.sort_ws = pad(mhb_sort_workspace_bytes(n, 2));
+  L.sort_ws = pad256(mhb_sort_workspace_bytes(n, 2));
   size_t p = L.sort_ws;
   L.off_bounds = p;
-  p += pad(65537 * 8);
+  p += pad256(65537 * 8);
   L.off_bcnt = p;
-  p += pad(65537 * 4);
+  p += pad256(65537 * 4);
   L.off_soff = p;
-  p += pad(65537 * 8);
+  p += pad256(65537 * 8);
   L.off_bsum = p;
-  p += pad((L.max_slices / kScanTile + 4) * 8);
+  p += pad256((L.max_slices / kScanTile + 4) * 8);
   L.off_misc = p;
   p += 256;
   L.off_scount = p;
-  p += pad(L.max_slices * 4);
+  p += pad256(L.max_slices * 4);
   L.off_sdst = p;
-  p += pad(L.max_slices * 8);
+  p += pad256(L.max_slices * 8);
   L.off_sbase = p;
-  p += pad(L.max_slices * 8);
+  p += pad256(L.max_slices * 8);
   L.off_sbucket = p;
-  p += pad(L.max_slices * 4);
+  p += pad256(L.max_slices * 4);
   L.off_plan = p;
-  p += pad(L.max_slices * 16);
+  p += pad256(L.max_slices * 16);
   L.off_list = p;
-  p += pad((size_t)(n / (uint64_t)(m < 1 ? 1 : m) + L.max_slices + 8) * 8);
+  p += pad256((size_t)(n / (uint64_t)(m < 1 ? 1 : m) + L.max_slices + 8) * 8);
   L.total = p;
   return L;
 }

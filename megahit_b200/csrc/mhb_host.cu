@@ -11,22 +11,9 @@
 
 #include "mhb.h"
 #include "mhb_bits.cuh"
-#include "mhb_internal.h"
+#include "mhb_common.cuh"
 
 using namespace mhb;
-
-#define CK(call)                                                                                   \
-  do {                                                                                             \
-    cudaError_t e_ = (call);                                                                       \
-    if (e_ != cudaSuccess)                                                                         \
-      return mhb_set_error(MHB_ERR_CUDA, "%s failed at %s:%d: %s", #call, __FILE__, __LINE__,      \
-                           cudaGetErrorString(e_));                                                \
-  } while (0)
-#define CKR(call)           \
-  do {                      \
-    int rc_ = (call);       \
-    if (rc_) return rc_;    \
-  } while (0)
 
 namespace {
 
@@ -49,35 +36,15 @@ struct Arena {
   }
   template <class T>
   T *take(size_t count) {
-    size_t bytes = (count * sizeof(T) + 255) & ~(size_t)255;
     char *p = base + used;
-    used += bytes;
+    used += pad256(count * sizeof(T));
     return reinterpret_cast<T *>(p);
   }
-  static size_t pad(size_t bytes) { return (bytes + 255) & ~(size_t)255; }
 };
 Arena g_arena;
 
-struct Timer {
-  cudaEvent_t a, b;
-  cudaStream_t st;
-  explicit Timer(cudaStream_t s) : st(s) {
-    cudaEventCreate(&a);
-    cudaEventCreate(&b);
-  }
-  ~Timer() {
-    cudaEventDestroy(a);
-    cudaEventDestroy(b);
-  }
-  void start() { cudaEventRecord(a, st); }
-  double stop() {
-    cudaEventRecord(b, st);
-    cudaEventSynchronize(b);
-    float ms = 0;
-    cudaEventElapsedTime(&ms, a, b);
-    return ms;
-  }
-};
+// what a plan may take: 92 % of the free device memory and of the arena, which the call may reallocate
+double arena_avail_bytes() { return 0.92 * (double)(free_device_bytes() + g_arena.cap); }
 
 }  // namespace
 
@@ -136,8 +103,8 @@ CountWork count_work_plan(uint64_t n, uint32_t k, int32_t m) {
   } else {
     uint8_t sb[72];
     mhb_count_sort_bytes(k, sb);
-    cw.ws_bytes = Arena::pad(mhb_sort_workspace_bytes(n, count_record_words(k)));
-    cw.bytes = cw.ws_bytes + Arena::pad(mhb_count_solid_scratch_bytes(n));
+    cw.ws_bytes = pad256(mhb_sort_workspace_bytes(n, count_record_words(k)));
+    cw.bytes = cw.ws_bytes + pad256(mhb_count_solid_scratch_bytes(n));
     cw.hist_byte = sb[0];
   }
   return cw;
@@ -170,8 +137,8 @@ namespace {
 // bytes of device memory one round of `n` records needs besides the read library
 size_t round_bytes(uint64_t n, uint32_t WR, uint32_t WE, int32_t m, uint32_t k) {
   const uint64_t cap_edges = n / (uint64_t)std::max(1, m) + 1;
-  return 2 * Arena::pad((size_t)n * WR * 4 + 16) + Arena::pad(count_work_plan(n, k, m).bytes) +
-         Arena::pad((size_t)cap_edges * WE * 4) + Arena::pad(cap_edges);
+  return 2 * pad256((size_t)n * WR * 4 + 16) + pad256(count_work_plan(n, k, m).bytes) +
+         pad256((size_t)cap_edges * WE * 4) + pad256(cap_edges);
 }
 }  // namespace
 
@@ -314,7 +281,7 @@ static int count_host_rounds(const mhb_count_args *args, mhb_count_result *res, 
   const uint32_t WR = count_record_words(k), WE = words_per_edge(k);
   const int top_byte = (int)(4 * WR - 1);
   cudaStream_t st = 0;
-  Timer t_all(st), t(st);
+  EventTimer t_all(st), t(st);
   t_all.start();
   auto restart_streamed = [&]() {
     const uint32_t we = res->words_per_edge;
@@ -330,26 +297,22 @@ static int count_host_rounds(const mhb_count_args *args, mhb_count_result *res, 
   CKR(rs.init(args->bin, args->bin_words, n_reads, ix, stream ? chunk_cap : 0));
   const uint64_t chunk_reads = rs.max_chunk_reads();  // reads the per-read arrays hold
   // besides the round buffers: the library (or its chunk slots), the mercy marks, the histograms and scalars
-  size_t fixed = Arena::pad(rs.device_bytes()) + Arena::pad(65536 * 8) + Arena::pad(256 * 8) + 4096;
-  if (args->want_mercy) fixed += 2 * Arena::pad((size_t)(chunk_reads + 1) * 4);
+  size_t fixed = pad256(rs.device_bytes()) + pad256(65536 * 8) + pad256(256 * 8) + 4096;
+  if (args->want_mercy) fixed += 2 * pad256((size_t)(chunk_reads + 1) * 4);
   bool one_pass = false;
   if (!stream && !(g_round_limit && n > g_round_limit)) {
     const size_t need = fixed + round_bytes(n, WR, WE, m, k);
     one_pass = need <= g_arena.cap;
     if (!one_pass) {
-      size_t free_b = 0, total_b = 0;
-      CK(cudaMemGetInfo(&free_b, &total_b));
-      one_pass = (double)need <= 0.92 * (double)(free_b + g_arena.cap);
+      one_pass = (double)need <= arena_avail_bytes();
     }
   }
   uint64_t max_records = n;
   if (!one_pass) {  // + the per-read counts of the extraction and the second-byte histograms
-    fixed += Arena::pad((chunk_reads + 2) * 8) + Arena::pad(256 * 256 * 8) + Arena::pad(256 * 8) + Arena::pad(64) + 4096;
+    fixed += pad256((chunk_reads + 2) * 8) + pad256(256 * 256 * 8) + pad256(256 * 8) + pad256(64) + 4096;
     max_records = g_round_limit;
     if (!max_records) {
-      size_t free_b = 0, total_b = 0;
-      CK(cudaMemGetInfo(&free_b, &total_b));
-      const size_t avail = (size_t)((double)(free_b + g_arena.cap) * 0.92);
+      const size_t avail = (size_t)arena_avail_bytes();
       if (!stream && mhb_read_stream_decide(fixed, avail, 0, read_chunk_limit())) return restart_streamed();
       max_records = largest_round(n, fixed, avail, [&](uint64_t r) { return round_bytes(r, WR, WE, m, k); });
       if (!max_records)
@@ -531,18 +494,16 @@ static int count_host_rounds(const mhb_count_args *args, mhb_count_result *res, 
     uint64_t n_tip = h_tip_aux.size();
     if (tips_on_device) CKR(mhb_count_tip_edges(st, d_aux, n_solid_total, &n_tip));
     const size_t ts_bytes = mhb_tipset_bytes(n_tip, k);
-    const size_t list_bytes = Arena::pad(h_tip_edges.size() * 4 + 16) + Arena::pad(h_tip_aux.size() + 16);
+    const size_t list_bytes = pad256(h_tip_edges.size() * 4 + 16) + pad256(h_tip_aux.size() + 16);
     // the per-round buffers are free now
-    char *d_tmp = nullptr;
-    bool own = false;
-    const size_t have = (size_t)max_records * WR * 4 * 2;
-    if (ts_bytes + list_bytes + 512 <= have) d_tmp = (char *)d_a;
-    else {
-      CK(cudaMalloc((void **)&d_tmp, ts_bytes + list_bytes + 512));
-      own = true;
+    DevBuf own;
+    char *d_tmp = (char *)d_a;
+    if (ts_bytes + list_bytes + 512 > (size_t)max_records * WR * 4 * 2) {
+      CKR(own.alloc(ts_bytes + list_bytes + 512, "count: mercy tip set"));
+      d_tmp = own.as<char>();
     }
     const uint32_t *d_tip_edges = tips_on_device ? d_edges : (uint32_t *)d_tmp;
-    const uint8_t *d_tip_aux = tips_on_device ? d_aux : (uint8_t *)(d_tmp + Arena::pad(h_tip_edges.size() * 4 + 16));
+    const uint8_t *d_tip_aux = tips_on_device ? d_aux : (uint8_t *)(d_tmp + pad256(h_tip_edges.size() * 4 + 16));
     char *d_tips = d_tmp + list_bytes;
     int rc = MHB_OK;
     if (!h_tip_aux.empty()) {
@@ -563,7 +524,7 @@ static int count_host_rounds(const mhb_count_args *args, mhb_count_result *res, 
       if (cudaStreamSynchronize(st) != cudaSuccess) return mhb_set_error(MHB_ERR_CUDA, "mercy marking failed: %s", cudaGetErrorString(cudaGetLastError()));
       return MHB_OK;
     });
-    if (own) cudaFree(d_tmp);
+    own.release();
     if (rc) return rc;
     res->t_mercy_ms = t.stop();
   }
@@ -624,22 +585,14 @@ StreamStats g_s2s_st, g_mercy_st;
 uint64_t g_s2s_rounds = 0;
 
 size_t s2s_round_bytes(uint64_t n, uint32_t W, uint32_t k) {
-  return 2 * Arena::pad((size_t)n * W * 4 + 16) + Arena::pad(mhb_s2s_sort_workspace_bytes(n, k)) +
-         Arena::pad(mhb_s2s_emit_scratch_bytes(n, k)) + Arena::pad((size_t)n * (4ull + 4ull * words_per_tip_label(k)) + 16);
+  return 2 * pad256((size_t)n * W * 4 + 16) + pad256(mhb_s2s_sort_workspace_bytes(n, k)) +
+         pad256(mhb_s2s_emit_scratch_bytes(n, k)) + pad256((size_t)n * (4ull + 4ull * words_per_tip_label(k)) + 16);
 }
 // what the rounds keep next to the sequences: bucket table, the histogram of the sort's first byte, totals and, to plan
 // rounds, the top-byte histogram, the second-byte rows of oversized bytes and the cursor
 size_t s2s_table_bytes(bool plan) {
-  return Arena::pad((size_t)MHB_NUM_BUCKETS * 4 * 8) + Arena::pad(256 * 8) + Arena::pad(16 * 8) +
-         (plan ? Arena::pad(256 * 8) + Arena::pad(256 * 256 * 8) + Arena::pad(64) + 8192 : 4096);
-}
-double device_avail_bytes() {
-  size_t free_b = 0, total_b = 0;
-  if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) {
-    cudaGetLastError();
-    return 0;
-  }
-  return 0.92 * (double)(free_b + g_arena.cap);
+  return pad256((size_t)MHB_NUM_BUCKETS * 4 * 8) + pad256(256 * 8) + pad256(16 * 8) +
+         (plan ? pad256(256 * 8) + pad256(256 * 256 * 8) + pad256(64) + 8192 : 4096);
 }
 
 // The layout of mhb_s2s_args: item offsets (exclusive prefix of 2 * (len - k + 2) over sequences of len >= k + 1) and
@@ -695,16 +648,16 @@ class SeqSource {
       }
     }
     const bool arrays = resident_ || !ly_.fixed;  // the resident form keeps all four arrays, as it always did
-    o_wo_ = Arena::pad(max_words * 4 + 64);
-    o_io_ = o_wo_ + (arrays ? Arena::pad((max_n + 1) * 8) : 0);
-    o_len_ = o_io_ + (arrays ? Arena::pad((max_n + 1) * 8) : 0);
-    o_mult_ = o_len_ + (arrays ? Arena::pad((max_n + 1) * 4) : 0);
-    slot_bytes_ = o_mult_ + Arena::pad((max_n + 1) * 2);
+    o_wo_ = pad256(max_words * 4 + 64);
+    o_io_ = o_wo_ + (arrays ? pad256((max_n + 1) * 8) : 0);
+    o_len_ = o_io_ + (arrays ? pad256((max_n + 1) * 8) : 0);
+    o_mult_ = o_len_ + (arrays ? pad256((max_n + 1) * 4) : 0);
+    slot_bytes_ = o_mult_ + pad256((max_n + 1) * 2);
     g_s2s_st.chunks = n_chunks();
     return resident_ ? MHB_OK : stager_.init(slot_bytes_, n_chunks(), &g_s2s_st);
   }
   static size_t resident_bytes(uint64_t ns, uint64_t n_words) {
-    return Arena::pad(n_words * 4 + 64) + 2 * Arena::pad((ns + 1) * 8) + Arena::pad((ns + 1) * 4) + Arena::pad((ns + 1) * 2);
+    return pad256(n_words * 4 + 64) + 2 * pad256((ns + 1) * 8) + pad256((ns + 1) * 4) + pad256((ns + 1) * 2);
   }
   size_t device_bytes() const { return (resident_ ? 1 : 2) * slot_bytes_; }
   uint64_t n_chunks() const { return resident_ ? 0 : first_.size() - 1; }
@@ -801,7 +754,7 @@ static int s2s_host_rounds(const mhb_s2s_args *args, mhb_s2s_result *res, SeqSou
   const uint32_t W = s2s_record_words(k), WPT = words_per_tip_label(k);
   const int top_byte = (int)(4 * W - 1);
   cudaStream_t st = 0;
-  Timer t_all(st), t(st);
+  EventTimer t_all(st), t(st);
   t_all.start();
 
   const size_t fixed_b = src.device_bytes() + s2s_table_bytes(!one_pass);
@@ -809,7 +762,7 @@ static int s2s_host_rounds(const mhb_s2s_args *args, mhb_s2s_result *res, SeqSou
     max_items = n_items;
   } else {
     if (!max_items) {
-      const size_t avail = (size_t)device_avail_bytes();
+      const size_t avail = (size_t)arena_avail_bytes();
       max_items = largest_round(n_items, fixed_b, avail, [&](uint64_t n) { return s2s_round_bytes(n, W, k); });
       if (!max_items)
         return mhb_set_error(MHB_ERR_NOMEM, "the sequences%s alone (%zu bytes) do not fit the device",
@@ -1010,12 +963,10 @@ extern "C" int mhb_s2s_host(const mhb_s2s_args *args, mhb_s2s_result *res) {
                       s2s_round_bytes(n_items, s2s_record_words(k), k);
   bool rounds = g_s2s_round_limit && n_items > g_s2s_round_limit;
   if (!rounds && need > g_arena.cap) {
-    size_t free_b = 0, total_b = 0;
-    CK(cudaMemGetInfo(&free_b, &total_b));
-    rounds = (double)need > 0.92 * (double)(free_b + g_arena.cap);
+    rounds = (double)need > arena_avail_bytes();
   }
   const bool stream = g_s2s_chunk_limit != 0 ||
-                      (rounds && mhb_read_stream_decide(s2s_resident_round_bytes(ns, n_words, k), (uint64_t)device_avail_bytes(), 0, 0));
+                      (rounds && mhb_read_stream_decide(s2s_resident_round_bytes(ns, n_words, k), (uint64_t)arena_avail_bytes(), 0, 0));
   SeqSource src(args, ly);
   CKR(src.init(stream ? (g_s2s_chunk_limit ? g_s2s_chunk_limit : read_chunk_auto_bytes()) : 0));
   return s2s_host_rounds(args, res, src, n_items, g_s2s_round_limit, !rounds && !stream);
@@ -1170,7 +1121,7 @@ static int build_host_impl(const mhb_build_args *args, mhb_build_result *res, bo
   res->words_per_tip_label = WPT;
 
   ReadLibIndex ix;
-  CKR(index_read_lib(args->bin, args->bin_words, args->n_reads, k, &ix, !full_index));
+  CKR(index_read_lib(args->bin, args->bin_words, args->n_reads, k, &ix, full_index ? FixedCheck::kFull : FixedCheck::kSampled));
   const bool verify_fixed = !full_index && ix.fixed_len != 0;  // the device checks every length word (below)
   const uint64_t n = ix.n_units, n_reads = args->n_reads;
   res->n_edge_records = n;
@@ -1179,7 +1130,7 @@ static int build_host_impl(const mhb_build_args *args, mhb_build_result *res, bo
     for (uint64_t r = 0; r < n_reads; ++r) max_len = std::max(max_len, args->bin[ix.rec_off[r]]);
 
   cudaStream_t st = 0;
-  Timer t_all(st), t(st);
+  EventTimer t_all(st), t(st);
   t_all.start();
 
   uint8_t cbytes[72];
@@ -1188,13 +1139,13 @@ static int build_host_impl(const mhb_build_args *args, mhb_build_result *res, bo
   const uint64_t cap_edges = n / (uint64_t)std::max(1, m) + 1;
   const size_t bin_bytes = (args->bin_words * 4 + 15) & ~(size_t)15;
   const CountWork cw = count_work_plan(n, k, m);
-  const size_t count_work = 2 * Arena::pad((size_t)n * WR * 4 + 16) + Arena::pad(cw.bytes);
+  const size_t count_work = 2 * pad256((size_t)n * WR * 4 + 16) + pad256(cw.bytes);
   // fixed part
-  size_t fixed = Arena::pad(bin_bytes + 16) + Arena::pad((size_t)cap_edges * WE * 4) + Arena::pad(cap_edges) +
-                 Arena::pad(65536 * 8) + 2 * Arena::pad(256 * 8) + Arena::pad(64) + Arena::pad((size_t)MHB_NUM_BUCKETS * 32) +
-                 Arena::pad(128) + 8192;
-  if (!ix.fixed_len) fixed += 2 * Arena::pad((n_reads + 1) * 8);
-  if (args->need_mercy) fixed += 2 * Arena::pad((n_reads + 1) * 4) + Arena::pad((n_reads + 1) * 8);
+  size_t fixed = pad256(bin_bytes + 16) + pad256((size_t)cap_edges * WE * 4) + pad256(cap_edges) +
+                 pad256(65536 * 8) + 2 * pad256(256 * 8) + pad256(64) + pad256((size_t)MHB_NUM_BUCKETS * 32) +
+                 pad256(128) + 8192;
+  if (!ix.fixed_len) fixed += 2 * pad256((n_reads + 1) * 8);
+  if (args->need_mercy) fixed += 2 * pad256((n_reads + 1) * 4) + pad256((n_reads + 1) * 8);
   CKR(g_arena.reserve(fixed + count_work));
 
   uint32_t *d_bin = g_arena.take<uint32_t>(bin_bytes / 4 + 4);
@@ -1219,14 +1170,8 @@ static int build_host_impl(const mhb_build_args *args, mhb_build_result *res, bo
   }
   char *work = g_arena.take<char>(count_work);
   size_t work_bytes = count_work;
-  char *extra = nullptr;  // separately allocated work area when the SdBG stage outgrows the count stage's
-  char *big_edges = nullptr;  // solid + mercy edges when the mercy edges do not fit behind the solid ones in d_edges
-  struct ExtraGuard {
-    char *&p;
-    ~ExtraGuard() {
-      if (p) cudaFree(p);
-    }
-  } guard{extra}, guard2{big_edges};
+  DevBuf extra;      // separately allocated work area when a later stage outgrows the count stage's
+  DevBuf big_edges;  // solid + mercy edges when the mercy edges do not fit behind the solid ones in d_edges
   uint32_t *d_all_edges = d_edges;
 
   // ---- H2D ----
@@ -1259,8 +1204,8 @@ static int build_host_impl(const mhb_build_args *args, mhb_build_result *res, bo
   // ---- count stage ----
   t.start();
   uint32_t *c_a = (uint32_t *)work;
-  uint32_t *c_b = (uint32_t *)(work + Arena::pad((size_t)n * WR * 4 + 16));
-  char *c_wsp = work + 2 * Arena::pad((size_t)n * WR * 4 + 16);
+  uint32_t *c_b = (uint32_t *)(work + pad256((size_t)n * WR * 4 + 16));
+  char *c_wsp = work + 2 * pad256((size_t)n * WR * 4 + 16);
   if (!chunked) {
     CKR(mhb_count_extract(st, &reads, k, c_a, n, d_hist0, cw.hist_byte));
   } else {
@@ -1313,27 +1258,23 @@ static int build_host_impl(const mhb_build_args *args, mhb_build_result *res, bo
     const size_t ts_bytes = mhb_tipset_bytes(n_tip, k);
     const size_t cs_bytes = mhb_mercy_candidates_scratch_bytes(n_reads);
     // the count stage's work area is free now; small inputs may need more than it offers (12-mer look-up table)
-    auto work_area = [&](size_t bytes) -> char * {
-      if (bytes <= work_bytes) return work;
-      if (extra) cudaFree(extra);
-      extra = nullptr;
-      if (cudaMalloc((void **)&extra, bytes) != cudaSuccess) {
-        cudaGetLastError();
-        return nullptr;
-      }
-      return extra;
-    };
-    char *d_tips = work_area(Arena::pad(ts_bytes) + Arena::pad(cs_bytes));
-    if (!d_tips) return mhb_set_error(MHB_ERR_NOMEM, "cudaMalloc for the mercy stage failed");
-    char *d_cs = d_tips + Arena::pad(ts_bytes);
+    char *d_tips = work;
+    if (pad256(ts_bytes) + pad256(cs_bytes) > work_bytes) {
+      CKR(extra.alloc(pad256(ts_bytes) + pad256(cs_bytes), "build: mercy tip set"));
+      d_tips = extra.as<char>();
+    }
+    char *d_cs = d_tips + pad256(ts_bytes);
     CKR(mhb_tipset_build(st, d_edges, d_aux, n_solid, k, d_tips, ts_bytes, n_tip));
     CKR(mhb_count_mark_mercy(st, &reads, k, d_tips, ts_bytes, n_tip, d_first, d_last));
     CKR(mhb_mercy_candidates(st, d_first, d_last, n_reads, d_cand, &n_cand, d_cs, cs_bytes));
     if (n_cand) {
       const size_t ms_bytes = mhb_mercy_edges_scratch_bytes(n_cand, max_len);
-      CK(cudaStreamSynchronize(st));  // the tip set / candidate scratch may be released by work_area()
-      char *d_ms = work_area(ms_bytes);
-      if (!d_ms) return mhb_set_error(MHB_ERR_NOMEM, "cudaMalloc for the mercy stage failed");
+      CK(cudaStreamSynchronize(st));  // the tip set / candidate scratch may be released below
+      char *d_ms = work;
+      if (ms_bytes > work_bytes) {
+        CKR(extra.alloc(ms_bytes, "build: mercy edge scratch"));
+        d_ms = extra.as<char>();
+      }
       // count first (probe + per-read counts + scan), then size the destination: reads that overlap only at their ends
       // can put more mercy edges between two tips than n/m + 1 - n_solid (the reference reserves +25 % and grows,
       // seq_to_sdbg.cpp:371-379; here the exact number is known before anything is written)
@@ -1345,13 +1286,9 @@ static int build_host_impl(const mhb_build_args *args, mhb_build_result *res, bo
       const void *seg_l[1] = {lut};
       CKR(mhb_mercy_edges_count(st, &reads, d_cand, n_cand, max_len, k, 1, seg_e, seg_n, seg_l, nullptr, &n_mercy, d_ms, core));
       if (n_mercy > cap_edges - n_solid) {
-        const size_t eb = Arena::pad((size_t)(n_solid + n_mercy) * WE * 4 + 16);
-        if (cudaMalloc((void **)&big_edges, eb) != cudaSuccess) {
-          cudaGetLastError();
-          return mhb_set_error(MHB_ERR_NOMEM, "cudaMalloc of %zu bytes for solid + mercy edges failed", eb);
-        }
-        CK(cudaMemcpyAsync(big_edges, d_edges, (size_t)n_solid * WE * 4, cudaMemcpyDeviceToDevice, st));
-        d_all_edges = (uint32_t *)big_edges;
+        CKR(big_edges.alloc((size_t)(n_solid + n_mercy) * WE * 4 + 16, "build: solid + mercy edges"));
+        CK(cudaMemcpyAsync(big_edges.p, d_edges, (size_t)n_solid * WE * 4, cudaMemcpyDeviceToDevice, st));
+        d_all_edges = big_edges.as<uint32_t>();
       }
       CKR(mhb_mercy_edges_write(st, &reads, d_cand, n_cand, max_len, k, d_all_edges + (size_t)n_solid * WE, n_mercy, n_mercy,
                                 d_ms, core));
@@ -1368,23 +1305,17 @@ static int build_host_impl(const mhb_build_args *args, mhb_build_result *res, bo
   res->n_sort_items = n_items;
   const size_t s_ws = mhb_s2s_sort_emit_workspace_bytes(n_items, k);
   const uint64_t cap_bytes = n_items * (4ull + 4ull * WPT) + 16;
-  const size_t s2s_work = 2 * Arena::pad((size_t)n_items * W2 * 4 + 16) + Arena::pad(s_ws) + Arena::pad(cap_bytes);
+  const size_t s2s_work = 2 * pad256((size_t)n_items * W2 * 4 + 16) + pad256(s_ws) + pad256(cap_bytes);
   char *sw = work;
   if (s2s_work > work_bytes) {
     CK(cudaStreamSynchronize(st));
-    if (extra) cudaFree(extra);
-    extra = nullptr;
-    cudaError_t e = cudaMalloc((void **)&extra, s2s_work);
-    if (e != cudaSuccess) {
-      cudaGetLastError();
-      return mhb_set_error(MHB_ERR_NOMEM, "cudaMalloc of %zu bytes for the SdBG stage failed", s2s_work);
-    }
-    sw = extra;
+    CKR(extra.alloc(s2s_work, "build: SdBG stage"));
+    sw = extra.as<char>();
   }
   uint32_t *s_a = (uint32_t *)sw;
-  uint32_t *s_b = (uint32_t *)(sw + Arena::pad((size_t)n_items * W2 * 4 + 16));
-  char *s_wsp = sw + 2 * Arena::pad((size_t)n_items * W2 * 4 + 16);
-  uint8_t *d_bytes = (uint8_t *)(s_wsp + Arena::pad(s_ws));
+  uint32_t *s_b = (uint32_t *)(sw + pad256((size_t)n_items * W2 * 4 + 16));
+  char *s_wsp = sw + 2 * pad256((size_t)n_items * W2 * 4 + 16);
+  uint8_t *d_bytes = (uint8_t *)(s_wsp + pad256(s_ws));
   mhb_dev_seqs seqs;
   memset(&seqs, 0, sizeof(seqs));
   seqs.words = d_all_edges;
@@ -1480,8 +1411,8 @@ int plan_mercy_segments(const uint64_t start[257], uint32_t WE, uint64_t target,
 // device bytes of a streamed search besides its two segment slots: candidate reads, scratch and the answer planes
 size_t mercy_stream_fixed_bytes(uint64_t n_reads, uint64_t cand_words, uint32_t max_len) {
   const size_t bin_bytes = (cand_words * 4 + 15) & ~(size_t)15;
-  return Arena::pad(bin_bytes + 16) + 3 * Arena::pad((n_reads + 1) * 8) + Arena::pad(mhb_mercy_edges_scratch_bytes(n_reads, max_len)) +
-         4096 + Arena::pad(mhb_mercy_planes_words(n_reads, max_len) * 4);
+  return pad256(bin_bytes + 16) + 3 * pad256((n_reads + 1) * 8) + pad256(mhb_mercy_edges_scratch_bytes(n_reads, max_len)) +
+         4096 + pad256(mhb_mercy_planes_words(n_reads, max_len) * 4);
 }
 // Segment sizes of a search streamed because its edges do not fit (no cap set): segments are packed to 1 GiB, which
 // keeps the pinned staging small and the uploads overlapping, but a leading byte may take a slot of up to half the room
@@ -1495,8 +1426,8 @@ void mercy_auto_segment_bytes(double avail, size_t fixed, uint64_t *target, uint
 // the resident search: candidate reads (image, record and edge offsets, ids), the sorted edges and the scratch
 size_t mercy_resident_bytes(uint64_t n_edges, uint32_t k, uint64_t n_reads, uint64_t cand_words, uint32_t max_len) {
   const size_t bin_bytes = (cand_words * 4 + 15) & ~(size_t)15;
-  return Arena::pad(bin_bytes + 16) + 3 * Arena::pad((n_reads + 1) * 8) + Arena::pad((size_t)n_edges * words_per_edge(k) * 4 + 16) +
-         Arena::pad(mhb_mercy_edges_scratch_bytes(n_reads, max_len)) + 4096;
+  return pad256(bin_bytes + 16) + 3 * pad256((n_reads + 1) * 8) + pad256((size_t)n_edges * words_per_edge(k) * 4 + 16) +
+         pad256(mhb_mercy_edges_scratch_bytes(n_reads, max_len)) + 4096;
 }
 }  // namespace
 
@@ -1541,7 +1472,7 @@ extern "C" int mhb_selftest_mercy_auto_plan(const uint64_t *byte_edges, uint32_t
   memcpy(first_byte_out, first.data(), first.size() * 4);
   uint64_t max_seg = 0;
   for (size_t i = 0; i + 1 < first.size(); ++i) max_seg = std::max(max_seg, start[first[i + 1]] - start[first[i]]);
-  *slot_bytes = Arena::pad(max_seg * words_per_edge(k) * 4 + 16);
+  *slot_bytes = pad256(max_seg * words_per_edge(k) * 4 + 16);
   return (int)(first.size() - 1);
 }
 
@@ -1591,7 +1522,7 @@ extern "C" int mhb_mercy_host(uint32_t k, const uint32_t *edges, uint64_t n_edge
   // The edges are streamed in leading-byte segments when they do not fit next to the candidate reads and the scratch,
   // or when a chunk cap is set: every search stays inside one 12-base prefix, so inside one leading byte and one segment
   const bool stream = g_s2s_chunk_limit != 0 ||
-                      (need > g_arena.cap && mhb_read_stream_decide(need, (uint64_t)device_avail_bytes(), 0, 0));
+                      (need > g_arena.cap && mhb_read_stream_decide(need, (uint64_t)arena_avail_bytes(), 0, 0));
   const size_t pw = stream ? mhb_mercy_planes_words(n_reads, max_len) : 0;
   const size_t fixed_b = mercy_stream_fixed_bytes(n_reads, bin.size(), max_len);
   uint64_t start[257];
@@ -1599,12 +1530,12 @@ extern "C" int mhb_mercy_host(uint32_t k, const uint32_t *edges, uint64_t n_edge
   size_t slot_bytes = 0;
   if (stream) {
     uint64_t target = g_s2s_chunk_limit, limit = g_s2s_chunk_limit;
-    if (!target) mercy_auto_segment_bytes(device_avail_bytes(), fixed_b, &target, &limit);
+    if (!target) mercy_auto_segment_bytes(arena_avail_bytes(), fixed_b, &target, &limit);
     edge_byte_starts(edges, n_edges, WE, start);
     CKR(plan_mercy_segments(start, WE, target, limit, &seg_first));
     uint64_t max_seg = 0;
     for (size_t i = 0; i + 1 < seg_first.size(); ++i) max_seg = std::max(max_seg, start[seg_first[i + 1]] - start[seg_first[i]]);
-    slot_bytes = Arena::pad(max_seg * WE * 4 + 16);
+    slot_bytes = pad256(max_seg * WE * 4 + 16);
   }
   CKR(g_arena.reserve(stream ? fixed_b + 2 * slot_bytes : need));
   cudaStream_t st = 0;
@@ -1675,14 +1606,14 @@ extern "C" int mhb_mercy_host(uint32_t k, const uint32_t *edges, uint64_t n_edge
   *mercy_out = (uint32_t *)malloc(std::max<size_t>(4, (size_t)n_mercy * WE * 4));
   if (!*mercy_out) return mhb_set_error(MHB_ERR_NOMEM, "host malloc failed");
   if (n_mercy) {
-    uint32_t *d_out = nullptr;
-    CK(cudaMalloc((void **)&d_out, (size_t)n_mercy * WE * 4));
-    int rc = mhb_mercy_edges_write(st, &reads, d_ids, n_reads, max_len, k, d_out, n_mercy, n_mercy, d_ms, core);
-    if (!rc && cudaMemcpyAsync(*mercy_out, d_out, (size_t)n_mercy * WE * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess)
+    DevBuf out;
+    int rc = out.alloc((size_t)n_mercy * WE * 4, "mercy: edges");
+    if (!rc) rc = mhb_mercy_edges_write(st, &reads, d_ids, n_reads, max_len, k, out.as<uint32_t>(), n_mercy, n_mercy, d_ms, core);
+    if (!rc && cudaMemcpyAsync(*mercy_out, out.p, (size_t)n_mercy * WE * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess)
       rc = mhb_set_error(MHB_ERR_CUDA, "mercy edge download failed");
     if (!rc && cudaStreamSynchronize(st) != cudaSuccess)
       rc = mhb_set_error(MHB_ERR_CUDA, "mercy edge kernels failed: %s", cudaGetErrorString(cudaGetLastError()));
-    cudaFree(d_out);
+    out.release();
     if (rc) {
       free(*mercy_out);
       *mercy_out = nullptr;

@@ -12,6 +12,41 @@
 
 int mhb_set_error(int code, const char *fmt, ...);
 
+// ---- host helpers of every stage (device-side ones, which need CUDA types: mhb_common.cuh) ----
+// return a non-zero status code at once
+#define CKR(call)        \
+  do {                   \
+    int rc_ = (call);    \
+    if (rc_) return rc_; \
+  } while (0)
+
+// the 256-byte alignment of every device sub-allocation
+inline size_t pad256(size_t bytes) { return (bytes + 255) & ~(size_t)255; }
+
+// free memory of the current device; 0 when cudaMemGetInfo fails (the error is cleared) (mhb_stream.cu)
+size_t free_device_bytes();
+
+// One device allocation, released with the object (mhb_stream.cu).  alloc rounds max(bytes, 1) up to 256 and
+// reallocates; ensure only grows, and contents do not survive growth.  A failed cudaMalloc clears the CUDA error and is
+// MHB_ERR_NOMEM, its message "<what>: cudaMalloc of <bytes> bytes failed" (what starts with the stage).
+struct DevBuf {
+  void *p = nullptr;
+  size_t bytes = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf &) = delete;
+  DevBuf &operator=(const DevBuf &) = delete;
+  ~DevBuf() { release(); }
+  int alloc(size_t b, const char *what);
+  int ensure(size_t b, const char *what) { return p && bytes >= b ? MHB_OK : alloc(b, what); }
+  void release();
+  void swap(DevBuf &o) {
+    std::swap(p, o.p);
+    std::swap(bytes, o.bytes);
+  }
+  template <class T>
+  T *as() const { return reinterpret_cast<T *>(p); }
+};
+
 // largest n <= n_max with fixed + bytes(n) <= avail (bytes(n) grows with n); 0 when not even one fits
 template <class F>
 uint64_t largest_round(uint64_t n_max, size_t fixed, size_t avail, F bytes) {
@@ -47,13 +82,24 @@ struct ReadLibIndex {
   uint32_t fixed_len = 0;
   std::vector<uint64_t> rec_off, unit_off;
   uint64_t n_units = 0;  // sum of max(0, L - k) over all reads
+  // the first word of read r (its length word); r = n_reads: the end of the image (0 for an empty library, which
+  // index_read_lib leaves without offsets)
+  uint64_t word_of(uint64_t r) const {
+    return fixed_len ? r * (1 + (fixed_len + 15) / 16) : rec_off.empty() ? 0 : rec_off[r];
+  }
 };
-// sampled = true: a library whose size matches n_reads x (1 + ceil(L0/16)) is taken as fixed-length after looking at
-// ~2048 of its length words only; the caller must then verify ALL of them on the device (mhb_check_fixed_len) and come
-// back with sampled = false when that fails.  (The full host scan touches every cache line of the image: ~10 ms for
-// 10 M reads, all of it inside the end-to-end time of the fused build.)
+// How index_read_lib checks a library whose size matches n_reads x (1 + ceil(L0/16)) for fixed-length reads:
+// - kFull: every length word, on all host threads;
+// - kSerial: every length word on the calling thread, for a process that forks workers afterwards (GNU OpenMP's
+//   thread pool does not survive fork(): the first parallel region of a child would wait for the parent's threads);
+// - kSampled: ~2048 of its length words only; the caller must then verify ALL of them on the device
+//   (mhb_check_fixed_len) and come back with kFull when that fails.  (The full host scan touches every cache line of
+//   the image: ~10 ms for 10 M reads, all of it inside the end-to-end time of the fused build.)
+enum class FixedCheck { kFull, kSerial, kSampled };
 int index_read_lib(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, uint32_t k, ReadLibIndex *ix,
-                   bool sampled = false);
+                   FixedCheck check = FixedCheck::kFull);
+// A read library from disk (mhb_files.cpp): the counts of `prefix.lib_info` and the image of `prefix.bin`
+int load_read_lib(const std::string &prefix, std::vector<uint32_t> *bin, long long *n_reads, long long *total_bases);
 
 // Streaming statistics of one host-level call: chunks (0 = resident), passes, bytes host to device, and the copy-engine
 // and compute-stream busy time, host fill time and wall time of the passes (ms).
@@ -128,6 +174,7 @@ class ReadStream {
   ReadStream(const ReadStream &) = delete;
   ReadStream &operator=(const ReadStream &) = delete;
   // host library and its index; max_chunk_bytes = 0: resident, otherwise streamed in chunks planned here
+  // (the index is read by every pass: it must outlive them)
   int init(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, const ReadLibIndex &ix, uint64_t max_chunk_bytes);
   size_t device_bytes() const { return (resident_ ? 1 : 2) * slot_bytes_; }  // the library, or both chunk slots
   // device_bytes() bytes, 256-byte aligned; the resident form uploads the library there on `stream`
@@ -144,15 +191,14 @@ class ReadStream {
   ReadChunkView view(uint64_t i, const char *slot) const;
   bool resident_ = false;
   const uint32_t *bin_ = nullptr;
-  uint64_t bin_words_ = 0, stride_ = 0;
-  uint32_t fixed_len_ = 0;
-  const uint64_t *rec_off_ = nullptr, *aux_off_ = nullptr;
+  uint64_t bin_words_ = 0;
+  const ReadLibIndex *ix_ = nullptr;
+  const uint64_t *aux_off_ = nullptr;
   std::vector<uint64_t> first_;
   uint64_t max_reads_ = 0;
   size_t off_at_ = 0, slot_bytes_ = 0;
   char *dev_ = nullptr;
   ChunkStager stager_;
-  uint64_t word_of(uint64_t r) const { return fixed_len_ ? r * stride_ : rec_off_[r]; }
 };
 // streaming statistics of the current host-level call (mhb_read_stream_stats)
 void read_stream_stats_reset();
@@ -204,31 +250,19 @@ void plan_shares(uint64_t n, uint32_t n_ranks, Weight weight, uint64_t *first) {
 }
 
 // ---- iterate's device pieces (mhb_iter.cu), shared by mhb_iterate_host and the multi-GPU worker ----
-// a device allocation released with the object; a failed cudaMalloc is MHB_ERR_NOMEM naming the bytes
-struct IterBuf {
-  void *p = nullptr;
-  IterBuf() = default;
-  IterBuf(const IterBuf &) = delete;
-  IterBuf &operator=(const IterBuf &) = delete;
-  ~IterBuf();
-  int alloc(size_t bytes, const char *what);
-  void release();
-  template <class T>
-  T *as() const { return reinterpret_cast<T *>(p); }
-};
 // the checks of mhb_iterate_host on k and step (main_iterate.cpp:73-93, and the 17-word records of the device sort)
 int iterate_check_args(uint32_t k, uint32_t step);
 // The flank index (FeedBatchContigs) of a's contigs on the current device: n unique records of ceil((k+1)/16) + 2
 // words in tab, and its 65537-entry prefix table in lut.  Every caller gets the same table from the same contigs.
 struct IterFlanks {
-  IterBuf tab, lut;
+  DevBuf tab, lut;
   uint64_t n = 0;
 };
 int iter_build_flanks(const mhb_iterate_args *a, IterFlanks *f);
 // The read pass (FindNextKmersFromReads) over a's reads against the flank index: resident, or streamed in chunks when a
 // chunk cap is set or when the resident buffers do not fit.  *set = the n_set unique candidate edges, ascending, on the
 // device (nothing allocated when there are none); n_cand = candidates before the dedup; n_aligned = reads with one.
-int iter_collect(const mhb_iterate_args *a, const IterFlanks &f, IterBuf *set, uint64_t *n_set, uint64_t *n_cand,
+int iter_collect(const mhb_iterate_args *a, const IterFlanks &f, DevBuf *set, uint64_t *n_set, uint64_t *n_cand,
                  uint64_t *n_aligned);
 // KmerCollector's set semantics on n edge records of k + step in a (b: a buffer of the same size): sort, then the first
 // record of every run of equal ones; *out = where the n_out unique records are (a or b)

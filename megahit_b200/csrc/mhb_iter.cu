@@ -14,36 +14,7 @@ using namespace mhb;
 
 int scan32(cudaStream_t st, const uint32_t *in, uint64_t n, uint64_t *out, uint64_t *total_dev, uint64_t *bsum);
 
-IterBuf::~IterBuf() { release(); }
-void IterBuf::release() {
-  if (p) cudaFree(p);
-  p = nullptr;
-}
-int IterBuf::alloc(size_t b, const char *what) {
-  release();
-  b = ((b ? b : 1) + 255) & ~(size_t)255;
-  if (cudaMalloc(&p, b) != cudaSuccess) {
-    cudaGetLastError();
-    p = nullptr;
-    return mhb_set_error(MHB_ERR_NOMEM, "iterate: cudaMalloc of %zu bytes for %s failed", b, what);
-  }
-  return MHB_OK;
-}
-
 namespace {
-
-#define CKR(call)        \
-  do {                   \
-    int rc_ = (call);    \
-    if (rc_) return rc_; \
-  } while (0)
-
-unsigned igrid(uint64_t n, unsigned threads, unsigned per_sm = 16) {
-  uint64_t g = (n + threads - 1) / threads;
-  const uint64_t cap = (uint64_t)sm_count() * per_sm;
-  if (g > cap) g = cap;
-  return (unsigned)(g < 1 ? 1 : g);
-}
 
 // ascending byte positions of a record of `words` words that hold the first `bits` bits (from the top)
 uint32_t top_bytes(uint32_t words, uint32_t bits, uint8_t *out) {
@@ -60,7 +31,7 @@ int cap_class(uint32_t words) { return words <= 2 ? 2 : words <= 4 ? 4 : words <
 // the kernels' capacity class of (k, step): the wider of the (k+1)-mer keys and the (k+step+1)-mers
 int iter_class(uint32_t k, uint32_t step) { return cap_class(std::max(div_ceil(k + step + 1, 16), div_ceil(k + 1, 16))); }
 
-int iter_reads(const mhb_iterate_args *a, const ReadLibIndex &ix, const FlankTable &tab, bool stream, IterBuf *set,
+int iter_reads(const mhb_iterate_args *a, const ReadLibIndex &ix, const FlankTable &tab, bool stream, DevBuf *set,
                uint64_t *n_set_out, uint64_t *n_cand_out, uint64_t *n_aligned_out);
 
 // mhb_selftest_iterate_narrow: the narrow flank index at a k whose wide records fit, to compare the two layouts
@@ -81,17 +52,17 @@ int iter_build_flanks(const mhb_iterate_args *a, IterFlanks *f) {
   const uint32_t k = a->k, step = a->step, K1 = k + 1, wk = div_ceil(K1, 16), frw = wk + 2;
   const int WCc = iter_class(k, step);
   cudaStream_t st = 0;
-  IterBuf d_cw, d_co, d_cl, d_fl, d_fl2, d_val, d_ws, d_flag, d_off, d_bsum, d_cnt;
-  CKR(d_cnt.alloc(64, "counters"));
+  DevBuf d_cw, d_co, d_cl, d_fl, d_fl2, d_val, d_ws, d_flag, d_off, d_bsum, d_cnt;
+  CKR(d_cnt.alloc(64, "iterate: counters"));
   CK(cudaMemsetAsync(d_cnt.p, 0, 64, st));
   unsigned long long *cnt = d_cnt.as<unsigned long long>();
   f->n = 0;
   f->tab.release();
   if (a->n_contigs) {
     const uint64_t cw = a->contig_word_off[a->n_contigs];
-    CKR(d_cw.alloc(cw * 4 + 64, "contigs"));
-    CKR(d_co.alloc((a->n_contigs + 1) * 8, "contig offsets"));
-    CKR(d_cl.alloc(a->n_contigs * 4, "contig lengths"));
+    CKR(d_cw.alloc(cw * 4 + 64, "iterate: contigs"));
+    CKR(d_co.alloc((a->n_contigs + 1) * 8, "iterate: contig offsets"));
+    CKR(d_cl.alloc(a->n_contigs * 4, "iterate: contig lengths"));
     CK(cudaMemcpyAsync(d_cw.p, a->contig_words, cw * 4, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_co.p, a->contig_word_off, (a->n_contigs + 1) * 8, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_cl.p, a->contig_len, a->n_contigs * 4, cudaMemcpyHostToDevice, st));
@@ -101,13 +72,13 @@ int iter_build_flanks(const mhb_iterate_args *a, IterFlanks *f) {
     const bool narrow = frw > 17 || g_iter_force_narrow;
     const uint32_t srw = narrow ? wk + 1 : frw;
     if (cap >= (1ull << 32) && narrow) return mhb_set_error(MHB_ERR_ARG, "iterate: too many contigs for 32-bit flank rows");
-    CKR(d_fl.alloc(cap * srw * 4 + 16, "flank records"));
-    CKR(d_fl2.alloc(cap * srw * 4 + 16, "flank records (sort buffer)"));
-    if (narrow) CKR(d_val.alloc(cap * 8 + 16, "flank values"));
+    CKR(d_fl.alloc(cap * srw * 4 + 16, "iterate: flank records"));
+    CKR(d_fl2.alloc(cap * srw * 4 + 16, "iterate: flank records (sort buffer)"));
+    if (narrow) CKR(d_val.alloc(cap * 8 + 16, "iterate: flank values"));
     IterContigs cs{d_cw.as<u32>(), d_co.as<u64>(), d_cl.as<u32>(), a->n_contigs};
 #define M(WW)                                                                                                    \
   if (WCc == WW)                                                                                                 \
-    k_iter_flanks<WW><<<igrid(cap, 256), 256, 0, st>>>(cs, k, step, wk, d_fl.as<u32>(), narrow ? d_val.as<u64>() : nullptr, \
+    k_iter_flanks<WW><<<grid_cap(cap, 256, 16), 256, 0, st>>>(cs, k, step, wk, d_fl.as<u32>(), narrow ? d_val.as<u64>() : nullptr, \
                                                        cnt);
     IT_FOR_WC(M)
 #undef M
@@ -128,33 +99,33 @@ int iter_build_flanks(const mhb_iterate_args *a, IterFlanks *f) {
         for (uint32_t i = 0; i < nkb; ++i) bytes[nb++] = (uint8_t)(kb[i] + 8);  // the key bytes above them
       }
       const size_t wsb = mhb_sort_workspace_bytes(nf, srw);
-      CKR(d_ws.alloc(wsb, "sort workspace"));
+      CKR(d_ws.alloc(wsb, "iterate: sort workspace"));
       int in_b = 0;
       if (narrow)
         CKR(mhb_sort_records_relaxed(st, d_fl.as<u32>(), d_fl2.as<u32>(), nf, srw, bytes, nb, nullptr, d_ws.p, wsb, &in_b));
       else
         CKR(mhb_sort_records(st, d_fl.as<u32>(), d_fl2.as<u32>(), nf, srw, bytes, nb, nullptr, d_ws.p, wsb, &in_b));
       const u32 *sorted = in_b ? d_fl2.as<u32>() : d_fl.as<u32>();
-      CKR(d_flag.alloc(nf * 4 + 16, "flags"));
-      CKR(d_off.alloc(nf * 8 + 16, "offsets"));
-      CKR(d_bsum.alloc((nf / 4096 + 4) * 8, "scan sums"));
-      k_iter_heads<<<igrid(nf, 256), 256, 0, st>>>(sorted, nf, srw, wk, d_flag.as<u32>());
+      CKR(d_flag.alloc(nf * 4 + 16, "iterate: flags"));
+      CKR(d_off.alloc(nf * 8 + 16, "iterate: offsets"));
+      CKR(d_bsum.alloc((nf / 4096 + 4) * 8, "iterate: scan sums"));
+      k_iter_heads<<<grid_cap(nf, 256, 16), 256, 0, st>>>(sorted, nf, srw, wk, d_flag.as<u32>());
       CK_LAUNCH();
       CKR(scan32(st, d_flag.as<u32>(), nf, d_off.as<u64>(), (uint64_t *)(cnt + 2), d_bsum.as<u64>()));
       unsigned long long nu = 0;
       CK(cudaMemcpyAsync(&nu, cnt + 2, 8, cudaMemcpyDeviceToHost, st));
       CK(cudaStreamSynchronize(st));
-      CKR(f->tab.alloc((size_t)nu * frw * 4 + 16, "flank table"));
+      CKR(f->tab.alloc((size_t)nu * frw * 4 + 16, "iterate: flank table"));
       if (narrow)
-        k_iter_best<<<igrid(nf, 256), 256, 0, st>>>(sorted, nf, wk, d_val.as<u64>(), d_flag.as<u32>(), d_off.as<u64>(),
+        k_iter_best<<<grid_cap(nf, 256, 16), 256, 0, st>>>(sorted, nf, wk, d_val.as<u64>(), d_flag.as<u32>(), d_off.as<u64>(),
                                                     f->tab.as<u32>());
       else
-        k_iter_compact<<<igrid(nf, 256), 256, 0, st>>>(sorted, nf, frw, d_flag.as<u32>(), d_off.as<u64>(), f->tab.as<u32>());
+        k_iter_compact<<<grid_cap(nf, 256, 16), 256, 0, st>>>(sorted, nf, frw, d_flag.as<u32>(), d_off.as<u64>(), f->tab.as<u32>());
       CK_LAUNCH();
       f->n = nu;
     }
   }
-  CKR(f->lut.alloc(65537 * 4, "flank prefix table"));
+  CKR(f->lut.alloc(65537 * 4, "iterate: flank prefix table"));
   CK(cudaMemsetAsync(f->lut.p, 0, 65537 * 4, st));
   if (f->n) {
     k_iter_lut<<<(65537 + 255) / 256, 256, 0, st>>>(f->tab.as<u32>(), f->n, frw, f->lut.as<u32>());
@@ -164,7 +135,7 @@ int iter_build_flanks(const mhb_iterate_args *a, IterFlanks *f) {
   return MHB_OK;
 }
 
-int iter_collect(const mhb_iterate_args *a, const IterFlanks &f, IterBuf *set, uint64_t *n_set, uint64_t *n_cand,
+int iter_collect(const mhb_iterate_args *a, const IterFlanks &f, DevBuf *set, uint64_t *n_set, uint64_t *n_cand,
                  uint64_t *n_aligned) {
   *n_set = *n_cand = *n_aligned = 0;
   set->release();
@@ -187,23 +158,12 @@ extern "C" int mhb_iterate_host(const mhb_iterate_args *a, mhb_iterate_result *r
   res->words_per_edge = w2;
   read_stream_stats_reset();
   cudaStream_t st = 0;
-  struct Events {
-    cudaEvent_t a, b;
-    Events() {
-      cudaEventCreate(&a);
-      cudaEventCreate(&b);
-    }
-    ~Events() {
-      cudaEventDestroy(a);
-      cudaEventDestroy(b);
-    }
-  } ev;
-  cudaEvent_t e0 = ev.a, e1 = ev.b;
-  cudaEventRecord(e0, st);
+  EventTimer t(st);
+  t.start();
   IterFlanks flanks;
   CKR(iter_build_flanks(a, &flanks));
   res->n_flanks = flanks.n;
-  IterBuf set;
+  DevBuf set;
   uint64_t n_set = 0, n_cand = 0, n_aligned = 0;
   CKR(iter_collect(a, flanks, &set, &n_set, &n_cand, &n_aligned));
   res->edges = (uint32_t *)malloc(std::max<size_t>(4, (size_t)n_set * w2 * 4));
@@ -212,64 +172,43 @@ extern "C" int mhb_iterate_host(const mhb_iterate_args *a, mhb_iterate_result *r
   res->n_aligned_reads = n_aligned;
   res->n_candidates = n_cand;
   res->n_edges = n_set;
-  cudaEventRecord(e1, st);
-  cudaEventSynchronize(e1);
-  float ms = 0;
-  cudaEventElapsedTime(&ms, e0, e1);
-  res->t_total_ms = ms;
+  res->t_total_ms = t.stop();
   return MHB_OK;
 }
 
 namespace {
-// a device buffer that only grows (its contents do not survive growth)
-struct Grow {
-  IterBuf b;
-  size_t cap = 0;
-  int need(size_t bytes, const char *what) {
-    if (bytes <= cap) return MHB_OK;
-    CKR(b.alloc(bytes, what));
-    cap = bytes;
-    return MHB_OK;
-  }
-};
-
 // KmerCollector's set semantics on n records in a (b: same-sized buffer): relaxed sort on the key bytes, then the first
 // record of every run of equal records; *out points at the n_out unique records (in a or b)
-int sort_unique(cudaStream_t st, u32 *a, u32 *b, uint64_t n, uint32_t w2, uint32_t KN, Grow &ws, Grow &flag, Grow &off,
-                Grow &bsum, unsigned long long *cnt_slot, u32 **out, uint64_t *n_out) {
+int sort_unique(cudaStream_t st, u32 *a, u32 *b, uint64_t n, uint32_t w2, uint32_t KN, DevBuf &ws, DevBuf &flag, DevBuf &off,
+                DevBuf &bsum, unsigned long long *cnt_slot, u32 **out, uint64_t *n_out) {
   uint8_t bytes[72];
   const uint32_t nb = top_bytes(w2, 2 * KN, bytes);
   const size_t wsb = mhb_sort_workspace_bytes(n, w2);
-  CKR(ws.need(wsb, "sort workspace"));
+  CKR(ws.ensure(wsb, "iterate: sort workspace"));
   int in_b = 0;
-  CKR(mhb_sort_records_relaxed(st, a, b, n, w2, bytes, nb, nullptr, ws.b.p, wsb, &in_b));
+  CKR(mhb_sort_records_relaxed(st, a, b, n, w2, bytes, nb, nullptr, ws.p, wsb, &in_b));
   const u32 *sorted = in_b ? b : a;
   u32 *uniq = in_b ? a : b;
-  CKR(flag.need(n * 4 + 16, "flags"));
-  CKR(off.need(n * 8 + 16, "offsets"));
-  CKR(bsum.need((n / 4096 + 4) * 8, "scan sums"));
-  k_iter_heads<<<igrid(n, 256), 256, 0, st>>>(sorted, n, w2, w2, flag.b.as<u32>());
+  CKR(flag.ensure(n * 4 + 16, "iterate: flags"));
+  CKR(off.ensure(n * 8 + 16, "iterate: offsets"));
+  CKR(bsum.ensure((n / 4096 + 4) * 8, "iterate: scan sums"));
+  k_iter_heads<<<grid_cap(n, 256, 16), 256, 0, st>>>(sorted, n, w2, w2, flag.as<u32>());
   CK_LAUNCH();
-  CKR(scan32(st, flag.b.as<u32>(), n, off.b.as<u64>(), (uint64_t *)cnt_slot, bsum.b.as<u64>()));
+  CKR(scan32(st, flag.as<u32>(), n, off.as<u64>(), (uint64_t *)cnt_slot, bsum.as<u64>()));
   unsigned long long nu = 0;
   CK(cudaMemcpyAsync(&nu, cnt_slot, 8, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  k_iter_compact<<<igrid(n, 256), 256, 0, st>>>(sorted, n, w2, flag.b.as<u32>(), off.b.as<u64>(), uniq);
+  k_iter_compact<<<grid_cap(n, 256, 16), 256, 0, st>>>(sorted, n, w2, flag.as<u32>(), off.as<u64>(), uniq);
   CK_LAUNCH();
   *out = uniq;
   *n_out = nu;
   return MHB_OK;
 }
 
-void swap_bufs(Grow &x, Grow &y) {
-  std::swap(x.b.p, y.b.p);
-  std::swap(x.cap, y.cap);
-}
-
 // The reads (ReadStream: resident, or streamed from host memory in chunks), the flank index resident: per chunk mark +
 // emit into a mark array of the chunk's bases, make the chunk's candidates unique and merge them into the running set by
 // the same sort + unique over the union.  KmerCollector is a set, so the result does not depend on the chunks.
-int iter_reads(const mhb_iterate_args *a, const ReadLibIndex &ix, const FlankTable &tab, bool stream, IterBuf *set,
+int iter_reads(const mhb_iterate_args *a, const ReadLibIndex &ix, const FlankTable &tab, bool stream, DevBuf *set,
                uint64_t *n_set_out, uint64_t *n_cand_out, uint64_t *n_aligned_out) {
   const uint32_t k = a->k, step = a->step, KN = k + step + 1, w2 = words_per_edge(k + step);
   const int WCc = iter_class(k, step);
@@ -281,13 +220,13 @@ int iter_reads(const mhb_iterate_args *a, const ReadLibIndex &ix, const FlankTab
   auto bases_of = [&](uint64_t b, uint64_t e) { return ix.fixed_len ? (e - b) * ix.fixed_len : ix.unit_off[e] - ix.unit_off[b]; };
   uint64_t max_bases = 0;
   for (uint64_t i = 0; i + 1 < first.size(); ++i) max_bases = std::max(max_bases, bases_of(first[i], first[i + 1]));
-  IterBuf d_lib, d_exist, d_cnt;
-  CKR(d_cnt.alloc(64, "counters"));
+  DevBuf d_lib, d_exist, d_cnt;
+  CKR(d_cnt.alloc(64, "iterate: counters"));
   unsigned long long *cnt = d_cnt.as<unsigned long long>();
-  CKR(d_lib.alloc(rs.device_bytes(), stream ? "read chunk buffers" : ".bin image"));
+  CKR(d_lib.alloc(rs.device_bytes(), stream ? "iterate: read chunk buffers" : "iterate: .bin image"));
   CKR(rs.bind(d_lib.p, st));
-  CKR(d_exist.alloc((max_bases / 32 + 2) * 4, "position marks"));
-  Grow c, c2, u, u2, ws, flag, off, bsum;
+  CKR(d_exist.alloc((max_bases / 32 + 2) * 4, "iterate: position marks"));
+  DevBuf c, c2, u, u2, ws, flag, off, bsum;
   uint64_t n_cand = 0, n_set = 0, n_aligned = 0;
   auto chunk = [&](const ReadChunkView &v) -> int {
     IterReads rd{v.bin, v.n_reads, ix.fixed_len, v.rec_off, v.aux_off};
@@ -296,8 +235,8 @@ int iter_reads(const mhb_iterate_args *a, const ReadLibIndex &ix, const FlankTab
     CK(cudaMemsetAsync(cnt + 4, 0, 16, st));
 #define M(WW)                                                                                                         \
   if (WCc == WW) {                                                                                                    \
-    k_iter_mark<WW><<<igrid(v.n_reads, 128, 32), 128, 0, st>>>(rd, k, step, tab, d_exist.as<u32>());                   \
-    k_iter_emit<WW, false><<<igrid(v.n_reads, 128, 32), 128, 0, st>>>(rd, k, step, d_exist.as<u32>(), w2, nullptr,     \
+    k_iter_mark<WW><<<grid_cap(v.n_reads, 128, 32), 128, 0, st>>>(rd, k, step, tab, d_exist.as<u32>());               \
+    k_iter_emit<WW, false><<<grid_cap(v.n_reads, 128, 32), 128, 0, st>>>(rd, k, step, d_exist.as<u32>(), w2, nullptr, \
                                                                        cnt + 4, 0);                                   \
   }
     IT_FOR_WC(M)
@@ -310,46 +249,45 @@ int iter_reads(const mhb_iterate_args *a, const ReadLibIndex &ix, const FlankTab
     n_aligned += hc[1];
     if (!hc[0]) return MHB_OK;
     const uint64_t nc = hc[0];
-    CKR(c.need((size_t)nc * w2 * 4 + 16, "edges"));
-    CKR(c2.need((size_t)nc * w2 * 4 + 16, "edges (sort buffer)"));
+    CKR(c.ensure((size_t)nc * w2 * 4 + 16, "iterate: edges"));
+    CKR(c2.ensure((size_t)nc * w2 * 4 + 16, "iterate: edges (sort buffer)"));
     CK(cudaMemsetAsync(cnt + 6, 0, 8, st));
 #define M(WW)                                                                                                        \
   if (WCc == WW)                                                                                                     \
-    k_iter_emit<WW, true><<<igrid(v.n_reads, 128, 32), 128, 0, st>>>(rd, k, step, d_exist.as<u32>(), w2, c.b.as<u32>(), \
+    k_iter_emit<WW, true><<<grid_cap(v.n_reads, 128, 32), 128, 0, st>>>(rd, k, step, d_exist.as<u32>(), w2, c.as<u32>(), \
                                                                      cnt + 6, nc);
     IT_FOR_WC(M)
 #undef M
     CK_LAUNCH();
     u32 *cu = nullptr;
     uint64_t ncu = 0;
-    CKR(sort_unique(st, c.b.as<u32>(), c2.b.as<u32>(), nc, w2, KN, ws, flag, off, bsum, cnt + 7, &cu, &ncu));
+    CKR(sort_unique(st, c.as<u32>(), c2.as<u32>(), nc, w2, KN, ws, flag, off, bsum, cnt + 7, &cu, &ncu));
     if (n_set == 0) {  // the first candidates are the set: take over their buffers
-      const bool in_c = cu == c.b.as<u32>();
-      swap_bufs(u, in_c ? c : c2);
-      swap_bufs(u2, in_c ? c2 : c);
+      const bool in_c = cu == c.as<u32>();
+      u.swap(in_c ? c : c2);
+      u2.swap(in_c ? c2 : c);
       n_set = ncu;
       return MHB_OK;
     }
     // union = running set followed by this chunk's unique candidates
     const size_t need = (size_t)(n_set + ncu) * w2 * 4 + 16;
-    if (need > u.cap) {
-      Grow g;
-      CKR(g.need(std::max(need, 2 * u.cap), "edge set"));
-      if (n_set) CK(cudaMemcpyAsync(g.b.p, u.b.p, (size_t)n_set * w2 * 4, cudaMemcpyDeviceToDevice, st));
+    if (need > u.bytes) {
+      DevBuf g;
+      CKR(g.alloc(std::max(need, 2 * u.bytes), "iterate: edge set"));
+      if (n_set) CK(cudaMemcpyAsync(g.p, u.p, (size_t)n_set * w2 * 4, cudaMemcpyDeviceToDevice, st));
       CK(cudaStreamSynchronize(st));
-      std::swap(u.b.p, g.b.p);
-      std::swap(u.cap, g.cap);
-      CKR(u2.need(u.cap, "edge set (sort buffer)"));
+      u.swap(g);
+      CKR(u2.ensure(u.bytes, "iterate: edge set (sort buffer)"));
     }
-    CK(cudaMemcpyAsync(u.b.as<u32>() + (size_t)n_set * w2, cu, (size_t)ncu * w2 * 4, cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(u.as<u32>() + (size_t)n_set * w2, cu, (size_t)ncu * w2 * 4, cudaMemcpyDeviceToDevice, st));
     u32 *su = nullptr;
-    CKR(sort_unique(st, u.b.as<u32>(), u2.b.as<u32>(), n_set + ncu, w2, KN, ws, flag, off, bsum, cnt + 7, &su, &n_set));
-    if (su != u.b.as<u32>()) std::swap(u.b.p, u2.b.p);
+    CKR(sort_unique(st, u.as<u32>(), u2.as<u32>(), n_set + ncu, w2, KN, ws, flag, off, bsum, cnt + 7, &su, &n_set));
+    if (su != u.as<u32>()) u.swap(u2);
     return MHB_OK;
   };
   CKR(rs.pass(st, chunk));
   CK(cudaStreamSynchronize(st));
-  std::swap(set->p, u.b.p);  // the set leaves with the caller; every other buffer is freed here
+  set->swap(u);  // the set leaves with the caller; every other buffer is freed here
   *n_set_out = n_set;
   *n_cand_out = n_cand;
   *n_aligned_out = n_aligned;
@@ -361,9 +299,9 @@ int iter_sort_unique(uint32_t *a, uint32_t *b, uint64_t n, uint32_t k, uint32_t 
   *out = a;
   *n_out = 0;
   if (!n) return MHB_OK;
-  IterBuf cnt;
-  CKR(cnt.alloc(64, "counters"));
-  Grow ws, flag, off, bsum;
+  DevBuf cnt;
+  CKR(cnt.alloc(64, "iterate: counters"));
+  DevBuf ws, flag, off, bsum;
   CKR(sort_unique(0, a, b, n, words_per_edge(k + step), k + step + 1, ws, flag, off, bsum, cnt.as<unsigned long long>(), out,
                   n_out));
   CK(cudaStreamSynchronize(0));

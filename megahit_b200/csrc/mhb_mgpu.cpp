@@ -38,7 +38,6 @@
 #include <unistd.h>
 
 #include <algorithm>
-#include <fstream>
 #include <string>
 #include <vector>
 
@@ -833,22 +832,9 @@ void s2s_worker(const SeqJob &J, Exchange &X) {
 // ================================================================================================
 // iterate on several GPUs: the reads are dealt in contiguous shares, the candidate sets meet on their owners
 // ================================================================================================
-// rec_off[i] = first word of read i of the `.bin` image, n_reads + 1 entries; false when the image ends inside a read
-bool read_offsets(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, std::vector<uint64_t> *rec_off) {
-  rec_off->assign(n_reads + 1, 0);
-  uint64_t pos = 0;
-  for (uint64_t i = 0; i < n_reads; ++i) {
-    if (pos >= bin_words) return false;
-    (*rec_off)[i] = pos;
-    pos += 1 + div_ceil(bin[pos], 16);
-  }
-  (*rec_off)[n_reads] = pos;
-  return pos <= bin_words;
-}
-
-// n_ranks contiguous shares of the reads, balanced on their bases: the mark pass scans every base of every read
-void plan_read_shares(const uint32_t *bin, const std::vector<uint64_t> &rec_off, uint32_t n_ranks, uint64_t *first) {
-  plan_shares(rec_off.size() - 1, n_ranks, [&](uint64_t i) { return (uint64_t)bin[rec_off[i]]; }, first);
+// n_ranks contiguous shares of the n_reads reads, balanced on their bases: the mark pass scans every base of every read
+void plan_read_shares(const uint32_t *bin, const ReadLibIndex &ix, uint64_t n_reads, uint32_t n_ranks, uint64_t *first) {
+  plan_shares(n_reads, n_ranks, [&](uint64_t i) { return (uint64_t)bin[ix.word_of(i)]; }, first);
 }
 
 struct IterJob {
@@ -877,7 +863,7 @@ void iter_worker(const IterJob &J, Exchange &X) {
   a.bin = J.a.bin + J.word[r];
   a.bin_words = J.word[r + 1] - J.word[r];
   a.n_reads = J.first[r + 1] - J.first[r];
-  IterBuf set;
+  DevBuf set;
   uint64_t n_flanks = 0, n_set = 0, n_cand = 0, n_aligned = 0, n_chunks = 0;
   read_stream_stats_reset();
   {
@@ -1024,28 +1010,14 @@ extern "C" int mhb_count_run_multi(const mhb_count_opts *o, int n_gpus) {
   const std::string lib = o->read_lib_file, prefix = o->output_prefix ? o->output_prefix : "out";
   const double t0 = now_s();
   long long total_bases = 0, n_reads = 0;
-  {
-    std::ifstream is(lib + ".lib_info");
-    if (!(is >> total_bases >> n_reads)) return mhb_set_error(MHB_ERR_IO, "cannot read %s.lib_info", lib.c_str());
-  }
   std::vector<uint32_t> bin;
-  {
-    FILE *f = fopen((lib + ".bin").c_str(), "rb");
-    if (!f) return mhb_set_error(MHB_ERR_IO, "cannot open %s.bin", lib.c_str());
-    fseek(f, 0, SEEK_END);
-    const long sz = ftell(f);
-    fseek(f, 0, SEEK_SET);
-    bin.resize(((size_t)sz + 3) / 4 + 16, 0);
-    const size_t got = sz ? fread(bin.data(), 1, (size_t)sz, f) : 0;
-    fclose(f);
-    if (got != (size_t)sz) return mhb_set_error(MHB_ERR_IO, "short read on %s.bin", lib.c_str());
-    bin.resize(((size_t)sz + 3) / 4);
-  }
-  // the partitioned build deals contiguous blocks of a FIXED-length library to the GPUs; anything else: one GPU
-  const uint32_t L = (n_reads > 0 && !bin.empty()) ? bin[0] : 0;
-  const uint64_t stride = 1 + div_ceil(L, 16);
-  bool fixed = L > 0 && bin.size() == (uint64_t)n_reads * stride && o->k >= 12 && (uint64_t)n_reads >= (uint64_t)n_gpus;
-  for (long long i = 0; fixed && i < n_reads; ++i) fixed = bin[(uint64_t)i * stride] == L;
+  if (int rc = load_read_lib(lib, &bin, &n_reads, &total_bases)) return rc;
+  // the partitioned build deals contiguous blocks of a FIXED-length library to the GPUs; anything else (a truncated
+  // image included, which the single-GPU count reports): one GPU.  Indexed serially: the workers are forked next.
+  ReadLibIndex ix;
+  const bool fixed = o->k >= 12 && n_reads >= n_gpus &&
+                     !index_read_lib(bin.data(), bin.size(), n_reads, 0, &ix, FixedCheck::kSerial) && ix.fixed_len;
+  const uint32_t L = ix.fixed_len;
   if (!fixed) {
     XINFO("variable-length or tiny library: running on one GPU\n");
     return mhb_count_run(o);
@@ -1094,8 +1066,8 @@ extern "C" int mhb_iterate_run_multi(const mhb_iterate_opts *o, int n_gpus) {
   std::vector<uint32_t> bin;
   uint64_t n_reads = 0;
   if (int rc = iterate_load(o, &seqs, &bin, &n_reads)) return rc;
-  std::vector<uint64_t> rec_off;
-  if (!read_offsets(bin.data(), bin.size(), n_reads, &rec_off))
+  ReadLibIndex ix;  // indexed serially: the workers are forked next
+  if (index_read_lib(bin.data(), bin.size(), n_reads, 0, &ix, FixedCheck::kSerial))
     return mhb_set_error(MHB_ERR_IO, "%s ends inside a read", o->read_file);
   IterJob J;
   memset(&J.a, 0, sizeof(J.a));
@@ -1110,8 +1082,8 @@ extern "C" int mhb_iterate_run_multi(const mhb_iterate_opts *o, int n_gpus) {
   J.a.bin_words = bin.size();
   J.a.n_reads = n_reads;
   J.first.resize(n_gpus + 1);
-  plan_read_shares(bin.data(), rec_off, (uint32_t)n_gpus, J.first.data());
-  for (uint64_t f : J.first) J.word.push_back(rec_off[f]);
+  plan_read_shares(bin.data(), ix, n_reads, (uint32_t)n_gpus, J.first.data());
+  for (uint64_t f : J.first) J.word.push_back(ix.word_of(f));
   J.prefix = o->output_prefix;
   J.fd = open((J.prefix + ".edges.0").c_str(), O_WRONLY | O_CREAT | O_TRUNC, 0666);
   if (J.fd < 0) return mhb_set_error(MHB_ERR_IO, "cannot open %s.edges.0 for writing", J.prefix.c_str());
@@ -1126,9 +1098,9 @@ extern "C" int mhb_iterate_run_multi(const mhb_iterate_opts *o, int n_gpus) {
 extern "C" int mhb_plan_read_shares(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, uint32_t n_ranks,
                                     uint64_t *first_out) {
   if ((!bin && bin_words) || !first_out || n_ranks < 1) return mhb_set_error(MHB_ERR_ARG, "bad args");
-  std::vector<uint64_t> rec_off;
-  if (!read_offsets(bin, bin_words, n_reads, &rec_off)) return mhb_set_error(MHB_ERR_ARG, "the image ends inside a read");
-  plan_read_shares(bin, rec_off, n_ranks, first_out);
+  ReadLibIndex ix;  // serially, as mhb_iterate_run_multi before its fork
+  CKR(index_read_lib(bin, bin_words, n_reads, 0, &ix, FixedCheck::kSerial));
+  plan_read_shares(bin, ix, n_reads, n_ranks, first_out);
   return MHB_OK;
 }
 

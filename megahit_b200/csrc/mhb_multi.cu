@@ -129,9 +129,7 @@ extern "C" int mhb_compact_tip_edges(void *stream, const uint32_t *edges, const 
                                      uint32_t *tips_out, uint8_t *tip_aux_out, uint64_t capacity, uint64_t *cursor_dev) {
   if (n_solid == 0) return MHB_OK;
   if (!edges || !aux || !tips_out || !tip_aux_out || !cursor_dev) return mhb_set_error(MHB_ERR_ARG, "null buffer");
-  u64 g = (n_solid + 255) / 256;
-  if (g > (u64)sm_count() * 16) g = (u64)sm_count() * 16;
-  k_compact_tips<<<(unsigned)g, 256, 0, (cudaStream_t)stream>>>(edges, aux, n_solid, words_per_edge(k), tips_out, tip_aux_out,
+  k_compact_tips<<<grid_cap(n_solid, 256, 16), 256, 0, (cudaStream_t)stream>>>(edges, aux, n_solid, words_per_edge(k), tips_out, tip_aux_out,
                                                               capacity, (unsigned long long *)cursor_dev);
   CK_LAUNCH();
   return MHB_OK;
@@ -305,16 +303,15 @@ int mercy_probe_owned(void *stream, const mhb_dev_reads *reads, const uint64_t *
   OwnerTab ot;
   memcpy(ot.owner, owner_of_byte, 256);
   const u32 wpr = (max_read_len + 31) / 32 + 1, WE = words_per_edge(k), WM = div_ceil(k + 1, 16);
-  u64 g64 = (n_cand + 7) / 8;
-  if (g64 > (u64)sm_count() * 16) g64 = (u64)sm_count() * 16;
+  const unsigned g64 = grid_cap(n_cand, 8, 16);
   cudaStream_t st = (cudaStream_t)stream;
 #define M(WW)                                                                                                               \
   if (WM == WW) {                                                                                                           \
     if (accumulate)                                                                                                         \
-      k_mercy_probe_owned<WW, true><<<(unsigned)g64, 256, 0, st>>>(rv, cand_ids, n_cand, k, edges, (long long)n_edges,       \
+      k_mercy_probe_owned<WW, true><<<g64, 256, 0, st>>>(rv, cand_ids, n_cand, k, edges, (long long)n_edges,                 \
                                                                    (const uint2 *)lut, ot, me, WE, planes_out, wpr);         \
     else                                                                                                                    \
-      k_mercy_probe_owned<WW, false><<<(unsigned)g64, 256, 0, st>>>(rv, cand_ids, n_cand, k, edges, (long long)n_edges,      \
+      k_mercy_probe_owned<WW, false><<<g64, 256, 0, st>>>(rv, cand_ids, n_cand, k, edges, (long long)n_edges,                \
                                                                     (const uint2 *)lut, ot, me, WE, planes_out, wpr);        \
   }
   MHB_FOR_W(M)

@@ -20,46 +20,11 @@ int scan32(cudaStream_t st, const uint32_t *in, uint64_t n, uint64_t *out, uint6
 
 namespace {
 
-struct DevBuf {  // cudaMalloc'ed scratch released on scope exit
-  void *p = nullptr;
-  size_t bytes = 0;
-  ~DevBuf() { release(); }
-  void release() {
-    if (p) cudaFree(p);
-    p = nullptr;
-    bytes = 0;
-  }
-  int alloc(size_t b, const char *what) {
-    release();
-    b = (b + 255) & ~(size_t)255;
-    if (b == 0) b = 256;
-    cudaError_t e = cudaMalloc(&p, b);
-    if (e != cudaSuccess) {
-      cudaGetLastError();
-      p = nullptr;
-      return mhb_set_error(MHB_ERR_NOMEM, "read2sdbg: cudaMalloc of %zu bytes for %s failed: %s", b, what,
-                           cudaGetErrorString(e));
-    }
-    bytes = b;
-    return MHB_OK;
-  }
-  // keep the allocation when it is already large enough (the two stages share their big buffers)
-  int ensure(size_t b, const char *what) { return bytes >= b ? MHB_OK : alloc(b, what); }
-  template <class T>
-  T *as() const { return reinterpret_cast<T *>(p); }
-};
-
 // the record / item ping-pong buffers and the sort workspace, shared by stage 1 and stage 2 (cudaMalloc + cudaFree of
 // 20-GB buffers between the stages cost ~0.2 s at 10 M reads)
 struct BigBufs {
   DevBuf a, b, ws;
 };
-
-#define CKR(call)        \
-  do {                   \
-    int rc_ = (call);    \
-    if (rc_) return rc_; \
-  } while (0)
 
 // phase marks on the stream: deltas include host-side gaps (allocations, synchronisations) between the marks
 struct PhaseTrace {
@@ -95,36 +60,22 @@ struct PhaseTrace {
   }
 };
 
-unsigned grid_for(uint64_t n, unsigned threads, unsigned per_sm = 16) {
-  uint64_t g = (n + threads - 1) / threads;
-  const uint64_t cap = (uint64_t)sm_count() * per_sm;
-  if (g > cap) g = cap;
-  if (g < 1) g = 1;
-  return (unsigned)g;
-}
-
-// host index of the `.bin` image: package geometry of every read
+// host index of the `.bin` image: package geometry of every read, derived from the record offsets of index_read_lib
 struct PkgIndex {
+  ReadLibIndex li;  // fixed-length check and record offsets (no unit offsets: streamed chunks derive theirs on the device)
   uint32_t fixed_len = 0, fixed_words = 0, max_len = 0;
   uint64_t n_reads = 0, n_words = 0, n_bases = 0, n_s1 = 0, n_edges = 0;
-  std::vector<uint64_t> rec_off, word_off, base_off, s1_off, edge_off;
+  std::vector<uint64_t> word_off, base_off, s1_off, edge_off;
   std::vector<uint32_t> len;
 };
 
 int index_pkg(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, uint32_t k, PkgIndex *ix) {
   ix->n_reads = n_reads;
+  CKR(index_read_lib(bin, bin_words, n_reads, 0, &ix->li));
+  std::vector<uint64_t>().swap(ix->li.unit_off);
   if (n_reads == 0) return MHB_OK;
-  if (bin_words == 0) return mhb_set_error(MHB_ERR_ARG, "empty .bin image for %llu reads", (unsigned long long)n_reads);
-  const uint32_t L0 = bin[0];
-  const uint64_t stride = 1 + div_ceil(L0, 16);
-  bool fixed = L0 > 0 && bin_words == n_reads * stride;
-  if (fixed) {
-    int bad = 0;
-#pragma omp parallel for reduction(| : bad) schedule(static)
-    for (long long r = 0; r < (long long)n_reads; ++r) bad |= bin[(uint64_t)r * stride] != L0;
-    fixed = !bad;
-  }
-  if (fixed) {
+  const uint32_t L0 = ix->li.fixed_len;
+  if (L0) {
     ix->fixed_len = ix->max_len = L0;
     ix->fixed_words = div_ceil(L0, 16);
     ix->n_words = n_reads * ix->fixed_words;
@@ -135,25 +86,21 @@ int index_pkg(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, uint32_
     }
     return MHB_OK;
   }
-  ix->rec_off.resize(n_reads + 1);
   ix->word_off.resize(n_reads + 1);
   ix->base_off.resize(n_reads + 1);
   ix->s1_off.resize(n_reads + 1);
   ix->edge_off.resize(n_reads + 1);
   ix->len.resize(n_reads);
-  uint64_t pos = 0, w = 0, b = 0, s1 = 0, e = 0;
+  uint64_t w = 0, b = 0, s1 = 0, e = 0;
   for (uint64_t r = 0; r < n_reads; ++r) {
-    if (pos >= bin_words) return mhb_set_error(MHB_ERR_ARG, ".bin image truncated at read %llu", (unsigned long long)r);
-    const uint32_t L = bin[pos];
+    const uint32_t L = bin[ix->li.rec_off[r]];
     const uint32_t eff = L == 0 ? 1 : L;  // sequence_package.h:276-281
-    ix->rec_off[r] = pos;
     ix->word_off[r] = w;
     ix->base_off[r] = b;
     ix->s1_off[r] = s1;
     ix->edge_off[r] = e;
     ix->len[r] = eff;
     ix->max_len = std::max(ix->max_len, eff);
-    pos += 1 + div_ceil(L, 16);
     w += div_ceil(eff, 16);
     b += eff;
     if (eff >= k + 1) {
@@ -161,8 +108,6 @@ int index_pkg(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, uint32_
       e += eff - k;
     }
   }
-  if (pos > bin_words) return mhb_set_error(MHB_ERR_ARG, ".bin image truncated");
-  ix->rec_off[n_reads] = pos;
   ix->word_off[n_reads] = w;
   ix->base_off[n_reads] = b;
   ix->s1_off[n_reads] = s1;
@@ -184,17 +129,6 @@ int upload(DevBuf &d, const std::vector<T> &v, const char *what) {
 // ---- device memory plan ----
 // Caps on the records / items of one round (mhb_set_r2s_round_limit); 0 = derive from free device memory
 uint64_t g_r2s_s1_limit = 0, g_r2s_s2_limit = 0;
-
-size_t pad(size_t b) { return (b + 255) & ~(size_t)255; }
-
-size_t free_device_bytes() {
-  size_t f = 0, t = 0;
-  if (cudaMemGetInfo(&f, &t) != cudaSuccess) {
-    cudaGetLastError();
-    return 0;
-  }
-  return f;
-}
 
 // The stage-1 record layout of k (DESIGN.md §4.10).  Wide: NW key words + the 2 read_info words, sorted as whole
 // records.  Narrow, where that exceeds the 17-word records of mhb_sort_records (k > 237): NW key words + a 32-bit row
@@ -219,9 +153,9 @@ size_t s1_ws_bytes(uint64_t n, const S1Layout &l) { return mhb_sort_workspace_by
 // read_info side array and the two pair buffers
 size_t s1_pass_bytes(uint64_t n, const S1Layout &l) {
   const uint64_t seg_cap = n / (kKmInsertThreshold + 1) + 2;
-  return 2 * pad((size_t)n * l.RW * 4 + 16) + pad(s1_ws_bytes(n, l)) + pad((MHB_NUM_BUCKETS + 1) * 8) +
-         2 * pad(seg_cap * sizeof(KmSeg)) + 2 * pad((n / 32 + 2) * 4) + pad((size_t)n * 2 + 64) + 256 +
-         (l.narrow ? 3 * pad((size_t)n * 8 + 16) : 0);
+  return 2 * pad256((size_t)n * l.RW * 4 + 16) + pad256(s1_ws_bytes(n, l)) + pad256((MHB_NUM_BUCKETS + 1) * 8) +
+         2 * pad256(seg_cap * sizeof(KmSeg)) + 2 * pad256((n / 32 + 2) * 4) + pad256((size_t)n * 2 + 64) + 256 +
+         (l.narrow ? 3 * pad256((size_t)n * 8 + 16) : 0);
 }
 
 // The stage-1 round plan: *max_n = 0 for one pass over all n_s1 records, else the most records of one round - the
@@ -233,8 +167,8 @@ int s1_plan_round(const S1Layout &l, uint64_t n_s1, uint64_t max_reads, size_t a
   if (!((limit && n_s1 > limit) || s1_pass_bytes(n_s1, l) > avail || n_s1 > cap)) return 0;
   uint64_t mx = limit;
   if (!mx) {
-    const size_t fixed = pad(max_reads * 4) + pad((max_reads + 1) * 8) + pad((max_reads / 4096 + 4) * 8) +
-                         pad(MHB_NUM_BUCKETS * 8) + 256;
+    const size_t fixed = pad256(max_reads * 4) + pad256((max_reads + 1) * 8) + pad256((max_reads / 4096 + 4) * 8) +
+                         pad256(MHB_NUM_BUCKETS * 8) + 256;
     mx = largest_round(n_s1, fixed, avail, [&](uint64_t n) { return s1_pass_bytes(n, l); });
     if (!mx) return 1;
   }
@@ -245,9 +179,9 @@ int s1_plan_round(const S1Layout &l, uint64_t n_s1, uint64_t max_reads, size_t a
 // device bytes of one stage-2 pass over n items: items, sort buffer and workspace, run collapse, emitter scratch + stream
 size_t s2_pass_bytes(uint64_t n, uint32_t W, uint32_t k) {
   const uint64_t n_tiles = (n + kDdTile - 1) / kDdTile;
-  return 2 * pad((size_t)n * W * 4 + 16) + pad(mhb_s2s_sort_workspace_bytes(n, k)) + pad(n_tiles * 4) + pad(n_tiles * 8) +
-         pad((n_tiles / 4096 + 4) * 8) + pad((size_t)n * 8) + pad(mhb_s2s_emit_scratch_bytes(n, k)) +
-         pad((size_t)n * (4ull + 4ull * words_per_tip_label(k)) + 16);
+  return 2 * pad256((size_t)n * W * 4 + 16) + pad256(mhb_s2s_sort_workspace_bytes(n, k)) + pad256(n_tiles * 4) + pad256(n_tiles * 8) +
+         pad256((n_tiles / 4096 + 4) * 8) + pad256((size_t)n * 8) + pad256(mhb_s2s_emit_scratch_bytes(n, k)) +
+         pad256((size_t)n * (4ull + 4ull * words_per_tip_label(k)) + 16);
 }
 
 // contiguous ranges of 16-bit bucket ids of at most max_n entries each, from the histogram of bucket ids (its rows are
@@ -315,16 +249,14 @@ class PkgSource {
   std::vector<PkgChunk> chunks;  // host geometry of every chunk (none for an empty library)
   uint64_t max_reads = 0, max_words = 0, max_plane_words = 0;
 
-  int plan(const mhb_build_args *a, PkgIndex &ix, uint32_t k, bool stream, uint64_t chunk_bytes) {
+  int plan(const mhb_build_args *a, const PkgIndex &ix, uint32_t k, bool stream, uint64_t chunk_bytes) {
     args_ = a;
     k_ = k;
     streamed_ = stream;
     fixed_ = ix.fixed_len != 0;
     std::vector<uint64_t> first = {0, ix.n_reads};
     if (stream) {
-      li_.fixed_len = ix.fixed_len;
-      li_.rec_off.swap(ix.rec_off);  // no unit offsets: the chunk's offsets are derived on the device
-      CKR(rs_.init(a->bin, a->bin_words, ix.n_reads, li_, chunk_bytes));
+      CKR(rs_.init(a->bin, a->bin_words, ix.n_reads, ix.li, chunk_bytes));
       first = rs_.first_reads();
     }
     for (size_t i = 0; i + 1 < first.size() && ix.n_reads; ++i) {
@@ -338,42 +270,42 @@ class PkgSource {
   }
   // device bytes of the streamed form: both `.bin` chunk slots, the package slot, the chunk's offsets and their scratch
   size_t streamed_bytes() const {
-    return pad(rs_.device_bytes()) + pad((size_t)max_words * 4 + 64) +
-           (fixed_ ? 0 : 4 * pad((max_reads + 1) * 8) + 4 * pad(max_reads * 4) + pad((max_reads / 4096 + 4) * 8));
+    return pad256(rs_.device_bytes()) + pad256((size_t)max_words * 4 + 64) +
+           (fixed_ ? 0 : 4 * pad256((max_reads + 1) * 8) + 4 * pad256(max_reads * 4) + pad256((max_reads / 4096 + 4) * 8));
   }
   // resident: upload + reverse now; streamed: the chunk buffers
   int bind(cudaStream_t st, const PkgIndex &ix) {
-    CKR(pkg_.alloc((size_t)max_words * 4 + 64, streamed_ ? "package chunk" : "package"));
+    CKR(pkg_.alloc((size_t)max_words * 4 + 64, streamed_ ? "read2sdbg: package chunk" : "read2sdbg: package"));
     if (streamed_) {
-      CKR(lib_.alloc(rs_.device_bytes(), ".bin chunk slots"));
+      CKR(lib_.alloc(rs_.device_bytes(), "read2sdbg: .bin chunk slots"));
       CKR(rs_.bind(lib_.p, st));
       if (!fixed_) {
-        CKR(word_off_.alloc((max_reads + 1) * 8, "chunk word offsets"));
-        CKR(len_.alloc(max_reads * 4, "chunk lengths"));
-        CKR(base_off_.alloc((max_reads + 1) * 8, "chunk base offsets"));
-        CKR(s1_off_.alloc((max_reads + 1) * 8, "chunk stage-1 offsets"));
-        CKR(edge_off_.alloc((max_reads + 1) * 8, "chunk edge offsets"));
-        CKR(geom_.alloc(3 * pad(max_reads * 4), "chunk read geometry"));
-        CKR(bsum_.alloc((max_reads / 4096 + 4) * 8, "scan sums"));
+        CKR(word_off_.alloc((max_reads + 1) * 8, "read2sdbg: chunk word offsets"));
+        CKR(len_.alloc(max_reads * 4, "read2sdbg: chunk lengths"));
+        CKR(base_off_.alloc((max_reads + 1) * 8, "read2sdbg: chunk base offsets"));
+        CKR(s1_off_.alloc((max_reads + 1) * 8, "read2sdbg: chunk stage-1 offsets"));
+        CKR(edge_off_.alloc((max_reads + 1) * 8, "read2sdbg: chunk edge offsets"));
+        CKR(geom_.alloc(3 * pad256(max_reads * 4), "read2sdbg: chunk read geometry"));
+        CKR(bsum_.alloc((max_reads / 4096 + 4) * 8, "read2sdbg: scan sums"));
       }
       return MHB_OK;
     }
     if (chunks.empty()) return MHB_OK;
     PkgChunk &c = chunks[0];
     DevBuf d_bin, d_rec_off;
-    CKR(d_bin.alloc((size_t)args_->bin_words * 4 + 64, ".bin image"));
+    CKR(d_bin.alloc((size_t)args_->bin_words * 4 + 64, "read2sdbg: .bin image"));
     CK(cudaMemcpyAsync(d_bin.p, args_->bin, (size_t)args_->bin_words * 4, cudaMemcpyHostToDevice, st));
     if (!fixed_) {
-      CKR(upload(d_rec_off, ix.rec_off, "record offsets"));
-      CKR(upload(word_off_, ix.word_off, "word offsets"));
-      CKR(upload(len_, ix.len, "lengths"));
-      CKR(upload(base_off_, ix.base_off, "base offsets"));
-      CKR(upload(s1_off_, ix.s1_off, "stage-1 offsets"));
-      CKR(upload(edge_off_, ix.edge_off, "edge offsets"));
+      CKR(upload(d_rec_off, ix.li.rec_off, "read2sdbg: record offsets"));
+      CKR(upload(word_off_, ix.word_off, "read2sdbg: word offsets"));
+      CKR(upload(len_, ix.len, "read2sdbg: lengths"));
+      CKR(upload(base_off_, ix.base_off, "read2sdbg: base offsets"));
+      CKR(upload(s1_off_, ix.s1_off, "read2sdbg: stage-1 offsets"));
+      CKR(upload(edge_off_, ix.edge_off, "read2sdbg: edge offsets"));
       set_offsets(c.pv);
     }
     if (c.n_words) {
-      k_r2s_reverse<<<grid_for(c.n_words, 256), 256, 0, st>>>(d_bin.as<u32>(), c.pv.n_reads, c.pv.fixed_len,
+      k_r2s_reverse<<<grid_cap(c.n_words, 256, 16), 256, 0, st>>>(d_bin.as<u32>(), c.pv.n_reads, c.pv.fixed_len,
                                                              d_rec_off.as<u64>(), c.pv, pkg_.as<u32>(), c.n_words);
       CK_LAUNCH();
     }
@@ -387,8 +319,8 @@ class PkgSource {
       PkgChunk c = chunks[v.index];
       const uint64_t n = c.pv.n_reads;
       if (!fixed_) {
-        u32 *words = geom_.as<u32>(), *s1 = words + pad(max_reads * 4) / 4, *edges = s1 + pad(max_reads * 4) / 4;
-        k_r2s_chunk_geom<<<grid_for(n, 256), 256, 0, st>>>(v.bin, v.rec_off, n, k_, len_.as<u32>(), words, s1, edges);
+        u32 *words = geom_.as<u32>(), *s1 = words + pad256(max_reads * 4) / 4, *edges = s1 + pad256(max_reads * 4) / 4;
+        k_r2s_chunk_geom<<<grid_cap(n, 256, 16), 256, 0, st>>>(v.bin, v.rec_off, n, k_, len_.as<u32>(), words, s1, edges);
         CK_LAUNCH();
         u64 *bs = bsum_.as<u64>();
         CKR(scan32(st, words, n, word_off_.as<u64>(), word_off_.as<u64>() + n, bs));
@@ -398,7 +330,7 @@ class PkgSource {
         set_offsets(c.pv);
       }
       if (c.n_words) {
-        k_r2s_reverse<<<grid_for(c.n_words, 256), 256, 0, st>>>(v.bin, n, c.pv.fixed_len, v.rec_off, c.pv, pkg_.as<u32>(),
+        k_r2s_reverse<<<grid_cap(c.n_words, 256, 16), 256, 0, st>>>(v.bin, n, c.pv.fixed_len, v.rec_off, c.pv, pkg_.as<u32>(),
                                                                c.n_words);
         CK_LAUNCH();
       }
@@ -418,7 +350,6 @@ class PkgSource {
   const mhb_build_args *args_ = nullptr;
   uint32_t k_ = 0;
   bool streamed_ = false, fixed_ = false;
-  ReadLibIndex li_;
   ReadStream rs_;
   DevBuf lib_, pkg_, word_off_, len_, base_off_, s1_off_, edge_off_, geom_, bsum_;
 };
@@ -432,11 +363,11 @@ struct ResidentPlan {
 };
 ResidentPlan resident_plan(const PkgIndex &ix, uint64_t bin_words, int32_t m, bool mercy) {
   const uint64_t bit_words = ix.n_bases / 32 + 2;
-  const size_t planes = (m > 1 ? pad(bit_words * 4) : 0) + (mercy ? 4 * pad(bit_words * 4) : 0);
+  const size_t planes = (m > 1 ? pad256(bit_words * 4) : 0) + (mercy ? 4 * pad256(bit_words * 4) : 0);
   ResidentPlan p;
-  p.resident = pad((size_t)ix.n_words * 4 + 64) + (ix.fixed_len ? 0 : 5 * pad((ix.n_reads + 1) * 8) + pad(ix.n_reads * 4)) +
-               planes + pad(65536 * 8) + pad(64) + pad((size_t)MHB_NUM_BUCKETS * 32) + pad(128);
-  p.upload = pad((size_t)bin_words * 4 + 64) + (ix.fixed_len ? 0 : pad((ix.n_reads + 1) * 8));
+  p.resident = pad256((size_t)ix.n_words * 4 + 64) + (ix.fixed_len ? 0 : 5 * pad256((ix.n_reads + 1) * 8) + pad256(ix.n_reads * 4)) +
+               planes + pad256(65536 * 8) + pad256(64) + pad256((size_t)MHB_NUM_BUCKETS * 32) + pad256(128);
+  p.upload = pad256((size_t)bin_words * 4 + 64) + (ix.fixed_len ? 0 : pad256((ix.n_reads + 1) * 8));
   return p;
 }
 
@@ -446,8 +377,8 @@ ResidentPlan resident_plan(const PkgIndex &ix, uint64_t bin_words, int32_t m, bo
 bool stream_decide(const ResidentPlan &p, const PkgIndex &ix, uint32_t k, int32_t m, size_t free_b, uint64_t chunk_limit) {
   const double room = free_b > p.resident ? 0.92 * (double)(free_b - p.resident) : 0.0;
   const uint32_t W = s2s_record_words(k);
-  const size_t s1_fixed = pad(ix.n_reads * 4) + pad((ix.n_reads + 1) * 8) + pad((ix.n_reads / 4096 + 4) * 8) +
-                          pad(MHB_NUM_BUCKETS * 8) + 256;
+  const size_t s1_fixed = pad256(ix.n_reads * 4) + pad256((ix.n_reads + 1) * 8) + pad256((ix.n_reads / 4096 + 4) * 8) +
+                          pad256(MHB_NUM_BUCKETS * 8) + 256;
   const bool no_round = (m > 1 && ix.n_s1 && (double)(s1_fixed + s1_pass_bytes(1, s1_layout(k))) > room) ||
                         (ix.n_edges && (double)s2_pass_bytes(1, W, k) > room);
   return mhb_read_stream_decide(p.resident + p.upload, free_b, no_round ? 1 : 0, chunk_limit) != 0;
@@ -476,28 +407,28 @@ int run_stage1(cudaStream_t st, const EachChunk &each, const PkgView &shape, con
   const bool one_pass = max_n == 0;
   if (one_pass) max_n = ix.n_s1;
   if (max_n > s1_round_cap(l)) return mhb_set_error(MHB_ERR_ARG, "read2sdbg: too many stage-1 records for one round");
-  CKR(big.a.ensure(std::max((size_t)max_n * RW * 4 + 16, min_rec_bytes), "records"));
-  CKR(big.b.ensure(std::max((size_t)max_n * RW * 4 + 16, min_rec_bytes), "records (sort buffer)"));
-  CKR(big.ws.ensure(std::max(s1_ws_bytes(max_n, l), min_ws_bytes), "sort workspace"));
+  CKR(big.a.ensure(std::max((size_t)max_n * RW * 4 + 16, min_rec_bytes), "read2sdbg: records"));
+  CKR(big.b.ensure(std::max((size_t)max_n * RW * 4 + 16, min_rec_bytes), "read2sdbg: records (sort buffer)"));
+  CKR(big.ws.ensure(std::max(s1_ws_bytes(max_n, l), min_ws_bytes), "read2sdbg: sort workspace"));
   S1Side side;
   if (l.narrow) {
-    CKR(side.info.alloc((size_t)max_n * 8 + 16, "stage-1 read_info"));
-    CKR(side.pa.alloc((size_t)max_n * 8 + 16, "bucket partition pairs"));
-    CKR(side.pb.alloc((size_t)max_n * 8 + 16, "bucket partition pairs (sort buffer)"));
+    CKR(side.info.alloc((size_t)max_n * 8 + 16, "read2sdbg: stage-1 read_info"));
+    CKR(side.pa.alloc((size_t)max_n * 8 + 16, "read2sdbg: bucket partition pairs"));
+    CKR(side.pb.alloc((size_t)max_n * 8 + 16, "read2sdbg: bucket partition pairs (sort buffer)"));
   }
   u64 *d_info = l.narrow ? side.info.as<u64>() : nullptr;
   std::vector<std::pair<uint32_t, uint32_t>> ranges = {{0u, 65535u}};
   DevBuf per_read, off, bsum, total;
   if (!one_pass) {
     DevBuf h16;
-    CKR(per_read.alloc(chunk_reads * 4, "per-read record counts"));
-    CKR(off.alloc((chunk_reads + 1) * 8, "per-read record offsets"));
-    CKR(bsum.alloc((chunk_reads / 4096 + 4) * 8, "scan sums"));
-    CKR(h16.alloc(MHB_NUM_BUCKETS * 8, "bucket histogram"));
-    CKR(total.alloc(8, "round size"));
+    CKR(per_read.alloc(chunk_reads * 4, "read2sdbg: per-read record counts"));
+    CKR(off.alloc((chunk_reads + 1) * 8, "read2sdbg: per-read record offsets"));
+    CKR(bsum.alloc((chunk_reads / 4096 + 4) * 8, "read2sdbg: scan sums"));
+    CKR(h16.alloc(MHB_NUM_BUCKETS * 8, "read2sdbg: bucket histogram"));
+    CKR(total.alloc(8, "read2sdbg: round size"));
     CK(cudaMemsetAsync(h16.p, 0, MHB_NUM_BUCKETS * 8, st));
     if (int rc_ = each([&](const PkgChunk &c) -> int {
-      const unsigned grid = grid_for(c.pv.n_reads * 32, 256);  // one warp per read
+      const unsigned grid = grid_cap(c.pv.n_reads * 32, 256, 16);  // one warp per read
 #define M(WW)   \
   if (NW == WW) \
     k_r2s_s1_range<WW, kS1Hist><<<grid, 256, 0, st>>>(c.pv, k, 0, 65535, h16.as<unsigned long long>(), nullptr, nullptr, nullptr);
@@ -521,7 +452,7 @@ int run_stage1(cudaStream_t st, const EachChunk &each, const PkgView &shape, con
         if (c.n_s1) {
 #define M(WW)                                                                                                      \
   if (NW == WW)                                                                                                    \
-    k_r2s_s1_extract<WW><<<grid_for(c.n_s1, 256), 256, 0, st>>>(c.pv, k, big.a.as<u32>(), d_info, c.s1_0, c.n_s1);
+    k_r2s_s1_extract<WW><<<grid_cap(c.n_s1, 256, 16), 256, 0, st>>>(c.pv, k, big.a.as<u32>(), d_info, c.s1_0, c.n_s1);
           MHB_FOR_WR(M)
 #undef M
           CK_LAUNCH();
@@ -529,7 +460,7 @@ int run_stage1(cudaStream_t st, const EachChunk &each, const PkgView &shape, con
         n += c.n_s1;
         return MHB_OK;
       }
-      const unsigned grid = grid_for(c.pv.n_reads * 32, 256);
+      const unsigned grid = grid_cap(c.pv.n_reads * 32, 256, 16);
 #define M(WW)                                                                                                          \
   if (NW == WW)                                                                                                        \
     k_r2s_s1_range<WW, kS1Count><<<grid, 256, 0, st>>>(c.pv, k, rg.first, rg.second, nullptr, per_read.as<u32>(), nullptr, \
@@ -577,23 +508,23 @@ int s1_sort_post(cudaStream_t st, const PkgView &pv, uint32_t k, int32_t m, bool
   DevBuf bstart, segs0, segs1, counter, bnd;
   DevBuf &a = big.a, &b = big.b, &ws = big.ws;
   const size_t ws_bytes = s1_ws_bytes(n, l);
-  CKR(bstart.alloc((MHB_NUM_BUCKETS + 1) * 8, "bucket bounds"));
+  CKR(bstart.alloc((MHB_NUM_BUCKETS + 1) * 8, "read2sdbg: bucket bounds"));
   const uint64_t seg_cap = n / (kKmInsertThreshold + 1) + 2;
-  CKR(segs0.alloc(seg_cap * sizeof(KmSeg), "kmsort ranges"));
-  CKR(segs1.alloc(seg_cap * sizeof(KmSeg), "kmsort ranges"));
-  CKR(counter.alloc(8, "counter"));
-  CKR(bnd.alloc((n / 32 + 2) * 4, "range marks"));
+  CKR(segs0.alloc(seg_cap * sizeof(KmSeg), "read2sdbg: kmsort ranges"));
+  CKR(segs1.alloc(seg_cap * sizeof(KmSeg), "read2sdbg: kmsort ranges"));
+  CKR(counter.alloc(8, "read2sdbg: counter"));
+  CKR(bnd.alloc((n / 32 + 2) * 4, "read2sdbg: range marks"));
   CK(cudaMemsetAsync(bnd.p, 0, (n / 32 + 2) * 4, st));
   // the reference's bucket input order: records of one 16-bit bucket in global read order = a STABLE sort on the two
   // leading key bytes (base_engine.cpp:323-348 fills every bucket thread by thread, i.e. in read order)
   int in_b = 0;
   if (l.narrow) {
     const uint8_t bytes[2] = {6, 7};  // the two leading bytes of a (word 0, row) pair
-    k_r2s_s1_pairs<<<grid_for(n, 256), 256, 0, st>>>(a.as<u32>(), n, RW, side.pa.as<u32>());
+    k_r2s_s1_pairs<<<grid_cap(n, 256, 16), 256, 0, st>>>(a.as<u32>(), n, RW, side.pa.as<u32>());
     CK_LAUNCH();
     int in_pb = 0;
     CKR(mhb_sort_records(st, side.pa.as<u32>(), side.pb.as<u32>(), n, 2, bytes, 2, nullptr, ws.p, ws_bytes, &in_pb));
-    k_r2s_s1_gather<<<grid_for(n * RW, 256), 256, 0, st>>>(a.as<u32>(), in_pb ? side.pb.as<u32>() : side.pa.as<u32>(), n,
+    k_r2s_s1_gather<<<grid_cap(n * RW, 256, 16), 256, 0, st>>>(a.as<u32>(), in_pb ? side.pb.as<u32>() : side.pa.as<u32>(), n,
                                                            RW, b.as<u32>());
     CK_LAUNCH();
     in_b = 1;
@@ -625,9 +556,9 @@ int s1_sort_post(cudaStream_t st, const PkgView &pv, uint32_t k, int32_t m, bool
     uint32_t cap = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(max_bucket, 1024), 65535);
     cap = (cap + 1023) & ~1023u;
     if (const char *e = getenv("MHB_R2S_KM_CAP")) cap = std::max(1024u, (uint32_t)atoi(e) & ~1023u);  // tests: force the fall-back
-    CKR(todo.alloc((n / 32 + 2) * 4, "unsorted-range marks"));
+    CKR(todo.alloc((n / 32 + 2) * 4, "read2sdbg: unsorted-range marks"));
     CK(cudaMemsetAsync(todo.p, 0, (n / 32 + 2) * 4, st));
-    CKR(src16.alloc((size_t)n * 2 + 64, "kmsort source indices"));
+    CKR(src16.alloc((size_t)n * 2 + 64, "read2sdbg: kmsort source indices"));
     d_todo = todo.as<u32>();
     u32 *other = in_b ? a.as<u32>() : b.as<u32>();
 #define M(WW)                                                                                                           \
@@ -670,9 +601,7 @@ int s1_sort_post(cudaStream_t st, const PkgView &pv, uint32_t k, int32_t m, bool
       CK(cudaFuncSetAttribute(k_r2s_km_warp<WW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));               \
       attr = true;                                                                                                       \
     }                                                                                                                    \
-    uint64_t g = (n_next + kKmWarps - 1) / kKmWarps;                                                                     \
-    if (g > (uint64_t)sm_count() * 8) g = (uint64_t)sm_count() * 8;                                                      \
-    k_r2s_km_warp<WW><<<(unsigned)g, kKmWarps * 32, smem, st>>>(recs, NW, kb, cur, n_next, nxt, d_cnt, seg_cap,           \
+    k_r2s_km_warp<WW><<<grid_cap(n_next, kKmWarps, 8), kKmWarps * 32, smem, st>>>(recs, NW, kb, cur, n_next, nxt, d_cnt, seg_cap, \
                                                               bnd.as<u32>(), d_todo);                                    \
   }
       MHB_FOR_RW(M)
@@ -688,14 +617,14 @@ int s1_sort_post(cudaStream_t st, const PkgView &pv, uint32_t k, int32_t m, bool
     CK_LAUNCH();
   }
 #define M(WW) \
-  if (RW == WW) k_r2s_kmsort_finish<WW><<<grid_for(n, 256, 32), 256, 0, st>>>(recs, n, NW, bnd.as<u32>(), d_todo);
+  if (RW == WW) k_r2s_kmsort_finish<WW><<<grid_cap(n, 256, 32), 256, 0, st>>>(recs, n, NW, bnd.as<u32>(), d_todo);
   MHB_FOR_RW(M)
 #undef M
   CK_LAUNCH();
   tr.mark("s1.kmsort.finish");
 #define M(WW)                                                                                                          \
   if (RW == WW)                                                                                                        \
-    k_r2s_s1_post<WW><<<grid_for(n, 256, 32), 256, 0, st>>>(recs, l.narrow ? side.info.as<u64>() : nullptr, n, NW, k, m, \
+    k_r2s_s1_post<WW><<<grid_cap(n, 256, 32), 256, 0, st>>>(recs, l.narrow ? side.info.as<u64>() : nullptr, n, NW, k, m, \
                                                             pv, out, need_mercy ? 1 : 0, d_mul_hist);
   MHB_FOR_RW(M)
 #undef M
@@ -724,9 +653,9 @@ int s2_sort_emit(cudaStream_t st, uint32_t k, BigBufs &big, S2Bufs &sb, uint64_t
   u32 *uniq = in_b ? a.as<u32>() : b.as<u32>();
   // equal items -> one item carrying the run length (read_to_sdbg_s2.cpp:560-572)
   const uint64_t n_tiles = (n + kDdTile - 1) / kDdTile;
-  CKR(sb.tile_heads.ensure(n_tiles * 4, "tile counts"));
-  CKR(sb.tile_off.ensure(n_tiles * 8, "tile offsets"));
-  CKR(sb.bsum.ensure((n_tiles / 4096 + 4) * 8, "scan sums"));
+  CKR(sb.tile_heads.ensure(n_tiles * 4, "read2sdbg: tile counts"));
+  CKR(sb.tile_off.ensure(n_tiles * 8, "read2sdbg: tile offsets"));
+  CKR(sb.bsum.ensure((n_tiles / 4096 + 4) * 8, "read2sdbg: scan sums"));
 #define M(WW) \
   if (W == WW) k_r2s_dd_count<WW><<<(unsigned)n_tiles, kDdThreads, 0, st>>>(sorted, n, sb.tile_heads.as<u32>());
   MHB_FOR_WR(M)
@@ -736,7 +665,7 @@ int s2_sort_emit(cudaStream_t st, uint32_t k, BigBufs &big, S2Bufs &sb, uint64_t
   unsigned long long n_u = 0;
   CK(cudaMemcpyAsync(&n_u, d_counter + 2, 8, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  CKR(sb.heads.ensure((size_t)n_u * 8, "run heads"));
+  CKR(sb.heads.ensure((size_t)n_u * 8, "read2sdbg: run heads"));
 #define M(WW)                                                                                                             \
   if (W == WW)                                                                                                            \
     k_r2s_dd_heads<WW><<<(unsigned)n_tiles, kDdThreads, 0, st>>>(sorted, n, sb.tile_off.as<u64>(), sb.heads.as<u64>());
@@ -744,15 +673,15 @@ int s2_sort_emit(cudaStream_t st, uint32_t k, BigBufs &big, S2Bufs &sb, uint64_t
 #undef M
   CK_LAUNCH();
 #define M(WW) \
-  if (W == WW) k_r2s_dd_build<WW><<<grid_for(n_u, 256), 256, 0, st>>>(sorted, n, sb.heads.as<u64>(), n_u, uniq);
+  if (W == WW) k_r2s_dd_build<WW><<<grid_cap(n_u, 256, 16), 256, 0, st>>>(sorted, n, sb.heads.as<u64>(), n_u, uniq);
   MHB_FOR_WR(M)
 #undef M
   CK_LAUNCH();
   tr.mark("s2.collapse");
   const size_t scr_bytes = mhb_s2s_emit_scratch_bytes(n_u, k);
   *cap_bytes = (uint64_t)n_u * (4ull + 4ull * WPT) + 16;
-  CKR(sb.scr.ensure(scr_bytes, "emit scratch"));
-  CKR(sb.bytes.ensure(*cap_bytes, "SdBG stream"));
+  CKR(sb.scr.ensure(scr_bytes, "read2sdbg: emit scratch"));
+  CKR(sb.bytes.ensure(*cap_bytes, "read2sdbg: SdBG stream"));
   CKR(mhb_s2s_emit_fmt(st, uniq, n_u, k, sb.bytes.as<uint8_t>(), *cap_bytes, d_table, d_totals, sb.scr.p, scr_bytes, 1));
   *n_u_out = n_u;
   return MHB_OK;
@@ -778,16 +707,16 @@ int mercy_count_pass(cudaStream_t st, const EachChunk &each, uint32_t k, int32_t
     if (mercy) {
       const uint64_t nw = c.w_end - c.w0;
       CK(cudaMemsetAsync(d_mplane, 0, nw * 4, st));
-      k_r2s_mercy<<<grid_for(c.pv.n_reads, 256), 256, 0, st>>>(c.pv, k, so, d_mplane - c.w0, d_counter + 1);
+      k_r2s_mercy<<<grid_cap(c.pv.n_reads, 256, 16), 256, 0, st>>>(c.pv, k, so, d_mplane - c.w0, d_counter + 1);
       CK_LAUNCH();
-      k_r2s_or_words<<<grid_for(nw, 256), 256, 0, st>>>(so.is_solid + c.w0, d_mplane, nw);
+      k_r2s_or_words<<<grid_cap(nw, 256, 16), 256, 0, st>>>(so.is_solid + c.w0, d_mplane, nw);
       CK_LAUNCH();
       tr.mark("s1.mercy");
     }
     if (c.n_edges) {
 #define M(WW)                                                                                                 \
   if (W == WW)                                                                                                \
-    k_r2s_s2_extract<WW, kS2Count><<<grid_for(c.n_edges, 256), 256, 0, st>>>(c.pv, k, so.is_solid, m == 1, \
+    k_r2s_s2_extract<WW, kS2Count><<<grid_cap(c.n_edges, 256, 16), 256, 0, st>>>(c.pv, k, so.is_solid, m == 1, \
                                                                             c.n_edges, nullptr, d_counter, 0);
       MHB_FOR_WR(M)
 #undef M
@@ -823,7 +752,7 @@ int run_stage2(const mhb_build_args *args, mhb_build_result *res, cudaStream_t s
     big.b.release();
     big.ws.release();
     DevBuf h16;
-    CKR(h16.alloc(MHB_NUM_BUCKETS * 8, "bucket histogram"));
+    CKR(h16.alloc(MHB_NUM_BUCKETS * 8, "read2sdbg: bucket histogram"));
     max_items = g_r2s_s2_limit;
     if (!max_items) {
       const size_t avail = (size_t)(0.92 * (double)free_device_bytes());
@@ -837,7 +766,7 @@ int run_stage2(const mhb_build_args *args, mhb_build_result *res, cudaStream_t s
       if (!c.n_edges) return MHB_OK;
 #define M(WW)                                                                                                          \
   if (W == WW)                                                                                                         \
-    k_r2s_s2_extract<WW, kS2Hist><<<grid_for(c.n_edges, 256), 256, 0, st>>>(c.pv, k, d_solid, all, c.n_edges, nullptr, \
+    k_r2s_s2_extract<WW, kS2Hist><<<grid_cap(c.n_edges, 256, 16), 256, 0, st>>>(c.pv, k, d_solid, all, c.n_edges, nullptr, \
                                                                            nullptr, 0, 0, 65535,                      \
                                                                            h16.as<unsigned long long>());
       MHB_FOR_WR(M)
@@ -852,9 +781,9 @@ int run_stage2(const mhb_build_args *args, mhb_build_result *res, cudaStream_t s
     tr.mark("s2.extract.plan");
     CKR(plan_bucket_ranges(h_h16, max_items, &ranges));
   }
-  CKR(big.a.ensure((size_t)max_items * W * 4 + 16, "stage-2 items"));
-  CKR(big.b.ensure((size_t)max_items * W * 4 + 16, "stage-2 items (sort buffer)"));
-  CKR(big.ws.ensure(mhb_s2s_sort_workspace_bytes(max_items, k), "sort workspace"));
+  CKR(big.a.ensure((size_t)max_items * W * 4 + 16, "read2sdbg: stage-2 items"));
+  CKR(big.b.ensure((size_t)max_items * W * 4 + 16, "read2sdbg: stage-2 items (sort buffer)"));
+  CKR(big.ws.ensure(mhb_s2s_sort_workspace_bytes(max_items, k), "read2sdbg: sort workspace"));
   S2Bufs sb;
   SdbgStitch out;
   uint64_t seen = 0;
@@ -866,14 +795,14 @@ int run_stage2(const mhb_build_args *args, mhb_build_result *res, cudaStream_t s
       if (one_pass) {
 #define M(WW)                                                                                                       \
   if (W == WW)                                                                                                      \
-    k_r2s_s2_extract<WW, kS2Write><<<grid_for(c.n_edges, 256), 256, 0, st>>>(c.pv, k, d_solid, all, c.n_edges, dst, \
+    k_r2s_s2_extract<WW, kS2Write><<<grid_cap(c.n_edges, 256, 16), 256, 0, st>>>(c.pv, k, d_solid, all, c.n_edges, dst, \
                                                                             d_counter, n_items);
         MHB_FOR_WR(M)
 #undef M
       } else {
 #define M(WW)                                                                                                       \
   if (W == WW)                                                                                                      \
-    k_r2s_s2_extract<WW, kS2Range><<<grid_for(c.n_edges, 256), 256, 0, st>>>(c.pv, k, d_solid, all, c.n_edges, dst, \
+    k_r2s_s2_extract<WW, kS2Range><<<grid_cap(c.n_edges, 256, 16), 256, 0, st>>>(c.pv, k, d_solid, all, c.n_edges, dst, \
                                                                             d_counter, max_items, rg.first,        \
                                                                             rg.second, nullptr);
         MHB_FOR_WR(M)
@@ -988,10 +917,10 @@ extern "C" int mhb_read2sdbg_host(const mhb_build_args *args, mhb_build_result *
   CKR(src.plan(args, ix, k, stream, read_chunk_limit() ? read_chunk_limit() : read_chunk_auto_bytes()));
   const char *held = stream ? "the bit planes and read chunk buffers leave" : "the resident read library leaves";
   if (stream) {  // resident: the solid plane, the mercy planes (the fourth one chunk-sized) and the chunk buffers
-    const size_t solid_b = m > 1 ? pad(bit_words * 4) : 0,
-                 mercy_b = mercy ? 3 * pad(bit_words * 4) + pad(src.max_plane_words * 4) : 0;
-    const size_t need = solid_b + mercy_b + src.streamed_bytes() + pad(65536 * 8) + pad(64) +
-                        pad((size_t)MHB_NUM_BUCKETS * 32) + pad(128);
+    const size_t solid_b = m > 1 ? pad256(bit_words * 4) : 0,
+                 mercy_b = mercy ? 3 * pad256(bit_words * 4) + pad256(src.max_plane_words * 4) : 0;
+    const size_t need = solid_b + mercy_b + src.streamed_bytes() + pad256(65536 * 8) + pad256(64) +
+                        pad256((size_t)MHB_NUM_BUCKETS * 32) + pad256(128);
     if (need > free_device_bytes())
       return mhb_set_error(MHB_ERR_NOMEM,
                            "read2sdbg: the streamed read library needs %zu bytes of device memory (solid plane %zu, "
@@ -1010,29 +939,29 @@ extern "C" int mhb_read2sdbg_host(const mhb_build_args *args, mhb_build_result *
   // ---- stage 1 (only when the threshold can reject anything, main_sdbg_build.cpp:141-147) ----
   DevBuf d_solid, d_planes, d_mplane, d_hist, d_cnt;
   if (m > 1) {  // m == 1: stage 2 takes every edge and never reads the solid plane
-    CKR(d_solid.alloc(bit_words * 4, "solid plane"));
+    CKR(d_solid.alloc(bit_words * 4, "read2sdbg: solid plane"));
     CK(cudaMemsetAsync(d_solid.p, 0, bit_words * 4, st));
   }
-  CKR(d_hist.alloc(65536 * 8, "multiplicity histogram"));
+  CKR(d_hist.alloc(65536 * 8, "read2sdbg: multiplicity histogram"));
   CK(cudaMemsetAsync(d_hist.p, 0, 65536 * 8, st));
-  CKR(d_cnt.alloc(64, "counters"));
+  CKR(d_cnt.alloc(64, "read2sdbg: counters"));
   CK(cudaMemsetAsync(d_cnt.p, 0, 64, st));
   unsigned long long *d_counter = d_cnt.as<unsigned long long>();
   DevBuf d_table, d_totals;
-  CKR(d_table.alloc((size_t)MHB_NUM_BUCKETS * 32, "bucket table"));
-  CKR(d_totals.alloc(16 * 8, "totals"));
+  CKR(d_table.alloc((size_t)MHB_NUM_BUCKETS * 32, "read2sdbg: bucket table"));
+  CKR(d_totals.alloc(16 * 8, "read2sdbg: totals"));
   BigBufs big;
   S1Out so;
   memset(&so, 0, sizeof(so));
   so.is_solid = d_solid.as<u32>();
   if (s1_runs) {
     if (mercy) {
-      CKR(d_planes.alloc(bit_words * 4 * 3, "mercy candidate planes"));
+      CKR(d_planes.alloc(bit_words * 4 * 3, "read2sdbg: mercy candidate planes"));
       CK(cudaMemsetAsync(d_planes.p, 0, bit_words * 4 * 3, st));
       so.no_in = d_planes.as<u32>();
       so.no_out = so.no_in + bit_words;
       so.any = so.no_out + bit_words;
-      CKR(d_mplane.alloc(src.max_plane_words * 4, "mercy plane of a chunk"));
+      CKR(d_mplane.alloc(src.max_plane_words * 4, "read2sdbg: mercy plane of a chunk"));
     }
     // one pass when the records fit (and no cap is set), else rounds over bucket ranges
     const size_t avail = (size_t)(0.92 * (double)free_device_bytes());
@@ -1043,8 +972,8 @@ extern "C" int mhb_read2sdbg_host(const mhb_build_args *args, mhb_build_result *
     if (max_n == 0) {
       // size the shared buffers for stage 2 as well when that fits: ~1.6 items per edge position on a 30x library, 2.2
       // to be safe (stage 2 reallocates when its count launch says more)
-      const size_t rec1 = pad((size_t)ix.n_s1 * l1.RW * 4 + 16), ws1 = pad(s1_ws_bytes(ix.n_s1, l1));
-      const size_t rec2 = pad((size_t)est_items * W * 4 + 16), ws2 = pad(mhb_s2s_sort_workspace_bytes(est_items, k));
+      const size_t rec1 = pad256((size_t)ix.n_s1 * l1.RW * 4 + 16), ws1 = pad256(s1_ws_bytes(ix.n_s1, l1));
+      const size_t rec2 = pad256((size_t)est_items * W * 4 + 16), ws2 = pad256(mhb_s2s_sort_workspace_bytes(est_items, k));
       if (s1_one - 2 * rec1 - ws1 + 2 * std::max(rec1, rec2) + std::max(ws1, ws2) <= avail) {
         min_rec = (size_t)est_items * W * 4 + 16;
         min_ws = mhb_s2s_sort_workspace_bytes(est_items, k);
@@ -1323,11 +1252,8 @@ extern "C" int mhb_selftest_r2s_chunk_index(const uint32_t *bin, uint64_t bin_wo
     *base0_out = ix.base_off[first];
     return MHB_OK;
   }
-  ReadLibIndex li;
-  CKR(index_read_lib(bin, bin_words, n_reads, 0, &li));
-  const uint64_t stride = li.fixed_len ? 1 + div_ceil(li.fixed_len, 16) : 0;
-  auto rec = [&](uint64_t r) { return li.fixed_len ? r * stride : li.rec_off[r]; };
-  const uint32_t *chunk = bin + rec(first);
+  const ReadLibIndex &li = ix.li;
+  const uint32_t *chunk = bin + li.word_of(first);
   uint64_t w = 0, b = 0, s = 0, e = 0;
   for (uint64_t r = 0; r <= count; ++r) {
     word_off_out[r] = w;
@@ -1336,7 +1262,7 @@ extern "C" int mhb_selftest_r2s_chunk_index(const uint32_t *bin, uint64_t bin_wo
     edge_off_out[r] = e;
     if (r == count) break;
     u32 l, lw, ls, le;
-    r2s_read_geom(chunk[rec(first + r) - rec(first)], k, l, lw, ls, le);
+    r2s_read_geom(chunk[li.word_of(first + r) - li.word_of(first)], k, l, lw, ls, le);
     len_out[r] = l;
     w += lw;
     b += l;

@@ -394,7 +394,6 @@ bool s2s_local_path(uint32_t k) {
   const u32 w = s2s_record_words(k);
   return k >= 9 && (w == 2 || w == 3);
 }
-size_t pad256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 // ids / n_ids / mid / eo: as k_s2s_local_sort
 template <int W, u32 CAP, int THREADS, bool EMIT>

@@ -258,7 +258,7 @@ extern "C" int mhb_partition_scatter_hist(void *stream, const uint32_t *recs, ui
 }
 
 extern "C" int mhb_dev_malloc(void **ptr, size_t bytes) {
-  CK(cudaMalloc(ptr, bytes));
+  CK(cudaMalloc(ptr, bytes));  // the caller owns it (mhb_dev_free)
   return MHB_OK;
 }
 extern "C" int mhb_dev_free(void *ptr) {

@@ -16,19 +16,38 @@
 
 using namespace mhb;
 
-#define CKR(call)        \
-  do {                   \
-    int rc_ = (call);    \
-    if (rc_) return rc_; \
-  } while (0)
-
 namespace {
 uint64_t g_chunk_limit = 0;
 StreamStats g_st;
-
-inline size_t pad256(size_t b) { return (b + 255) & ~(size_t)255; }
-
 }  // namespace
+
+size_t free_device_bytes() {
+  size_t free_b = 0, total_b = 0;
+  if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) {
+    cudaGetLastError();
+    return 0;
+  }
+  return free_b;
+}
+
+void DevBuf::release() {
+  if (p) cudaFree(p);
+  p = nullptr;
+  bytes = 0;
+}
+
+int DevBuf::alloc(size_t b, const char *what) {
+  release();
+  b = pad256(std::max<size_t>(b, 1));
+  const cudaError_t e = cudaMalloc(&p, b);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    p = nullptr;
+    return mhb_set_error(MHB_ERR_NOMEM, "%s: cudaMalloc of %zu bytes failed: %s", what, b, cudaGetErrorString(e));
+  }
+  bytes = b;
+  return MHB_OK;
+}
 
 void plan_chunks(const uint64_t *word_off, uint64_t stride_words, uint64_t extra_bytes, uint64_t n, uint64_t max_bytes,
                  std::vector<uint64_t> *first) {
@@ -55,18 +74,21 @@ static void plan_read_chunks(const ReadLibIndex &ix, uint64_t n_reads, uint64_t 
   plan_chunks(ix.fixed_len ? nullptr : ix.rec_off.data(), 1 + div_ceil(ix.fixed_len, 16), 0, n_reads, max_bytes, first);
 }
 
-int index_read_lib(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, uint32_t k, ReadLibIndex *ix, bool sampled) {
+int index_read_lib(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, uint32_t k, ReadLibIndex *ix,
+                   FixedCheck check) {
   *ix = ReadLibIndex();
   if (n_reads == 0) return MHB_OK;
   if (bin_words == 0) return mhb_set_error(MHB_ERR_ARG, "empty .bin image for %llu reads", (unsigned long long)n_reads);
   const uint32_t L0 = bin[0];
   const uint64_t stride = 1 + div_ceil(L0, 16);
   bool fixed = L0 > 0 && bin_words == n_reads * stride;
-  if (fixed && sampled) {
+  if (fixed && check == FixedCheck::kSampled) {
     const uint64_t step = std::max<uint64_t>(1, n_reads / 1024);
     for (uint64_t r = 0; r < n_reads && fixed; r += step) fixed = bin[r * stride] == L0;
     for (uint64_t r = 0; r < std::min<uint64_t>(n_reads, 1024) && fixed; ++r) fixed = bin[r * stride] == L0;
     fixed = fixed && bin[(n_reads - 1) * stride] == L0;
+  } else if (fixed && check == FixedCheck::kSerial) {
+    for (uint64_t r = 0; r < n_reads && fixed; ++r) fixed = bin[r * stride] == L0;
   } else if (fixed) {
     int bad = 0;
 #pragma omp parallel for reduction(| : bad) schedule(static)
@@ -227,9 +249,7 @@ int ReadStream::init(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, 
   resident_ = max_chunk_bytes == 0;
   bin_ = bin;
   bin_words_ = bin_words;
-  fixed_len_ = ix.fixed_len;
-  stride_ = fixed_len_ ? 1 + div_ceil(fixed_len_, 16) : 0;
-  rec_off_ = ix.rec_off.data();
+  ix_ = &ix;
   aux_off_ = ix.unit_off.empty() ? nullptr : ix.unit_off.data();  // an index without unit offsets streams none
   uint64_t max_words = bin_words;
   if (resident_) {
@@ -240,12 +260,12 @@ int ReadStream::init(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, 
     max_words = max_reads_ = 0;
     for (uint64_t i = 0; i < n_chunks(); ++i) {
       max_reads_ = std::max(max_reads_, first_[i + 1] - first_[i]);
-      max_words = std::max(max_words, word_of(first_[i + 1]) - word_of(first_[i]));
+      max_words = std::max(max_words, ix_->word_of(first_[i + 1]) - ix_->word_of(first_[i]));
     }
   }
   // the image 16-byte aligned + 16 bytes: the extraction's bulk copies end on a 16-byte boundary
   off_at_ = pad256(((max_words * 4 + 15) & ~(size_t)15) + 16);
-  slot_bytes_ = off_at_ + (fixed_len_ ? 0 : (aux_off_ ? 2 : 1) * pad256((max_reads_ + 1) * 8));
+  slot_bytes_ = off_at_ + (ix_->fixed_len ? 0 : (aux_off_ ? 2 : 1) * pad256((max_reads_ + 1) * 8));
   g_st.chunks = n_chunks();
   return stager_.init(slot_bytes_, n_chunks(), &g_st);
 }
@@ -257,8 +277,8 @@ int ReadStream::bind(void *device, void *stream) {
   cudaStream_t st = (cudaStream_t)stream;
   const uint64_t n_reads = first_[1];
   if (bin_words_) CK(cudaMemcpyAsync(dev_, bin_, bin_words_ * 4, cudaMemcpyHostToDevice, st));
-  if (!fixed_len_ && n_reads) {
-    CK(cudaMemcpyAsync(dev_ + off_at_, rec_off_, (n_reads + 1) * 8, cudaMemcpyHostToDevice, st));
+  if (!ix_->fixed_len && n_reads) {
+    CK(cudaMemcpyAsync(dev_ + off_at_, ix_->rec_off.data(), (n_reads + 1) * 8, cudaMemcpyHostToDevice, st));
     if (aux_off_)
       CK(cudaMemcpyAsync(dev_ + off_at_ + pad256((n_reads + 1) * 8), aux_off_, (n_reads + 1) * 8, cudaMemcpyHostToDevice, st));
   }
@@ -271,15 +291,15 @@ ReadChunkView ReadStream::view(uint64_t i, const char *slot) const {
   v.first_read = first_[i];
   v.n_reads = first_[i + 1] - first_[i];
   v.bin = (const uint32_t *)slot;
-  v.bin_words = resident_ ? bin_words_ : word_of(first_[i + 1]) - word_of(first_[i]);
-  v.rec_off = fixed_len_ ? nullptr : (const uint64_t *)(slot + off_at_);
-  v.aux_off = fixed_len_ || !aux_off_ ? nullptr : (const uint64_t *)(slot + off_at_ + pad256((max_reads_ + 1) * 8));
+  v.bin_words = resident_ ? bin_words_ : ix_->word_of(first_[i + 1]) - ix_->word_of(first_[i]);
+  v.rec_off = ix_->fixed_len ? nullptr : (const uint64_t *)(slot + off_at_);
+  v.aux_off = ix_->fixed_len || !aux_off_ ? nullptr : (const uint64_t *)(slot + off_at_ + pad256((max_reads_ + 1) * 8));
   return v;
 }
 
 // chunk i into a staging buffer: its image, and for a variable-length library its offsets rebased to the chunk
 int ReadStream::fill(uint64_t i, char *h, ChunkStager::Copies *up) const {
-  const uint64_t b = first_[i], e = first_[i + 1], w0 = word_of(b), nw = word_of(e) - w0;
+  const uint64_t b = first_[i], e = first_[i + 1], w0 = ix_->word_of(b), nw = ix_->word_of(e) - w0;
   {
     const uint64_t bytes = nw * 4, blk = 4ull << 20, nblk = (bytes + blk - 1) / blk;
 #pragma omp parallel for schedule(static)
@@ -289,13 +309,13 @@ int ReadStream::fill(uint64_t i, char *h, ChunkStager::Copies *up) const {
     }
   }
   up->add(0, nw * 4);
-  if (fixed_len_) return MHB_OK;
+  if (ix_->fixed_len) return MHB_OK;
   const uint64_t nr = e - b, ao_at = off_at_ + pad256((max_reads_ + 1) * 8);
   uint64_t *ro = (uint64_t *)(h + off_at_), *ao = (uint64_t *)(h + ao_at);
-  const uint64_t r0 = rec_off_[b], a0 = aux_off_ ? aux_off_[b] : 0;
+  const uint64_t r0 = ix_->rec_off[b], a0 = aux_off_ ? aux_off_[b] : 0;
 #pragma omp parallel for schedule(static)
   for (long long r = 0; r <= (long long)nr; ++r) {
-    ro[r] = rec_off_[b + r] - r0;
+    ro[r] = ix_->rec_off[b + r] - r0;
     if (aux_off_) ao[r] = aux_off_[b + r] - a0;
   }
   up->add(off_at_, (nr + 1) * 8);
