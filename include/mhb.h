@@ -742,6 +742,23 @@ int mhb_plan_seq_shares(const uint32_t *len, uint64_t n_seqs, uint32_t k, uint32
  * owners' ascending runs follow each other in rank order in the one P.edges.0; rank 0 writes P.edges.info.  A rank
  * whose received edges do not fit returns MHB_ERR_NOMEM.  The caller must not have initialised CUDA in this process. */
 int mhb_iterate_run_multi(const mhb_iterate_opts *opts, int n_gpus);
+/* `read2sdbg` on n_gpus GPUs of this node: the same options, checks and output files as mhb_read2sdbg_run, except that
+ * rank r writes P.sdbg.<r> and P.sdbg_info has num_files = n_gpus; the canonical SdBG stream is the single-GPU one.
+ * n_gpus <= 1, or a library with fewer reads than GPUs, runs mhb_read2sdbg_run.  Otherwise the `.bin` image is loaded
+ * on the host and the reads dealt in contiguous shares balanced on their bases (mhb_plan_read_shares) to one forked
+ * worker per GPU (devices shared as in mhb_count_run_multi).  Each worker extracts its share's stage-1 records straight
+ * into the receive buffers of the ranks owning their leading byte, in global read order, so every owner's stable
+ * bucket partition and kmsort emulation see the reference's bucket input order; the owners mark their solid edges and
+ * mercy candidates into bit planes of the whole library, which every rank merges over its share's words before the
+ * mercy step.  The stage-2 items meet on their owners in the same way; each owner sorts, collapses and emits its bucket
+ * range.  Rank 0 writes P.sdbg_info and P.counting (m > 1).  Resident only: every rank holds the planes of the whole
+ * library (1 bit per base, 4 with need_mercy) next to its share and receive buffers; what does not fit is
+ * MHB_ERR_NOMEM.  The caller must not have initialised CUDA in this process. */
+int mhb_read2sdbg_run_multi(const mhb_read2sdbg_opts *opts, int n_gpus);
+/* The owner ranges of a multi-GPU read2sdbg stage (host only): the 65536-bin bucket histogram hist16 folded into its
+ * 256 leading bytes, cut into n_ranks contiguous byte ranges as the count exchange cuts them; rank o owns the buckets
+ * [bucket_lo[o], bucket_hi[o]]. */
+int mhb_plan_r2s_owners(const uint64_t *hist16, uint32_t n_ranks, uint32_t *bucket_lo, uint32_t *bucket_hi);
 /* The shares of mhb_iterate_run_multi (host only): n_ranks contiguous runs [first[r], first[r+1]) of the n_reads reads of
  * the `.bin` image bin (bin_words words, fixed or variable read length), every cut at the read boundary whose base count
  * before it is closest to r / n_ranks of the total.  first_out gets n_ranks + 1 entries. */

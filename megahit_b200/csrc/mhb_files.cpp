@@ -487,14 +487,13 @@ extern "C" int mhb_seq2sdbg_run(const mhb_seq2sdbg_opts *o) {
 // ================================================================================================
 // read2sdbg (main_read2sdbg, main_sdbg_build.cpp:88-156)
 // ================================================================================================
-extern "C" int mhb_read2sdbg_run(const mhb_read2sdbg_opts *o) {
+int read2sdbg_load(const mhb_read2sdbg_opts *o, std::vector<uint32_t> *bin, long long *n_reads_out) {
   if (!o || !o->read_lib_file || !o->read_lib_file[0]) return mhb_set_error(MHB_ERR_ARG, "No input file!");
   if (o->host_mem == 0) return mhb_set_error(MHB_ERR_ARG, "Please specify the host memory!");
   const std::string lib = o->read_lib_file, prefix = o->output_prefix ? o->output_prefix : "out";
-  const double t0 = now_s();
   long long total_bases = 0, n_reads = 0;
-  std::vector<uint32_t> bin;
-  if (int rc = load_read_lib(lib, &bin, &n_reads, &total_bases)) return rc;
+  if (int rc = load_read_lib(lib, bin, &n_reads, &total_bases)) return rc;
+  *n_reads_out = n_reads;
   XINFO("%lld reads, %lld total bases; k = %u, m = %d, need_mercy = %d\n", n_reads, total_bases, o->k, o->m, o->need_mercy);
   // the candidate files stage 1 hands to stage 2 inside the reference process (read_to_sdbg_s1.cpp:111-126: 1, 2, 4 .. 64
   // files by read count); here the candidates never leave the device (three bit planes), the files are created empty so
@@ -506,6 +505,11 @@ extern "C" int mhb_read2sdbg_run(const mhb_read2sdbg_opts *o) {
     if (!f) return mhb_set_error(MHB_ERR_IO, "cannot open %s.mercy_cand.%d", prefix.c_str(), i);
     fclose(f);
   }
+  return MHB_OK;
+}
+
+int read2sdbg_build(const mhb_read2sdbg_opts *o, std::vector<uint32_t> &bin, long long n_reads, double t0) {
+  const std::string prefix = o->output_prefix ? o->output_prefix : "out";
   mhb_build_args a;
   memset(&a, 0, sizeof(a));
   a.k = o->k;
@@ -542,6 +546,14 @@ extern "C" int mhb_read2sdbg_run(const mhb_read2sdbg_opts *o) {
   mhb_free(res.bucket_table);
   mhb_free(res.counting);
   return rc;
+}
+
+extern "C" int mhb_read2sdbg_run(const mhb_read2sdbg_opts *o) {
+  const double t0 = now_s();
+  std::vector<uint32_t> bin;
+  long long n_reads = 0;
+  if (int rc = read2sdbg_load(o, &bin, &n_reads)) return rc;
+  return read2sdbg_build(o, bin, n_reads, t0);
 }
 
 // ================================================================================================

@@ -270,6 +270,63 @@ int iter_sort_unique(uint32_t *a, uint32_t *b, uint64_t n, uint32_t k, uint32_t 
 // hist[v] += records among the n of `words` words whose byte `byte` (the sort's numbering) is v (mhb_sortdisp.cu)
 int hist_byte(void *stream, const uint32_t *recs, uint64_t n, uint32_t words, int byte, uint64_t *hist);
 
+// The two halves of mhb_read2sdbg_run, which mhb_read2sdbg_run_multi shares (mhb_files.cpp): the option checks, the
+// library and the (empty) P.mercy_cand.<i> files; then the single-GPU build and its files and summary lines.
+int read2sdbg_load(const mhb_read2sdbg_opts *o, std::vector<uint32_t> *bin, long long *n_reads);
+int read2sdbg_build(const mhb_read2sdbg_opts *o, std::vector<uint32_t> &bin, long long n_reads, double t0);
+
+// ---- read2sdbg's device pieces (mhb_r2s.cu), driven step by step by the multi-GPU worker ----
+// One rank's share [first, end) of the reads of a build, resident on the current device as one package chunk: read
+// indices are local, bases - stage-1 payload positions and bit-plane indices - global, and the bit planes (solid; with
+// need_mercy the three candidate planes after it, in one allocation) cover the whole library's word grid.  Owners are
+// ranks of contiguous leading-byte ranges (owner_of_byte); device addresses are passed as uint64_t.
+class R2sShare {
+ public:
+  R2sShare();
+  ~R2sShare();
+  R2sShare(const R2sShare &) = delete;
+  R2sShare &operator=(const R2sShare &) = delete;
+  // a: the whole library and the build's k, m, need_mercy; li: its index_read_lib (made before the fork)
+  int load(const mhb_build_args *a, const ReadLibIndex &li, uint64_t first, uint64_t end);
+  uint32_t s1_record_words() const;  // words of a stage-1 record row
+  bool s1_narrow() const;            // read_info in a side array of 8 bytes per row
+  uint64_t s1_round_cap() const;     // most stage-1 records one owner may sort
+  // hist[65536] = the 16-bit bucket ids of the share's stage-1 records / stage-2 items (s2 after mercy_count)
+  int s1_hist(uint64_t *hist);
+  int s2_hist(uint64_t *hist);
+  // the share's stage-1 records into their owners' buffers in global read order (rec_base / info_base: device address
+  // of row 0 of owner o's record / read_info buffer, info_base nullptr unless s1_narrow; my_off[o]: the rows of the
+  // lower ranks).  Counts first: an error, and nothing stored, unless owner o gets expect[o] records.
+  int s1_send(const uint8_t *owner_of_byte, int n_owners, const uint64_t *rec_base, const uint64_t *info_base,
+              const uint64_t *my_off, const uint64_t *expect);
+  // owner: stable bucket partition, kmsort and Lv2Postprocess of the n records received (overwritten), into the local
+  // planes and multiplicity histogram
+  int s1_own(uint32_t *recs, uint64_t *info, uint64_t n);
+  void *planes() const;  // the allocation of the planes, for CUDA IPC (nullptr when m == 1)
+  // OR another rank's planes (same layout) into mine over my share's words
+  int or_planes(const void *peer_planes);
+  // the mercy step and the stage-2 item count over the share
+  int mercy_count(uint64_t *n_items, uint64_t *n_mercy);
+  // every stage-2 item of the share to its owner: owner_base[o] = device address of this rank's segment of owner o's
+  // buffer, capacity[o] items (host arrays); sent[o] = items sent
+  int s2_send(const uint8_t *owner_of_byte, int n_owners, const uint64_t *owner_base, const uint64_t *capacity,
+              uint64_t *sent);
+  // owner: relaxed sort, collapse and emitter (label_fmt 1) of the n items received (overwritten); SdBG bytes, bucket
+  // table (65536 x {offset, items, tips, large_mul}) and the emitter's 16 totals
+  int s2_own(uint32_t *items, uint64_t n, std::vector<uint8_t> *bytes, std::vector<uint64_t> *table, uint64_t *totals);
+  int counting(uint64_t *hist);  // the multiplicity histogram (65536) of the records this rank owned
+  uint64_t n_reads() const;
+
+ private:
+  struct Impl;
+  Impl *d_;
+};
+// the 256 leading-byte bins of a 65536-bin bucket histogram
+inline void fold_bucket_hist(const uint64_t *h16, uint64_t *h256) {
+  for (int b = 0; b < 256; ++b) h256[b] = 0;
+  for (int b = 0; b < 65536; ++b) h256[b >> 8] += h16[b];
+}
+
 // mhb_mercy_probe_owned, with accumulate = true OR-ing the answers into planes_out instead of storing them (mhb_multi.cu)
 int mercy_probe_owned(void *stream, const mhb_dev_reads *reads, const uint64_t *cand_ids, uint64_t n_cand,
                       uint32_t max_read_len, uint32_t k, const uint32_t *edges, uint64_t n_edges, const void *lut,

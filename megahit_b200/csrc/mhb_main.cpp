@@ -248,7 +248,7 @@ int main_read2sdbg(int argc, char **argv, char **full_argv) {
   RssRecorder rec;
   const std::vector<Opt> opts = {{"kmer_k", "k", false},         {"min_kmer_frequency", "m", false}, {"host_mem", "", false},
                                  {"num_cpu_threads", "", false}, {"read_lib_file", "", false},       {"output_prefix", "", false},
-                                 {"mem_flag", "", false},        {"need_mercy", "", true}};
+                                 {"mem_flag", "", false},        {"need_mercy", "", true},           {"gpus", "", false}};
   const char *usage = "Usage: sdbg_builder read2sdbg --read_lib_file fastx_file -o out";
   std::map<std::string, std::string> v;
   std::string err;
@@ -266,7 +266,9 @@ int main_read2sdbg(int argc, char **argv, char **full_argv) {
   o.output_prefix = out.c_str();
   if (lib.empty()) return fail_usage("No input file!", usage);
   if (o.host_mem == 0) return fail_usage("Please specify the host memory!", usage);
-  if (int rc = mhb_read2sdbg_run(&o)) {
+  // --gpus N / MHB_GPUS=N (not an option of the reference, which the Python driver never passes): one worker per GPU
+  const int gpus = v.count("gpus") ? atoi(v["gpus"].c_str()) : (getenv("MHB_GPUS") ? atoi(getenv("MHB_GPUS")) : 1);
+  if (int rc = gpus > 1 ? mhb_read2sdbg_run_multi(&o, gpus) : mhb_read2sdbg_run(&o)) {
     fprintf(stderr, "FATAL megahit_b200: %s\n", mhb_last_error());
     (void)rc;
     exit(1);

@@ -23,6 +23,11 @@
 // `iterate` (mhb_iterate_run_multi) deals contiguous read shares, balanced on bases; each rank builds the whole flank
 // index, runs the single-GPU read pass over its share and sends its unique candidates to their owners, which sort and
 // dedup them; the owners' ascending runs, written in rank order, are the single-GPU P.edges.0.
+//
+// `read2sdbg` (mhb_read2sdbg_run_multi) deals contiguous read shares too; each rank sends its stage-1 records to their
+// owners in global read order (R2sShare::s1_send), the owners run stage 1 into planes of the whole library, every rank
+// ORs all planes over its share's words, runs the mercy step over its share and sends its stage-2 items to their
+// owners, which sort, collapse and emit as the single-GPU read2sdbg does.
 #include <cuda_runtime.h>
 #include <fcntl.h>
 #include <pthread.h>
@@ -69,7 +74,7 @@ struct Control {
   int world;
   char err[kMaxRanks][512];
   uint64_t hist[2][kMaxRanks][256];
-  uint8_t ipc[2][kMaxRanks][64];
+  uint8_t ipc[4][kMaxRanks][64];
   uint64_t n_solid[kMaxRanks], n_tip[kMaxRanks], n_cand[kMaxRanks], n_mercy[kMaxRanks], n_records[kMaxRanks];
   uint64_t sdbg_totals[kMaxRanks][16];
   uint64_t has_tips[kMaxRanks];
@@ -268,26 +273,35 @@ struct PeerBuf {
   size_t bytes = 0;
 };
 
-// The exchange of one stage, up to the stores: all-gather the leading-byte histograms (d_hist), plan the owner ranges,
-// allocate, export and open the receive buffers.  Returns the plan; *d_addr (256, in pool) = where this rank's records
-// for owner o begin, *d_lut = the owner of every leading byte.
-Plan open_receive(Exchange &X, int stage, const uint64_t *d_hist, uint32_t words, DevPool &pool, PeerBuf *pb,
-                  uint64_t **d_addr, uint8_t **d_lut) {
+// A receive buffer of `bytes` on every rank (the same size everywhere), exported through IPC slot `slot` and opened by
+// every other rank.
+void open_peers(Exchange &X, int slot, size_t bytes, PeerBuf *pb) {
   Control *C = X.C;
   const int W = X.world, r = X.rank;
-  CKC(cudaMemcpy(C->hist[stage][r], d_hist, 256 * 8, cudaMemcpyDeviceToHost));
+  pb->bytes = bytes;
+  pb->mine = dev_alloc(pb->bytes);
+  CKM(mhb_ipc_export(pb->mine, C->ipc[slot][r]));
+  X.barrier();
+  for (int o = 0; o < W; ++o) {
+    if (o == r) pb->peer[o] = pb->mine;
+    else CKM(mhb_ipc_open(C->ipc[slot][o], &pb->peer[o]));
+  }
+}
+
+// The exchange of one stage, up to the stores: all-gather the leading-byte histograms (d_hist on the device, or hist
+// on the host), plan the owner ranges, allocate, export and open the receive buffers.  Returns the plan; *d_addr (256,
+// in pool) = where this rank's records for owner o begin, *d_lut = the owner of every leading byte.
+Plan open_receive(Exchange &X, int stage, const uint64_t *d_hist, uint32_t words, DevPool &pool, PeerBuf *pb,
+                  uint64_t **d_addr, uint8_t **d_lut, const uint64_t *hist = nullptr) {
+  Control *C = X.C;
+  const int W = X.world, r = X.rank;
+  if (hist) memcpy(C->hist[stage][r], hist, 256 * 8);
+  else CKC(cudaMemcpy(C->hist[stage][r], d_hist, 256 * 8, cudaMemcpyDeviceToHost));
   X.barrier();
   const Plan P = plan_partition_host(C->hist[stage], W, r);
   uint64_t mx = 0;
   for (int o = 0; o < W; ++o) mx = std::max(mx, P.recv_tot[o]);
-  pb->bytes = (size_t)mx * words * 4 + 256;  // the same size on every rank
-  pb->mine = dev_alloc(pb->bytes);
-  CKM(mhb_ipc_export(pb->mine, C->ipc[stage][r]));
-  X.barrier();
-  for (int o = 0; o < W; ++o) {
-    if (o == r) pb->peer[o] = pb->mine;
-    else CKM(mhb_ipc_open(C->ipc[stage][o], &pb->peer[o]));
-  }
+  open_peers(X, stage, (size_t)mx * words * 4 + 256, pb);
   uint64_t addr[256] = {0};
   for (int o = 0; o < W; ++o) addr[o] = (uint64_t)(uintptr_t)pb->peer[o] + P.my_off[o] * (uint64_t)words * 4;
   *d_addr = pool.get<uint64_t>(256);
@@ -337,7 +351,15 @@ void write_file(const std::string &path, const void *data, size_t bytes) {
   fclose(f);
 }
 
-// ---- the owner side of the SdBG stage, the same in both workers ----
+// My P.sdbg.<r> and, for rank 0, my totals (C->sdbg_totals) and bucket table ("stab")
+void sdbg_publish(Exchange &X, const uint64_t *totals, const std::vector<uint8_t> &sdbg_bytes,
+                  const std::vector<uint64_t> &table, const std::string &prefix) {
+  memcpy(X.C->sdbg_totals[X.rank], totals, 16 * 8);
+  write_file(prefix + ".sdbg." + std::to_string(X.rank), sdbg_bytes.data(), sdbg_bytes.size());
+  X.publish("stab", table.data(), 65536 * 32);
+}
+
+// ---- the owner side of the SdBG stage, the same in the count and seq2sdbg workers ----
 // Sort and emit the n_own SdBG items of my receive buffer (my bucket range), close the exchange, write P.sdbg.<r> and
 // publish my totals (C->sdbg_totals) and bucket table ("stab") for rank 0.
 void sdbg_owner_stage(Exchange &X, PeerBuf *ps, uint64_t n_own, uint32_t k, const std::string &prefix, DevPool &pool) {
@@ -371,9 +393,7 @@ void sdbg_owner_stage(Exchange &X, PeerBuf *ps, uint64_t n_own, uint32_t k, cons
     for (void *p : {(void *)d_tmp, d_e, (void *)d_out, (void *)d_table, (void *)d_tot}) pool.drop(p);
   }
   close_peers(X, ps);
-  memcpy(X.C->sdbg_totals[r], totals, sizeof(totals));
-  write_file(prefix + ".sdbg." + std::to_string(r), sdbg_bytes.data(), sdbg_bytes.size());
-  X.publish("stab", table.data(), 65536 * 32);
+  sdbg_publish(X, totals, sdbg_bytes, table, prefix);
 }
 
 // Rank 0, once every rank's sdbg_owner_stage is behind a barrier: the merged P.sdbg_info (sdbg_meta.cpp:44-61: records
@@ -932,6 +952,135 @@ void iter_worker(const IterJob &J, Exchange &X) {
   }
 }
 
+// ================================================================================================
+// read2sdbg on several GPUs: the reads are dealt in contiguous shares; the stage-1 records meet on their owners in
+// global read order, the bit planes are merged per share, the stage-2 items meet on their owners
+// ================================================================================================
+struct R2sJob {
+  mhb_build_args a;             // the whole `.bin` image (host, inherited by the workers), k, m, need_mercy
+  const ReadLibIndex *li;       // its index, made before the fork
+  std::vector<uint64_t> first;  // read shares
+  std::string prefix;
+};
+
+// the owner plan of a stage from my 65536-bin bucket histogram (stages 0 and 1 use Control::hist[0] / [1])
+Plan r2s_plan(Exchange &X, int stage, const uint64_t *h16, uint32_t words, DevPool &pool, PeerBuf *pb, uint64_t **d_addr,
+              uint8_t **d_lut) {
+  uint64_t h256[256];
+  fold_bucket_hist(h16, h256);
+  return open_receive(X, stage, nullptr, words, pool, pb, d_addr, d_lut, h256);
+}
+
+void r2s_worker(const R2sJob &J, Exchange &X) {
+  Control *C = X.C;
+  const int W = X.world, r = X.rank;
+  const uint32_t k = J.a.k, W2 = mhb_s2s_record_words(k);
+  const int32_t m = J.a.m;
+  bind_device(r, W);
+  DevPool pool;
+  R2sShare sh;
+  CKI(sh.load(&J.a, *J.li, J.first[r], J.first[r + 1]));
+  std::vector<uint64_t> h16(65536);
+  uint64_t n_s1_own = 0;
+
+  // ---- stage 1: my records straight into their owners' buffers, in global read order; each owner's planes ----
+  if (m > 1) {
+    CKI(sh.s1_hist(h16.data()));
+    const uint32_t RW = sh.s1_record_words();
+    PeerBuf pr, pi;
+    uint64_t *d_addr = nullptr;
+    uint8_t *d_lut = nullptr;
+    const Plan P = r2s_plan(X, 0, h16.data(), RW, pool, &pr, &d_addr, &d_lut);
+    n_s1_own = P.recv_tot[r];
+    if (n_s1_own > sh.s1_round_cap())
+      fail_nomem("%llu stage-1 records in my bucket range, more than the %llu one pass sorts (%llu bytes)",
+                 (unsigned long long)n_s1_own, (unsigned long long)sh.s1_round_cap(),
+                 (unsigned long long)(n_s1_own * RW * 4));
+    uint64_t mx = 0;
+    for (int o = 0; o < W; ++o) mx = std::max(mx, P.recv_tot[o]);
+    if (sh.s1_narrow()) open_peers(X, 2, (size_t)mx * 8 + 256, &pi);
+    uint64_t rec_base[kMaxRanks], info_base[kMaxRanks];
+    for (int o = 0; o < W; ++o) {
+      rec_base[o] = (uint64_t)(uintptr_t)pr.peer[o];
+      info_base[o] = (uint64_t)(uintptr_t)pi.peer[o];
+    }
+    CKI(sh.s1_send(P.owner, W, rec_base, sh.s1_narrow() ? info_base : nullptr, P.my_off, P.send));
+    X.barrier();  // every rank's stores have completed: my receive buffer is complete
+    CKI(sh.s1_own((uint32_t *)pr.mine, (uint64_t *)pi.mine, n_s1_own));
+    close_peers(X, &pr);
+    if (sh.s1_narrow()) close_peers(X, &pi);
+
+    // ---- plane merge: the words of my share's reads, OR-ed over every rank's planes (read through CUDA IPC) ----
+    CKM(mhb_ipc_export(sh.planes(), C->ipc[3][r]));
+    X.barrier();
+    for (int o = 0; o < W; ++o) {
+      if (o == r) continue;
+      void *peer = nullptr;
+      CKM(mhb_ipc_open(C->ipc[3][o], &peer));
+      CKI(sh.or_planes(peer));
+      CKM(mhb_ipc_close(peer));
+    }
+    X.barrier();  // nobody reads my planes any more: the mercy step may add to them
+  }
+
+  // ---- the mercy step and the stage-2 item count over my share ----
+  uint64_t n_items = 0, n_mercy = 0;
+  CKI(sh.mercy_count(&n_items, &n_mercy));
+  C->n_mercy[r] = n_mercy;
+
+  // ---- stage 2: every item straight into its owner's buffer; the owner sorts, collapses and emits ----
+  CKI(sh.s2_hist(h16.data()));
+  PeerBuf ps;
+  uint64_t *d_addr = nullptr;
+  uint8_t *d_lut = nullptr;
+  const Plan P2 = r2s_plan(X, 1, h16.data(), W2, pool, &ps, &d_addr, &d_lut);
+  uint64_t base[kMaxRanks], sent[kMaxRanks];
+  for (int o = 0; o < W; ++o) base[o] = (uint64_t)(uintptr_t)ps.peer[o] + P2.my_off[o] * (uint64_t)W2 * 4;
+  CKI(sh.s2_send(P2.owner, W, base, P2.send, sent));
+  for (int o = 0; o < W; ++o)
+    if (sent[o] != P2.send[o])
+      fail("internal: %llu stage-2 items for rank %d, the histogram said %llu", (unsigned long long)sent[o], o,
+           (unsigned long long)P2.send[o]);
+  X.barrier();  // every rank's stores have completed: my receive buffer is complete
+  const uint64_t n_own = P2.recv_tot[r];
+  std::vector<uint8_t> bytes;
+  std::vector<uint64_t> table;
+  uint64_t totals[16];
+  CKI(sh.s2_own((uint32_t *)ps.mine, n_own, &bytes, &table, totals));
+  close_peers(X, &ps);
+  sdbg_publish(X, totals, bytes, table, J.prefix);
+  if (m > 1) {
+    CKI(sh.counting(h16.data()));
+    X.publish("mul", h16.data(), 65536 * 8);
+  }
+  XINFO("rank %d: %llu reads, %llu stage-1 records owned, %llu mercy edges, %llu items sent, %llu owned; peak device "
+        "memory %.1f MiB\n", r, (unsigned long long)sh.n_reads(), (unsigned long long)n_s1_own, (unsigned long long)n_mercy,
+        (unsigned long long)n_items, (unsigned long long)n_own, g_dev.peak / 1048576.0);
+  X.barrier();
+  if (r == 0) {
+    if (m > 1) {  // Read2SdbgS1::Lv0Postprocess, read_to_sdbg_s1.cpp:557-566: the histogram over every owner's groups
+      std::vector<uint64_t> mul(65536, 0);
+      for (int o = 0; o < W; ++o) {
+        const std::vector<char> v = X.fetch("mul", o);
+        const uint64_t *h = (const uint64_t *)v.data();
+        for (int i = 0; i < 65536; ++i) mul[i] += h[i];
+      }
+      FILE *f = fopen((J.prefix + ".counting").c_str(), "w");
+      if (!f) throw Fail{"cannot open " + J.prefix + ".counting", MHB_ERR_IO};
+      for (int i = 1; i <= MHB_MAX_MUL; ++i) fprintf(f, "%d %lld\n", i, (long long)mul[i]);
+      fclose(f);
+      if (J.a.need_mercy) {
+        uint64_t n_mercy_tot = 0;
+        for (int o = 0; o < W; ++o) n_mercy_tot += C->n_mercy[o];
+        XINFO("Number mercy: %llu\n", (unsigned long long)n_mercy_tot);
+      }
+    }
+    sdbg_merge_info(X, k, J.prefix);
+  }
+  X.barrier();
+  for (const char *t : {"stab", "mul"}) X.cleanup(t);
+}
+
 // Forks one worker per rank around a fresh control block and waits for all of them.  A worker that dies would leave
 // the others at a barrier: the first abnormal exit takes the rest down.  A failure is reported with the error code of
 // the first failed rank that set one (MHB_ERR_CUDA otherwise) and every rank's message; the exchange files of `tags`
@@ -1107,5 +1256,51 @@ extern "C" int mhb_plan_read_shares(const uint32_t *bin, uint64_t bin_words, uin
 extern "C" int mhb_plan_seq_shares(const uint32_t *len, uint64_t n_seqs, uint32_t k, uint32_t n_ranks, uint64_t *first_out) {
   if ((!len && n_seqs) || !first_out || n_ranks < 1) return mhb_set_error(MHB_ERR_ARG, "bad args");
   plan_seq_shares(len, n_seqs, k, n_ranks, first_out);
+  return MHB_OK;
+}
+
+extern "C" int mhb_read2sdbg_run_multi(const mhb_read2sdbg_opts *o, int n_gpus) {
+  if (n_gpus <= 1) return mhb_read2sdbg_run(o);
+  if (n_gpus > kMaxRanks) return mhb_set_error(MHB_ERR_ARG, "at most %d GPUs of one node are supported", kMaxRanks);
+  const double t0 = now_s();
+  std::vector<uint32_t> bin;
+  long long n_reads = 0;
+  if (int rc = read2sdbg_load(o, &bin, &n_reads)) return rc;  // no CUDA in this process
+  if (n_reads < n_gpus) {
+    XINFO("%lld reads for %d GPUs: running on one GPU\n", n_reads, n_gpus);
+    return read2sdbg_build(o, bin, n_reads, t0);
+  }
+  ReadLibIndex ix;  // indexed serially: the workers are forked next
+  if (index_read_lib(bin.data(), bin.size(), (uint64_t)n_reads, 0, &ix, FixedCheck::kSerial))
+    return mhb_set_error(MHB_ERR_IO, "%s.bin ends inside a read", o->read_lib_file);
+  R2sJob J;
+  memset(&J.a, 0, sizeof(J.a));
+  J.a.k = o->k;
+  J.a.m = o->m;
+  J.a.bin = bin.data();
+  J.a.bin_words = bin.size();
+  J.a.n_reads = (uint64_t)n_reads;
+  J.a.need_mercy = o->need_mercy;
+  J.li = &ix;
+  J.first.resize(n_gpus + 1);
+  plan_read_shares(bin.data(), ix, (uint64_t)n_reads, (uint32_t)n_gpus, J.first.data());
+  J.prefix = o->output_prefix ? o->output_prefix : "out";
+  XINFO("read2sdbg: %lld reads; k = %u, m = %d; %d GPUs\n", n_reads, o->k, o->m, n_gpus);
+  const int rc = run_workers(n_gpus, "read2sdbg", {"stab", "mul"}, [&](Exchange &X) { r2s_worker(J, X); });
+  if (!rc) XINFO("read2sdbg on %d GPUs done. Time elapsed: %.4f\n", n_gpus, now_s() - t0);
+  return rc;
+}
+
+extern "C" int mhb_plan_r2s_owners(const uint64_t *hist16, uint32_t n_ranks, uint32_t *bucket_lo, uint32_t *bucket_hi) {
+  if (!hist16 || !bucket_lo || !bucket_hi || n_ranks < 1 || n_ranks > (uint32_t)kMaxRanks)
+    return mhb_set_error(MHB_ERR_ARG, "bad args");
+  static uint64_t h[kMaxRanks][256];  // rank 0's histogram holds everything
+  memset(h, 0, sizeof(h));
+  fold_bucket_hist(hist16, h[0]);
+  const Plan P = plan_partition_host(h, (int)n_ranks, 0);
+  for (uint32_t o = 0; o < n_ranks; ++o) {
+    bucket_lo[o] = P.bounds[o] << 8;
+    bucket_hi[o] = (P.bounds[o + 1] << 8) - 1;
+  }
   return MHB_OK;
 }

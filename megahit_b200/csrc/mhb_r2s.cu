@@ -69,11 +69,10 @@ struct PkgIndex {
   std::vector<uint32_t> len;
 };
 
-int index_pkg(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, uint32_t k, PkgIndex *ix) {
-  ix->n_reads = n_reads;
-  CKR(index_read_lib(bin, bin_words, n_reads, 0, &ix->li));
-  std::vector<uint64_t>().swap(ix->li.unit_off);
-  if (n_reads == 0) return MHB_OK;
+// the package geometry of every read, from the record offsets in ix->li and ix->n_reads
+void pkg_geometry(const uint32_t *bin, uint32_t k, PkgIndex *ix) {
+  const uint64_t n_reads = ix->n_reads;
+  if (n_reads == 0) return;
   const uint32_t L0 = ix->li.fixed_len;
   if (L0) {
     ix->fixed_len = ix->max_len = L0;
@@ -84,7 +83,7 @@ int index_pkg(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, uint32_
       ix->n_s1 = n_reads * (uint64_t)(L0 - k + 4);
       ix->n_edges = n_reads * (uint64_t)(L0 - k);
     }
-    return MHB_OK;
+    return;
   }
   ix->word_off.resize(n_reads + 1);
   ix->base_off.resize(n_reads + 1);
@@ -116,6 +115,13 @@ int index_pkg(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, uint32_
   ix->n_bases = b;
   ix->n_s1 = s1;
   ix->n_edges = e;
+}
+
+int index_pkg(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, uint32_t k, PkgIndex *ix) {
+  ix->n_reads = n_reads;
+  CKR(index_read_lib(bin, bin_words, n_reads, 0, &ix->li));
+  std::vector<uint64_t>().swap(ix->li.unit_off);
+  pkg_geometry(bin, k, ix);
   return MHB_OK;
 }
 
@@ -388,8 +394,16 @@ bool stream_decide(const ResidentPlan &p, const PkgIndex &ix, uint32_t k, int32_
 struct S1Side {  // the narrow layout's read_info side array and the pair buffers of its bucket partition
   DevBuf info, pa, pb;
 };
+// the buffers of one stage-1 pass over n records: the records (a, overwritten), a sort buffer of as many records (b),
+// the workspace s1_ws_bytes(n); narrow layout: the read_info side array and the two pair buffers, n entries each
+struct S1Bufs {
+  u32 *a, *b;
+  void *ws;
+  u64 *info;
+  u32 *pa, *pb;
+};
 int s1_sort_post(cudaStream_t st, const PkgView &pv, uint32_t k, int32_t m, bool need_mercy, const S1Out &out,
-                 unsigned long long *d_mul_hist, PhaseTrace &tr, BigBufs &big, S1Side &side, uint64_t n);
+                 unsigned long long *d_mul_hist, PhaseTrace &tr, const S1Bufs &bufs, uint64_t n);
 
 // Stage 1 in rounds over contiguous ranges of bucket ids, each of at most max_n records; *n_rounds counts the
 // non-empty ones.  max_n == 0: one pass, the one range over all bucket ids, known without a pass: each chunk's records
@@ -491,7 +505,8 @@ int run_stage1(cudaStream_t st, const EachChunk &each, const PkgView &shape, con
     seen += n;
     if (n == 0) continue;
     tr.mark("s1.extract");
-    CKR(s1_sort_post(st, shape, k, m, need_mercy, out, d_mul_hist, tr, big, side, n));
+    const S1Bufs bufs{big.a.as<u32>(), big.b.as<u32>(), big.ws.p, d_info, side.pa.as<u32>(), side.pb.as<u32>()};
+    CKR(s1_sort_post(st, shape, k, m, need_mercy, out, d_mul_hist, tr, bufs, n));
     ++*n_rounds;
   }
   if (seen != ix.n_s1)
@@ -500,13 +515,13 @@ int run_stage1(cudaStream_t st, const EachChunk &each, const PkgView &shape, con
   return MHB_OK;
 }
 
-// stable bucket partition, kmsort emulation and Lv2Postprocess of the n records in big.a
+// stable bucket partition, kmsort emulation and Lv2Postprocess of the n records in bufs.a
 int s1_sort_post(cudaStream_t st, const PkgView &pv, uint32_t k, int32_t m, bool need_mercy, const S1Out &out,
-                 unsigned long long *d_mul_hist, PhaseTrace &tr, BigBufs &big, S1Side &side, uint64_t n) {
+                 unsigned long long *d_mul_hist, PhaseTrace &tr, const S1Bufs &bufs, uint64_t n) {
   const S1Layout l = s1_layout(k);
   const uint32_t NW = l.NW, RW = l.RW;
   DevBuf bstart, segs0, segs1, counter, bnd;
-  DevBuf &a = big.a, &b = big.b, &ws = big.ws;
+  u32 *const a = bufs.a, *const b = bufs.b;
   const size_t ws_bytes = s1_ws_bytes(n, l);
   CKR(bstart.alloc((MHB_NUM_BUCKETS + 1) * 8, "read2sdbg: bucket bounds"));
   const uint64_t seg_cap = n / (kKmInsertThreshold + 1) + 2;
@@ -520,19 +535,18 @@ int s1_sort_post(cudaStream_t st, const PkgView &pv, uint32_t k, int32_t m, bool
   int in_b = 0;
   if (l.narrow) {
     const uint8_t bytes[2] = {6, 7};  // the two leading bytes of a (word 0, row) pair
-    k_r2s_s1_pairs<<<grid_cap(n, 256, 16), 256, 0, st>>>(a.as<u32>(), n, RW, side.pa.as<u32>());
+    k_r2s_s1_pairs<<<grid_cap(n, 256, 16), 256, 0, st>>>(a, n, RW, bufs.pa);
     CK_LAUNCH();
     int in_pb = 0;
-    CKR(mhb_sort_records(st, side.pa.as<u32>(), side.pb.as<u32>(), n, 2, bytes, 2, nullptr, ws.p, ws_bytes, &in_pb));
-    k_r2s_s1_gather<<<grid_cap(n * RW, 256, 16), 256, 0, st>>>(a.as<u32>(), in_pb ? side.pb.as<u32>() : side.pa.as<u32>(), n,
-                                                           RW, b.as<u32>());
+    CKR(mhb_sort_records(st, bufs.pa, bufs.pb, n, 2, bytes, 2, nullptr, bufs.ws, ws_bytes, &in_pb));
+    k_r2s_s1_gather<<<grid_cap(n * RW, 256, 16), 256, 0, st>>>(a, in_pb ? bufs.pb : bufs.pa, n, RW, b);
     CK_LAUNCH();
     in_b = 1;
   } else {
     const uint8_t bytes[2] = {(uint8_t)(4 * RW - 2), (uint8_t)(4 * RW - 1)};
-    CKR(mhb_sort_records(st, a.as<u32>(), b.as<u32>(), n, RW, bytes, 2, nullptr, ws.p, ws_bytes, &in_b));
+    CKR(mhb_sort_records(st, a, b, n, RW, bytes, 2, nullptr, bufs.ws, ws_bytes, &in_b));
   }
-  u32 *recs = in_b ? b.as<u32>() : a.as<u32>();
+  u32 *recs = in_b ? b : a;
   tr.mark("s1.partition");
   k_r2s_bucket_bounds<<<(MHB_NUM_BUCKETS + 1 + 255) / 256, 256, 0, st>>>(recs, n, RW, bstart.as<u64>());
   CK_LAUNCH();
@@ -560,7 +574,7 @@ int s1_sort_post(cudaStream_t st, const PkgView &pv, uint32_t k, int32_t m, bool
     CK(cudaMemsetAsync(todo.p, 0, (n / 32 + 2) * 4, st));
     CKR(src16.alloc((size_t)n * 2 + 64, "read2sdbg: kmsort source indices"));
     d_todo = todo.as<u32>();
-    u32 *other = in_b ? a.as<u32>() : b.as<u32>();
+    u32 *other = in_b ? a : b;
 #define M(WW)                                                                                                           \
   if (RW == WW) {                                                                                                       \
     CK(cudaFuncSetAttribute(k_r2s_km_bucket<WW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cap));               \
@@ -624,7 +638,7 @@ int s1_sort_post(cudaStream_t st, const PkgView &pv, uint32_t k, int32_t m, bool
   tr.mark("s1.kmsort.finish");
 #define M(WW)                                                                                                          \
   if (RW == WW)                                                                                                        \
-    k_r2s_s1_post<WW><<<grid_cap(n, 256, 32), 256, 0, st>>>(recs, l.narrow ? side.info.as<u64>() : nullptr, n, NW, k, m, \
+    k_r2s_s1_post<WW><<<grid_cap(n, 256, 32), 256, 0, st>>>(recs, l.narrow ? bufs.info : nullptr, n, NW, k, m, \
                                                             pv, out, need_mercy ? 1 : 0, d_mul_hist);
   MHB_FOR_RW(M)
 #undef M
@@ -639,18 +653,18 @@ struct S2Bufs {  // collapse and emitter buffers, kept across rounds
   DevBuf tile_heads, tile_off, bsum, heads, scr, bytes;
 };
 
-// relaxed sort -> collapse of equal items -> emitter, on the n items in big.a; leaves the SdBG stream in sb.bytes
-// (capacity *cap_bytes) and the bucket table / totals in d_table / d_totals; *n_u = distinct items
-int s2_sort_emit(cudaStream_t st, uint32_t k, BigBufs &big, S2Bufs &sb, uint64_t n, u64 *d_table, u64 *d_totals,
+// relaxed sort -> collapse of equal items -> emitter, on the n items in a (b: a buffer of as many items, ws: the sort
+// workspace); leaves the SdBG stream in sb.bytes (capacity *cap_bytes) and the bucket table / totals in d_table /
+// d_totals; *n_u = distinct items
+int s2_sort_emit(cudaStream_t st, uint32_t k, u32 *a, u32 *b, void *ws, S2Bufs &sb, uint64_t n, u64 *d_table, u64 *d_totals,
                  unsigned long long *d_counter, PhaseTrace &tr, uint64_t *n_u_out, uint64_t *cap_bytes) {
   const uint32_t W = s2s_record_words(k), WPT = words_per_tip_label(k);
-  DevBuf &a = big.a, &b = big.b, &ws = big.ws;
   const size_t ws_bytes = mhb_s2s_sort_workspace_bytes(n, k);
   int in_b = 0;
-  CKR(mhb_s2s_sort(st, a.as<u32>(), b.as<u32>(), n, k, nullptr, ws.p, ws_bytes, &in_b));
+  CKR(mhb_s2s_sort(st, a, b, n, k, nullptr, ws, ws_bytes, &in_b));
   tr.mark("s2.sort");
-  const u32 *sorted = in_b ? b.as<u32>() : a.as<u32>();
-  u32 *uniq = in_b ? a.as<u32>() : b.as<u32>();
+  const u32 *sorted = in_b ? b : a;
+  u32 *uniq = in_b ? a : b;
   // equal items -> one item carrying the run length (read_to_sdbg_s2.cpp:560-572)
   const uint64_t n_tiles = (n + kDdTile - 1) / kDdTile;
   CKR(sb.tile_heads.ensure(n_tiles * 4, "read2sdbg: tile counts"));
@@ -824,7 +838,8 @@ int run_stage2(const mhb_build_args *args, mhb_build_result *res, cudaStream_t s
     seen += n;
     if (n == 0) continue;
     uint64_t n_u = 0, cap_bytes = 0;
-    CKR(s2_sort_emit(st, k, big, sb, n, d_table, d_totals, d_counter, tr, &n_u, &cap_bytes));
+    CKR(s2_sort_emit(st, k, big.a.as<u32>(), big.b.as<u32>(), big.ws.p, sb, n, d_table, d_totals, d_counter, tr, &n_u,
+                     &cap_bytes));
     tr.mark("s2.emit");
     if (ranges.size() > 1) {
       CKR(out.append(st, sb.bytes.as<uint8_t>(), cap_bytes, d_table, d_totals));
@@ -855,6 +870,311 @@ int run_stage2(const mhb_build_args *args, mhb_build_result *res, cudaStream_t s
 }
 
 }  // namespace
+
+// ------------------------------------------------------------------------------------------------
+// One rank's share of a build on several GPUs (R2sShare, mhb_internal.h; the steps of mhb_read2sdbg_run_multi)
+// ------------------------------------------------------------------------------------------------
+struct R2sShare::Impl {
+  mhb_build_args a;
+  uint32_t k = 0;
+  int32_t m = 0;
+  bool mercy = false;  // need_mercy with a stage 1
+  PkgIndex ix;         // the whole library
+  PkgChunk c;          // the share, package words in pkg
+  PkgView shape;       // the library's shape for the post-processing of stage 1
+  uint64_t bit_words = 0;
+  int n_planes = 0;
+  DevBuf pkg, word_off, len, base_off, s1_off, edge_off, planes, mplane, hist, cnt, table, totals;
+  S1Out so;
+  PhaseTrace tr;
+  cudaStream_t st = 0;
+};
+
+R2sShare::R2sShare() : d_(new Impl) {}
+R2sShare::~R2sShare() { delete d_; }
+uint32_t R2sShare::s1_record_words() const { return s1_layout(d_->k).RW; }
+bool R2sShare::s1_narrow() const { return s1_layout(d_->k).narrow; }
+uint64_t R2sShare::s1_round_cap() const { return ::s1_round_cap(s1_layout(d_->k)); }
+void *R2sShare::planes() const { return d_->planes.p; }
+uint64_t R2sShare::n_reads() const { return d_->c.pv.n_reads; }
+
+namespace {
+// the slice [f, e] of a whole-library offset array, rebased to its first entry, on the device
+int upload_slice(DevBuf &d, const std::vector<uint64_t> &v, uint64_t f, uint64_t e, const char *what) {
+  std::vector<uint64_t> s(v.begin() + f, v.begin() + e + 1);
+  for (uint64_t &x : s) x -= v[f];
+  return upload(d, s, what);
+}
+}  // namespace
+
+int R2sShare::load(const mhb_build_args *a, const ReadLibIndex &li, uint64_t first, uint64_t end) {
+  Impl &d = *d_;
+  d.a = *a;
+  d.k = a->k;
+  d.m = a->m;
+  if (d.k < 9 || d.k > MHB_MAX_K || d.m < 1) return mhb_set_error(MHB_ERR_ARG, "read2sdbg: need 9 <= k <= 255 and m >= 1");
+  PkgIndex &ix = d.ix;
+  ix.n_reads = a->n_reads;
+  ix.li = li;
+  pkg_geometry(a->bin, d.k, &ix);
+  d.mercy = a->need_mercy && d.m > 1 && ix.n_s1 > 0;
+  memset(&d.shape, 0, sizeof(d.shape));
+  d.shape.n_reads = ix.n_reads;
+  d.shape.fixed_len = ix.fixed_len;
+  d.shape.fixed_words = ix.fixed_words;
+  PkgChunk &c = d.c;
+  c = chunk_of(ix, first, end, d.k);
+  const uint64_t n = c.pv.n_reads;
+  const cudaStream_t st = d.st;
+  CKR(d.pkg.alloc((size_t)c.n_words * 4 + 64, "read2sdbg: package of the share"));
+  if (n) {
+    const uint64_t w0 = li.word_of(first), nw = li.word_of(end) - w0;
+    DevBuf d_bin, d_rec_off;
+    CKR(d_bin.alloc((size_t)nw * 4 + 64, "read2sdbg: .bin image of the share"));
+    CK(cudaMemcpyAsync(d_bin.p, a->bin + w0, (size_t)nw * 4, cudaMemcpyHostToDevice, st));
+    if (!ix.fixed_len) {
+      CKR(upload_slice(d_rec_off, li.rec_off, first, end, "read2sdbg: record offsets of the share"));
+      CKR(upload_slice(d.word_off, ix.word_off, first, end, "read2sdbg: word offsets of the share"));
+      CKR(upload_slice(d.base_off, ix.base_off, first, end, "read2sdbg: base offsets of the share"));
+      CKR(upload_slice(d.s1_off, ix.s1_off, first, end, "read2sdbg: stage-1 offsets of the share"));
+      CKR(upload_slice(d.edge_off, ix.edge_off, first, end, "read2sdbg: edge offsets of the share"));
+      CKR(upload(d.len, std::vector<uint32_t>(ix.len.begin() + first, ix.len.begin() + end), "read2sdbg: lengths of the share"));
+      c.pv.word_off = d.word_off.as<u64>();
+      c.pv.len = d.len.as<u32>();
+      c.pv.base_off = d.base_off.as<u64>();
+      c.pv.s1_off = d.s1_off.as<u64>();
+      c.pv.edge_off = d.edge_off.as<u64>();
+    }
+    if (c.n_words) {
+      k_r2s_reverse<<<grid_cap(c.n_words, 256, 16), 256, 0, st>>>(d_bin.as<u32>(), n, c.pv.fixed_len, d_rec_off.as<u64>(),
+                                                                   c.pv, d.pkg.as<u32>(), c.n_words);
+      CK_LAUNCH();
+    }
+    CK(cudaStreamSynchronize(st));  // d_bin / d_rec_off go out of scope
+  }
+  c.pv.words = d.pkg.as<u32>();
+  d.bit_words = ix.n_bases / 32 + 2;
+  memset(&d.so, 0, sizeof(d.so));
+  if (d.m > 1) {  // m == 1: stage 2 takes every edge and never reads the solid plane
+    d.n_planes = d.mercy ? 4 : 1;
+    const size_t pb = (size_t)d.n_planes * d.bit_words * 4;
+    CKR(d.planes.alloc(pb, "read2sdbg: bit planes of the whole library"));
+    CK(cudaMemsetAsync(d.planes.p, 0, pb, st));
+    d.so.is_solid = d.planes.as<u32>();
+    if (d.mercy) {
+      d.so.no_in = d.so.is_solid + d.bit_words;
+      d.so.no_out = d.so.no_in + d.bit_words;
+      d.so.any = d.so.no_out + d.bit_words;
+      CKR(d.mplane.alloc((c.w_end - c.w0) * 4, "read2sdbg: mercy plane of the share"));
+    }
+  }
+  CKR(d.hist.alloc(65536 * 8, "read2sdbg: multiplicity histogram"));
+  CK(cudaMemsetAsync(d.hist.p, 0, 65536 * 8, st));
+  CKR(d.cnt.alloc(64, "read2sdbg: counters"));
+  CK(cudaMemsetAsync(d.cnt.p, 0, 64, st));
+  CKR(d.table.alloc((size_t)MHB_NUM_BUCKETS * 32, "read2sdbg: bucket table"));
+  CKR(d.totals.alloc(16 * 8, "read2sdbg: totals"));
+  CK(cudaStreamSynchronize(st));
+  return MHB_OK;
+}
+
+int R2sShare::s1_hist(uint64_t *hist) {
+  Impl &d = *d_;
+  memset(hist, 0, 65536 * 8);
+  const PkgChunk &c = d.c;
+  if (d.m < 2 || !c.n_s1) return MHB_OK;
+  const uint32_t NW = s1_layout(d.k).NW;
+  DevBuf h16;
+  CKR(h16.alloc(MHB_NUM_BUCKETS * 8, "read2sdbg: bucket histogram"));
+  CK(cudaMemsetAsync(h16.p, 0, MHB_NUM_BUCKETS * 8, d.st));
+  const unsigned grid = grid_cap(c.pv.n_reads * 32, 256, 16);  // one warp per read
+#define M(WW) \
+  if (NW == WW) k_r2s_s1_range<WW, kS1Hist><<<grid, 256, 0, d.st>>>(c.pv, d.k, 0, 65535, h16.as<unsigned long long>(), nullptr, nullptr, nullptr);
+  MHB_FOR_WR(M)
+#undef M
+  CK_LAUNCH();
+  CK(cudaMemcpyAsync(hist, h16.p, MHB_NUM_BUCKETS * 8, cudaMemcpyDeviceToHost, d.st));
+  CK(cudaStreamSynchronize(d.st));
+  return MHB_OK;
+}
+
+int R2sShare::s1_send(const uint8_t *owner_of_byte, int n_owners, const uint64_t *rec_base, const uint64_t *info_base,
+                      const uint64_t *my_off, const uint64_t *expect) {
+  Impl &d = *d_;
+  const PkgChunk &c = d.c;
+  const uint64_t n = c.pv.n_reads;
+  if (n_owners < 1 || n_owners > kS1MaxOwners) return mhb_set_error(MHB_ERR_ARG, "read2sdbg: 1 .. %d owners", kS1MaxOwners);
+  if (d.m < 2 || !c.n_s1) {
+    for (int o = 0; o < n_owners; ++o)
+      if (expect[o]) return mhb_set_error(MHB_ERR_CUDA, "read2sdbg: internal: records expected from an empty share");
+    return MHB_OK;
+  }
+  const uint32_t NW = s1_layout(d.k).NW;
+  const cudaStream_t st = d.st;
+  DevBuf lut, bases, infos, offs, per_read, off, bsum;
+  CKR(lut.alloc(256, "read2sdbg: owner table"));
+  CKR(bases.alloc(kS1MaxOwners * 8, "read2sdbg: owner buffers"));
+  CKR(offs.alloc(kS1MaxOwners * 8, "read2sdbg: owner offsets"));
+  CKR(per_read.alloc((size_t)n_owners * n * 4, "read2sdbg: per-read record counts per owner"));
+  CKR(off.alloc((size_t)n_owners * (n + 1) * 8, "read2sdbg: per-read record offsets per owner"));
+  CKR(bsum.alloc((n / 4096 + 4) * 8, "read2sdbg: scan sums"));
+  CK(cudaMemcpyAsync(lut.p, owner_of_byte, 256, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(bases.p, rec_base, n_owners * 8, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(offs.p, my_off, n_owners * 8, cudaMemcpyHostToDevice, st));
+  if (info_base) {
+    CKR(infos.alloc(kS1MaxOwners * 8, "read2sdbg: owner read_info buffers"));
+    CK(cudaMemcpyAsync(infos.p, info_base, n_owners * 8, cudaMemcpyHostToDevice, st));
+  }
+  const unsigned grid = grid_cap(n * 32, 256, 16);  // one warp per read
+#define M(WW)                                                                                                        \
+  if (NW == WW)                                                                                                      \
+    k_r2s_s1_owners<WW, kS1OwnerCount><<<grid, 256, 0, st>>>(c.pv, d.k, lut.as<uint8_t>(), (u32)n_owners,             \
+                                                             per_read.as<u32>(), nullptr, nullptr, nullptr, nullptr);
+  MHB_FOR_WR(M)
+#undef M
+  CK_LAUNCH();
+  std::vector<uint64_t> sent(n_owners);
+  for (int o = 0; o < n_owners; ++o) {
+    u64 *oo = off.as<u64>() + (size_t)o * (n + 1);
+    CKR(scan32(st, per_read.as<u32>() + (size_t)o * n, n, oo, oo + n, bsum.as<u64>()));
+    CK(cudaMemcpyAsync(&sent[o], oo + n, 8, cudaMemcpyDeviceToHost, st));
+  }
+  CK(cudaStreamSynchronize(st));
+  for (int o = 0; o < n_owners; ++o)
+    if (sent[o] != expect[o])
+      return mhb_set_error(MHB_ERR_CUDA, "read2sdbg: internal: %llu stage-1 records for rank %d, the histogram said %llu",
+                           (unsigned long long)sent[o], o, (unsigned long long)expect[o]);
+#define M(WW)                                                                                                          \
+  if (NW == WW)                                                                                                        \
+    k_r2s_s1_owners<WW, kS1OwnerWrite><<<grid, 256, 0, st>>>(c.pv, d.k, lut.as<uint8_t>(), (u32)n_owners, nullptr,       \
+                                                             off.as<u64>(), bases.as<u64>(), infos.as<u64>(), offs.as<u64>());
+  MHB_FOR_WR(M)
+#undef M
+  CK_LAUNCH();
+  CK(cudaStreamSynchronize(st));
+  return MHB_OK;
+}
+
+int R2sShare::s1_own(uint32_t *recs, uint64_t *info, uint64_t n) {
+  Impl &d = *d_;
+  if (!n) return MHB_OK;
+  const S1Layout l = s1_layout(d.k);
+  DevBuf b, ws, pa, pb;
+  CKR(b.alloc((size_t)n * l.RW * 4 + 16, "read2sdbg: records (sort buffer)"));
+  CKR(ws.alloc(s1_ws_bytes(n, l), "read2sdbg: sort workspace"));
+  if (l.narrow) {
+    CKR(pa.alloc((size_t)n * 8 + 16, "read2sdbg: bucket partition pairs"));
+    CKR(pb.alloc((size_t)n * 8 + 16, "read2sdbg: bucket partition pairs (sort buffer)"));
+  }
+  const S1Bufs bufs{recs, b.as<u32>(), ws.p, l.narrow ? info : nullptr, pa.as<u32>(), pb.as<u32>()};
+  return s1_sort_post(d.st, d.shape, d.k, d.m, d.mercy, d.so, d.hist.as<unsigned long long>(), d.tr, bufs, n);
+}
+
+int R2sShare::or_planes(const void *peer_planes) {
+  Impl &d = *d_;
+  const PkgChunk &c = d.c;
+  if (!d.n_planes || !c.pv.n_reads) return MHB_OK;
+  const uint64_t nw = c.w_end - c.w0;
+  for (int p = 0; p < d.n_planes; ++p) {
+    const uint64_t at = (uint64_t)p * d.bit_words + c.w0;
+    k_r2s_or_words<<<grid_cap(nw, 256, 16), 256, 0, d.st>>>(d.planes.as<u32>() + at, (const u32 *)peer_planes + at, nw);
+    CK_LAUNCH();
+  }
+  CK(cudaStreamSynchronize(d.st));
+  return MHB_OK;
+}
+
+int R2sShare::mercy_count(uint64_t *n_items, uint64_t *n_mercy) {
+  Impl &d = *d_;
+  *n_items = *n_mercy = 0;
+  if (!d.c.pv.n_reads) return MHB_OK;
+  const EachChunk each = [&](const ChunkFn &fn) { return fn(d.c); };
+  return mercy_count_pass(d.st, each, d.k, d.m, d.mercy, d.so, d.mplane.as<u32>(), d.cnt.as<unsigned long long>(), d.tr,
+                          n_items, n_mercy);
+}
+
+int R2sShare::s2_hist(uint64_t *hist) {
+  Impl &d = *d_;
+  memset(hist, 0, 65536 * 8);
+  const PkgChunk &c = d.c;
+  if (!c.n_edges) return MHB_OK;
+  const uint32_t W = s2s_record_words(d.k);
+  DevBuf h16;
+  CKR(h16.alloc(MHB_NUM_BUCKETS * 8, "read2sdbg: bucket histogram"));
+  CK(cudaMemsetAsync(h16.p, 0, MHB_NUM_BUCKETS * 8, d.st));
+#define M(WW)                                                                                                          \
+  if (W == WW)                                                                                                         \
+    k_r2s_s2_extract<WW, kS2Hist><<<grid_cap(c.n_edges, 256, 16), 256, 0, d.st>>>(c.pv, d.k, d.so.is_solid, d.m == 1,     \
+                                                                                c.n_edges, nullptr, nullptr, 0, 0, 65535, \
+                                                                                h16.as<unsigned long long>());
+  MHB_FOR_WR(M)
+#undef M
+  CK_LAUNCH();
+  CK(cudaMemcpyAsync(hist, h16.p, MHB_NUM_BUCKETS * 8, cudaMemcpyDeviceToHost, d.st));
+  CK(cudaStreamSynchronize(d.st));
+  return MHB_OK;
+}
+
+int R2sShare::s2_send(const uint8_t *owner_of_byte, int n_owners, const uint64_t *owner_base, const uint64_t *capacity,
+                      uint64_t *sent) {
+  Impl &d = *d_;
+  const PkgChunk &c = d.c;
+  for (int o = 0; o < n_owners; ++o) sent[o] = 0;
+  if (!c.n_edges) return MHB_OK;
+  const uint32_t W = s2s_record_words(d.k);
+  const cudaStream_t st = d.st;
+  DevBuf lut, bases, cursor, cap;
+  CKR(lut.alloc(256, "read2sdbg: owner table"));
+  CKR(bases.alloc(n_owners * 8, "read2sdbg: owner buffers"));
+  CKR(cursor.alloc(n_owners * 8, "read2sdbg: owner cursors"));
+  CKR(cap.alloc(n_owners * 8, "read2sdbg: owner capacities"));
+  CK(cudaMemcpyAsync(lut.p, owner_of_byte, 256, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(bases.p, owner_base, n_owners * 8, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(cap.p, capacity, n_owners * 8, cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(cursor.p, 0, n_owners * 8, st));
+  const OwnerSink sink{lut.as<uint8_t>(), bases.as<u64>(), cursor.as<unsigned long long>(), cap.as<u64>()};
+#define M(WW)                                                                                                       \
+  if (W == WW)                                                                                                      \
+    k_r2s_s2_extract<WW, kS2Owner><<<grid_cap(c.n_edges, 256, 16), 256, 0, st>>>(c.pv, d.k, d.so.is_solid, d.m == 1, \
+                                                                               c.n_edges, nullptr, nullptr, 0, 0, 0, \
+                                                                               nullptr, sink);
+  MHB_FOR_WR(M)
+#undef M
+  CK_LAUNCH();
+  CK(cudaMemcpyAsync(sent, cursor.p, n_owners * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return MHB_OK;
+}
+
+int R2sShare::s2_own(uint32_t *items, uint64_t n, std::vector<uint8_t> *bytes, std::vector<uint64_t> *table,
+                     uint64_t *totals) {
+  Impl &d = *d_;
+  bytes->clear();
+  table->assign((size_t)MHB_NUM_BUCKETS * 4, 0);
+  memset(totals, 0, 16 * 8);
+  if (!n) return MHB_OK;
+  const uint32_t W = s2s_record_words(d.k);
+  DevBuf b, ws;
+  CKR(b.alloc((size_t)n * W * 4 + 16, "read2sdbg: stage-2 items (sort buffer)"));
+  CKR(ws.alloc(mhb_s2s_sort_workspace_bytes(n, d.k), "read2sdbg: sort workspace"));
+  S2Bufs sb;
+  uint64_t n_u = 0, cap_bytes = 0;
+  CKR(s2_sort_emit(d.st, d.k, items, b.as<u32>(), ws.p, sb, n, d.table.as<u64>(), d.totals.as<u64>(),
+                   d.cnt.as<unsigned long long>(), d.tr, &n_u, &cap_bytes));
+  CK(cudaMemcpyAsync(totals, d.totals.p, 16 * 8, cudaMemcpyDeviceToHost, d.st));
+  CK(cudaStreamSynchronize(d.st));
+  if (totals[0] > cap_bytes) return mhb_set_error(MHB_ERR_NOMEM, "internal: SdBG byte stream exceeds capacity");
+  bytes->resize(totals[0]);
+  if (totals[0]) CK(cudaMemcpyAsync(bytes->data(), sb.bytes.p, totals[0], cudaMemcpyDeviceToHost, d.st));
+  CK(cudaMemcpyAsync(table->data(), d.table.p, (size_t)MHB_NUM_BUCKETS * 32, cudaMemcpyDeviceToHost, d.st));
+  CK(cudaStreamSynchronize(d.st));
+  return MHB_OK;
+}
+
+int R2sShare::counting(uint64_t *hist) {
+  CK(cudaMemcpy(hist, d_->hist.p, 65536 * 8, cudaMemcpyDeviceToHost));
+  return MHB_OK;
+}
 
 extern "C" int mhb_set_r2s_round_limit(uint64_t max_s1_records, uint64_t max_s2_items) {
   g_r2s_s1_limit = max_s1_records;

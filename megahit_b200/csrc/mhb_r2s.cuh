@@ -16,6 +16,9 @@
 #pragma once
 #include "mhb.h"
 #include "mhb_kernels.cuh"
+#if defined(__CUDACC__)
+#include "mhb_s2s.cuh"  // OwnerSink
+#endif
 
 namespace mhb {
 
@@ -631,6 +634,59 @@ __global__ void __launch_bounds__(256) k_r2s_s1_range(PkgView pv, u32 k, u32 lo,
   }
 }
 
+// Stage 1 on several GPUs: every record of a rank's share straight into the receive buffer of the rank that owns its
+// leading byte, in global read order.  One warp per read, lane = emission index, as k_r2s_s1_range; the lanes of a
+// batch are grouped by owner (__match_any_sync) and s_run holds, per owner, the read's records placed so far.
+//   kS1OwnerCount: per_read[o * n_reads + r] = records of read r for owner o
+//   kS1OwnerWrite: the record goes to row my_off[o] + off[o * (n_reads + 1) + r] + its rank among read r's records for
+//                  o, of owner o's buffer rec_base[o] (narrow layout: read_info at that row of info_base[o]; the row
+//                  index the record carries is that owner-local row)
+// The shares ascend with the rank and my_off[o] puts this rank's block after those of the lower ranks, so every owner
+// holds its records in global read order - the reference's bucket input order - without an atomic.
+static constexpr int kS1MaxOwners = 16;
+enum { kS1OwnerCount = 0, kS1OwnerWrite = 1 };
+template <int NW, int MODE>
+__global__ void __launch_bounds__(256) k_r2s_s1_owners(PkgView pv, u32 k, const uint8_t *__restrict__ owner, u32 n_owners,
+                                                      u32 *__restrict__ per_read, const u64 *__restrict__ off,
+                                                      const u64 *__restrict__ rec_base, const u64 *__restrict__ info_base,
+                                                      const u64 *__restrict__ my_off) {
+  __shared__ u32 s_run[8][kS1MaxOwners];
+  const u32 lane = lane_id(), lt = lanemask_lt(), warp = threadIdx.x >> 5;
+  const u64 n_warps = (u64)gridDim.x * 8;
+  for (u64 r = ((u64)blockIdx.x * 256 + threadIdx.x) >> 5; r < pv.n_reads; r += n_warps) {  // warp-uniform
+    if (lane < (u32)kS1MaxOwners) s_run[warp][lane] = 0;
+    __syncwarp();
+    const u32 L = pv.L(r);
+    if (L >= k + 1) {
+      const u32 n_e = L - k + 4, nwords = div_ceil(L, 16);
+      const u32 *s = pv.ptr(r);
+      const u64 base = pv.base(r);
+      for (u32 e0 = 0; e0 < n_e; e0 += 32) {
+        const u32 e = e0 + lane;
+        u32 rec[NW + 2];
+        u32 o = 0xFFFFFFFFu;
+        if (e < n_e) {
+          u32 p, want;
+          s1_emission(L, k, e, p, want);
+          make_s1_record<NW>(s, nwords, L, k, p, want, base, rec);
+          o = __ldg(owner + (rec[0] >> 24));
+        }
+        const u32 peers = __match_any_sync(0xffffffffu, o);
+        if (MODE == kS1OwnerWrite && e < n_e) {
+          const u64 row = my_off[o] + off[(u64)o * (pv.n_reads + 1) + r] + s_run[warp][o] + __popc(peers & lt);
+          s1_store<NW>(reinterpret_cast<u32 *>(rec_base[o]), info_base ? reinterpret_cast<u64 *>(info_base[o]) : nullptr,
+                       row, rec);
+        }
+        __syncwarp();
+        if (e < n_e && lane == (u32)__ffs(peers) - 1) s_run[warp][o] += __popc(peers);
+        __syncwarp();
+      }
+    }
+    if (MODE == kS1OwnerCount && lane < n_owners) per_read[(u64)lane * pv.n_reads + r] = s_run[warp][lane];
+    __syncwarp();
+  }
+}
+
 // The bucket partition of the narrow layout, whose records may be wider than mhb_sort_records takes: (word 0, row)
 // pairs are sorted stably on the bucket id, then the records gathered in that order.  Row r sits at position r and its
 // index word says r, so the gathered records keep their side-array rows.
@@ -951,12 +1007,15 @@ MHB_HD u32 r2s_edge_types(const u32 *is_solid, bool sure, u64 b, u32 i, u32 L, u
 
 // MODE kS2Count: total number of items -> *cursor.  kS2Write: items appended at recs[*cursor ...] in no particular
 // order (whole-record sort keys).  For stage 2 in rounds: kS2Hist adds every item's 16-bit bucket id (top of word 0)
-// to hist[65536]; kS2Range appends only the items whose bucket id lies in [lo, hi].  One thread per (k+1)-mer position.
-enum { kS2Count = 0, kS2Write = 1, kS2Hist = 2, kS2Range = 3 };
+// to hist[65536]; kS2Range appends only the items whose bucket id lies in [lo, hi].  On several GPUs, kS2Owner hands
+// every item to `sink`, which stores it in the receive buffer of the rank owning its leading byte.  One thread per
+// (k+1)-mer position.
+enum { kS2Count = 0, kS2Write = 1, kS2Hist = 2, kS2Range = 3, kS2Owner = 4 };
 template <int W, int MODE>
 __global__ void __launch_bounds__(256) k_r2s_s2_extract(PkgView pv, u32 k, const u32 *__restrict__ is_solid, int sure, u64 n_edges,
                                                        u32 *__restrict__ recs, unsigned long long *__restrict__ cursor, u64 capacity,
-                                                       u32 lo = 0, u32 hi = 0, unsigned long long *__restrict__ hist = nullptr) {
+                                                       u32 lo = 0, u32 hi = 0, unsigned long long *__restrict__ hist = nullptr,
+                                                       OwnerSink sink = {}) {
   const u32 lane = lane_id();
   u64 t0 = (u64)blockIdx.x * 256 + threadIdx.x;
   const u64 step = (u64)gridDim.x * 256;
@@ -983,7 +1042,7 @@ __global__ void __launch_bounds__(256) k_r2s_s2_extract(PkgView pv, u32 k, const
       local_total += cnt;
       continue;
     }
-    if (MODE == kS2Hist || MODE == kS2Range) {
+    if (MODE == kS2Hist || MODE == kS2Range || MODE == kS2Owner) {
       // one (type, strand) slot at a time: a warp-aggregated append per slot for the items in range
       const u32 *s = pv.ptr(r);
       const u32 nwords = div_ceil(L, 16);
@@ -995,11 +1054,15 @@ __global__ void __launch_bounds__(256) k_r2s_s2_extract(PkgView pv, u32 k, const
           make_r2s_item<W>(s, nwords, k, i, strand, type, rec);
           const u32 b = rec[0] >> 16;
           if (MODE == kS2Hist) atomicAdd(&hist[b], 1ull);
-          in = b >= lo && b <= hi;
+          in = MODE == kS2Owner || (b >= lo && b <= hi);
         }
         if (MODE == kS2Hist) continue;
         const u32 mask = __ballot_sync(0xffffffffu, in);
         if (!mask) continue;
+        if (MODE == kS2Owner) {
+          sink.template put<W>(in, rec, mask, lane, lanemask_lt());
+          continue;
+        }
         unsigned long long wbase = 0;
         if (lane == 0) wbase = atomicAdd(cursor, (unsigned long long)__popc(mask));
         wbase = __shfl_sync(0xffffffffu, wbase, 0);

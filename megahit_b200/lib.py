@@ -146,7 +146,7 @@ SYMBOLS = [
     "mhb_mercy_candidates_scratch_bytes", "mhb_mercy_candidates", "mhb_mercy_edges_scratch_bytes", "mhb_mercy_edges", "mhb_mercy_edges_count", "mhb_mercy_edges_write", "mhb_mercy_edges_segs", "mhb_mercy_host", "mhb_mercy_planes_words", "mhb_mercy_probe_owned", "mhb_mercy_count_planes", "mhb_edge_lut_bytes", "mhb_edge_lut_build",
     "mhb_release", "mhb_count_run", "mhb_count_run_multi", "mhb_seq2sdbg_run", "mhb_seq2sdbg_run_multi",
     "mhb_plan_seq_shares", "mhb_s2s_extract_owners","mhb_selftest_count_record", "mhb_selftest_count_records_roll", "mhb_selftest_s2s_record",
-    "mhb_iterate_host", "mhb_iterate_run", "mhb_iterate_run_multi", "mhb_plan_read_shares", "mhb_selftest_iterate", "mhb_s2s_extract_edges_pruned", "mhb_s2s_emit_fmt", "mhb_read2sdbg_host", "mhb_read2sdbg_run", "mhb_selftest_r2s_s1_record", "mhb_selftest_r2s_item",
+    "mhb_iterate_host", "mhb_iterate_run", "mhb_iterate_run_multi", "mhb_plan_read_shares", "mhb_selftest_iterate", "mhb_s2s_extract_edges_pruned", "mhb_s2s_emit_fmt", "mhb_read2sdbg_host", "mhb_read2sdbg_run", "mhb_read2sdbg_run_multi", "mhb_plan_r2s_owners", "mhb_selftest_r2s_s1_record", "mhb_selftest_r2s_item",
     "mhb_selftest_kmsort", "mhb_selftest_kmsort_smem", "mhb_selftest_r2s_s1_group", "mhb_selftest_r2s_mercy_read",
     "mhb_selftest_r2s_chunk_index", "mhb_selftest_r2s_stream_decide",
     "mhb_selftest_kmsort_narrow", "mhb_selftest_r2s_s1_plan", "mhb_selftest_read2sdbg_narrow", "mhb_selftest_iterate_narrow",
@@ -283,6 +283,8 @@ def load():
                                                C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_int]
     L.mhb_read2sdbg_host.argtypes = [C.POINTER(BuildArgs), C.POINTER(BuildResult)]
     L.mhb_read2sdbg_run.argtypes = [C.POINTER(Read2SdbgOpts)]
+    L.mhb_read2sdbg_run_multi.argtypes = [C.POINTER(Read2SdbgOpts), C.c_int]
+    L.mhb_plan_r2s_owners.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
     L.mhb_selftest_r2s_s1_record.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64, C.c_void_p]
     L.mhb_selftest_r2s_item.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
                                         C.c_void_p, C.POINTER(C.c_uint32)]
@@ -784,10 +786,24 @@ def plan_read_shares(bin_words: np.ndarray, n_reads: int, n_ranks: int) -> list[
 
 
 def read2sdbg_run(read_lib_file: str, output_prefix: str, k: int = 21, m: int = 2, need_mercy: bool = False,
-                  host_mem: float = 1e9, num_cpu_threads: int = 0, mem_flag: int = 1) -> None:
+                  host_mem: float = 1e9, num_cpu_threads: int = 0, mem_flag: int = 1, gpus: int = 1) -> None:
+    """gpus > 1: mhb_read2sdbg_run_multi, which forks one worker per GPU and so must be called from a process that has
+    not initialised CUDA (torch included); it writes one P.sdbg.<r> per rank."""
     o = Read2SdbgOpts(k, m, host_mem, num_cpu_threads, read_lib_file.encode(), output_prefix.encode(), mem_flag,
                       int(need_mercy))
-    _check(load().mhb_read2sdbg_run(C.byref(o)))
+    L = load()
+    _check(L.mhb_read2sdbg_run_multi(C.byref(o), int(gpus)) if gpus > 1 else L.mhb_read2sdbg_run(C.byref(o)))
+
+
+def plan_r2s_owners(hist16: np.ndarray, n_ranks: int) -> list[tuple[int, int]]:
+    """The owner ranges of a multi-GPU read2sdbg stage (host logic only): (first, last) bucket id of every rank, from the
+    65536-bin bucket histogram of the stage's records."""
+    h = np.ascontiguousarray(hist16, np.uint64)
+    assert len(h) == 65536
+    lo = np.zeros(n_ranks, np.uint32)
+    hi = np.zeros(n_ranks, np.uint32)
+    _check(load().mhb_plan_r2s_owners(h.ctypes.data, n_ranks, lo.ctypes.data, hi.ctypes.data))
+    return [(int(a), int(b)) for a, b in zip(lo, hi)]
 
 
 # ------------------------------------------------------------------------------------------------
