@@ -2,6 +2,8 @@
 #pragma once
 #include <stddef.h>
 #include <stdint.h>
+#include <stdio.h>
+#include <sys/time.h>
 
 #include <algorithm>
 #include <functional>
@@ -11,6 +13,20 @@
 #include "mhb.h"
 
 int mhb_set_error(int code, const char *fmt, ...);
+
+// an INFO line on stderr, in the reference's log format
+#define XINFO(...)                                                    \
+  do {                                                                \
+    fprintf(stderr, "INFO  %-30s: %4d - ", "megahit_b200", __LINE__); \
+    fprintf(stderr, __VA_ARGS__);                                     \
+  } while (0)
+
+// wall-clock seconds, for the "Time elapsed" lines
+inline double now_s() {
+  timeval tv;
+  gettimeofday(&tv, nullptr);
+  return tv.tv_sec + tv.tv_usec * 1e-6;
+}
 
 // ---- host helpers of every stage (device-side ones, which need CUDA types: mhb_common.cuh) ----
 // return a non-zero status code at once
@@ -28,7 +44,8 @@ size_t free_device_bytes();
 
 // One device allocation, released with the object (mhb_stream.cu).  alloc rounds max(bytes, 1) up to 256 and
 // reallocates; ensure only grows, and contents do not survive growth.  A failed cudaMalloc clears the CUDA error and is
-// MHB_ERR_NOMEM, its message "<what>: cudaMalloc of <bytes> bytes failed" (what starts with the stage).
+// MHB_ERR_NOMEM, its message "<what>: cudaMalloc of <bytes> bytes failed" (what starts with the stage).  The process
+// counts the bytes all its DevBufs hold: peak_bytes() is the most they have held since the last reset_peak().
 struct DevBuf {
   void *p = nullptr;
   size_t bytes = 0;
@@ -45,6 +62,8 @@ struct DevBuf {
   }
   template <class T>
   T *as() const { return reinterpret_cast<T *>(p); }
+  static void reset_peak();
+  static size_t peak_bytes();
 };
 
 // largest n <= n_max with fixed + bytes(n) <= avail (bytes(n) grows with n); 0 when not even one fits
@@ -100,6 +119,26 @@ int index_read_lib(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, ui
                    FixedCheck check = FixedCheck::kFull);
 // A read library from disk (mhb_files.cpp): the counts of `prefix.lib_info` and the image of `prefix.bin`
 int load_read_lib(const std::string &prefix, std::vector<uint32_t> *bin, long long *n_reads, long long *total_bases);
+
+// ---- the reference's output formats (mhb_files.cpp), each written in one place for the single- and multi-GPU paths;
+// a file that cannot be written is MHB_ERR_IO ----
+// n raw bytes: `.sdbg.<i>`, `.edges.<i>`, `.cand`
+int write_bytes(const std::string &path, const void *data, size_t n);
+// P.sdbg_info (sdbg_meta.cpp:44-61).  tables: one 65536 x {byte offset, items, tips, large_mul} bucket table per
+// `.sdbg.<i>` file, in file order.  Rows of the used buckets, files in order and buckets ascending, then unused rows.
+int write_sdbg_info(const std::string &prefix, uint32_t k, uint32_t words_per_tip_label, int num_files,
+                    const std::vector<const uint64_t *> &tables);
+// P.edges.info of sorted edges (edge_io_meta.h:25-44).  counts: one 65536-bin bucket histogram per `.edges.<i>` file,
+// whose edges are in bucket order; offsets run per file, and a bucket with edges in two files is MHB_ERR_ARG.
+int write_edges_info(const std::string &prefix, uint32_t k, uint32_t words_per_edge,
+                     const std::vector<std::vector<int64_t>> &counts);
+// P.counting (edge_counter.h:44-52): multiplicities 1 .. MHB_MAX_MUL of hist
+int write_counting(const std::string &prefix, const int64_t *hist);
+// one read of a `.bin` image, given at its length word, appended to a `.cand` image in the reversed orientation
+// KmerCounter holds candidate reads in (kmer_counter.cpp:387-401; sequence_package.h:284-295: reverse, no complement)
+void append_cand_reversed(const uint32_t *read, std::vector<uint32_t> *out);
+// the closing lines of the reference's seq2sdbg / read2sdbg, from the emitter's totals (SdbgStitch::tot layout)
+void log_sdbg_summary(const uint64_t tot[16]);
 
 // Streaming statistics of one host-level call: chunks (0 = resident), passes, bytes host to device, and the copy-engine
 // and compute-stream busy time, host fill time and wall time of the passes (ms).
@@ -354,4 +393,15 @@ void set_sdbg_totals(R *res, const uint64_t tot[16]) {
   res->n_large_mul = tot[3];
   for (int i = 0; i < 9; ++i) res->w_count[i] = tot[4 + i];
   res->ones_in_last = tot[13];
+}
+// ... and back
+template <class R>
+void get_sdbg_totals(const R &res, uint64_t tot[16]) {
+  std::fill(tot, tot + 16, 0);
+  tot[0] = res.n_bytes;
+  tot[1] = res.n_items;
+  tot[2] = res.n_tips;
+  tot[3] = res.n_large_mul;
+  for (int i = 0; i < 9; ++i) tot[4 + i] = res.w_count[i];
+  tot[13] = res.ones_in_last;
 }

@@ -19,6 +19,7 @@ using namespace mhb;
 namespace {
 uint64_t g_chunk_limit = 0;
 StreamStats g_st;
+size_t g_dev_live = 0, g_dev_peak = 0;  // bytes the process's DevBufs hold, and the most since DevBuf::reset_peak
 }  // namespace
 
 size_t free_device_bytes() {
@@ -31,7 +32,10 @@ size_t free_device_bytes() {
 }
 
 void DevBuf::release() {
-  if (p) cudaFree(p);
+  if (p) {
+    cudaFree(p);
+    g_dev_live -= bytes;
+  }
   p = nullptr;
   bytes = 0;
 }
@@ -46,8 +50,13 @@ int DevBuf::alloc(size_t b, const char *what) {
     return mhb_set_error(MHB_ERR_NOMEM, "%s: cudaMalloc of %zu bytes failed: %s", what, b, cudaGetErrorString(e));
   }
   bytes = b;
+  g_dev_live += b;
+  g_dev_peak = std::max(g_dev_peak, g_dev_live);
   return MHB_OK;
 }
+
+void DevBuf::reset_peak() { g_dev_peak = g_dev_live; }
+size_t DevBuf::peak_bytes() { return g_dev_peak; }
 
 void plan_chunks(const uint64_t *word_off, uint64_t stride_words, uint64_t extra_bytes, uint64_t n, uint64_t max_bytes,
                  std::vector<uint64_t> *first) {
