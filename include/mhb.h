@@ -108,6 +108,20 @@ int mhb_count_extract_range(void *stream, const mhb_dev_reads *reads, uint32_t k
                             uint64_t *per_read, uint32_t *records, uint64_t *hist256, int hist_byte,
                             uint64_t *total_dev);
 
+/* The extraction of a multi-GPU count, the records of one rank's share of the reads in two modes:
+ *   hist16 != NULL: count only - hist16[b] (device uint64[65536], caller-zeroed) += the records whose 16-bit bucket id
+ *                   (first eight bases) is b; the other arguments are ignored;
+ *   hist16 == NULL: every record of bucket id b whose owner o = owner_of_byte[b >> 8] has round_lo[o] <= b <=
+ *                   round_hi[o] is stored straight into o's buffer (an empty range, lo > hi, sends nothing to o).
+ *                   Device arrays: owner_of_byte[256]; owner_base[o] = the address where this rank's records for o begin
+ *                   (a segment of o's receive buffer, possibly opened through CUDA IPC); cursor_dev[o] (caller-zeroed)
+ *                   ends at the number of records sent to o; records beyond capacity_dev[o] are counted but not
+ *                   stored; round_lo / round_hi: one entry per owner.  The order inside a segment is unspecified.
+ * Records as mhb_count_extract; variable-length reads need rec_off and edge_off. */
+int mhb_count_extract_owners(void *stream, const mhb_dev_reads *reads, uint32_t k, uint64_t *hist16,
+                             const uint8_t *owner_of_byte, const uint64_t *owner_base, uint64_t *cursor_dev,
+                             const uint64_t *capacity_dev, const uint32_t *round_lo, const uint32_t *round_hi);
+
 /* A4: stable LSD radix sort of n records of `words` uint32 each, ascending on the given byte
  * positions (least significant first).  `first_hist` = histogram of bytes[0] if the caller already has
  * it (from mhb_count_extract / mhb_s2s_extract), else NULL.  Result is left in `a` if *result_in_b == 0
@@ -708,17 +722,34 @@ int mhb_read2sdbg_run(const mhb_read2sdbg_opts *opts);
  * forward to the reference. */
 int mhb_buildlib_run(const char *lib_file, const char *out_prefix);
 
-/* `count` on n_gpus GPUs of this node (fixed-length read libraries; anything else, or n_gpus <= 1, runs mhb_count_run).
- * One worker process per GPU is forked; each takes a contiguous block of the reads, the records meet on the rank that
- * owns their leading byte (fused partition + exchange into CUDA-IPC peer buffers, SURVEY.md 8e), every rank counts its
- * bucket range, the mercy searches are answered by the owners of the searched prefixes, and - because the solid
- * edges are already on the devices - the k_min SdBG is built in the same run.  Files: rank r writes P.edges.<r> and
+/* `count` on n_gpus GPUs of this node, for fixed- and variable-length read libraries.  n_gpus <= 1, fewer reads than
+ * GPUs, k < 12 or a truncated `.bin` image (which the single-GPU count reports) run mhb_count_run.  One worker process
+ * per GPU is forked; each takes a contiguous share of the reads balanced on bases (mhb_plan_read_shares), histograms
+ * its records' 16-bit bucket ids, and every rank plans the same owner byte ranges and, when an owner's records do not
+ * fit its device at once (or exceed mhb_set_round_limit), the same rounds over ascending bucket sub-ranges
+ * (mhb_plan_count_owner_rounds).  Per round every rank extracts its records straight into the owners' CUDA-IPC receive
+ * buffers (mhb_count_extract_owners) and every owner counts what it received; a single bucket larger than one round
+ * is MHB_ERR_NOMEM before any round buffer is allocated.  The mercy searches are answered by the owners of the
+ * searched prefixes, and - because the solid edges are already on the devices - the k_min SdBG is built in the same
+ * run (resident).  Files: rank r writes P.edges.<r> and
  * P.sdbg.<r>, rank 0 the merged P.edges.info (num_files = n_gpus, edge_io_meta.h:25-44), P.sdbg_info
  * (sdbg_meta.cpp:44-61), P.cand, P.counting, and the marker P.sdbg_fused ("k need_mercy n_gpus") that lets a following
  * `seq2sdbg --need_mercy --input_prefix P -o P` return at once instead of rebuilding the same graph.  The caller must not
  * have initialised CUDA in this process (the workers are forked).  Rank r runs on device r % device_count: with more
  * ranks than devices, ranks share a device (its compute mode must admit several processes). */
 int mhb_count_run_multi(const mhb_count_opts *opts, int n_gpus);
+/* The plan of mhb_count_run_multi (host only).  hist16: n_ranks x 65536 bucket histograms, one per rank's share.
+ * Owners: the leading bytes cut into n_ranks contiguous ranges as the count exchange cuts them; owner o owns the
+ * buckets [owner_lo[o], owner_hi[o]].  Rounds: every owner's bucket range cut greedily into ascending sub-ranges of at
+ * most max_records records (0 = no cap: one round, the owner ranges), a leading byte that alone exceeds the cap cut on
+ * bucket ids; *n_rounds_out = R = the most sub-ranges of any owner, and an owner with fewer gets empty ranges (lo > hi)
+ * in its last rounds.  round_lo / round_hi[t * n_ranks + o]: owner o's range in round t; block_n / block_off[(t *
+ * n_ranks + o) * n_ranks + s]: the records rank s sends to o in round t and where they start in o's buffer.  Arrays
+ * sized for max_rounds rounds.  MHB_ERR_NOMEM when a single bucket exceeds the cap (the message names the bucket and
+ * the owner) or more than max_rounds rounds are needed. */
+int mhb_plan_count_owner_rounds(const uint64_t *hist16, uint32_t n_ranks, uint64_t max_records, uint32_t max_rounds,
+                                uint32_t *owner_lo, uint32_t *owner_hi, uint32_t *round_lo, uint32_t *round_hi,
+                                uint64_t *block_n, uint64_t *block_off, uint32_t *n_rounds_out);
 
 /* `seq2sdbg` on n_gpus GPUs of this node: the same options and inputs as mhb_seq2sdbg_run.  n_gpus <= 1 runs
  * mhb_seq2sdbg_run; so does --need_mercy (the mercy search over edge files stays on one GPU), except where the multi-GPU

@@ -205,6 +205,49 @@ __global__ void __launch_bounds__(kExtractThreads)
 }
 
 // ------------------------------------------------------------------------------------------------
+// K-extract on several GPUs: the records of a rank's share of the reads, straight into the receive buffers of the ranks
+// owning their leading byte (no local record array), in rounds over bucket ranges when the owners cannot take all their
+// records at once.  Same reads walk and records as k_count_extract.
+//   kCountOwnHist : hist16[bucket id] += 1 for every record (the planner's input); nothing is stored.  The lanes of a
+//                   warp holding the same bucket id add once, so a skewed library costs one atomic per distinct bucket.
+//   kCountOwnWrite: a record of bucket id b with owner o = sink.owner[b >> 8] goes to o when round_lo[o] <= b <=
+//                   round_hi[o] (an empty range, lo > hi, sends nothing to o); stored through the OwnerSink.
+// ------------------------------------------------------------------------------------------------
+enum { kCountOwnHist = 0, kCountOwnWrite = 1 };
+template <int W, int WR, int MODE>
+__global__ void __launch_bounds__(kExtractThreads)
+    k_count_extract_owners(ReadsView rv, u32 k, unsigned long long *__restrict__ hist16, OwnerSink sink,
+                           const u32 *__restrict__ round_lo, const u32 *__restrict__ round_hi) {
+  const u32 lane = lane_id(), lt = lanemask_lt();
+  const u32 K1 = k + 1;
+  for_each_read(rv, [&](u64, const u32 *s, u32 nwords, u32 L) {  // warp-uniform
+    if (L < K1) return;  // kmer_counter.cpp:124
+    const u32 n_e = L - k;
+    for (u32 q0 = 0; q0 < n_e; q0 += 32) {
+      const u32 q = q0 + lane;
+      u32 rec[WR], strand;
+      bool in = q < n_e;
+      u32 b = 0xFFFFFFFFu;
+      if (in) {
+        make_count_record<W, WR>(s, nwords, L, k, q, rec, strand);
+        b = rec[0] >> 16;  // the 8-base bucket id (base_engine.h kNumBuckets)
+      }
+      if constexpr (MODE == kCountOwnHist) {
+        const u32 peers = __match_any_sync(0xffffffffu, b);
+        if (in && lane == (u32)__ffs(peers) - 1) atomicAdd(hist16 + b, (unsigned long long)__popc(peers));
+      } else {
+        if (in) {
+          const u32 o = __ldg(sink.owner + (b >> 8));
+          in = b >= __ldg(round_lo + o) && b <= __ldg(round_hi + o);
+        }
+        const u32 mask = __ballot_sync(0xffffffffu, in);
+        if (mask) sink.template put<WR>(in, rec, mask, lane, lt);
+      }
+    }
+  });
+}
+
+// ------------------------------------------------------------------------------------------------
 // K-count helpers (A5/A6; kmer_counter.cpp:254-381)
 // ------------------------------------------------------------------------------------------------
 template <int WR>

@@ -215,6 +215,36 @@ extern "C" int mhb_count_extract_range(void *stream, const mhb_dev_reads *reads,
   return MHB_OK;
 }
 
+// the extraction of a multi-GPU count: bucket histogram of the share (hist16 != NULL) or one round's records into
+// their owners (k_count_extract_owners)
+extern "C" int mhb_count_extract_owners(void *stream, const mhb_dev_reads *reads, uint32_t k, uint64_t *hist16,
+                                        const uint8_t *owner_of_byte, const uint64_t *owner_base, uint64_t *cursor_dev,
+                                        const uint64_t *capacity_dev, const uint32_t *round_lo, const uint32_t *round_hi) {
+  if (int rc = check_reads(reads, k)) return rc;
+  if (!hist16 && (!owner_of_byte || !owner_base || !cursor_dev || !capacity_dev || !round_lo || !round_hi))
+    return mhb_set_error(MHB_ERR_ARG, "bad args");
+  if (reads->n_reads == 0) return MHB_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  const ReadsView rv = make_reads_view(reads);
+  const u32 W = count_key_words(k), WR = count_record_words(k);
+  const int grid = (int)grid_cap(rv.n_reads, kReadsPerBatch, 8);
+  const OwnerSink sink{owner_of_byte, owner_base, (unsigned long long *)cursor_dev, capacity_dev};
+  unsigned long long *h = (unsigned long long *)hist16;
+#define M2(WW, WRR)                                                                                                         \
+  if (W == WW && WR == WRR) {                                                                                               \
+    if (hist16)                                                                                                             \
+      k_count_extract_owners<WW, WRR, kCountOwnHist><<<grid, kExtractThreads, 0, st>>>(rv, k, h, sink, round_lo, round_hi);  \
+    else                                                                                                                    \
+      k_count_extract_owners<WW, WRR, kCountOwnWrite><<<grid, kExtractThreads, 0, st>>>(rv, k, h, sink, round_lo, round_hi); \
+  } else
+#define M(WW) M2(WW, WW) M2(WW, WW + 1)
+  MHB_FOR_W(M) return mhb_set_error(MHB_ERR_ARG, "unsupported k=%u", k);
+#undef M
+#undef M2
+  CK_LAUNCH();
+  return MHB_OK;
+}
+
 // ------------------------------------------------------------------------------------------------
 // count: solid edges
 // ------------------------------------------------------------------------------------------------

@@ -85,13 +85,6 @@ int SdbgStitch::append(void *stream, const uint8_t *d_bytes, uint64_t cap_bytes,
 // aggregation (mhb_count_solid_hashed).  MHB_COUNT_MODE=sort forces the former.  Both leave the same edges / aux /
 // histogram; both clobber d_a and d_b.
 // ------------------------------------------------------------------------------------------------
-namespace {
-struct CountWork {
-  bool hashed;
-  size_t bytes;      // one work area: sort workspace + count scratch, or the hashed path's workspace
-  size_t ws_bytes;   // sort path: size of the leading sort workspace
-  int hist_byte;     // record byte whose histogram the extraction must deliver
-};
 CountWork count_work_plan(uint64_t n, uint32_t k, int32_t m) {
   static const bool force_sort = getenv("MHB_COUNT_MODE") && !strcmp(getenv("MHB_COUNT_MODE"), "sort");
   CountWork cw;
@@ -109,9 +102,10 @@ CountWork count_work_plan(uint64_t n, uint32_t k, int32_t m) {
   }
   return cw;
 }
-int run_count_stage(cudaStream_t st, const CountWork &cw, uint32_t *d_a, uint32_t *d_b, uint64_t n, uint32_t k, int32_t m,
+int run_count_stage(void *stream, const CountWork &cw, uint32_t *d_a, uint32_t *d_b, uint64_t n, uint32_t k, int32_t m,
                     const uint64_t *d_hist0, uint32_t *d_edges, uint8_t *d_aux, uint64_t cap_edges, uint64_t *d_mul_hist,
                     uint64_t *d_nsolid, char *work, double *pass_ms, uint32_t *n_passes) {
+  cudaStream_t st = (cudaStream_t)stream;
   const uint32_t WR = count_record_words(k);
   if (cw.hashed) {
     if (n_passes) *n_passes = n ? 2 : 0;
@@ -131,16 +125,13 @@ int run_count_stage(cudaStream_t st, const CountWork &cw, uint32_t *d_a, uint32_
   return mhb_count_solid(st, in_b ? d_b : d_a, n, k, m, d_edges, d_aux, cap_edges, d_mul_hist, d_nsolid, work + cw.ws_bytes,
                          cw.bytes - cw.ws_bytes);
 }
-}  // namespace
 
-namespace {
 // bytes of device memory one round of `n` records needs besides the read library
 size_t round_bytes(uint64_t n, uint32_t WR, uint32_t WE, int32_t m, uint32_t k) {
   const uint64_t cap_edges = n / (uint64_t)std::max(1, m) + 1;
   return 2 * pad256((size_t)n * WR * 4 + 16) + pad256(count_work_plan(n, k, m).bytes) +
          pad256((size_t)cap_edges * WE * 4) + pad256(cap_edges);
 }
-}  // namespace
 
 // ================================================================================================
 // count (A13): one round over all records, or rounds over ranges of bucket ids
@@ -249,6 +240,8 @@ extern "C" int mhb_plan_rounds16(const uint64_t *hist256, const uint64_t *sub_hi
   mhb_set_error(MHB_ERR_NOMEM, "round plan needs more than %u ranges", cap_out);
   return -1;
 }
+
+uint64_t count_round_limit() { return g_round_limit; }
 
 extern "C" int mhb_set_round_limit(uint64_t max_records_per_round) {
   g_round_limit = max_records_per_round;

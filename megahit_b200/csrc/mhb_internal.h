@@ -79,6 +79,28 @@ uint64_t largest_round(uint64_t n_max, size_t fixed, size_t avail, F bytes) {
   return lo;
 }
 
+// ---- the count stage (mhb_host.cu), shared by the single-GPU rounds and the owners of a multi-GPU count ----
+// Its work area for n records: either the LSD sort on every key byte followed by the run-length count, or - 8-byte
+// records, the default where available - two partition passes + per-bucket hash aggregation (mhb_count_solid_hashed).
+// MHB_COUNT_MODE=sort forces the former.
+struct CountWork {
+  bool hashed;
+  size_t bytes;      // one work area: sort workspace + count scratch, or the hashed path's workspace
+  size_t ws_bytes;   // sort path: size of the leading sort workspace
+  int hist_byte;     // record byte whose histogram the extraction must deliver
+};
+CountWork count_work_plan(uint64_t n, uint32_t k, int32_t m);
+// The count stage on the n records in d_a (d_b: a buffer of the same size; both clobbered): solid edges and flags into
+// d_edges / d_aux (cap_edges), the multiplicity histogram added to d_mul_hist, the number of solid edges to *d_nsolid.
+// d_hist0: the histogram of record byte cw.hist_byte, or NULL.  pass_ms / n_passes (may be NULL): per-pass timings.
+int run_count_stage(void *stream, const CountWork &cw, uint32_t *d_a, uint32_t *d_b, uint64_t n, uint32_t k, int32_t m,
+                    const uint64_t *d_hist0, uint32_t *d_edges, uint8_t *d_aux, uint64_t cap_edges, uint64_t *d_mul_hist,
+                    uint64_t *d_nsolid, char *work, double *pass_ms, uint32_t *n_passes);
+// bytes of device memory one count round of n records needs: two record buffers, the work area, edges and flags
+size_t round_bytes(uint64_t n, uint32_t WR, uint32_t WE, int32_t m, uint32_t k);
+// the cap on the records of one count round (mhb_set_round_limit), 0 = none
+uint64_t count_round_limit();
+
 // mhb_sort_records + optional per-pass timings (host array of n_bytes doubles, ms; forces a stream sync)
 int mhb_sort_records_impl(void *stream, uint32_t *a, uint32_t *b, uint64_t n, uint32_t words, const uint8_t *bytes,
                           uint32_t n_bytes, const uint64_t *first_hist, void *ws, size_t ws_bytes, int *result_in_b,

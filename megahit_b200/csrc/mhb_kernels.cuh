@@ -228,6 +228,31 @@ __device__ __forceinline__ u32 lanemask_lt() {
   return m;
 }
 
+// Where the extraction kernels of the multi-GPU stages put a warp's records (in = this lane holds one, mask = the ballot
+// of `in`, lt = lanemask_lt; every lane of the warp calls put).  OwnerSink: record -> rank owner[leading record byte],
+// stored at base[owner] + cursor[owner] (base[o] = this rank's segment of owner o's receive buffer, which may be another
+// process's memory opened through CUDA IPC; the cursors are this rank's).  The lanes of a warp are grouped by owner;
+// one atomic per group, each lane stores at the group's base plus its rank in the group.  Records beyond
+// capacity[owner] are counted but not stored.
+struct OwnerSink {
+  const uint8_t *owner;  // 256 entries
+  const u64 *base;       // device addresses, one per owner
+  unsigned long long *cursor;
+  const u64 *capacity;
+  template <int W>
+  __device__ __forceinline__ void put(bool in, const u32 (&rec)[W], u32, u32 lane, u32 lt) const {
+    const u32 o = in ? (u32)__ldg(owner + (rec[0] >> 24)) : 0xFFFFFFFFu;
+    const u32 peers = __match_any_sync(0xffffffffu, o);
+    if (!in) return;
+    const u32 leader = (u32)__ffs(peers) - 1;
+    unsigned long long at = 0;
+    if (lane == leader) at = atomicAdd(cursor + o, (unsigned long long)__popc(peers));
+    at = __shfl_sync(peers, at, leader);
+    const u64 pos = at + __popc(peers & lt);
+    if (pos < capacity[o]) st_rec<W>(reinterpret_cast<u32 *>(base[o]), pos, rec);
+  }
+};
+
 // ------------------------------------------------------------------------------------------------
 // mbarrier + bulk async copy (TMA 1-D: cp.async.bulk, SASS UBLKCP)
 // ------------------------------------------------------------------------------------------------

@@ -1,14 +1,17 @@
 // mhb_mgpu.cpp -- `count` on several GPUs of one node behind the file-level C ABI (mhb_count_run_multi, include/mhb.h).
 //
 // One worker PROCESS per GPU (forked before CUDA is touched; libmhb keeps per-process state: arena, kernel attributes),
-// the same pipeline as megahit_b200/multigpu.py but with no Python, torch or NCCL underneath:
-//   * records travel GPU -> GPU inside the fused partition + exchange kernel (mhb_partition_scatter storing into the
-//     owners' receive buffers, opened through CUDA IPC);
-//   * the small collectives (256-bin histograms, counters, IPC handles) go through one MAP_SHARED control block with a
-//     process-shared barrier; the medium ones (tip edges, candidate reads, answer planes of the mercy searches, the
-//     per-bucket tables) through files in /dev/shm written by one rank and read by the others;
-//   * the plan of a stage (owner ranges from the all-gathered histograms) is computed by every rank from the same data
-//     (plan_partition_host = the rule of k_plan_partition / multigpu.plan_ranges).
+// with no Python, torch or NCCL underneath.  The reads, fixed- or variable-length, are dealt in contiguous shares
+// balanced on bases:
+//   * the count records are extracted straight into the receive buffers of the ranks owning their leading byte
+//     (mhb_count_extract_owners, opened through CUDA IPC), in rounds over ascending bucket sub-ranges when an owner
+//     cannot take all its records at once; the SdBG items travel inside the fused partition + exchange kernel
+//     (mhb_partition_scatter);
+//   * the small collectives (256-bin histograms, counters, budgets, IPC handles) go through one MAP_SHARED control
+//     block with a process-shared barrier; the medium ones (bucket histograms, tip edges, candidate reads, answer planes
+//     of the mercy searches, the per-bucket tables) through files in /dev/shm written by one rank and read by the others;
+//   * the plan of a stage (owner ranges and rounds from the all-gathered histograms) is computed by every rank from the
+//     same data (plan_partition_host = the rule of k_plan_partition / multigpu.plan_ranges; plan_count_rounds).
 // The mercy searches are answered by the owners of the searched prefixes (mhb_mercy_probe_owned); the k_min SdBG is
 // built in the same run because the solid edges are already on the devices.
 //
@@ -66,6 +69,7 @@ struct Control {
   uint64_t sdbg_totals[kMaxRanks][16];
   uint64_t has_tips[kMaxRanks];
   uint64_t n_edges[kMaxRanks], n_aligned[kMaxRanks];  // iterate
+  uint64_t budget[kMaxRanks];                          // count: the most records each owner takes in one round
   int err_code[kMaxRanks];  // MHB_ERR_* of a failed rank
 };
 
@@ -276,9 +280,9 @@ void close_peers(Exchange &X, PeerBuf *pb) {
 struct Job {
   uint32_t k;
   int32_t m;
-  const uint32_t *bin;  // whole library (host, inherited by the workers)
-  uint64_t n_reads;
-  uint32_t read_len;
+  const uint32_t *bin;          // whole library (host, inherited by the workers)
+  const ReadLibIndex *ix;       // its index for k, made before the fork
+  std::vector<uint64_t> first;  // read shares
   std::string prefix;
 };
 
@@ -358,88 +362,258 @@ std::vector<int64_t> sum_mul(Exchange &X) {
 // ================================================================================================
 // one worker = one GPU
 // ================================================================================================
+// The owner ranges of a multi-GPU count and its rounds over bucket ranges (mhb_plan_count_owner_rounds), computed by
+// every rank from the same all-gathered 65536-bin histograms.
+struct CountPlan {
+  Plan P;                         // owner byte ranges (P.bounds, P.owner)
+  int R = 1;                      // rounds
+  std::vector<uint32_t> lo, hi;   // [R][world]: owner o's bucket range in round t (lo > hi: empty)
+  std::vector<uint64_t> n, off;   // [R][world owner][world rank]: records rank s sends to o in round t, and where
+                                  // they start in o's receive buffer
+};
+// h16[s]: rank s's histogram; cap[o]: the most records owner o takes in one round (UINT64_MAX: no cap).  Each owner's
+// range is cut greedily into ascending sub-ranges of whole leading bytes, and of bucket ids inside a leading byte that
+// alone exceeds the cap (the rule of mhb_plan_rounds16).  MHB_ERR_NOMEM (message set) when one bucket exceeds a cap.
+int plan_count_rounds(const uint64_t *const *h16, int world, const uint64_t *cap, CountPlan *cp) {
+  std::vector<uint64_t> tot(65536, 0), pre((size_t)world * 65537, 0);  // pre[s][b] = rank s's records below bucket b
+  for (int s = 0; s < world; ++s)
+    for (uint32_t b = 0; b < 65536; ++b) {
+      tot[b] += h16[s][b];
+      pre[(size_t)s * 65537 + b + 1] = pre[(size_t)s * 65537 + b] + h16[s][b];
+    }
+  uint64_t h256[kMaxRanks][256] = {{0}};  // everything in rank 0's row: only the totals decide the owner ranges
+  for (uint32_t b = 0; b < 65536; ++b) h256[0][b >> 8] += tot[b];
+  cp->P = plan_partition_host(h256, world, 0);
+  std::vector<std::vector<std::pair<uint32_t, uint32_t>>> sub(world);
+  for (int o = 0; o < world; ++o) {
+    uint32_t lo = cp->P.bounds[o] << 8;
+    uint64_t acc = 0;
+    auto atom = [&](uint32_t a, uint64_t cnt) -> int {  // the next atom starts at bucket a and holds cnt records
+      if (cnt > cap[o])
+        return mhb_set_error(MHB_ERR_NOMEM, "bucket 0x%04x alone holds %llu records, more than one round of rank %d can "
+                             "take (%llu)", a, (unsigned long long)cnt, o, (unsigned long long)cap[o]);
+      if (acc + cnt > cap[o]) {  // acc > 0 here: close the open sub-range before this atom
+        sub[o].push_back({lo, a - 1});
+        lo = a;
+        acc = 0;
+      }
+      acc += cnt;
+      return MHB_OK;
+    };
+    for (uint32_t B = cp->P.bounds[o]; B < cp->P.bounds[o + 1]; ++B) {
+      uint64_t bt = 0;
+      for (uint32_t c = 0; c < 256; ++c) bt += tot[(B << 8) | c];
+      if (bt <= cap[o]) {
+        CKR(atom(B << 8, bt));
+      } else {
+        for (uint32_t c = 0; c < 256; ++c) CKR(atom((B << 8) | c, tot[(B << 8) | c]));
+      }
+    }
+    sub[o].push_back({lo, (cp->P.bounds[o + 1] << 8) - 1});
+  }
+  cp->R = 1;
+  for (int o = 0; o < world; ++o) cp->R = std::max(cp->R, (int)sub[o].size());
+  const size_t RW = (size_t)cp->R * world;
+  cp->lo.assign(RW, 1);
+  cp->hi.assign(RW, 0);
+  cp->n.assign(RW * world, 0);
+  cp->off.assign(RW * world, 0);
+  for (int t = 0; t < cp->R; ++t)
+    for (int o = 0; o < world; ++o) {
+      if (t >= (int)sub[o].size()) continue;  // empty range: nothing for o in this round
+      const uint32_t a = sub[o][t].first, b = sub[o][t].second;
+      cp->lo[(size_t)t * world + o] = a;
+      cp->hi[(size_t)t * world + o] = b;
+      uint64_t at = 0;
+      for (int s = 0; s < world; ++s) {
+        const size_t i = ((size_t)t * world + o) * world + s;
+        cp->n[i] = pre[(size_t)s * 65537 + b + 1] - pre[(size_t)s * 65537 + a];
+        cp->off[i] = at;
+        at += cp->n[i];
+      }
+    }
+  return MHB_OK;
+}
+
+// the records owner o receives in round t
+uint64_t round_total(const CountPlan &cp, int world, int t, int o) {
+  uint64_t s = 0;
+  for (int q = 0; q < world; ++q) s += cp.n[((size_t)t * world + o) * world + q];
+  return s;
+}
+
+// The most count records this rank may take in one round: the largest round (round_bytes, as the single-GPU count
+// plans it) that fits its part of the device's free memory - the ranks bound to one device split it evenly - capped by
+// mhb_set_round_limit.  Called by every rank between two barriers, when every share is on its device.
+uint64_t count_round_budget(int rank, int world, uint64_t n_total, uint32_t k, int32_t m) {
+  int n_dev = 1, sharers = 0;
+  CKC(cudaGetDeviceCount(&n_dev));
+  for (int q = 0; q < world; ++q) sharers += q % n_dev == rank % n_dev;
+  const size_t avail = (size_t)(0.92 * (double)free_device_bytes()) / (size_t)std::max(1, sharers);
+  const size_t fixed = (size_t)64 << 20;  // round arrays, counters, the exchange's small tables
+  const uint32_t WR = mhb_count_record_words(k), WE = mhb_words_per_edge(k);
+  uint64_t cap = largest_round(std::max<uint64_t>(n_total, 1), fixed, avail,
+                               [&](uint64_t n) { return round_bytes(n, WR, WE, m, k); });
+  if (!cap) fail_nomem("%zu free bytes for this rank: not even one count record fits", avail);
+  if (count_round_limit()) cap = std::min(cap, count_round_limit());
+  return cap;
+}
+
 void worker(const Job &J, Exchange &X) {
   Control *C = X.C;
   const int W = X.world, r = X.rank;
-  const uint32_t k = J.k, L = J.read_len;
+  const uint32_t k = J.k;
   const int32_t m = J.m;
   bind_device(r, W);
   const uint32_t WR = mhb_count_record_words(k), WE = mhb_words_per_edge(k), W2 = mhb_s2s_record_words(k);
-  const uint32_t stride = 1 + div_ceil(L, 16);
-  const uint64_t per = (J.n_reads + W - 1) / W;
-  const uint64_t r0 = std::min<uint64_t>(J.n_reads, (uint64_t)r * per), r1 = std::min<uint64_t>(J.n_reads, r0 + per);
-  const uint64_t nr = r1 - r0;                                    // my block of reads
-  const uint64_t n = L >= k + 1 ? nr * (uint64_t)(L - k) : 0;     // my edge records
-  const uint32_t *my_bin = J.bin + r0 * stride;
-  uint8_t cbytes[72];
-  const uint32_t n_csort = mhb_count_sort_bytes(k, cbytes);
-  const int top = (int)(4 * WR - 1), top2 = (int)(4 * W2 - 1);
+  const int top2 = (int)(4 * W2 - 1);
+  const ReadLibIndex &ix = *J.ix;
+  const uint64_t r0 = J.first[r], nr = J.first[r + 1] - r0;  // my share of the reads
+  const uint64_t w0 = ix.word_of(r0), nw = ix.word_of(r0 + nr) - w0;
+  const uint32_t *my_bin = J.bin + w0;
+  auto read_at = [&](uint64_t i) { return my_bin + (ix.word_of(r0 + i) - w0); };  // my read i, at its length word
 
-  // ---- reads to the device, extraction ----
-  DevBuf bin, recs, hist, ws;  // recs and ws: the records of an exchange and its workspace, once per stage
-  CKL(bin.alloc((nr * stride + 16) * 4, "count: reads"));
-  if (nr) CKC(cudaMemcpy(bin.p, my_bin, nr * stride * 4, cudaMemcpyHostToDevice));
+  // ---- my share to the device: the image slice and, for variable-length reads, its rebased offsets ----
+  DevBuf bin, roff, eoff;
+  CKL(bin.alloc((nw + 16) * 4, "count: reads"));
+  if (nw) CKC(cudaMemcpy(bin.p, my_bin, nw * 4, cudaMemcpyHostToDevice));
   mhb_dev_reads reads;
+  memset(&reads, 0, sizeof(reads));
   reads.bin = bin.as<uint32_t>();
-  reads.bin_words = nr * stride;
+  reads.bin_words = nw;
   reads.n_reads = nr;
-  reads.fixed_len = L;
-  reads.rec_off = nullptr;
-  reads.edge_off = nullptr;
-  CKL(recs.alloc((n * WR + 16) * 4, "count: edge records"));
-  CKL(hist.alloc(256 * 8, "count: leading-byte histogram"));
-  uint64_t *d_hist = hist.as<uint64_t>();
-  CKC(cudaMemset(d_hist, 0, 256 * 8));
-  CKL(mhb_count_extract(nullptr, &reads, k, recs.as<uint32_t>(), n, d_hist, top));
-  size_t ws_bytes = mhb_sort_workspace_bytes(std::max<uint64_t>(n, 1), WR);
-  CKL(ws.alloc(ws_bytes, "count: partition workspace"));
-  PeerBuf pc;
-  const Plan P = partition_and_exchange(X, 0, recs.as<uint32_t>(), n, WR, top, d_hist, ws.p, ws_bytes, &pc,
-                                        "count: edge records received");
-  recs.release();
-  ws.release();
-  const uint64_t n_own = P.recv_tot[r];
-  C->n_records[r] = n_own;
+  reads.fixed_len = ix.fixed_len;
+  if (!ix.fixed_len) {
+    std::vector<uint64_t> ro(nr + 1), eo(nr + 1);
+    for (uint64_t i = 0; i <= nr; ++i) {
+      ro[i] = ix.rec_off[r0 + i] - w0;
+      eo[i] = ix.unit_off[r0 + i] - ix.unit_off[r0];
+    }
+    CKL(roff.alloc((nr + 1) * 8, "count: read offsets"));
+    CKL(eoff.alloc((nr + 1) * 8, "count: edge offsets"));
+    CKC(cudaMemcpy(roff.p, ro.data(), (nr + 1) * 8, cudaMemcpyHostToDevice));
+    CKC(cudaMemcpy(eoff.p, eo.data(), (nr + 1) * 8, cudaMemcpyHostToDevice));
+    reads.rec_off = roff.as<uint64_t>();
+    reads.edge_off = eoff.as<uint64_t>();
+  }
 
-  // ---- count stage on the owned records ----
-  const uint64_t cap = n_own / (uint64_t)std::max(1, m) + 1;
-  DevBuf edges, aux, mul, ns;
-  CKL(edges.alloc((cap * WE + 16) * 4, "count: solid edges"));
-  CKL(aux.alloc(cap + 16, "count: edge flags"));
+  // ---- bucket histogram of my records -> every rank's round budget -> the same owner and round plan everywhere ----
+  DevBuf h16, mul, ns, hist;
   CKL(mul.alloc(65536 * 8, "count: multiplicity histogram"));
   CKL(ns.alloc(8 * 8, "count: counters"));
-  uint32_t *d_edges = edges.as<uint32_t>();
-  uint8_t *d_aux = aux.as<uint8_t>();
-  uint64_t *d_ns = ns.as<uint64_t>();
+  CKL(hist.alloc(256 * 8, "count: leading-byte histogram"));
+  uint64_t *d_ns = ns.as<uint64_t>(), *d_hist = hist.as<uint64_t>();
   CKC(cudaMemset(mul.p, 0, 65536 * 8));
   CKC(cudaMemset(d_ns, 0, 64));
   {
-    DevBuf tmp;
-    CKL(tmp.alloc((n_own * WR + 16) * 4, "count: sort buffer"));
-    uint32_t *d_own = pc.mine.as<uint32_t>(), *d_tmp = tmp.as<uint32_t>();
-    if (mhb_count_hashed_supported(k, m) && !(getenv("MHB_COUNT_MODE") && !strcmp(getenv("MHB_COUNT_MODE"), "sort"))) {
-      const size_t hb = mhb_count_hashed_workspace_bytes(std::max<uint64_t>(n_own, 1), k, m);
-      DevBuf h;
-      CKL(h.alloc(hb, "count: hash-count workspace"));
-      CKL(mhb_count_solid_hashed(nullptr, d_own, d_tmp, n_own, k, m, nullptr, d_edges, d_aux, cap, mul.as<uint64_t>(), d_ns,
-                                 h.p, hb));
-      CKC(cudaDeviceSynchronize());
-    } else {
-      const size_t sb = mhb_sort_workspace_bytes(std::max<uint64_t>(n_own, 1), WR), cb = mhb_count_solid_scratch_bytes(n_own);
-      DevBuf s, c;
-      CKL(s.alloc(sb, "count: sort workspace"));
-      CKL(c.alloc(cb, "count: count scratch"));
-      int in_b = 0;
-      CKL(mhb_sort_records_relaxed(nullptr, d_own, d_tmp, n_own, WR, cbytes, n_csort, nullptr, s.p, sb, &in_b));
-      CKL(mhb_count_solid(nullptr, in_b ? d_tmp : d_own, n_own, k, m, d_edges, d_aux, cap, mul.as<uint64_t>(), d_ns, c.p, cb));
-      CKC(cudaDeviceSynchronize());
+    std::vector<uint64_t> h(65536);
+    CKL(h16.alloc(65536 * 8, "count: bucket histogram"));
+    CKC(cudaMemset(h16.p, 0, 65536 * 8));
+    CKL(mhb_count_extract_owners(nullptr, &reads, k, h16.as<uint64_t>(), nullptr, nullptr, nullptr, nullptr, nullptr, nullptr));
+    CKC(cudaMemcpy(h.data(), h16.p, 65536 * 8, cudaMemcpyDeviceToHost));
+    h16.release();
+    X.publish("h16", h.data(), 65536 * 8);
+  }
+  X.barrier();  // every share is on its device: the free memory left is what the rounds may take
+  C->budget[r] = count_round_budget(r, W, ix.n_units, k, m);
+  X.barrier();
+  CountPlan cp;
+  {
+    std::vector<std::vector<char>> hs(W);
+    std::vector<const uint64_t *> hp(W);
+    for (int s = 0; s < W; ++s) {
+      hs[s] = X.fetch("h16", s);
+      hp[s] = (const uint64_t *)hs[s].data();
+    }
+    CKL(plan_count_rounds(hp.data(), W, C->budget, &cp));
+  }
+  const Plan &P = cp.P;
+  const int R = cp.R;
+  uint64_t n_own = 0, n_round_max = 0, n_sent = 0;
+  for (int t = 0; t < R; ++t) {
+    const uint64_t a = round_total(cp, W, t, r);
+    n_own += a;
+    n_round_max = std::max(n_round_max, a);
+    for (int o = 0; o < W; ++o) n_sent += cp.n[((size_t)t * W + o) * W + r];
+  }
+  C->n_records[r] = n_own;
+  if (r == 0) XINFO("count plan: %d round%s over bucket ranges\n", R, R > 1 ? "s" : "");
+
+  // ---- rounds: my records of the round straight into their owners, then every owner counts what it received ----
+  const uint64_t cap = n_round_max / (uint64_t)std::max(1, m) + 1;
+  DevBuf edges, aux;
+  CKL(edges.alloc((cap * WE + 16) * 4, "count: solid edges"));
+  CKL(aux.alloc(cap + 16, "count: edge flags"));
+  uint64_t n_solid = 0;
+  std::vector<uint32_t> edges_h;  // the edges and flags of every round, on the host, when there are several rounds
+  std::vector<uint8_t> aux_h;
+  {
+    PeerBuf pc;
+    open_peers(X, 0, n_round_max * WR * 4 + 256, &pc, "count: edge records received");
+    DevBuf tmp, work, lut, dbase, cursor, dcap, rlo, rhi;
+    CKL(tmp.alloc((n_round_max * WR + 16) * 4, "count: sort buffer"));
+    const CountWork cw = count_work_plan(std::max<uint64_t>(n_round_max, 1), k, m);
+    CKL(work.alloc(cw.bytes, "count: count work area"));
+    CKL(lut.alloc(256, "count: owner of each byte"));
+    CKL(dbase.alloc(kMaxRanks * 8, "count: owner addresses"));
+    CKL(cursor.alloc(kMaxRanks * 8, "count: owner cursors"));
+    CKL(dcap.alloc(kMaxRanks * 8, "count: owner capacities"));
+    CKL(rlo.alloc(kMaxRanks * 4, "count: round ranges"));
+    CKL(rhi.alloc(kMaxRanks * 4, "count: round ranges"));
+    CKC(cudaMemcpy(lut.p, P.owner, 256, cudaMemcpyHostToDevice));
+    for (int t = 0; t < R; ++t) {
+      uint64_t base[kMaxRanks], want[kMaxRanks], sent[kMaxRanks];
+      for (int o = 0; o < W; ++o) {
+        const size_t i = ((size_t)t * W + o) * W + r;
+        base[o] = (uint64_t)(uintptr_t)pc.peer[o] + cp.off[i] * (uint64_t)WR * 4;
+        want[o] = cp.n[i];
+      }
+      CKC(cudaMemcpy(dbase.p, base, W * 8, cudaMemcpyHostToDevice));
+      CKC(cudaMemcpy(dcap.p, want, W * 8, cudaMemcpyHostToDevice));
+      CKC(cudaMemcpy(rlo.p, &cp.lo[(size_t)t * W], W * 4, cudaMemcpyHostToDevice));
+      CKC(cudaMemcpy(rhi.p, &cp.hi[(size_t)t * W], W * 4, cudaMemcpyHostToDevice));
+      CKC(cudaMemset(cursor.p, 0, kMaxRanks * 8));
+      CKL(mhb_count_extract_owners(nullptr, &reads, k, nullptr, lut.as<uint8_t>(), dbase.as<uint64_t>(), cursor.as<uint64_t>(),
+                                   dcap.as<uint64_t>(), rlo.as<uint32_t>(), rhi.as<uint32_t>()));
+      CKC(cudaMemcpy(sent, cursor.p, W * 8, cudaMemcpyDeviceToHost));
+      check_sent(sent, want, W, "count records");
+      X.barrier();  // every rank's stores of the round have completed: my receive buffer is complete
+
+      const uint64_t n_t = round_total(cp, W, t, r);
+      uint64_t s_t = 0;
+      if (n_t) {
+        CKC(cudaMemset(d_ns, 0, 8));
+        CKL(run_count_stage(nullptr, cw, pc.mine.as<uint32_t>(), tmp.as<uint32_t>(), n_t, k, m, nullptr, edges.as<uint32_t>(),
+                            aux.as<uint8_t>(), cap, mul.as<uint64_t>(), d_ns, work.as<char>(), nullptr, nullptr));
+        CKC(cudaMemcpy(&s_t, d_ns, 8, cudaMemcpyDeviceToHost));
+        if (s_t > cap) fail("internal: solid edges exceed capacity");
+      }
+      if (R > 1 && s_t) {  // the round's edges follow those of the lower bucket ranges (count_host_rounds)
+        edges_h.resize((n_solid + s_t) * WE);
+        aux_h.resize(n_solid + s_t);
+        CKC(cudaMemcpy(edges_h.data() + n_solid * WE, edges.p, s_t * WE * 4, cudaMemcpyDeviceToHost));
+        CKC(cudaMemcpy(aux_h.data() + n_solid, aux.p, s_t, cudaMemcpyDeviceToHost));
+      }
+      n_solid += s_t;
+      X.barrier();  // nobody stores into my receive buffer before I have counted it
+    }
+    close_peers(X, &pc);  // the count records are gone: give the memory back before the mercy and SdBG stages
+  }
+  uint64_t cap_all = cap;  // edges the device arrays hold
+  if (R > 1) {  // exactly my n_solid edges and flags back to the device
+    edges.release();
+    aux.release();
+    cap_all = n_solid;
+    CKL(edges.alloc((n_solid * WE + 16) * 4, "count: solid edges"));
+    CKL(aux.alloc(n_solid + 16, "count: edge flags"));
+    if (n_solid) {
+      CKC(cudaMemcpy(edges.p, edges_h.data(), n_solid * WE * 4, cudaMemcpyHostToDevice));
+      CKC(cudaMemcpy(aux.p, aux_h.data(), n_solid, cudaMemcpyHostToDevice));
     }
   }
-  uint64_t n_solid = 0;
-  CKC(cudaMemcpy(&n_solid, d_ns, 8, cudaMemcpyDeviceToHost));
-  if (n_solid > cap) fail("internal: solid edges exceed capacity");
+  uint32_t *d_edges = edges.as<uint32_t>();
+  uint8_t *d_aux = aux.as<uint8_t>();
   C->n_solid[r] = n_solid;
-  close_peers(X, &pc);  // the count records are gone: give the memory back before the SdBG stage
   {
     std::vector<uint64_t> h(65536);
     CKC(cudaMemcpy(h.data(), mul.p, 65536 * 8, cudaMemcpyDeviceToHost));
@@ -502,7 +676,8 @@ void worker(const Job &J, Exchange &X) {
   C->n_cand[r] = n_cand;
   std::vector<uint64_t> cand_ids(n_cand);
   if (n_cand) CKC(cudaMemcpy(cand_ids.data(), d_cand, n_cand * 8, cudaMemcpyDeviceToHost));
-  {  // number of reads with both marks set (the "(%d)" of the reference's log line) + my candidate reads, file orientation
+  {  // number of reads with both marks set (the "(%d)" of the reference's log line) + my candidate reads as their
+     // image words (length word + payload)
     std::vector<uint32_t> f(nr), l(nr);
     if (nr) {
       CKC(cudaMemcpy(f.data(), first.p, nr * 4, cudaMemcpyDeviceToHost));
@@ -511,8 +686,11 @@ void worker(const Job &J, Exchange &X) {
     uint64_t ht = 0;
     for (uint64_t i = 0; i < nr; ++i) ht += f[i] != MHB_SENTINEL_OFFSET && l[i] != MHB_SENTINEL_OFFSET;
     C->has_tips[r] = ht;
-    std::vector<uint32_t> cr(n_cand * stride);
-    for (uint64_t c = 0; c < n_cand; ++c) memcpy(cr.data() + c * stride, my_bin + cand_ids[c] * stride, stride * 4);
+    std::vector<uint32_t> cr;
+    for (uint64_t c = 0; c < n_cand; ++c) {
+      const uint32_t *rd = read_at(cand_ids[c]);
+      cr.insert(cr.end(), rd, rd + 1 + div_ceil(rd[0], 16));
+    }
     X.publish("cand", cr.data(), cr.size() * 4);
   }
   X.barrier();
@@ -527,20 +705,36 @@ void worker(const Job &J, Exchange &X) {
   uint32_t *d_all_edges = d_edges;  // solid + mercy edges, the sequences of the SdBG stage
   DevBuf big;                       // ... when the mercy edges do not fit behind the solid ones in d_edges
   if (n_cand_all) {
-    std::vector<uint32_t> all(n_cand_all * stride + 4);
+    // the candidates of every rank, in rank order, indexed as a library of their own; the longest of them sizes the
+    // answer planes on every rank alike
+    std::vector<uint32_t> all;
     for (int o = 0; o < W; ++o)
       if (C->n_cand[o]) {
         const std::vector<char> v = X.fetch("cand", o);
-        memcpy(all.data() + cand_off[o] * stride, v.data(), v.size());
+        all.insert(all.end(), (const uint32_t *)v.data(), (const uint32_t *)(v.data() + v.size()));
       }
+    ReadLibIndex cix;
+    CKL(index_read_lib(all.data(), all.size(), n_cand_all, k, &cix, FixedCheck::kSerial));
+    uint32_t L = 0;
+    for (uint64_t c = 0; c < n_cand_all; ++c) L = std::max(L, all[cix.word_of(c)]);
     {
-      DevBuf call, lut, planes;
-      CKL(call.alloc((n_cand_all * stride + 16) * 4, "count: candidate reads of every rank"));
-      CKC(cudaMemcpy(call.p, all.data(), n_cand_all * stride * 4, cudaMemcpyHostToDevice));
-      mhb_dev_reads greads = reads;
+      DevBuf call, croff, ceoff, lut, planes;
+      CKL(call.alloc((all.size() + 16) * 4, "count: candidate reads of every rank"));
+      CKC(cudaMemcpy(call.p, all.data(), all.size() * 4, cudaMemcpyHostToDevice));
+      mhb_dev_reads greads;
+      memset(&greads, 0, sizeof(greads));
       greads.bin = call.as<uint32_t>();
-      greads.bin_words = n_cand_all * stride;
+      greads.bin_words = all.size();
       greads.n_reads = n_cand_all;
+      greads.fixed_len = cix.fixed_len;
+      if (!cix.fixed_len) {
+        CKL(croff.alloc((n_cand_all + 1) * 8, "count: candidate read offsets"));
+        CKL(ceoff.alloc((n_cand_all + 1) * 8, "count: candidate edge offsets"));
+        CKC(cudaMemcpy(croff.p, cix.rec_off.data(), (n_cand_all + 1) * 8, cudaMemcpyHostToDevice));
+        CKC(cudaMemcpy(ceoff.p, cix.unit_off.data(), (n_cand_all + 1) * 8, cudaMemcpyHostToDevice));
+        greads.rec_off = croff.as<uint64_t>();
+        greads.edge_off = ceoff.as<uint64_t>();
+      }
       CKL(lut.alloc(mhb_edge_lut_bytes(), "count: edge lookup table"));
       CKL(mhb_edge_lut_build(nullptr, d_edges, n_solid, k, lut.p));
       const size_t pw_all = mhb_mercy_planes_words(n_cand_all, L);
@@ -568,7 +762,7 @@ void worker(const Job &J, Exchange &X) {
       CKL(mhb_mercy_count_planes(nullptr, &reads, d_cand, n_cand, L, k, d_mine.as<uint32_t>(), (uint32_t)W, pw_mine, &n_mercy,
                                  ms.p, msb));
       if (n_mercy) {
-        if (n_solid + n_mercy > cap) {  // reads overlapping only at their ends: more mercy than solid edges
+        if (n_solid + n_mercy > cap_all) {  // reads overlapping only at their ends: more mercy than solid edges
           CKL(big.alloc(((n_solid + n_mercy) * WE + 16) * 4, "count: solid and mercy edges"));
           CKC(cudaMemcpy(big.p, d_edges, n_solid * WE * 4, cudaMemcpyDeviceToDevice));
           d_all_edges = big.as<uint32_t>();
@@ -592,6 +786,7 @@ void worker(const Job &J, Exchange &X) {
   seqs.n_seqs = n_seqs;
   seqs.fixed_len = k + 1;
   seqs.fixed_stride = WE;
+  DevBuf recs, ws;
   CKL(recs.alloc((n_items * W2 + 16) * 4, "count: SdBG items"));
   CKC(cudaMemset(d_hist, 0, 256 * 8));
   if (getenv("MHB_S2S_NO_PRUNE")) {
@@ -607,7 +802,7 @@ void worker(const Job &J, Exchange &X) {
     if (kept > n_items) fail("internal: pruned item count exceeds 6 per edge");
     n_items = kept;
   }
-  ws_bytes = mhb_sort_workspace_bytes(std::max<uint64_t>(n_items, 1), W2);
+  const size_t ws_bytes = mhb_sort_workspace_bytes(std::max<uint64_t>(n_items, 1), W2);
   CKL(ws.alloc(ws_bytes, "count: partition workspace"));
   PeerBuf ps;
   const Plan P2 = partition_and_exchange(X, 1, recs.as<uint32_t>(), n_items, W2, top2, d_hist, ws.p, ws_bytes, &ps,
@@ -615,17 +810,22 @@ void worker(const Job &J, Exchange &X) {
   recs.release();
   ws.release();
   sdbg_owner_stage(X, &ps, P2.recv_tot[r], k, J.prefix);
+  XINFO("rank %d: %llu reads, %llu records sent, %llu owned in %d round%s, %llu solid edges; peak device memory %.1f MiB\n",
+        r, (unsigned long long)nr, (unsigned long long)n_sent, (unsigned long long)n_own, R, R > 1 ? "s" : "",
+        (unsigned long long)n_solid, DevBuf::peak_bytes() / 1048576.0);
 
   // ---- files: my bucket range of the edges; the tables go to rank 0 ----
-  std::vector<uint32_t> edges_h(n_solid * WE);
-  if (n_solid) CKC(cudaMemcpy(edges_h.data(), d_edges, n_solid * WE * 4, cudaMemcpyDeviceToHost));
-  CKL(write_bytes(J.prefix + ".edges." + std::to_string(r), edges_h.data(), edges_h.size() * 4));
+  if (R == 1) {
+    edges_h.resize(n_solid * WE);
+    if (n_solid) CKC(cudaMemcpy(edges_h.data(), d_edges, n_solid * WE * 4, cudaMemcpyDeviceToHost));
+  }
+  CKL(write_bytes(J.prefix + ".edges." + std::to_string(r), edges_h.data(), n_solid * WE * 4));
   {
     std::vector<int64_t> cnt(65536, 0);
     for (uint64_t i = 0; i < n_solid; ++i) cnt[edges_h[i * WE] >> 16]++;
     X.publish("ecnt", cnt.data(), 65536 * 8);
     std::vector<uint32_t> rec;
-    for (uint64_t c = 0; c < n_cand; ++c) append_cand_reversed(my_bin + cand_ids[c] * stride, &rec);
+    for (uint64_t c = 0; c < n_cand; ++c) append_cand_reversed(read_at(cand_ids[c]), &rec);
     X.publish("candrev", rec.data(), rec.size() * 4);
   }
   X.barrier();
@@ -662,7 +862,7 @@ void worker(const Job &J, Exchange &X) {
     sdbg_merge_info(X, k, J.prefix);  // merged P.sdbg_info
   }
   X.barrier();
-  for (const char *t : {"mul", "tips", "cand", "planes", "ecnt", "stab", "candrev"}) X.cleanup(t);
+  for (const char *t : {"h16", "mul", "tips", "cand", "planes", "ecnt", "stab", "candrev"}) X.cleanup(t);
 }
 
 
@@ -1044,19 +1244,29 @@ extern "C" int mhb_count_run_multi(const mhb_count_opts *o, int n_gpus) {
   long long total_bases = 0, n_reads = 0;
   std::vector<uint32_t> bin;
   if (int rc = load_read_lib(lib, &bin, &n_reads, &total_bases)) return rc;
-  // the partitioned build deals contiguous blocks of a FIXED-length library to the GPUs; anything else (a truncated
-  // image included, which the single-GPU count reports): one GPU.  Indexed serially: the workers are forked next.
-  ReadLibIndex ix;
-  const bool fixed = o->k >= 12 && n_reads >= n_gpus &&
-                     !index_read_lib(bin.data(), bin.size(), n_reads, 0, &ix, FixedCheck::kSerial) && ix.fixed_len;
-  const uint32_t L = ix.fixed_len;
-  if (!fixed) {
-    XINFO("variable-length or tiny library: running on one GPU\n");
+  if (n_reads < n_gpus) {
+    XINFO("%lld reads for %d GPUs: running on one GPU\n", n_reads, n_gpus);
+    return mhb_count_run(o);
+  }
+  if (o->k < 12) {
+    XINFO("k = %u is below 12, the mercy search's 12-base look-up prefix: running on one GPU\n", o->k);
+    return mhb_count_run(o);
+  }
+  ReadLibIndex ix;  // indexed serially: the workers are forked next
+  if (index_read_lib(bin.data(), bin.size(), (uint64_t)n_reads, o->k, &ix, FixedCheck::kSerial)) {
+    XINFO("%s.bin ends inside a read: running on one GPU\n", lib.c_str());
     return mhb_count_run(o);
   }
   XINFO("%lld reads, %lld bases; k = %u, m = %d; %d GPUs\n", n_reads, total_bases, o->k, o->m, n_gpus);
-  const Job J{o->k, o->m, bin.data(), (uint64_t)n_reads, L, prefix};
-  const int rc = run_workers(n_gpus, "count", {"mul", "tips", "cand", "planes", "ecnt", "stab", "candrev"},
+  Job J;
+  J.k = o->k;
+  J.m = o->m;
+  J.bin = bin.data();
+  J.ix = &ix;
+  J.first.resize(n_gpus + 1);
+  plan_read_shares(bin.data(), ix, (uint64_t)n_reads, (uint32_t)n_gpus, J.first.data());
+  J.prefix = prefix;
+  const int rc = run_workers(n_gpus, "count", {"h16", "mul", "tips", "cand", "planes", "ecnt", "stab", "candrev"},
                              [&](Exchange &X) { worker(J, X); });
   if (!rc) XINFO("count (+ k_min SdBG) on %d GPUs done. Time elapsed: %.4f\n", n_gpus, now_s() - t0);
   return rc;
@@ -1185,5 +1395,32 @@ extern "C" int mhb_plan_r2s_owners(const uint64_t *hist16, uint32_t n_ranks, uin
     bucket_lo[o] = P.bounds[o] << 8;
     bucket_hi[o] = (P.bounds[o + 1] << 8) - 1;
   }
+  return MHB_OK;
+}
+
+extern "C" int mhb_plan_count_owner_rounds(const uint64_t *hist16, uint32_t n_ranks, uint64_t max_records, uint32_t max_rounds,
+                                           uint32_t *owner_lo, uint32_t *owner_hi, uint32_t *round_lo, uint32_t *round_hi,
+                                           uint64_t *block_n, uint64_t *block_off, uint32_t *n_rounds_out) {
+  if (!hist16 || !owner_lo || !owner_hi || !round_lo || !round_hi || !block_n || !block_off || !n_rounds_out || n_ranks < 1 ||
+      n_ranks > (uint32_t)kMaxRanks || max_rounds < 1)
+    return mhb_set_error(MHB_ERR_ARG, "bad args");
+  const int W = (int)n_ranks;
+  std::vector<const uint64_t *> h(W);
+  for (int s = 0; s < W; ++s) h[s] = hist16 + (size_t)s * 65536;
+  uint64_t cap[kMaxRanks];
+  for (int o = 0; o < W; ++o) cap[o] = max_records ? max_records : ~0ull;
+  CountPlan cp;
+  CKR(plan_count_rounds(h.data(), W, cap, &cp));
+  if ((uint32_t)cp.R > max_rounds)
+    return mhb_set_error(MHB_ERR_NOMEM, "the plan needs %d rounds, more than %u", cp.R, max_rounds);
+  for (int o = 0; o < W; ++o) {
+    owner_lo[o] = cp.P.bounds[o] << 8;
+    owner_hi[o] = (cp.P.bounds[o + 1] << 8) - 1;
+  }
+  std::copy(cp.lo.begin(), cp.lo.end(), round_lo);
+  std::copy(cp.hi.begin(), cp.hi.end(), round_hi);
+  std::copy(cp.n.begin(), cp.n.end(), block_n);
+  std::copy(cp.off.begin(), cp.off.end(), block_off);
+  *n_rounds_out = (uint32_t)cp.R;
   return MHB_OK;
 }

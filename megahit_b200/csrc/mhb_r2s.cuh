@@ -17,7 +17,7 @@
 #include "mhb.h"
 #include "mhb_kernels.cuh"
 #if defined(__CUDACC__)
-#include "mhb_s2s.cuh"  // OwnerSink
+#include "mhb_s2s.cuh"
 #endif
 
 namespace mhb {

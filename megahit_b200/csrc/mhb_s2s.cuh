@@ -87,28 +87,7 @@ struct RangeSink {
   }
 };
 
-// OwnerSink: item -> rank owner[leading record byte], stored at base[owner] + cursor[owner] (base[o] = this rank's
-// segment of owner o's receive buffer, which may be another process's memory opened through CUDA IPC; the cursors are
-// this rank's).  The lanes of a warp are grouped by owner; one atomic per group, each lane stores at the group's base
-// plus its rank in the group.  Items beyond capacity[owner] are counted but not stored.
-struct OwnerSink {
-  const uint8_t *owner;  // 256 entries
-  const u64 *base;       // device addresses, one per owner
-  unsigned long long *cursor;
-  const u64 *capacity;
-  template <int W>
-  __device__ __forceinline__ void put(bool in, const u32 (&rec)[W], u32, u32 lane, u32 lt) const {
-    const u32 o = in ? (u32)__ldg(owner + (rec[0] >> 24)) : 0xFFFFFFFFu;
-    const u32 peers = __match_any_sync(0xffffffffu, o);
-    if (!in) return;
-    const u32 leader = (u32)__ffs(peers) - 1;
-    unsigned long long at = 0;
-    if (lane == leader) at = atomicAdd(cursor + o, (unsigned long long)__popc(peers));
-    at = __shfl_sync(peers, at, leader);
-    const u64 pos = at + __popc(peers & lt);
-    if (pos < capacity[o]) st_rec<W>(reinterpret_cast<u32 *>(base[o]), pos, rec);
-  }
-};
+// OwnerSink (mhb_kernels.cuh): each item straight into the receive buffer of the rank owning its leading byte.
 
 // S-extract restricted to the items whose 16-bit bucket id (first eight bases) lies in [lo, hi] (A13: seq2sdbg in
 // rounds when the items of all sequences do not fit in HBM; base_engine.cpp:254-281), handed to `sink` a warp at a

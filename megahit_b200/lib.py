@@ -139,12 +139,12 @@ class BuildlibResult(C.Structure):
 SYMBOLS = [
     "mhb_last_error", "mhb_version", "mhb_device_count", "mhb_launch_count", "mhb_count_record_words", "mhb_words_per_edge",
     "mhb_s2s_record_words", "mhb_count_sort_bytes", "mhb_s2s_sort_bytes", "mhb_sort_workspace_bytes",
-    "mhb_count_extract", "mhb_check_fixed_len", "mhb_count_extract_range", "mhb_set_round_limit", "mhb_set_s2s_round_limit", "mhb_set_r2s_round_limit", "mhb_plan_rounds", "mhb_plan_rounds16", "mhb_sort_records", "mhb_sort_records_relaxed", "mhb_sort_pass_ms", "mhb_partition_scatter", "mhb_partition_scatter_hist", "mhb_plan_partition", "mhb_compact_tip_edges", "mhb_dev_malloc", "mhb_dev_free",
+    "mhb_count_extract", "mhb_count_extract_owners", "mhb_check_fixed_len", "mhb_count_extract_range", "mhb_set_round_limit", "mhb_set_s2s_round_limit", "mhb_set_r2s_round_limit", "mhb_plan_rounds", "mhb_plan_rounds16", "mhb_sort_records", "mhb_sort_records_relaxed", "mhb_sort_pass_ms", "mhb_partition_scatter", "mhb_partition_scatter_hist", "mhb_plan_partition", "mhb_compact_tip_edges", "mhb_dev_malloc", "mhb_dev_free",
     "mhb_ipc_export", "mhb_ipc_open", "mhb_ipc_close", "mhb_count_solid_scratch_bytes", "mhb_count_solid", "mhb_count_hashed_supported", "mhb_count_hashed_workspace_bytes", "mhb_count_solid_hashed", "mhb_tipset_bytes",
     "mhb_tipset_build", "mhb_count_mark_mercy", "mhb_count_tip_edges", "mhb_s2s_extract", "mhb_s2s_extract_range",
     "mhb_s2s_emit_scratch_bytes", "mhb_s2s_emit", "mhb_set_device", "mhb_count_host", "mhb_s2s_host", "mhb_build_host", "mhb_free",
     "mhb_mercy_candidates_scratch_bytes", "mhb_mercy_candidates", "mhb_mercy_edges_scratch_bytes", "mhb_mercy_edges", "mhb_mercy_edges_count", "mhb_mercy_edges_write", "mhb_mercy_edges_segs", "mhb_mercy_host", "mhb_mercy_planes_words", "mhb_mercy_probe_owned", "mhb_mercy_count_planes", "mhb_edge_lut_bytes", "mhb_edge_lut_build",
-    "mhb_release", "mhb_count_run", "mhb_count_run_multi", "mhb_seq2sdbg_run", "mhb_seq2sdbg_run_multi",
+    "mhb_release", "mhb_count_run", "mhb_count_run_multi", "mhb_plan_count_owner_rounds", "mhb_seq2sdbg_run", "mhb_seq2sdbg_run_multi",
     "mhb_plan_seq_shares", "mhb_s2s_extract_owners","mhb_selftest_count_record", "mhb_selftest_count_records_roll", "mhb_selftest_s2s_record",
     "mhb_iterate_host", "mhb_iterate_run", "mhb_iterate_run_multi", "mhb_plan_read_shares", "mhb_selftest_iterate", "mhb_s2s_extract_edges_pruned", "mhb_s2s_emit_fmt", "mhb_read2sdbg_host", "mhb_read2sdbg_run", "mhb_read2sdbg_run_multi", "mhb_plan_r2s_owners", "mhb_selftest_r2s_s1_record", "mhb_selftest_r2s_item",
     "mhb_selftest_kmsort", "mhb_selftest_kmsort_smem", "mhb_selftest_r2s_s1_group", "mhb_selftest_r2s_mercy_read",
@@ -260,6 +260,11 @@ def load():
     L.mhb_ipc_close.argtypes = [C.c_void_p]
     L.mhb_free.argtypes = [C.c_void_p]
     L.mhb_count_run.argtypes = [C.POINTER(CountOpts)]
+    L.mhb_count_run_multi.argtypes = [C.POINTER(CountOpts), C.c_int]
+    L.mhb_count_extract_owners.argtypes = [C.c_void_p, C.POINTER(DevReads), C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.mhb_plan_count_owner_rounds.argtypes = [C.c_void_p, C.c_uint32, C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p,
+                                              C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint32)]
     L.mhb_seq2sdbg_run.argtypes = [C.POINTER(Seq2SdbgOpts)]
     L.mhb_seq2sdbg_run_multi.argtypes = [C.POINTER(Seq2SdbgOpts), C.c_int]
     L.mhb_plan_seq_shares.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_void_p]
@@ -713,9 +718,33 @@ def sdbg_stream_from_table(table: np.ndarray, data: bytes) -> bytes:
 # file level (the sub-commands)
 # ------------------------------------------------------------------------------------------------
 def count_run(read_lib_file: str, output_prefix: str, k: int = 21, m: int = 2, host_mem: float = 1e9,
-              num_cpu_threads: int = 0, mem_flag: int = 1) -> None:
+              num_cpu_threads: int = 0, mem_flag: int = 1, gpus: int = 1) -> None:
+    """gpus > 1: mhb_count_run_multi, which forks one worker per GPU and so must be called from a process that has
+    not initialised CUDA (torch included); it writes one P.edges.<r> and P.sdbg.<r> per rank."""
     o = CountOpts(k, m, host_mem, num_cpu_threads, read_lib_file.encode(), output_prefix.encode(), mem_flag)
-    _check(load().mhb_count_run(C.byref(o)))
+    L = load()
+    _check(L.mhb_count_run_multi(C.byref(o), int(gpus)) if gpus > 1 else L.mhb_count_run(C.byref(o)))
+
+
+def plan_count_owner_rounds(hist16: np.ndarray, max_records: int = 0, max_rounds: int = 4096) -> dict:
+    """The owner and round plan of a multi-GPU count (host logic only) from the (n_ranks, 65536) bucket histograms of the
+    ranks' shares: owners = [(first, last) bucket of every owner], rounds = R, lo / hi = (R, n_ranks) range of every
+    owner in every round (lo > hi: empty), n / off = (R, owner, rank) records sent and where they start in the owner's
+    buffer.  max_records = 0: no cap."""
+    h = np.ascontiguousarray(hist16, np.uint64)
+    assert h.ndim == 2 and h.shape[1] == 65536
+    W = h.shape[0]
+    olo, ohi = np.zeros(W, np.uint32), np.zeros(W, np.uint32)
+    lo, hi = np.zeros(max_rounds * W, np.uint32), np.zeros(max_rounds * W, np.uint32)
+    n, off = np.zeros(max_rounds * W * W, np.uint64), np.zeros(max_rounds * W * W, np.uint64)
+    R = C.c_uint32(0)
+    _check(load().mhb_plan_count_owner_rounds(h.ctypes.data, W, int(max_records), max_rounds, olo.ctypes.data,
+                                              ohi.ctypes.data, lo.ctypes.data, hi.ctypes.data, n.ctypes.data,
+                                              off.ctypes.data, C.byref(R)))
+    R = R.value
+    return {"owners": [(int(a), int(b)) for a, b in zip(olo, ohi)], "rounds": R,
+            "lo": lo[: R * W].reshape(R, W), "hi": hi[: R * W].reshape(R, W),
+            "n": n[: R * W * W].reshape(R, W, W), "off": off[: R * W * W].reshape(R, W, W)}
 
 
 def seq2sdbg_run(output_prefix: str, k: int, k_from: int = 0, input_prefix: str = "", contig: str = "",
