@@ -1,10 +1,13 @@
 """The NumPy count reference (tests/count_reference.py) against a deliberately naive restatement of
 KmerCounter::Lv2Postprocess + PackEdge (kmer_counter.cpp:254-305, :32-52): a dict of per-key tallies and a loop per
-record.  No GPU: a bug in the yardstick must not be mistaken for a kernel bug."""
+record.  The any-k extraction and mercy-mark restatements against the C oracle at every record width.  No GPU: a bug in
+the yardstick must not be mistaken for a kernel bug."""
 import numpy as np
 import pytest
 
-from count_reference import count_records_reference, count_record_words, make_records, records_from_tallies, words_per_edge
+from count_reference import (count_key_words, count_records_reference, count_record_words, extract_records, make_records,
+                             make_records_wide, record_byte_hist, records_from_tallies, reference_marks, words_per_edge)
+from count_wide_cases import library, pack, palindrome, width_classes
 
 
 def naive_count(recs, k, m):
@@ -137,3 +140,105 @@ def test_reference_edge_layout_and_empty_input():
     assert n == 0 and e.shape == (0, 3) and len(a) == 0 and not h.any()
     with pytest.raises(AssertionError):  # a set bit between the (k+1)-mer and prev / next
         count_records_reference(np.array([[0, 1 << 6]], np.uint32), 27, 1)
+
+
+# ------------------------------------------------------------------------------------------------
+# every record width: the extraction restatement and the count reference against the C oracle
+# ------------------------------------------------------------------------------------------------
+WIDE_K = width_classes(9, 255)
+
+
+def test_width_classes_cover_every_record_geometry():
+    classes = {(count_key_words(k), count_record_words(k), words_per_edge(k)) for k in range(9, 256)}
+    assert len(WIDE_K) == len(classes) == 47 and WIDE_K[0] == 12 and WIDE_K[-1] == 255
+    assert {(count_key_words(k), count_record_words(k), words_per_edge(k)) for k in WIDE_K} == classes
+
+
+@pytest.mark.parametrize("k", WIDE_K)
+def test_extract_count_and_marks_match_the_oracle_at_every_width(k):
+    """extract_records -> count_records_reference == oracle.count (edges, .counting) and reference_marks == its
+    first_0_out / last_0_in, on variable-length reads with zero-length ones and (odd k) palindromic (k+1)-mers"""
+    from oracle import oracle as O
+    m = 2
+    binw, n_reads, lens = library(k, 70 + k)
+    assert (lens == 0).sum() >= 2 and (lens == k).any() and (lens == k + 1).any()
+    assert {0, 1, 15} <= set((lens[lens > k] % 16).tolist())
+    recs, strand = extract_records(binw, n_reads, k)
+    assert recs.shape == (np.maximum(lens - k, 0).sum(), count_record_words(k))
+    edges, aux, hist, n = count_records_reference(recs, k, m)
+    oc = O.count(O.unpack_bin(binw.tobytes(), reverse=True), k, m)
+    assert n == oc["n_solid"] > 0 and (edges == oc["edges"]).all()
+    assert (hist[1:] == oc["counting"][1:]).all()
+    first, last, _, _, n_tip = reference_marks(binw, n_reads, k, m)
+    assert n_tip > 0 and (first != 0xFFFFFFFF).any()
+    assert (first == oc["first_0_out"]).all() and (last == oc["last_0_in"]).all()
+    assert (strand == 0).any() and (strand == 1).any()
+
+
+@pytest.mark.parametrize("k", [31, 47, 63, 127, 255])
+def test_palindromes_take_strand_zero(k):
+    """a (k+1)-mer equal to its reverse complement keeps the package orientation (rc < fwd is false on a tie):
+    prev / next are the package neighbours, not their complements"""
+    rng = np.random.default_rng(k)
+    pal = palindrome(rng, k)
+    x, y = np.array([0, 1, 2], np.uint8), np.array([3, 0], np.uint8)  # file neighbours 2 (before) and 3 (after)
+    recs, strand = extract_records(pack([pal, np.concatenate([x, pal, y])]), 2, k)
+    assert len(recs) == 1 + (len(x) + len(y) + 1) and strand[0] == 0 and strand[1 + len(x)] == 0
+    assert recs[0, -1] & 63 == (4 << 3) | 4 and recs[1 + len(x), -1] & 63 == (3 << 3) | 2
+    assert ((recs[0] ^ recs[1 + len(x)]) & ~np.uint32(63) == 0).all()
+
+
+def _wide_set(rng, k, m):
+    """keys that share their leading words and differ in one word, tallies as random_set"""
+    w = count_key_words(k)
+    n_keys = int(rng.integers(1, 10))
+    keys = np.repeat(rng.integers(0, 1 << 32, (1, w), dtype=np.uint64).astype(np.uint32), n_keys, axis=0)
+    col = int(rng.integers(0, w))
+    keys[:, col] = rng.integers(0, 1 << 32, n_keys, dtype=np.uint64).astype(np.uint32)
+    choices = [1, max(1, m - 1), m, m + 1, 256, 257, int(rng.integers(1, 3 * m + 3))]
+    counts = [choices[int(rng.integers(0, len(choices)))] for _ in range(n_keys)]
+    kinds = ["random", "none", "exact_m", "below_m", "wrap"]
+    pt = np.array([_tally_row(rng, c, m, kinds[int(rng.integers(0, 5))]) for c in counts])
+    nt = np.array([_tally_row(rng, c, m, kinds[int(rng.integers(0, 5))]) for c in counts])
+    sym = np.tile(np.arange(5), n_keys)
+    kidx = np.repeat(np.arange(n_keys), pt.sum(axis=1))
+    recs = make_records_wide(keys[kidx], np.repeat(sym, pt.reshape(-1)), np.repeat(sym, nt.reshape(-1)), k)
+    return recs[rng.permutation(len(recs))]
+
+
+@pytest.mark.parametrize("m", [1, 2, 3])
+def test_reference_matches_naive_at_wide_records(m):
+    rng = np.random.default_rng(2000 + m)
+    for i in range(150):
+        k = (32, 39, 44, 47, 63, 127, 141, 199, 253, 255)[i % 10]
+        recs = _wide_set(rng, k, m)
+        assert recs.shape[1] == count_record_words(k) >= 3
+        e0, a0, h0, n0 = naive_count(recs, k, m)
+        e1, a1, h1, n1 = count_records_reference(recs, k, m)
+        assert n0 == n1 and (e0 == e1).all() and (a0 == a1).all() and (h0 == h1).all(), (m, i, k)
+
+
+def test_wide_record_layout_and_empty_input():
+    ones = np.full((2, 16), 0xFFFFFFFF, np.uint32)
+    # k = 47 (W = 3, WR = 4): the last record word holds prev / next only
+    r47 = make_records_wide(ones, [4, 0], [1, 4], 47)
+    assert r47.shape == (2, 4) and (r47[:, :3] == 0xFFFFFFFF).all() and r47[:, 3].tolist() == [33, 4]
+    e47, a47, h47, n47 = count_records_reference(r47, 47, 1)
+    assert n47 == 1 and e47.tolist() == [[0xFFFFFFFF] * 3 + [2]] and a47.tolist() == [0] and h47[2] == 1
+    # k = 39 (W = WR = WE = 3): 80 key bits, the multiplicity shares the last key word
+    e39 = count_records_reference(make_records_wide(ones[:1], [2], [3], 39), 39, 1)[0]
+    assert e39.tolist() == [[0xFFFFFFFF, 0xFFFFFFFF, 0xFFFF0001]]
+    # k = 44 (W = WR = 3, WE = 4): the key reaches record bit 6, the multiplicity takes a word of its own
+    r44 = make_records_wide(ones[:1], [1], [1], 44)
+    assert r44[0, 2] == 0xFFFFFFC0 | 9
+    assert count_records_reference(r44, 44, 1)[0].tolist() == [[0xFFFFFFFF, 0xFFFFFFFF, 0xFFFFFFC0, 1]]
+    # k = 255: 17-word records and edges
+    r255 = make_records_wide(np.zeros((3, 16), np.uint32), [0, 1, 2], [4, 4, 4], 255)
+    e255, a255, _, n255 = count_records_reference(r255, 255, 3)
+    assert n255 == 1 and e255.shape == (1, 17) and e255[0, -1] == 3 and a255.tolist() == [3]
+    e, a, h, n = count_records_reference(np.zeros((0, 17), np.uint32), 255, 2)
+    assert n == 0 and e.shape == (0, 17) and len(a) == 0 and not h.any()
+    recs, strand = extract_records(pack([np.zeros(0, np.uint8), np.zeros(255, np.uint8)]), 2, 255)
+    assert recs.shape == (0, 17) and len(strand) == 0 and not record_byte_hist(recs, 3).any()
+    with pytest.raises(AssertionError):  # a set bit between the (k+1)-mer and prev / next
+        count_records_reference(np.array([[0, 0, 0, 1 << 6]], np.uint32), 47, 1)

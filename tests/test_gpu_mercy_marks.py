@@ -1,7 +1,8 @@
 """The per-read mercy marks (first_0_out / last_0_in, kmer_counter.cpp:307-367) of mhb_count_mark_mercy, word for word,
 for every tip-set filter plan ($MHB_TIPSET_FILTER: the default, the global-memory filter, a filter of 1024 words and a
 saturated one of 4 words, where every position probes the table) against a NumPy restatement built on
-count_reference.py's solid edges and in/out flags.  The device tip set is built from those same edges."""
+count_reference.py's solid edges and in/out flags (count_reference.reference_marks, any k).  The device tip set is built
+from those same edges."""
 import ctypes as C
 import os
 
@@ -9,68 +10,12 @@ import numpy as np
 import pytest
 
 from conftest import GOLDEN
-from count_reference import count_records_reference, make_records
+from count_reference import SENTINEL, read_layout as _layout, reference_marks
+from count_wide_cases import library
 
 pytestmark = pytest.mark.gpu
 
-SENTINEL = 0xFFFFFFFF
 ARMS = ("default", "global", "1024", "1")
-
-
-def _layout(binw, n_reads):
-    """length and record start of every read of a `.bin` word stream"""
-    lens, starts, pos = np.empty(n_reads, np.int64), np.empty(n_reads, np.int64), 0
-    for r in range(n_reads):
-        lens[r], starts[r] = int(binw[pos]), pos
-        pos += 1 + (lens[r] + 15) // 16
-    return lens, starts
-
-
-def reference_marks(binw, n_reads, k, m):
-    """-> first, last (uint32 per read), edges, aux, n_tip.  Reads are processed in groups of equal length."""
-    K1 = k + 1
-    pw = np.array([1 << (2 * (K1 - 1 - i)) for i in range(K1)], np.uint64)
-    sh = np.arange(30, -1, -2, dtype=np.uint64)
-    lens, starts = _layout(binw, n_reads)
-    groups = []
-    for L in np.unique(lens):
-        if L < K1:
-            continue
-        ids = np.flatnonzero(lens == L)
-        nw = (L + 15) // 16
-        w = binw[starts[ids][:, None] + 1 + np.arange(nw)[None, :]].astype(np.uint64)
-        b = ((w[:, :, None] >> sh[None, None, :]) & np.uint64(3)).reshape(len(ids), -1)[:, :L].astype(np.int64)
-        win = np.lib.stride_tricks.sliding_window_view(b, K1, axis=1).astype(np.uint64)  # (g, L - k, K1), file order
-        fwd = win[:, :, ::-1] @ pw        # the package-orientation edge: reverse(S)
-        rc = (np.uint64(3) - win) @ pw    # its reverse complement: complement(S)
-        strand = rc < fwd
-        canon = np.where(strand, rc, fwd)
-        q = np.arange(L - k)[None, :]
-        prev = np.where(q + K1 < L, b[:, np.minimum(q[0] + K1, L - 1)], 4)
-        nxt = np.where(q > 0, b[:, np.maximum(q[0] - 1, 0)], 4)
-        p = np.where(strand, np.where(nxt == 4, 4, 3 - nxt), prev)
-        n = np.where(strand, np.where(prev == 4, 4, 3 - prev), nxt)
-        groups.append((ids, L, canon, strand, p, n))
-    recs = make_records(np.concatenate([g[2].reshape(-1) for g in groups]) << np.uint64(64 - 2 * K1),
-                        np.concatenate([g[4].reshape(-1) for g in groups]), np.concatenate([g[5].reshape(-1) for g in groups]), k)
-    edges, aux, _, n_solid = count_records_reference(recs, k, m)
-    ekey = ((edges[:, 0].astype(np.uint64) << np.uint64(32)) | edges[:, 1].astype(np.uint64)) >> np.uint64(64 - 2 * K1)
-    first = np.full(n_reads, SENTINEL, np.uint32)
-    last = np.full(n_reads, SENTINEL, np.uint32)
-    for ids, L, canon, strand, _, _ in groups:
-        flags = np.zeros(canon.shape, np.int64)
-        if n_solid:
-            i = np.minimum(np.searchsorted(ekey, canon), n_solid - 1)
-            flags = np.where(ekey[i] == canon, aux[i], 0).astype(np.int64)
-        off = (L - K1 - np.arange(L - k))[None, :].repeat(len(ids), axis=0)
-        no_in, no_out = (flags & 1) != 0, (flags & 2) != 0
-        to_last = (no_in & ~strand) | (no_out & strand)
-        to_first = (no_in & strand) | (no_out & ~strand)
-        lv = np.where(to_last, off, -1).max(axis=1)
-        fv = np.where(to_first, off + 1, SENTINEL).min(axis=1)
-        last[ids] = np.where(lv >= 0, lv, SENTINEL).astype(np.uint32)
-        first[ids] = fv.astype(np.uint32)
-    return first, last, edges, aux, int((aux != 0).sum())
 
 
 def device_marks(binw, n_reads, k, edges, aux, spec):
@@ -141,11 +86,17 @@ def test_marks_match_reference_on_fixtures(name, k, m):
     assert headers["1"][2] == 4 and headers["1"][4] == 1  # 4 words, no fold: saturated, every probe reaches the table
 
 
-@pytest.mark.parametrize("k", [13, 16, 28, 29, 31])
+@pytest.mark.parametrize("k", [13, 16, 28, 29, 31, 32, 39, 44, 47, 48, 63, 95, 127, 141, 199, 255])
 def test_marks_match_reference_across_widths(k):
     """k = 13: generic kernel, one-word keys; 16 and 28: the two ends of the rolling kernel; 29 and 31: generic
-    kernel, 3-word records"""
-    headers, n_tip, n_marked = _check_all_arms(*_lib("syn150_k27"), k, 2)
+    kernel, 3-word records.  Wider keys on a low-coverage variable-length library: 32, 39 (W = WR, the multiplicity
+    shares the last edge word), 44 (an edge word of its own), 47 (W = WR - 1), 48 (the first 256-thread kernel), 63, 95,
+    127, 141, 199, 255 (multi-word tip hashing and keys)"""
+    if k <= 31:
+        binw, n_reads = _lib("syn150_k27")
+    else:
+        binw, n_reads, _ = library(k, 900 + k, n_reads=800, genome_len=12_000)
+    headers, n_tip, n_marked = _check_all_arms(binw, n_reads, k, 2)
     assert n_tip > 0 and n_marked > 0
 
 
