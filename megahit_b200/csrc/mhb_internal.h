@@ -169,11 +169,58 @@ struct StreamStats {
   double copy_ms = 0, kernel_ms = 0, fill_ms = 0, pass_ms = 0;
 };
 
+// ---- the plans (mhb_plan.cpp): host logic only; every greedy cut is the one rule of greedy_cut there ----
+constexpr int kMaxRanks = 16;  // GPUs of one multi-GPU run
+// the sort items of a sequence of len bases at k
+inline uint64_t seq_items(uint32_t len, uint32_t k) { return len >= k + 1 ? 2ull * (len - k + 2) : 0; }
+// the 256 leading-byte bins of a 65536-bin bucket histogram
+inline void fold_bucket_hist(const uint64_t *h16, uint64_t *h256) {
+  for (int b = 0; b < 256; ++b) h256[b] = 0;
+  for (int b = 0; b < 65536; ++b) h256[b >> 8] += h16[b];
+}
+// Owner o takes the leading bytes [bounds[o], bounds[o+1]) (owner[b] = o): bound r is the byte whose cumulative count
+// in total256 is closest to r/world of the total, leaving at least one byte for every later rank (k_plan_partition).
+void owner_bounds(const uint64_t *total256, int world, uint32_t *bounds, uint8_t *owner);
+using BucketRanges = std::vector<std::pair<uint32_t, uint32_t>>;  // [lo, hi] of 16-bit bucket ids, ascending
+// Ranges tiling the leading bytes [byte_lo, byte_hi), of at most cap records each (cf. Lv1FindEndBuckets,
+// base_engine.cpp:254-281): a byte is one atom of h256[b] records when that fits cap, else its buckets are atoms of
+// h16[b << 8 | c] (h16 NULL: the byte stays one atom).  MHB_ERR_NOMEM naming the byte or bucket that alone exceeds cap
+// (and rank >= 0, the owner), or when more than cap_out ranges are needed; *ranges then holds those closed before.
+int plan_bucket_rounds(const uint64_t *h256, const uint64_t *h16, uint32_t byte_lo, uint32_t byte_hi, uint64_t cap,
+                       uint32_t cap_out, int rank, BucketRanges *ranges);
+// the rounds of a stage over all bucket ids from its 65536-bin histogram
+int plan_stage_rounds(const uint64_t *h16, uint64_t cap, BucketRanges *ranges);
+// The same from two histogram passes: top(h256) stores the leading-byte histogram; sub(bytes, h16), called when some
+// bytes alone exceed cap, the second-byte histogram of each listed byte b in h16[b << 8 | c].  *pre: prefix sums of
+// that histogram with every other byte's count in its first bucket, so the records of a range [lo, hi] are
+// pre[hi + 1] - pre[lo].  MHB_OK, a pass's error, or -1 (MHB_ERR_NOMEM message set) when the plan fails.
+int plan_bucket_passes(uint64_t cap, const std::function<int(uint64_t *)> &top,
+                       const std::function<int(const std::vector<uint32_t> &, uint64_t *)> &sub, BucketRanges *ranges,
+                       std::vector<uint64_t> *pre);
+// The owners of a multi-GPU count and its rounds (mhb_plan_count_owner_rounds), from every rank's 65536-bin histogram
+// h16[s] and the most records owner o takes in one round, cap[o] (UINT64_MAX: no cap)
+struct CountPlan {
+  uint32_t bounds[kMaxRanks + 1];
+  uint8_t owner[256];
+  int R = 1;                       // rounds
+  std::vector<uint32_t> lo, hi;    // [R][world]: owner o's bucket range in round t (lo > hi: empty)
+  std::vector<uint64_t> n, off;    // [R][world owner][world rank]: records rank s sends to o in round t, and where
+                                   // they start in o's receive buffer
+};
+int plan_count_rounds(const uint64_t *const *h16, int world, const uint64_t *cap, CountPlan *cp);
 // Greedy cut of n items into contiguous chunks [first[i], first[i+1]) of at most max_bytes each; a larger item gets a
 // chunk of its own.  Item r takes 4 * (word_off[r+1] - word_off[r]) + extra_bytes, or with word_off == NULL
 // 4 * stride_words + extra_bytes, cut in closed form.  first gets n_chunks + 1 entries ({0} when n == 0).
 void plan_chunks(const uint64_t *word_off, uint64_t stride_words, uint64_t extra_bytes, uint64_t n, uint64_t max_bytes,
                  std::vector<uint64_t> *first);
+// first edge of every leading byte in a sorted edge array (start[256] = n_edges)
+void edge_byte_starts(const uint32_t *edges, uint64_t n_edges, uint32_t WE, uint64_t start[257]);
+// Leading-byte segments [first[i], first[i+1]) of a streamed mercy search, packed to target bytes of edges; a byte above
+// target is a segment of its own, one above limit (a device slot) MHB_ERR_NOMEM.
+int plan_mercy_segments(const uint64_t start[257], uint32_t WE, uint64_t target, uint64_t limit, std::vector<uint32_t> *first);
+// n_ranks contiguous shares (n_ranks + 1 entries) of the sequences balanced on their items, of the reads on their bases
+void plan_seq_shares(const uint32_t *len, uint64_t n, uint32_t k, uint32_t n_ranks, uint64_t *first);
+void plan_read_shares(const uint32_t *bin, const ReadLibIndex &ix, uint64_t n_reads, uint32_t n_ranks, uint64_t *first);
 
 // The uploads of data kept in host memory, chunk by chunk, through two device slots (mhb_stream.cu): two pinned staging
 // buffers, a non-blocking copy stream and four events per chunk.  While host threads fill the staging buffer of chunk
@@ -292,23 +339,6 @@ int seq2sdbg_load(const mhb_seq2sdbg_opts *o, HostSeqs *seqs);
 int iterate_check_opts(const mhb_iterate_opts *o);
 int iterate_load(const mhb_iterate_opts *o, HostSeqs *contigs, std::vector<uint32_t> *bin, uint64_t *n_reads);
 int iterate_write_info(const std::string &prefix, uint32_t k_out, uint32_t words_per_edge, uint64_t n);
-// n_ranks contiguous shares of n items, cut r at the item boundary whose weight before it is closest to r / n_ranks of
-// the total (so a share is off its ideal weight by at most one item's); first gets n_ranks + 1 entries
-template <class Weight>
-void plan_shares(uint64_t n, uint32_t n_ranks, Weight weight, uint64_t *first) {
-  uint64_t total = 0;
-  for (uint64_t i = 0; i < n; ++i) total += weight(i);
-  first[0] = 0;
-  uint64_t b = 0, cum = 0;  // cum = weight of the items before b
-  for (uint32_t r = 1; r < n_ranks; ++r) {
-    const uint64_t target = (uint64_t)((unsigned __int128)total * r / n_ranks);
-    while (b < n && cum + weight(b) <= target) cum += weight(b++);
-    // the previous cut may already lie beyond this target (cum > target): then the cut stays where it is
-    if (b < n && cum < target && cum + weight(b) - target < target - cum) cum += weight(b++);
-    first[r] = b;
-  }
-  first[n_ranks] = n;
-}
 
 // ---- iterate's device pieces (mhb_iter.cu), shared by mhb_iterate_host and the multi-GPU worker ----
 // the checks of mhb_iterate_host on k and step (main_iterate.cpp:73-93, and the 17-word records of the device sort)
@@ -382,12 +412,6 @@ class R2sShare {
   struct Impl;
   Impl *d_;
 };
-// the 256 leading-byte bins of a 65536-bin bucket histogram
-inline void fold_bucket_hist(const uint64_t *h16, uint64_t *h256) {
-  for (int b = 0; b < 256; ++b) h256[b] = 0;
-  for (int b = 0; b < 65536; ++b) h256[b >> 8] += h16[b];
-}
-
 // mhb_mercy_probe_owned, with accumulate = true OR-ing the answers into planes_out instead of storing them (mhb_multi.cu)
 int mercy_probe_owned(void *stream, const mhb_dev_reads *reads, const uint64_t *cand_ids, uint64_t n_cand,
                       uint32_t max_read_len, uint32_t k, const uint32_t *edges, uint64_t n_edges, const void *lut,

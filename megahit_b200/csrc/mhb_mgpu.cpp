@@ -11,7 +11,7 @@
 //     block with a process-shared barrier; the medium ones (bucket histograms, tip edges, candidate reads, answer planes
 //     of the mercy searches, the per-bucket tables) through files in /dev/shm written by one rank and read by the others;
 //   * the plan of a stage (owner ranges and rounds from the all-gathered histograms) is computed by every rank from the
-//     same data (plan_partition_host = the rule of k_plan_partition / multigpu.plan_ranges; plan_count_rounds).
+//     same data (owner_bounds and plan_count_rounds, mhb_plan.cpp).
 // The mercy searches are answered by the owners of the searched prefixes (mhb_mercy_probe_owned); the k_min SdBG is
 // built in the same run because the solid edges are already on the devices.
 //
@@ -55,8 +55,6 @@
 using namespace mhb;
 
 namespace {
-
-constexpr int kMaxRanks = 16;
 
 // control block shared by the workers (anonymous MAP_SHARED mapping created before the fork)
 struct Control {
@@ -158,8 +156,7 @@ struct Exchange {
   void cleanup(const char *tag) { unlink(path(tag, rank).c_str()); }
 };
 
-// owner ranges from the all-gathered top-byte histograms: bound r = the byte value whose cumulative count is closest
-// to r/world of the total, leaving at least one value for every later rank (k_plan_partition, multigpu.plan_ranges)
+// the owner ranges of the all-gathered top-byte histograms (owner_bounds of their sum), and this rank's part in them
 struct Plan {
   uint32_t bounds[kMaxRanks + 1];
   uint8_t owner[256];
@@ -167,32 +164,11 @@ struct Plan {
 };
 Plan plan_partition_host(const uint64_t (*hist)[256], int world, int rank) {
   Plan p;
-  uint64_t cum[257];
-  cum[0] = 0;
-  for (int b = 0; b < 256; ++b) {
-    uint64_t a = 0;
-    for (int r = 0; r < world; ++r) a += hist[r][b];
-    cum[b + 1] = cum[b] + a;
-  }
-  const uint64_t total = cum[256];
-  p.bounds[0] = 0;
-  for (int r = 1; r < world; ++r) {
-    const uint32_t lo = p.bounds[r - 1] + 1, hi = 256 - (world - r);
-    const uint64_t target = total * r / world;
-    uint32_t best = lo;
-    uint64_t bestd = ~0ull;
-    for (uint32_t c = lo; c <= hi; ++c) {
-      const uint64_t d = cum[c] > target ? cum[c] - target : target - cum[c];
-      if (d < bestd) {
-        bestd = d;
-        best = c;
-      }
-    }
-    p.bounds[r] = best;
-  }
-  p.bounds[world] = 256;
+  uint64_t total[256] = {0};
+  for (int r = 0; r < world; ++r)
+    for (int b = 0; b < 256; ++b) total[b] += hist[r][b];
+  owner_bounds(total, world, p.bounds, p.owner);
   for (int o = 0; o < world; ++o) {
-    for (uint32_t b = p.bounds[o]; b < p.bounds[o + 1]; ++b) p.owner[b] = (uint8_t)o;
     uint64_t before = 0, tot = 0, mine = 0;
     for (int r = 0; r < world; ++r) {
       uint64_t s = 0;
@@ -362,79 +338,6 @@ std::vector<int64_t> sum_mul(Exchange &X) {
 // ================================================================================================
 // one worker = one GPU
 // ================================================================================================
-// The owner ranges of a multi-GPU count and its rounds over bucket ranges (mhb_plan_count_owner_rounds), computed by
-// every rank from the same all-gathered 65536-bin histograms.
-struct CountPlan {
-  Plan P;                         // owner byte ranges (P.bounds, P.owner)
-  int R = 1;                      // rounds
-  std::vector<uint32_t> lo, hi;   // [R][world]: owner o's bucket range in round t (lo > hi: empty)
-  std::vector<uint64_t> n, off;   // [R][world owner][world rank]: records rank s sends to o in round t, and where
-                                  // they start in o's receive buffer
-};
-// h16[s]: rank s's histogram; cap[o]: the most records owner o takes in one round (UINT64_MAX: no cap).  Each owner's
-// range is cut greedily into ascending sub-ranges of whole leading bytes, and of bucket ids inside a leading byte that
-// alone exceeds the cap (the rule of mhb_plan_rounds16).  MHB_ERR_NOMEM (message set) when one bucket exceeds a cap.
-int plan_count_rounds(const uint64_t *const *h16, int world, const uint64_t *cap, CountPlan *cp) {
-  std::vector<uint64_t> tot(65536, 0), pre((size_t)world * 65537, 0);  // pre[s][b] = rank s's records below bucket b
-  for (int s = 0; s < world; ++s)
-    for (uint32_t b = 0; b < 65536; ++b) {
-      tot[b] += h16[s][b];
-      pre[(size_t)s * 65537 + b + 1] = pre[(size_t)s * 65537 + b] + h16[s][b];
-    }
-  uint64_t h256[kMaxRanks][256] = {{0}};  // everything in rank 0's row: only the totals decide the owner ranges
-  for (uint32_t b = 0; b < 65536; ++b) h256[0][b >> 8] += tot[b];
-  cp->P = plan_partition_host(h256, world, 0);
-  std::vector<std::vector<std::pair<uint32_t, uint32_t>>> sub(world);
-  for (int o = 0; o < world; ++o) {
-    uint32_t lo = cp->P.bounds[o] << 8;
-    uint64_t acc = 0;
-    auto atom = [&](uint32_t a, uint64_t cnt) -> int {  // the next atom starts at bucket a and holds cnt records
-      if (cnt > cap[o])
-        return mhb_set_error(MHB_ERR_NOMEM, "bucket 0x%04x alone holds %llu records, more than one round of rank %d can "
-                             "take (%llu)", a, (unsigned long long)cnt, o, (unsigned long long)cap[o]);
-      if (acc + cnt > cap[o]) {  // acc > 0 here: close the open sub-range before this atom
-        sub[o].push_back({lo, a - 1});
-        lo = a;
-        acc = 0;
-      }
-      acc += cnt;
-      return MHB_OK;
-    };
-    for (uint32_t B = cp->P.bounds[o]; B < cp->P.bounds[o + 1]; ++B) {
-      uint64_t bt = 0;
-      for (uint32_t c = 0; c < 256; ++c) bt += tot[(B << 8) | c];
-      if (bt <= cap[o]) {
-        CKR(atom(B << 8, bt));
-      } else {
-        for (uint32_t c = 0; c < 256; ++c) CKR(atom((B << 8) | c, tot[(B << 8) | c]));
-      }
-    }
-    sub[o].push_back({lo, (cp->P.bounds[o + 1] << 8) - 1});
-  }
-  cp->R = 1;
-  for (int o = 0; o < world; ++o) cp->R = std::max(cp->R, (int)sub[o].size());
-  const size_t RW = (size_t)cp->R * world;
-  cp->lo.assign(RW, 1);
-  cp->hi.assign(RW, 0);
-  cp->n.assign(RW * world, 0);
-  cp->off.assign(RW * world, 0);
-  for (int t = 0; t < cp->R; ++t)
-    for (int o = 0; o < world; ++o) {
-      if (t >= (int)sub[o].size()) continue;  // empty range: nothing for o in this round
-      const uint32_t a = sub[o][t].first, b = sub[o][t].second;
-      cp->lo[(size_t)t * world + o] = a;
-      cp->hi[(size_t)t * world + o] = b;
-      uint64_t at = 0;
-      for (int s = 0; s < world; ++s) {
-        const size_t i = ((size_t)t * world + o) * world + s;
-        cp->n[i] = pre[(size_t)s * 65537 + b + 1] - pre[(size_t)s * 65537 + a];
-        cp->off[i] = at;
-        at += cp->n[i];
-      }
-    }
-  return MHB_OK;
-}
-
 // the records owner o receives in round t
 uint64_t round_total(const CountPlan &cp, int world, int t, int o) {
   uint64_t s = 0;
@@ -527,7 +430,6 @@ void worker(const Job &J, Exchange &X) {
     }
     CKL(plan_count_rounds(hp.data(), W, C->budget, &cp));
   }
-  const Plan &P = cp.P;
   const int R = cp.R;
   uint64_t n_own = 0, n_round_max = 0, n_sent = 0;
   for (int t = 0; t < R; ++t) {
@@ -560,7 +462,7 @@ void worker(const Job &J, Exchange &X) {
     CKL(dcap.alloc(kMaxRanks * 8, "count: owner capacities"));
     CKL(rlo.alloc(kMaxRanks * 4, "count: round ranges"));
     CKL(rhi.alloc(kMaxRanks * 4, "count: round ranges"));
-    CKC(cudaMemcpy(lut.p, P.owner, 256, cudaMemcpyHostToDevice));
+    CKC(cudaMemcpy(lut.p, cp.owner, 256, cudaMemcpyHostToDevice));
     for (int t = 0; t < R; ++t) {
       uint64_t base[kMaxRanks], want[kMaxRanks], sent[kMaxRanks];
       for (int o = 0; o < W; ++o) {
@@ -739,7 +641,7 @@ void worker(const Job &J, Exchange &X) {
       CKL(mhb_edge_lut_build(nullptr, d_edges, n_solid, k, lut.p));
       const size_t pw_all = mhb_mercy_planes_words(n_cand_all, L);
       CKL(planes.alloc(pw_all * 4, "count: mercy answer planes"));
-      CKL(mhb_mercy_probe_owned(nullptr, &greads, nullptr, n_cand_all, L, k, d_edges, n_solid, lut.p, P.owner, (uint32_t)r,
+      CKL(mhb_mercy_probe_owned(nullptr, &greads, nullptr, n_cand_all, L, k, d_edges, n_solid, lut.p, cp.owner, (uint32_t)r,
                                 planes.as<uint32_t>()));
       std::vector<uint32_t> hp(pw_all);
       CKC(cudaMemcpy(hp.data(), planes.p, pw_all * 4, cudaMemcpyDeviceToHost));
@@ -869,13 +771,6 @@ void worker(const Job &J, Exchange &X) {
 // ================================================================================================
 // seq2sdbg on several GPUs: the sequences are dealt in contiguous shares, the items meet on their owners
 // ================================================================================================
-uint64_t seq_items(uint32_t len, uint32_t k) { return len >= k + 1 ? 2ull * (len - k + 2) : 0; }
-
-// n_ranks contiguous shares of the sequences, balanced on their items (plan_shares)
-void plan_seq_shares(const uint32_t *len, uint64_t n, uint32_t k, uint32_t n_ranks, uint64_t *first) {
-  plan_shares(n, n_ranks, [&](uint64_t i) { return seq_items(len[i], k); }, first);
-}
-
 struct SeqJob {
   uint32_t k;
   const HostSeqs *seqs;                // every sequence (host, inherited by the workers)
@@ -954,11 +849,6 @@ void s2s_worker(const SeqJob &J, Exchange &X) {
 // ================================================================================================
 // iterate on several GPUs: the reads are dealt in contiguous shares, the candidate sets meet on their owners
 // ================================================================================================
-// n_ranks contiguous shares of the n_reads reads, balanced on their bases: the mark pass scans every base of every read
-void plan_read_shares(const uint32_t *bin, const ReadLibIndex &ix, uint64_t n_reads, uint32_t n_ranks, uint64_t *first) {
-  plan_shares(n_reads, n_ranks, [&](uint64_t i) { return (uint64_t)bin[ix.word_of(i)]; }, first);
-}
-
 struct IterJob {
   mhb_iterate_args a;          // every contig and the whole `.bin` image (host, inherited by the workers)
   std::vector<uint64_t> first;  // read shares
@@ -1337,21 +1227,6 @@ extern "C" int mhb_iterate_run_multi(const mhb_iterate_opts *o, int n_gpus) {
   return rc;
 }
 
-extern "C" int mhb_plan_read_shares(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, uint32_t n_ranks,
-                                    uint64_t *first_out) {
-  if ((!bin && bin_words) || !first_out || n_ranks < 1) return mhb_set_error(MHB_ERR_ARG, "bad args");
-  ReadLibIndex ix;  // serially, as mhb_iterate_run_multi before its fork
-  CKR(index_read_lib(bin, bin_words, n_reads, 0, &ix, FixedCheck::kSerial));
-  plan_read_shares(bin, ix, n_reads, n_ranks, first_out);
-  return MHB_OK;
-}
-
-extern "C" int mhb_plan_seq_shares(const uint32_t *len, uint64_t n_seqs, uint32_t k, uint32_t n_ranks, uint64_t *first_out) {
-  if ((!len && n_seqs) || !first_out || n_ranks < 1) return mhb_set_error(MHB_ERR_ARG, "bad args");
-  plan_seq_shares(len, n_seqs, k, n_ranks, first_out);
-  return MHB_OK;
-}
-
 extern "C" int mhb_read2sdbg_run_multi(const mhb_read2sdbg_opts *o, int n_gpus) {
   if (n_gpus <= 1) return mhb_read2sdbg_run(o);
   if (n_gpus > kMaxRanks) return mhb_set_error(MHB_ERR_ARG, "at most %d GPUs of one node are supported", kMaxRanks);
@@ -1382,45 +1257,4 @@ extern "C" int mhb_read2sdbg_run_multi(const mhb_read2sdbg_opts *o, int n_gpus) 
   const int rc = run_workers(n_gpus, "read2sdbg", {"stab", "mul"}, [&](Exchange &X) { r2s_worker(J, X); });
   if (!rc) XINFO("read2sdbg on %d GPUs done. Time elapsed: %.4f\n", n_gpus, now_s() - t0);
   return rc;
-}
-
-extern "C" int mhb_plan_r2s_owners(const uint64_t *hist16, uint32_t n_ranks, uint32_t *bucket_lo, uint32_t *bucket_hi) {
-  if (!hist16 || !bucket_lo || !bucket_hi || n_ranks < 1 || n_ranks > (uint32_t)kMaxRanks)
-    return mhb_set_error(MHB_ERR_ARG, "bad args");
-  static uint64_t h[kMaxRanks][256];  // rank 0's histogram holds everything
-  memset(h, 0, sizeof(h));
-  fold_bucket_hist(hist16, h[0]);
-  const Plan P = plan_partition_host(h, (int)n_ranks, 0);
-  for (uint32_t o = 0; o < n_ranks; ++o) {
-    bucket_lo[o] = P.bounds[o] << 8;
-    bucket_hi[o] = (P.bounds[o + 1] << 8) - 1;
-  }
-  return MHB_OK;
-}
-
-extern "C" int mhb_plan_count_owner_rounds(const uint64_t *hist16, uint32_t n_ranks, uint64_t max_records, uint32_t max_rounds,
-                                           uint32_t *owner_lo, uint32_t *owner_hi, uint32_t *round_lo, uint32_t *round_hi,
-                                           uint64_t *block_n, uint64_t *block_off, uint32_t *n_rounds_out) {
-  if (!hist16 || !owner_lo || !owner_hi || !round_lo || !round_hi || !block_n || !block_off || !n_rounds_out || n_ranks < 1 ||
-      n_ranks > (uint32_t)kMaxRanks || max_rounds < 1)
-    return mhb_set_error(MHB_ERR_ARG, "bad args");
-  const int W = (int)n_ranks;
-  std::vector<const uint64_t *> h(W);
-  for (int s = 0; s < W; ++s) h[s] = hist16 + (size_t)s * 65536;
-  uint64_t cap[kMaxRanks];
-  for (int o = 0; o < W; ++o) cap[o] = max_records ? max_records : ~0ull;
-  CountPlan cp;
-  CKR(plan_count_rounds(h.data(), W, cap, &cp));
-  if ((uint32_t)cp.R > max_rounds)
-    return mhb_set_error(MHB_ERR_NOMEM, "the plan needs %d rounds, more than %u", cp.R, max_rounds);
-  for (int o = 0; o < W; ++o) {
-    owner_lo[o] = cp.P.bounds[o] << 8;
-    owner_hi[o] = (cp.P.bounds[o + 1] << 8) - 1;
-  }
-  std::copy(cp.lo.begin(), cp.lo.end(), round_lo);
-  std::copy(cp.hi.begin(), cp.hi.end(), round_hi);
-  std::copy(cp.n.begin(), cp.n.end(), block_n);
-  std::copy(cp.off.begin(), cp.off.end(), block_off);
-  *n_rounds_out = (uint32_t)cp.R;
-  return MHB_OK;
 }

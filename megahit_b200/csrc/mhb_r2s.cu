@@ -190,19 +190,6 @@ size_t s2_pass_bytes(uint64_t n, uint32_t W, uint32_t k) {
          pad256((size_t)n * (4ull + 4ull * words_per_tip_label(k)) + 16);
 }
 
-// contiguous ranges of 16-bit bucket ids of at most max_n entries each, from the histogram of bucket ids (its rows are
-// the second-byte histograms mhb_plan_rounds16 reads for leading bytes that exceed a round)
-int plan_bucket_ranges(const std::vector<uint64_t> &h16, uint64_t max_n, std::vector<std::pair<uint32_t, uint32_t>> *out) {
-  uint64_t h256[256] = {0};
-  for (size_t b = 0; b < (size_t)MHB_NUM_BUCKETS; ++b) h256[b >> 8] += h16[b];
-  std::vector<uint32_t> lo(MHB_NUM_BUCKETS), hi(MHB_NUM_BUCKETS);
-  const int n = mhb_plan_rounds16(h256, h16.data(), max_n, lo.data(), hi.data(), MHB_NUM_BUCKETS);
-  if (n < 0) return MHB_ERR_NOMEM;  // message set by the planner
-  out->clear();
-  for (int i = 0; i < n; ++i) out->push_back({lo[i], hi[i]});
-  return MHB_OK;
-}
-
 // ---- the package, resident or streamed (DESIGN.md §4.9) ----
 // One chunk of the package on the device, handed to the stage code in read order: pv covers the chunk's reads (read
 // indices, words and offset arrays relative to the chunk, pv.base0 = global base of its first read, so every bit-plane
@@ -431,7 +418,7 @@ int run_stage1(cudaStream_t st, const EachChunk &each, const PkgView &shape, con
     CKR(side.pb.alloc((size_t)max_n * 8 + 16, "read2sdbg: bucket partition pairs (sort buffer)"));
   }
   u64 *d_info = l.narrow ? side.info.as<u64>() : nullptr;
-  std::vector<std::pair<uint32_t, uint32_t>> ranges = {{0u, 65535u}};
+  BucketRanges ranges = {{0u, 65535u}};
   DevBuf per_read, off, bsum, total;
   if (!one_pass) {
     DevBuf h16;
@@ -456,7 +443,7 @@ int run_stage1(cudaStream_t st, const EachChunk &each, const PkgView &shape, con
     CK(cudaMemcpyAsync(h_h16.data(), h16.p, MHB_NUM_BUCKETS * 8, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     tr.mark("s1.extract.plan");
-    CKR(plan_bucket_ranges(h_h16, max_n, &ranges));
+    CKR(plan_stage_rounds(h_h16.data(), max_n, &ranges));
   }
   uint64_t seen = 0;
   for (const auto &rg : ranges) {
@@ -760,7 +747,7 @@ int run_stage2(const mhb_build_args *args, mhb_build_result *res, cudaStream_t s
   const uint32_t k = args->k, W = s2s_record_words(k);
   const bool all = args->m == 1;  // stage 2 takes every edge
   uint64_t max_items = n_items;
-  std::vector<std::pair<uint32_t, uint32_t>> ranges = {{0u, 65535u}};
+  BucketRanges ranges = {{0u, 65535u}};
   if (!one_pass) {
     big.a.release();  // sized for stage 1
     big.b.release();
@@ -793,7 +780,7 @@ int run_stage2(const mhb_build_args *args, mhb_build_result *res, cudaStream_t s
     CK(cudaMemcpyAsync(h_h16.data(), h16.p, MHB_NUM_BUCKETS * 8, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     tr.mark("s2.extract.plan");
-    CKR(plan_bucket_ranges(h_h16, max_items, &ranges));
+    CKR(plan_stage_rounds(h_h16.data(), max_items, &ranges));
   }
   CKR(big.a.ensure((size_t)max_items * W * 4 + 16, "read2sdbg: stage-2 items"));
   CKR(big.b.ensure((size_t)max_items * W * 4 + 16, "read2sdbg: stage-2 items (sort buffer)"));

@@ -58,26 +58,6 @@ int DevBuf::alloc(size_t b, const char *what) {
 void DevBuf::reset_peak() { g_dev_peak = g_dev_live; }
 size_t DevBuf::peak_bytes() { return g_dev_peak; }
 
-void plan_chunks(const uint64_t *word_off, uint64_t stride_words, uint64_t extra_bytes, uint64_t n, uint64_t max_bytes,
-                 std::vector<uint64_t> *first) {
-  first->assign(1, 0);
-  if (!word_off) {
-    const uint64_t per = std::max<uint64_t>(1, max_bytes / (4 * stride_words + extra_bytes));
-    for (uint64_t r = per; r < n; r += per) first->push_back(r);
-  } else {
-    uint64_t acc = 0;
-    for (uint64_t r = 0; r < n; ++r) {
-      const uint64_t b = 4 * (word_off[r + 1] - word_off[r]) + extra_bytes;
-      if (r > first->back() && acc + b > max_bytes) {
-        first->push_back(r);
-        acc = 0;
-      }
-      acc += b;
-    }
-  }
-  if (n) first->push_back(n);
-}
-
 // a library's read chunks: the image only, a fixed-length library cut in closed form
 static void plan_read_chunks(const ReadLibIndex &ix, uint64_t n_reads, uint64_t max_bytes, std::vector<uint64_t> *first) {
   plan_chunks(ix.fixed_len ? nullptr : ix.rec_off.data(), 1 + div_ceil(ix.fixed_len, 16), 0, n_reads, max_bytes, first);
