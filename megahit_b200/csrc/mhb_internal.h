@@ -197,17 +197,20 @@ int plan_stage_rounds(const uint64_t *h16, uint64_t cap, BucketRanges *ranges);
 int plan_bucket_passes(uint64_t cap, const std::function<int(uint64_t *)> &top,
                        const std::function<int(const std::vector<uint32_t> &, uint64_t *)> &sub, BucketRanges *ranges,
                        std::vector<uint64_t> *pre);
-// The owners of a multi-GPU count and its rounds (mhb_plan_count_owner_rounds), from every rank's 65536-bin histogram
-// h16[s] and the most records owner o takes in one round, cap[o] (UINT64_MAX: no cap)
-struct CountPlan {
+// The plan of every multi-GPU owner exchange (mhb_plan_count_owner_rounds), from every rank's 65536-bin histogram
+// h16[s] and the most records owner o takes in one round, cap[o] (UINT64_MAX: no cap, one round).  A stage that
+// histograms 256 leading bytes places byte b at bucket b << 8.
+struct OwnerPlan {
+  int world = 0;
   uint32_t bounds[kMaxRanks + 1];
   uint8_t owner[256];
   int R = 1;                       // rounds
   std::vector<uint32_t> lo, hi;    // [R][world]: owner o's bucket range in round t (lo > hi: empty)
   std::vector<uint64_t> n, off;    // [R][world owner][world rank]: records rank s sends to o in round t, and where
                                    // they start in o's receive buffer
+  size_t at(int t, int o, int s) const { return ((size_t)t * world + o) * world + s; }
 };
-int plan_count_rounds(const uint64_t *const *h16, int world, const uint64_t *cap, CountPlan *cp);
+int plan_owner_rounds(const uint64_t *const *h16, int world, const uint64_t *cap, OwnerPlan *p);
 // Greedy cut of n items into contiguous chunks [first[i], first[i+1]) of at most max_bytes each; a larger item gets a
 // chunk of its own.  Item r takes 4 * (word_off[r+1] - word_off[r]) + extra_bytes, or with word_off == NULL
 // 4 * stride_words + extra_bytes, cut in closed form.  first gets n_chunks + 1 entries ({0} when n == 0).
@@ -366,11 +369,25 @@ int hist_byte(void *stream, const uint32_t *recs, uint64_t n, uint32_t words, in
 int read2sdbg_load(const mhb_read2sdbg_opts *o, std::vector<uint32_t> *bin, long long *n_reads);
 int read2sdbg_build(const mhb_read2sdbg_opts *o, std::vector<uint32_t> &bin, long long n_reads, double t0);
 
+// One round of a multi-GPU owner exchange on the device (OwnerExchange, mhb_mgpu.cpp); every pointer is device memory.
+// owner[b]: the rank owning leading byte b.  Per owner o: base[o] = where this rank's block of o's receive buffer
+// starts (256 entries, the rest 0: mhb_partition_scatter reads as many); row0[o] / info0[o] = row 0 of that buffer
+// and of its read_info buffer (info0 nullptr unless read2sdbg's narrow stage 1); off[o] = the rows of the lower
+// ranks' blocks; cap[o] = the rows of my block; cursor[o] = zeroed, the records the store counted; lo[o] .. hi[o] =
+// o's bucket range in the round.  Device addresses are uint64_t.
+struct OwnerRoute {
+  int n_owners;
+  const uint8_t *owner;
+  const uint64_t *base, *row0, *info0, *off, *cap;
+  uint64_t *cursor;
+  const uint32_t *lo, *hi;
+};
+
 // ---- read2sdbg's device pieces (mhb_r2s.cu), driven step by step by the multi-GPU worker ----
 // One rank's share [first, end) of the reads of a build, resident on the current device as one package chunk: read
 // indices are local, bases - stage-1 payload positions and bit-plane indices - global, and the bit planes (solid; with
-// need_mercy the three candidate planes after it, in one allocation) cover the whole library's word grid.  Owners are
-// ranks of contiguous leading-byte ranges (owner_of_byte); device addresses are passed as uint64_t.
+// need_mercy the three candidate planes after it, in one allocation) cover the whole library's word grid.  Records
+// reach their owners (ranks of contiguous leading-byte ranges) through an OwnerRoute.
 class R2sShare {
  public:
   R2sShare();
@@ -385,11 +402,11 @@ class R2sShare {
   // hist[65536] = the 16-bit bucket ids of the share's stage-1 records / stage-2 items (s2 after mercy_count)
   int s1_hist(uint64_t *hist);
   int s2_hist(uint64_t *hist);
-  // the share's stage-1 records into their owners' buffers in global read order (rec_base / info_base: device address
-  // of row 0 of owner o's record / read_info buffer, info_base nullptr unless s1_narrow; my_off[o]: the rows of the
-  // lower ranks).  Counts first: an error, and nothing stored, unless owner o gets expect[o] records.
-  int s1_send(const uint8_t *owner_of_byte, int n_owners, const uint64_t *rec_base, const uint64_t *info_base,
-              const uint64_t *my_off, const uint64_t *expect);
+  // the share's stage-1 records to their owners in global read order, in two passes: s1_count puts the records of
+  // every owner into rt.cursor, s1_store stores them at rt.row0 / rt.info0 from row rt.off (it has no capacity: the
+  // caller checks the counts in between)
+  int s1_count(const OwnerRoute &rt);
+  int s1_store(const OwnerRoute &rt);
   // owner: stable bucket partition, kmsort and Lv2Postprocess of the n records received (overwritten), into the local
   // planes and multiplicity histogram
   int s1_own(uint32_t *recs, uint64_t *info, uint64_t n);
@@ -398,10 +415,8 @@ class R2sShare {
   int or_planes(const void *peer_planes);
   // the mercy step and the stage-2 item count over the share
   int mercy_count(uint64_t *n_items, uint64_t *n_mercy);
-  // every stage-2 item of the share to its owner: owner_base[o] = device address of this rank's segment of owner o's
-  // buffer, capacity[o] items (host arrays); sent[o] = items sent
-  int s2_send(const uint8_t *owner_of_byte, int n_owners, const uint64_t *owner_base, const uint64_t *capacity,
-              uint64_t *sent);
+  // every stage-2 item of the share to its owner through rt (OwnerSink)
+  int s2_send(const OwnerRoute &rt);
   // owner: relaxed sort, collapse and emitter (label_fmt 1) of the n items received (overwritten); SdBG bytes, bucket
   // table (65536 x {offset, items, tips, large_mul}) and the emitter's 16 totals
   int s2_own(uint32_t *items, uint64_t n, std::vector<uint8_t> *bytes, std::vector<uint64_t> *table, uint64_t *totals);

@@ -136,7 +136,8 @@ int plan_bucket_passes(uint64_t cap, const std::function<int(uint64_t *)> &top,
   return MHB_OK;
 }
 
-int plan_count_rounds(const uint64_t *const *h16, int world, const uint64_t *cap, CountPlan *cp) {
+int plan_owner_rounds(const uint64_t *const *h16, int world, const uint64_t *cap, OwnerPlan *cp) {
+  cp->world = world;
   std::vector<uint64_t> tot(65536, 0);
   for (int s = 0; s < world; ++s)
     for (uint32_t b = 0; b < 65536; ++b) tot[b] += h16[s][b];
@@ -163,7 +164,7 @@ int plan_count_rounds(const uint64_t *const *h16, int world, const uint64_t *cap
       cp->hi[(size_t)t * world + o] = b;
       uint64_t at = 0;
       for (int s = 0; s < world; ++s) {
-        const size_t i = ((size_t)t * world + o) * world + s;
+        const size_t i = cp->at(t, o, s);
         cp->n[i] = pre[s][b + 1] - pre[s][a];
         cp->off[i] = at;
         at += cp->n[i];
@@ -275,8 +276,8 @@ extern "C" int mhb_plan_count_owner_rounds(const uint64_t *hist16, uint32_t n_ra
   for (int s = 0; s < W; ++s) h[s] = hist16 + (size_t)s * 65536;
   uint64_t cap[kMaxRanks];
   for (int o = 0; o < W; ++o) cap[o] = max_records ? max_records : ~0ull;
-  CountPlan cp;
-  CKR(plan_count_rounds(h.data(), W, cap, &cp));
+  OwnerPlan cp;
+  CKR(plan_owner_rounds(h.data(), W, cap, &cp));
   if ((uint32_t)cp.R > max_rounds)
     return mhb_set_error(MHB_ERR_NOMEM, "the plan needs %d rounds, more than %u", cp.R, max_rounds);
   for (int o = 0; o < W; ++o) {

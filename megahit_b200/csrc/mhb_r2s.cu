@@ -872,6 +872,7 @@ struct R2sShare::Impl {
   uint64_t bit_words = 0;
   int n_planes = 0;
   DevBuf pkg, word_off, len, base_off, s1_off, edge_off, planes, mplane, hist, cnt, table, totals;
+  DevBuf s1_per_read, s1_rows, s1_bsum;  // from s1_count to s1_store: records per read and owner, their scan
   S1Out so;
   PhaseTrace tr;
   cudaStream_t st = 0;
@@ -985,60 +986,47 @@ int R2sShare::s1_hist(uint64_t *hist) {
   return MHB_OK;
 }
 
-int R2sShare::s1_send(const uint8_t *owner_of_byte, int n_owners, const uint64_t *rec_base, const uint64_t *info_base,
-                      const uint64_t *my_off, const uint64_t *expect) {
+int R2sShare::s1_count(const OwnerRoute &rt) {
   Impl &d = *d_;
   const PkgChunk &c = d.c;
   const uint64_t n = c.pv.n_reads;
+  const int n_owners = rt.n_owners;
   if (n_owners < 1 || n_owners > kS1MaxOwners) return mhb_set_error(MHB_ERR_ARG, "read2sdbg: 1 .. %d owners", kS1MaxOwners);
-  if (d.m < 2 || !c.n_s1) {
-    for (int o = 0; o < n_owners; ++o)
-      if (expect[o]) return mhb_set_error(MHB_ERR_CUDA, "read2sdbg: internal: records expected from an empty share");
-    return MHB_OK;
-  }
+  if (d.m < 2 || !c.n_s1) return MHB_OK;
   const uint32_t NW = s1_layout(d.k).NW;
   const cudaStream_t st = d.st;
-  DevBuf lut, bases, infos, offs, per_read, off, bsum;
-  CKR(lut.alloc(256, "read2sdbg: owner table"));
-  CKR(bases.alloc(kS1MaxOwners * 8, "read2sdbg: owner buffers"));
-  CKR(offs.alloc(kS1MaxOwners * 8, "read2sdbg: owner offsets"));
-  CKR(per_read.alloc((size_t)n_owners * n * 4, "read2sdbg: per-read record counts per owner"));
-  CKR(off.alloc((size_t)n_owners * (n + 1) * 8, "read2sdbg: per-read record offsets per owner"));
-  CKR(bsum.alloc((n / 4096 + 4) * 8, "read2sdbg: scan sums"));
-  CK(cudaMemcpyAsync(lut.p, owner_of_byte, 256, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(bases.p, rec_base, n_owners * 8, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(offs.p, my_off, n_owners * 8, cudaMemcpyHostToDevice, st));
-  if (info_base) {
-    CKR(infos.alloc(kS1MaxOwners * 8, "read2sdbg: owner read_info buffers"));
-    CK(cudaMemcpyAsync(infos.p, info_base, n_owners * 8, cudaMemcpyHostToDevice, st));
-  }
+  CKR(d.s1_per_read.alloc((size_t)n_owners * n * 4, "read2sdbg: per-read record counts per owner"));
+  CKR(d.s1_rows.alloc((size_t)n_owners * (n + 1) * 8, "read2sdbg: per-read record offsets per owner"));
+  CKR(d.s1_bsum.alloc((n / 4096 + 4) * 8, "read2sdbg: scan sums"));
   const unsigned grid = grid_cap(n * 32, 256, 16);  // one warp per read
 #define M(WW)                                                                                                        \
   if (NW == WW)                                                                                                      \
-    k_r2s_s1_owners<WW, kS1OwnerCount><<<grid, 256, 0, st>>>(c.pv, d.k, lut.as<uint8_t>(), (u32)n_owners,             \
-                                                             per_read.as<u32>(), nullptr, nullptr, nullptr, nullptr);
+    k_r2s_s1_owners<WW, kS1OwnerCount><<<grid, 256, 0, st>>>(c.pv, d.k, rt.owner, (u32)n_owners,                     \
+                                                             d.s1_per_read.as<u32>(), nullptr, nullptr, nullptr, nullptr);
   MHB_FOR_WR(M)
 #undef M
   CK_LAUNCH();
-  std::vector<uint64_t> sent(n_owners);
   for (int o = 0; o < n_owners; ++o) {
-    u64 *oo = off.as<u64>() + (size_t)o * (n + 1);
-    CKR(scan32(st, per_read.as<u32>() + (size_t)o * n, n, oo, oo + n, bsum.as<u64>()));
-    CK(cudaMemcpyAsync(&sent[o], oo + n, 8, cudaMemcpyDeviceToHost, st));
+    u64 *oo = d.s1_rows.as<u64>() + (size_t)o * (n + 1);
+    CKR(scan32(st, d.s1_per_read.as<u32>() + (size_t)o * n, n, oo, rt.cursor + o, d.s1_bsum.as<u64>()));
   }
-  CK(cudaStreamSynchronize(st));
-  for (int o = 0; o < n_owners; ++o)
-    if (sent[o] != expect[o])
-      return mhb_set_error(MHB_ERR_CUDA, "read2sdbg: internal: %llu stage-1 records for rank %d, the histogram said %llu",
-                           (unsigned long long)sent[o], o, (unsigned long long)expect[o]);
+  return MHB_OK;
+}
+
+int R2sShare::s1_store(const OwnerRoute &rt) {
+  Impl &d = *d_;
+  const PkgChunk &c = d.c;
+  if (d.m < 2 || !c.n_s1) return MHB_OK;
+  const uint32_t NW = s1_layout(d.k).NW;
+  const unsigned grid = grid_cap(c.pv.n_reads * 32, 256, 16);
 #define M(WW)                                                                                                          \
   if (NW == WW)                                                                                                        \
-    k_r2s_s1_owners<WW, kS1OwnerWrite><<<grid, 256, 0, st>>>(c.pv, d.k, lut.as<uint8_t>(), (u32)n_owners, nullptr,       \
-                                                             off.as<u64>(), bases.as<u64>(), infos.as<u64>(), offs.as<u64>());
+    k_r2s_s1_owners<WW, kS1OwnerWrite><<<grid, 256, 0, d.st>>>(c.pv, d.k, rt.owner, (u32)rt.n_owners, nullptr,         \
+                                                               d.s1_rows.as<u64>(), rt.row0, rt.info0, rt.off);
   MHB_FOR_WR(M)
 #undef M
   CK_LAUNCH();
-  CK(cudaStreamSynchronize(st));
+  for (DevBuf *b : {&d.s1_per_read, &d.s1_rows, &d.s1_bsum}) b->release();  // after the pass (cudaFree waits for it)
   return MHB_OK;
 }
 
@@ -1102,34 +1090,20 @@ int R2sShare::s2_hist(uint64_t *hist) {
   return MHB_OK;
 }
 
-int R2sShare::s2_send(const uint8_t *owner_of_byte, int n_owners, const uint64_t *owner_base, const uint64_t *capacity,
-                      uint64_t *sent) {
+int R2sShare::s2_send(const OwnerRoute &rt) {
   Impl &d = *d_;
   const PkgChunk &c = d.c;
-  for (int o = 0; o < n_owners; ++o) sent[o] = 0;
   if (!c.n_edges) return MHB_OK;
   const uint32_t W = s2s_record_words(d.k);
-  const cudaStream_t st = d.st;
-  DevBuf lut, bases, cursor, cap;
-  CKR(lut.alloc(256, "read2sdbg: owner table"));
-  CKR(bases.alloc(n_owners * 8, "read2sdbg: owner buffers"));
-  CKR(cursor.alloc(n_owners * 8, "read2sdbg: owner cursors"));
-  CKR(cap.alloc(n_owners * 8, "read2sdbg: owner capacities"));
-  CK(cudaMemcpyAsync(lut.p, owner_of_byte, 256, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(bases.p, owner_base, n_owners * 8, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(cap.p, capacity, n_owners * 8, cudaMemcpyHostToDevice, st));
-  CK(cudaMemsetAsync(cursor.p, 0, n_owners * 8, st));
-  const OwnerSink sink{lut.as<uint8_t>(), bases.as<u64>(), cursor.as<unsigned long long>(), cap.as<u64>()};
-#define M(WW)                                                                                                       \
-  if (W == WW)                                                                                                      \
-    k_r2s_s2_extract<WW, kS2Owner><<<grid_cap(c.n_edges, 256, 16), 256, 0, st>>>(c.pv, d.k, d.so.is_solid, d.m == 1, \
-                                                                               c.n_edges, nullptr, nullptr, 0, 0, 0, \
-                                                                               nullptr, sink);
+  const OwnerSink sink{rt.owner, rt.base, (unsigned long long *)rt.cursor, rt.cap};
+#define M(WW)                                                                                                         \
+  if (W == WW)                                                                                                        \
+    k_r2s_s2_extract<WW, kS2Owner><<<grid_cap(c.n_edges, 256, 16), 256, 0, d.st>>>(c.pv, d.k, d.so.is_solid, d.m == 1, \
+                                                                                 c.n_edges, nullptr, nullptr, 0, 0, 0, \
+                                                                                 nullptr, sink);
   MHB_FOR_WR(M)
 #undef M
   CK_LAUNCH();
-  CK(cudaMemcpyAsync(sent, cursor.p, n_owners * 8, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
   return MHB_OK;
 }
 
