@@ -422,7 +422,7 @@ int mhb_plan_rounds16(const uint64_t *hist256, const uint64_t *sub_hist, uint64_
                       uint32_t *hi16_out, uint32_t cap_out);
 
 /* Read libraries larger than device memory (mhb_count_host, mhb_iterate_host, mhb_read2sdbg_host, and
- * mhb_build_host through its staged route): the `.bin` image stays in host memory and every pass over the reads
+ * mhb_build_host, whose count streams the same way): the `.bin` image stays in host memory and every pass over the reads
  * streams it through the device in chunks that end on read boundaries (two pinned staging buffers, two device chunk
  * slots; upload of chunk i overlaps the kernels of chunk i-1 and the host fill of chunk i+1).  The library is resident whenever it was before; it is streamed when the
  * resident part alone does not fit, when the plan next to it fails (count: one bucket exceeds the room left; iterate:
@@ -468,7 +468,7 @@ typedef struct {
 
 int mhb_s2s_host(const mhb_s2s_args *args, mhb_s2s_result *res);
 /* Sequence sets and edge arrays larger than device memory (mhb_s2s_host, mhb_mercy_host, and so `seq2sdbg` and the
- * staged mhb_build_host).  mhb_s2s_host keeps the sequences resident whenever they and a one-item round fit in 92 % of
+ * mhb_build_host when its seq2sdbg runs from host memory).  mhb_s2s_host keeps the sequences resident whenever they and a one-item round fit in 92 % of
  * the free device memory (a cached arena counts as free) and no chunk cap is set (mhb_read_stream_decide); otherwise
  * they stay in host memory and every pass streams them through the device in chunks that end on sequence boundaries
  * (a sequence larger than the cap gets a chunk of its own): a top-byte histogram pass, one more pass for the
@@ -545,9 +545,11 @@ typedef struct {
   uint32_t n_rounds_s1, n_rounds_s2;
 } mhb_build_result;
 
-/* A13: when the resident plan does not fit in device memory (cudaMalloc fails), or a round cap is set with
- * mhb_set_round_limit / mhb_set_s2s_round_limit, the same graph is built stage by stage - count in rounds over bucket
- * ranges -> mercy edges -> seq2sdbg in rounds - with the solid edges passing through host memory once; same outputs. */
+/* One chain of the stage drivers: count -> mercy edges -> seq2sdbg.  A stage that runs in one pass over resident data
+ * hands its result to the next on the device; otherwise (A13: it does not fit in device memory, a round cap is set with
+ * mhb_set_round_limit / mhb_set_s2s_round_limit, or the library is streamed) the result passes through host memory
+ * once, and each stage plans its rounds as mhb_count_host / mhb_mercy_host / mhb_s2s_host do.  Same outputs either
+ * way; n_sort_items is the pruned item count when seq2sdbg runs on the device, else six items per edge. */
 int mhb_build_host(const mhb_build_args *args, mhb_build_result *res);
 
 /* The 1-pass k_min build (main_read2sdbg, main_sdbg_build.cpp:88-156; `megahit --kmin-1pass`, and the route the driver

@@ -247,12 +247,16 @@ class ChunkStager {
   ChunkStager(const ChunkStager &) = delete;
   ChunkStager &operator=(const ChunkStager &) = delete;
   ~ChunkStager();
-  // n_chunks chunks of at most slot_bytes; the passes are counted into *stats
+  // n_chunks chunks of at most slot_bytes; the passes are counted into *stats.  slot_bytes = 0: no staging (upload)
   int init(size_t slot_bytes, uint64_t n_chunks, StreamStats *stats);
   size_t device_bytes() const { return 2 * slot_bytes_; }
   void bind(char *device) { dev_ = device; }  // device_bytes() bytes, 256-byte aligned
   // one pass: every chunk filled, uploaded and handed to run, in order
   int pass(void *stream, const Fill &fill, const Run &run);
+  // One pass over n_chunks pieces of host memory that need no staging: piece i, bytes [off[i], off[i+1]) of host, is
+  // copied to the same offsets of the bound device memory on the copy stream, behind the work already queued on
+  // `stream`, and run(i, its device address) is queued on `stream` behind that copy.  Counts nothing in the stats.
+  int upload(void *stream, const char *host, const std::vector<size_t> &off, const Run &run);
 
  private:
   int stage(uint64_t i, const Fill &fill);
@@ -267,6 +271,8 @@ class ChunkStager {
 
 // Every pass over a read library (mhb_stream.cu), in one of two forms:
 // - resident: the library is uploaded once into the device memory the caller binds, and a pass hands it over whole;
+//   a fixed-length library may instead go up in pieces during the first pass, which hands over each piece as a chunk
+//   while the next one is still being copied;
 // - streamed: the `.bin` image stays in host memory and goes through the device in chunks that end on read boundaries.
 //   Two pinned staging buffers and two device chunk slots: while host threads fill the staging buffer of chunk i+1,
 //   chunk i uploads on a copy stream and the compute stream works on chunk i-1.
@@ -285,8 +291,10 @@ class ReadStream {
   ReadStream(const ReadStream &) = delete;
   ReadStream &operator=(const ReadStream &) = delete;
   // host library and its index; max_chunk_bytes = 0: resident, otherwise streamed in chunks planned here
-  // (the index is read by every pass: it must outlive them)
-  int init(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, const ReadLibIndex &ix, uint64_t max_chunk_bytes);
+  // (the index is read by every pass: it must outlive them); pieces > 1: a resident fixed-length library goes up in
+  // that many pieces of a multiple of 4 reads (16-byte aligned) during the first pass
+  int init(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, const ReadLibIndex &ix, uint64_t max_chunk_bytes,
+           uint32_t pieces = 1);
   size_t device_bytes() const { return (resident_ ? 1 : 2) * slot_bytes_; }  // the library, or both chunk slots
   // device_bytes() bytes, 256-byte aligned; the resident form uploads the library there on `stream`
   int bind(void *device, void *stream);
@@ -305,7 +313,7 @@ class ReadStream {
   uint64_t bin_words_ = 0;
   const ReadLibIndex *ix_ = nullptr;
   const uint64_t *aux_off_ = nullptr;
-  std::vector<uint64_t> first_;
+  std::vector<uint64_t> first_, pieces_;  // pieces_: read bounds of the pieces still to upload
   uint64_t max_reads_ = 0;
   size_t off_at_ = 0, slot_bytes_ = 0;
   char *dev_ = nullptr;

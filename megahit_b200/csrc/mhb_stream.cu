@@ -173,7 +173,7 @@ int ChunkStager::init(size_t slot_bytes, uint64_t n_chunks, StreamStats *stats) 
   n_chunks_ = n_chunks;
   st_ = stats;
   if (!n_chunks) return MHB_OK;
-  for (int s = 0; s < 2; ++s) CK(cudaHostAlloc((void **)&host_[s], slot_bytes_, cudaHostAllocDefault));
+  for (int s = 0; s < 2 && slot_bytes_; ++s) CK(cudaHostAlloc((void **)&host_[s], slot_bytes_, cudaHostAllocDefault));
   cudaStream_t cs;
   CK(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
   copy_ = cs;
@@ -231,10 +231,24 @@ int ChunkStager::pass(void *stream, const Fill &fill, const Run &run) {
   return MHB_OK;
 }
 
+int ChunkStager::upload(void *stream, const char *host, const std::vector<size_t> &off, const Run &run) {
+  cudaStream_t st = (cudaStream_t)stream, cs = (cudaStream_t)copy_;
+  CK(cudaEventRecord((cudaEvent_t)ev_[0], st));
+  CK(cudaStreamWaitEvent(cs, (cudaEvent_t)ev_[0], 0));
+  for (uint64_t i = 0; i < n_chunks_; ++i) {
+    CK(cudaMemcpyAsync(dev_ + off[i], host + off[i], off[i + 1] - off[i], cudaMemcpyHostToDevice, cs));
+    CK(cudaEventRecord((cudaEvent_t)ev_[4 * i + 1], cs));
+    CK(cudaStreamWaitEvent(st, (cudaEvent_t)ev_[4 * i + 1], 0));
+    CKR(run(i, dev_ + off[i]));
+  }
+  return MHB_OK;
+}
+
 // ------------------------------------------------------------------------------------------------
 // ReadStream
 // ------------------------------------------------------------------------------------------------
-int ReadStream::init(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, const ReadLibIndex &ix, uint64_t max_chunk_bytes) {
+int ReadStream::init(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, const ReadLibIndex &ix, uint64_t max_chunk_bytes,
+                     uint32_t pieces) {
   resident_ = max_chunk_bytes == 0;
   bin_ = bin;
   bin_words_ = bin_words;
@@ -256,13 +270,20 @@ int ReadStream::init(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, 
   off_at_ = pad256(((max_words * 4 + 15) & ~(size_t)15) + 16);
   slot_bytes_ = off_at_ + (ix_->fixed_len ? 0 : (aux_off_ ? 2 : 1) * pad256((max_reads_ + 1) * 8));
   g_st.chunks = n_chunks();
+  pieces_.clear();
+  if (resident_ && ix.fixed_len && pieces > 1) {
+    const uint64_t per = ((n_reads + pieces - 1) / pieces + 3) & ~(uint64_t)3;
+    for (uint64_t r = 0; r < n_reads; r += per) pieces_.push_back(r);
+    pieces_.push_back(n_reads);
+    return stager_.init(0, pieces_.size() - 1, &g_st);
+  }
   return stager_.init(slot_bytes_, n_chunks(), &g_st);
 }
 
 int ReadStream::bind(void *device, void *stream) {
   dev_ = (char *)device;
   stager_.bind(dev_);
-  if (!resident_) return MHB_OK;
+  if (!resident_ || !pieces_.empty()) return MHB_OK;
   cudaStream_t st = (cudaStream_t)stream;
   const uint64_t n_reads = first_[1];
   if (bin_words_) CK(cudaMemcpyAsync(dev_, bin_, bin_words_ * 4, cudaMemcpyHostToDevice, st));
@@ -314,6 +335,20 @@ int ReadStream::fill(uint64_t i, char *h, ChunkStager::Copies *up) const {
 
 int ReadStream::pass(void *stream, const std::function<int(const ReadChunkView &)> &fn) {
   if (!dev_) return mhb_set_error(MHB_ERR_ARG, "internal: read library without device memory");
+  if (resident_ && !pieces_.empty()) {
+    std::vector<uint64_t> p;
+    p.swap(pieces_);
+    std::vector<size_t> off;
+    for (uint64_t r : p) off.push_back(ix_->word_of(r) * 4);
+    return stager_.upload(stream, (const char *)bin_, off, [&](uint64_t i, const char *piece) {
+      ReadChunkView v = view(0, piece);
+      v.index = i;
+      v.first_read = p[i];
+      v.n_reads = p[i + 1] - p[i];
+      v.bin_words = ix_->word_of(p[i + 1]) - ix_->word_of(p[i]);
+      return fn(v);
+    });
+  }
   if (resident_) return fn(view(0, dev_));
   return stager_.pass(
       stream, [this](uint64_t i, char *h, ChunkStager::Copies *up) { return fill(i, h, up); },
