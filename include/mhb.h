@@ -575,7 +575,8 @@ int mhb_build_host(const mhb_build_args *args, mhb_build_result *res);
  * returns MHB_ERR_NOMEM, as do bit planes and chunk buffers that alone do not fit. */
 int mhb_read2sdbg_host(const mhb_build_args *args, mhb_build_result *res);
 /* Caps the stage-1 records / stage-2 items of one read2sdbg round regardless of memory (0 = derive from free device
- * memory).  Independent of mhb_set_round_limit / mhb_set_s2s_round_limit.  The result does not depend on the caps. */
+ * memory), on one GPU and, per owner, on several (mhb_read2sdbg_run_multi).  Independent of mhb_set_round_limit /
+ * mhb_set_s2s_round_limit.  The result does not depend on the caps. */
 int mhb_set_r2s_round_limit(uint64_t max_s1_records, uint64_t max_s2_items);
 
 /* `megahit_core iterate` (SURVEY.md 8f N2; main_iterate.cpp:117-221, iterate/contig_flank_index.h:16-221,
@@ -784,9 +785,15 @@ int mhb_iterate_run_multi(const mhb_iterate_opts *opts, int n_gpus);
  * bucket partition and kmsort emulation see the reference's bucket input order; the owners mark their solid edges and
  * mercy candidates into bit planes of the whole library, which every rank merges over its share's words before the
  * mercy step.  The stage-2 items meet on their owners in the same way; each owner sorts, collapses and emits its bucket
- * range.  Rank 0 writes P.sdbg_info and P.counting (m > 1).  Resident only: every rank holds the planes of the whole
- * library (1 bit per base, 4 with need_mercy) next to its share and receive buffers; what does not fit is
- * MHB_ERR_NOMEM.  The caller must not have initialised CUDA in this process. */
+ * range.  Rank 0 writes P.sdbg_info and P.counting (m > 1).  Both sort stages run in rounds over ascending bucket
+ * sub-ranges of every owner's range when its records / items do not fit its device at once (92 % of the free memory,
+ * split evenly among the ranks sharing a device) or exceed mhb_set_r2s_round_limit (mhb_plan_count_owner_rounds); each
+ * round of stage 1 adds to the same planes and multiplicity histogram, and the rounds of stage 2 follow each other in
+ * P.sdbg.<r>.  A single bucket larger than one round is MHB_ERR_NOMEM, naming the bucket and the rank, before any
+ * receive buffer exists.  What stays resident on every rank: its share of the reads and the planes of the whole
+ * library (1 bit per base, 4 with need_mercy); what does not fit is MHB_ERR_NOMEM.  Rank 0 logs the plan ("read2sdbg
+ * plan: stage 1 in R1 rounds, stage 2 in R2 rounds") and each stage's loads (largest owner, leading byte and bucket).
+ * The caller must not have initialised CUDA in this process. */
 int mhb_read2sdbg_run_multi(const mhb_read2sdbg_opts *opts, int n_gpus);
 /* The owner ranges of a multi-GPU read2sdbg stage (host only): the 65536-bin bucket histogram hist16 folded into its
  * 256 leading bytes, cut into n_ranks contiguous byte ranges as the count exchange cuts them; rank o owns the buckets

@@ -395,7 +395,8 @@ struct OwnerRoute {
 // One rank's share [first, end) of the reads of a build, resident on the current device as one package chunk: read
 // indices are local, bases - stage-1 payload positions and bit-plane indices - global, and the bit planes (solid; with
 // need_mercy the three candidate planes after it, in one allocation) cover the whole library's word grid.  Records
-// reach their owners (ranks of contiguous leading-byte ranges) through an OwnerRoute.
+// reach their owners (ranks of contiguous leading-byte ranges) through an OwnerRoute, one round over ascending bucket
+// sub-ranges at a time (rt.lo / rt.hi).
 class R2sShare {
  public:
   R2sShare();
@@ -406,28 +407,37 @@ class R2sShare {
   int load(const mhb_build_args *a, const ReadLibIndex &li, uint64_t first, uint64_t end);
   uint32_t s1_record_words() const;  // words of a stage-1 record row
   bool s1_narrow() const;            // read_info in a side array of 8 bytes per row
-  uint64_t s1_round_cap() const;     // most stage-1 records one owner may sort
+  // The most stage-1 records / stage-2 items one owner takes in one round (at most n_total): the largest round whose
+  // receive buffer and sort pass fit `avail` device bytes next to the stage's fixed arrays (stage 1: the per-read
+  // arrays of n_owners owners), capped by mhb_set_r2s_round_limit and, stage 1, by the narrow layout's 2^32 rows.
+  // 0 when not even one fits.
+  uint64_t s1_round_budget(size_t avail, int n_owners, uint64_t n_total) const;
+  uint64_t s2_round_budget(size_t avail, uint64_t n_total) const;
   // hist[65536] = the 16-bit bucket ids of the share's stage-1 records / stage-2 items (s2 after mercy_count)
   int s1_hist(uint64_t *hist);
   int s2_hist(uint64_t *hist);
-  // the share's stage-1 records to their owners in global read order, in two passes: s1_count puts the records of
-  // every owner into rt.cursor, s1_store stores them at rt.row0 / rt.info0 from row rt.off (it has no capacity: the
-  // caller checks the counts in between)
+  // the share's stage-1 records of one round to their owners in global read order, in two passes: s1_count puts the
+  // records of every owner into rt.cursor, s1_store stores them at rt.row0 / rt.info0 from row rt.off (it has no
+  // capacity: the caller checks the counts in between).  The per-read arrays between them are kept for the stage.
   int s1_count(const OwnerRoute &rt);
   int s1_store(const OwnerRoute &rt);
-  // owner: stable bucket partition, kmsort and Lv2Postprocess of the n records received (overwritten), into the local
-  // planes and multiplicity histogram
-  int s1_own(uint32_t *recs, uint64_t *info, uint64_t n);
+  // owner, once per round: stable bucket partition, kmsort and Lv2Postprocess of the n records received (overwritten),
+  // into the local planes and multiplicity histogram.  Its buffers are sized for n_max, the largest round, and kept.
+  int s1_own(uint32_t *recs, uint64_t *info, uint64_t n, uint64_t n_max);
+  void s1_end();  // after the last round: the stage-1 round buffers go
   void *planes() const;  // the allocation of the planes, for CUDA IPC (nullptr when m == 1)
   // OR another rank's planes (same layout) into mine over my share's words
   int or_planes(const void *peer_planes);
   // the mercy step and the stage-2 item count over the share
   int mercy_count(uint64_t *n_items, uint64_t *n_mercy);
-  // every stage-2 item of the share to its owner through rt (OwnerSink)
+  // the share's stage-2 items of one round to their owners through rt (OwnerSink)
   int s2_send(const OwnerRoute &rt);
-  // owner: relaxed sort, collapse and emitter (label_fmt 1) of the n items received (overwritten); SdBG bytes, bucket
-  // table (65536 x {offset, items, tips, large_mul}) and the emitter's 16 totals
-  int s2_own(uint32_t *items, uint64_t n, std::vector<uint8_t> *bytes, std::vector<uint64_t> *table, uint64_t *totals);
+  // owner, once per round in ascending bucket order: relaxed sort, collapse and emitter (label_fmt 1) of the n items
+  // received (overwritten), appended to the owner's output (SdbgStitch); buffers sized for n_max and kept
+  int s2_own(uint32_t *items, uint64_t n, uint64_t n_max);
+  // after the last round: SdBG bytes, bucket table (65536 x {offset, items, tips, large_mul}) and the emitter's 16
+  // totals of every round; the round buffers go
+  void s2_result(std::vector<uint8_t> *bytes, std::vector<uint64_t> *table, uint64_t *totals);
   int counting(uint64_t *hist);  // the multiplicity histogram (65536) of the records this rank owned
   uint64_t n_reads() const;
 

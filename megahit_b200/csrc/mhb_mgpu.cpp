@@ -32,6 +32,8 @@
 // `read2sdbg` (mhb_read2sdbg_run_multi): the stage-1 records reach their owners in global read order, the owners run
 // stage 1 into planes of the whole library, every rank ORs all planes over its share's words, runs the mercy step over
 // its share and sends its stage-2 items to their owners, which sort, collapse and emit as the single-GPU read2sdbg does.
+// Both sort stages run in rounds over ascending bucket ranges when an owner's records do not fit its device at once
+// (or exceed mhb_set_r2s_round_limit), as the count's records do.
 #include <cuda_runtime.h>
 #include <dirent.h>
 #include <fcntl.h>
@@ -348,14 +350,19 @@ struct Job {
   std::string prefix;
 };
 
-// The most count records this rank may take in one round: the largest round (round_bytes, as the single-GPU count
-// plans it) that fits its part of the device's free memory - the ranks bound to one device split it evenly - capped by
-// mhb_set_round_limit.  Called by every rank between two barriers, when every share is on its device.
-uint64_t count_round_budget(int rank, int world, uint64_t n_total, uint32_t k, int32_t m) {
+// This rank's part of its device's free memory for the rounds of a stage: 92 % of it, split evenly among the ranks
+// bound to the device.  Called by every rank between two barriers, when nobody allocates.
+size_t rank_round_bytes(int rank, int world) {
   int n_dev = 1, sharers = 0;
   CKC(cudaGetDeviceCount(&n_dev));
   for (int q = 0; q < world; ++q) sharers += q % n_dev == rank % n_dev;
-  const size_t avail = (size_t)(0.92 * (double)free_device_bytes()) / (size_t)std::max(1, sharers);
+  return (size_t)(0.92 * (double)free_device_bytes()) / (size_t)std::max(1, sharers);
+}
+
+// The most count records this rank may take in one round: the largest round (round_bytes, as the single-GPU count
+// plans it) that fits rank_round_bytes, capped by mhb_set_round_limit.  Called when every share is on its device.
+uint64_t count_round_budget(int rank, int world, uint64_t n_total, uint32_t k, int32_t m) {
+  const size_t avail = rank_round_bytes(rank, world);
   const size_t fixed = (size_t)64 << 20;  // round arrays, counters, the exchange's small tables
   const uint32_t WR = mhb_count_record_words(k), WE = mhb_words_per_edge(k);
   uint64_t cap = largest_round(std::max<uint64_t>(n_total, 1), fixed, avail,
@@ -933,6 +940,29 @@ struct R2sJob {
   std::string prefix;
 };
 
+// Rank 0: the loads of a stage's plan - the records of the largest owner, leading byte and bucket - from which a
+// round cap (mhb_set_r2s_round_limit) can be chosen
+void log_r2s_loads(const Exchange &X, const OwnerExchange &ex, int stage) {
+  if (X.rank) return;
+  std::vector<uint64_t> tot(65536, 0);
+  for (int s = 0; s < X.world; ++s)
+    for (int b = 0; b < 65536; ++b) tot[b] += ex.hist[(size_t)s * 65536 + b];
+  uint64_t owner = 0, byte = 0, bucket = 0;
+  for (int o = 0; o < X.world; ++o) {
+    uint64_t n = 0;
+    for (uint32_t b = ex.plan.bounds[o] << 8; b < ex.plan.bounds[o + 1] << 8; ++b) n += tot[b];
+    owner = std::max(owner, n);
+  }
+  for (int b = 0; b < 256; ++b) {
+    uint64_t n = 0;
+    for (int c = 0; c < 256; ++c) n += tot[b << 8 | c];
+    byte = std::max(byte, n);
+  }
+  for (uint64_t n : tot) bucket = std::max(bucket, n);
+  XINFO("read2sdbg stage %d: largest owner %llu, largest leading byte %llu, largest bucket %llu\n", stage,
+        (unsigned long long)owner, (unsigned long long)byte, (unsigned long long)bucket);
+}
+
 void r2s_worker(const R2sJob &J, Exchange &X) {
   const int W = X.world, r = X.rank;
   const uint32_t k = J.a.k, W2 = mhb_s2s_record_words(k);
@@ -942,26 +972,34 @@ void r2s_worker(const R2sJob &J, Exchange &X) {
   CKL(sh.load(&J.a, *J.li, J.first[r], J.first[r + 1]));
   std::vector<uint64_t> h16(65536);
   uint64_t n_s1_own = 0;
+  int R1 = 0;
 
-  // ---- stage 1: my records straight into their owners' buffers, in global read order; each owner's planes ----
+  // ---- stage 1: my records straight into their owners' buffers, in global read order, in rounds over ascending
+  // bucket ranges; each owner's planes ----
   if (m > 1) {
     CKL(sh.s1_hist(h16.data()));
-    const uint32_t RW = sh.s1_record_words();
     OwnerExchange ex;
-    ex.gather(X, h16.data(), 65536);
-    ex.open(X, nullptr, RW * 4, "read2sdbg: stage-1 records received",
+    ex.gather(X, h16.data(), 65536);  // ... behind which every share and its planes are on the device
+    uint64_t n_s1 = 0;
+    for (uint64_t c : ex.hist) n_s1 += c;
+    const uint64_t budget = sh.s1_round_budget(rank_round_bytes(r, W), W, n_s1);
+    if (!budget) fail_nomem("%zu free bytes for this rank: not even a one-record stage-1 round fits", rank_round_bytes(r, W));
+    ex.open(X, X.gather(&budget, 1).data(), sh.s1_record_words() * 4, "read2sdbg: stage-1 records received",
             sh.s1_narrow() ? "read2sdbg: stage-1 read_info received" : nullptr);
+    log_r2s_loads(X, ex, 1);
+    R1 = ex.plan.R;
     n_s1_own = ex.n_own;
-    if (n_s1_own > sh.s1_round_cap())
-      fail_nomem("%llu stage-1 records in my bucket range, more than the %llu one pass sorts (%llu bytes)",
-                 (unsigned long long)n_s1_own, (unsigned long long)sh.s1_round_cap(),
-                 (unsigned long long)(n_s1_own * RW * 4));
-    ex.send(X, 0, "stage-1 records", [&](const OwnerRoute &rt) {
-      CKL(sh.s1_count(rt));
-      ex.check(X, 0, "stage-1 records");  // the stores have no capacity: they run once the counts match the plan
-      CKL(sh.s1_store(rt));
-    });
-    CKL(sh.s1_own(ex.mine.as<uint32_t>(), ex.info.as<uint64_t>(), n_s1_own));
+    const uint64_t n_max = *std::max_element(ex.own.begin(), ex.own.end());
+    for (int t = 0; t < R1; ++t) {
+      ex.send(X, t, "stage-1 records", [&](const OwnerRoute &rt) {
+        CKL(sh.s1_count(rt));
+        ex.check(X, t, "stage-1 records");  // the stores have no capacity: they run once the counts match the plan
+        CKL(sh.s1_store(rt));
+      });
+      CKL(sh.s1_own(ex.mine.as<uint32_t>(), ex.info.as<uint64_t>(), ex.own[t], n_max));
+      if (t + 1 < R1) X.barrier();  // nobody stores into my receive buffer before I have sorted it
+    }
+    sh.s1_end();
     ex.close(X);
 
     // ---- plane merge: the words of my share's reads, OR-ed over every rank's planes (read through CUDA IPC) ----
@@ -982,16 +1020,30 @@ void r2s_worker(const R2sJob &J, Exchange &X) {
   uint64_t n_items = 0, n_mercy = 0;
   CKL(sh.mercy_count(&n_items, &n_mercy));
 
-  // ---- stage 2: every item straight into its owner's buffer; the owner sorts, collapses and emits ----
+  // ---- stage 2: every item straight into its owner's buffer, in rounds over ascending bucket ranges; the owner sorts,
+  // collapses and emits each round, and its rounds follow each other in bucket order ----
   CKL(sh.s2_hist(h16.data()));
   OwnerExchange ex;
-  ex.gather(X, h16.data(), 65536);
-  ex.open(X, nullptr, W2 * 4, "read2sdbg: stage-2 items received");
-  ex.send(X, 0, "stage-2 items", [&](const OwnerRoute &rt) { CKL(sh.s2_send(rt)); });
+  ex.gather(X, h16.data(), 65536);  // ... behind which the stage-1 buffers are gone on every rank
+  uint64_t n_s2 = 0;
+  for (uint64_t c : ex.hist) n_s2 += c;
+  const uint64_t budget = sh.s2_round_budget(rank_round_bytes(r, W), n_s2);
+  if (!budget) fail_nomem("%zu free bytes for this rank: not even a one-item stage-2 round fits", rank_round_bytes(r, W));
+  ex.open(X, X.gather(&budget, 1).data(), W2 * 4, "read2sdbg: stage-2 items received");
+  log_r2s_loads(X, ex, 2);
+  const int R2 = ex.plan.R;
+  if (r == 0)
+    XINFO("read2sdbg plan: stage 1 in %d round%s, stage 2 in %d round%s\n", R1, R1 == 1 ? "" : "s", R2, R2 == 1 ? "" : "s");
+  const uint64_t n_max = *std::max_element(ex.own.begin(), ex.own.end());
+  for (int t = 0; t < R2; ++t) {
+    ex.send(X, t, "stage-2 items", [&](const OwnerRoute &rt) { CKL(sh.s2_send(rt)); });
+    CKL(sh.s2_own(ex.mine.as<uint32_t>(), ex.own[t], n_max));
+    if (t + 1 < R2) X.barrier();  // nobody stores into my receive buffer before I have sorted it
+  }
   std::vector<uint8_t> bytes;
   std::vector<uint64_t> table;
   uint64_t totals[16];
-  CKL(sh.s2_own(ex.mine.as<uint32_t>(), ex.n_own, &bytes, &table, totals));
+  sh.s2_result(&bytes, &table, totals);
   ex.close(X);
   sdbg_publish(X, totals, bytes, std::move(table), J.prefix);
   if (m > 1) {

@@ -873,6 +873,9 @@ struct R2sShare::Impl {
   int n_planes = 0;
   DevBuf pkg, word_off, len, base_off, s1_off, edge_off, planes, mplane, hist, cnt, table, totals;
   DevBuf s1_per_read, s1_rows, s1_bsum;  // from s1_count to s1_store: records per read and owner, their scan
+  DevBuf sort_b, sort_ws, pa, pb;        // the owner's sort buffer, workspace and narrow pairs, for the largest round
+  S2Bufs s2b;
+  SdbgStitch out;                        // the owner's stage-2 rounds
   S1Out so;
   PhaseTrace tr;
   cudaStream_t st = 0;
@@ -882,8 +885,28 @@ R2sShare::R2sShare() : d_(new Impl) {}
 R2sShare::~R2sShare() { delete d_; }
 uint32_t R2sShare::s1_record_words() const { return s1_layout(d_->k).RW; }
 bool R2sShare::s1_narrow() const { return s1_layout(d_->k).narrow; }
-uint64_t R2sShare::s1_round_cap() const { return ::s1_round_cap(s1_layout(d_->k)); }
 void *R2sShare::planes() const { return d_->planes.p; }
+
+// fixed: the exchange's route and small tables, counters, and the buffers an allocation rounds up to
+static constexpr size_t kOwnerFixed = (size_t)64 << 20;
+
+uint64_t R2sShare::s1_round_budget(size_t avail, int n_owners, uint64_t n_total) const {
+  const S1Layout l = s1_layout(d_->k);
+  const uint64_t n = d_->c.pv.n_reads;
+  const size_t fixed = kOwnerFixed + (size_t)n_owners * (pad256(n * 4) + pad256((n + 1) * 8)) + pad256((n / 4096 + 4) * 8);
+  // s1_pass_bytes holds the receive buffer (the records) and, narrow, its read_info rows
+  uint64_t cap = largest_round(std::max<uint64_t>(n_total, 1), fixed, avail, [&](uint64_t r) { return s1_pass_bytes(r, l); });
+  if (cap && g_r2s_s1_limit) cap = std::min(cap, g_r2s_s1_limit);
+  return std::min(cap, ::s1_round_cap(l));
+}
+
+uint64_t R2sShare::s2_round_budget(size_t avail, uint64_t n_total) const {
+  const uint32_t k = d_->k;
+  uint64_t cap = largest_round(std::max<uint64_t>(n_total, 1), kOwnerFixed, avail,
+                               [&](uint64_t r) { return s2_pass_bytes(r, s2s_record_words(k), k); });
+  if (cap && g_r2s_s2_limit) cap = std::min(cap, g_r2s_s2_limit);
+  return cap;
+}
 uint64_t R2sShare::n_reads() const { return d_->c.pv.n_reads; }
 
 namespace {
@@ -995,13 +1018,13 @@ int R2sShare::s1_count(const OwnerRoute &rt) {
   if (d.m < 2 || !c.n_s1) return MHB_OK;
   const uint32_t NW = s1_layout(d.k).NW;
   const cudaStream_t st = d.st;
-  CKR(d.s1_per_read.alloc((size_t)n_owners * n * 4, "read2sdbg: per-read record counts per owner"));
-  CKR(d.s1_rows.alloc((size_t)n_owners * (n + 1) * 8, "read2sdbg: per-read record offsets per owner"));
-  CKR(d.s1_bsum.alloc((n / 4096 + 4) * 8, "read2sdbg: scan sums"));
+  CKR(d.s1_per_read.ensure((size_t)n_owners * n * 4, "read2sdbg: per-read record counts per owner"));
+  CKR(d.s1_rows.ensure((size_t)n_owners * (n + 1) * 8, "read2sdbg: per-read record offsets per owner"));
+  CKR(d.s1_bsum.ensure((n / 4096 + 4) * 8, "read2sdbg: scan sums"));
   const unsigned grid = grid_cap(n * 32, 256, 16);  // one warp per read
 #define M(WW)                                                                                                        \
   if (NW == WW)                                                                                                      \
-    k_r2s_s1_owners<WW, kS1OwnerCount><<<grid, 256, 0, st>>>(c.pv, d.k, rt.owner, (u32)n_owners,                     \
+    k_r2s_s1_owners<WW, kS1OwnerCount><<<grid, 256, 0, st>>>(c.pv, d.k, rt.owner, (u32)n_owners, rt.lo, rt.hi,       \
                                                              d.s1_per_read.as<u32>(), nullptr, nullptr, nullptr, nullptr);
   MHB_FOR_WR(M)
 #undef M
@@ -1021,28 +1044,31 @@ int R2sShare::s1_store(const OwnerRoute &rt) {
   const unsigned grid = grid_cap(c.pv.n_reads * 32, 256, 16);
 #define M(WW)                                                                                                          \
   if (NW == WW)                                                                                                        \
-    k_r2s_s1_owners<WW, kS1OwnerWrite><<<grid, 256, 0, d.st>>>(c.pv, d.k, rt.owner, (u32)rt.n_owners, nullptr,         \
-                                                               d.s1_rows.as<u64>(), rt.row0, rt.info0, rt.off);
+    k_r2s_s1_owners<WW, kS1OwnerWrite><<<grid, 256, 0, d.st>>>(c.pv, d.k, rt.owner, (u32)rt.n_owners, rt.lo, rt.hi,   \
+                                                               nullptr, d.s1_rows.as<u64>(), rt.row0, rt.info0, rt.off);
   MHB_FOR_WR(M)
 #undef M
   CK_LAUNCH();
-  for (DevBuf *b : {&d.s1_per_read, &d.s1_rows, &d.s1_bsum}) b->release();  // after the pass (cudaFree waits for it)
   return MHB_OK;
 }
 
-int R2sShare::s1_own(uint32_t *recs, uint64_t *info, uint64_t n) {
+int R2sShare::s1_own(uint32_t *recs, uint64_t *info, uint64_t n, uint64_t n_max) {
   Impl &d = *d_;
   if (!n) return MHB_OK;
   const S1Layout l = s1_layout(d.k);
-  DevBuf b, ws, pa, pb;
-  CKR(b.alloc((size_t)n * l.RW * 4 + 16, "read2sdbg: records (sort buffer)"));
-  CKR(ws.alloc(s1_ws_bytes(n, l), "read2sdbg: sort workspace"));
+  CKR(d.sort_b.ensure((size_t)n_max * l.RW * 4 + 16, "read2sdbg: records (sort buffer)"));
+  CKR(d.sort_ws.ensure(s1_ws_bytes(n_max, l), "read2sdbg: sort workspace"));
   if (l.narrow) {
-    CKR(pa.alloc((size_t)n * 8 + 16, "read2sdbg: bucket partition pairs"));
-    CKR(pb.alloc((size_t)n * 8 + 16, "read2sdbg: bucket partition pairs (sort buffer)"));
+    CKR(d.pa.ensure((size_t)n_max * 8 + 16, "read2sdbg: bucket partition pairs"));
+    CKR(d.pb.ensure((size_t)n_max * 8 + 16, "read2sdbg: bucket partition pairs (sort buffer)"));
   }
-  const S1Bufs bufs{recs, b.as<u32>(), ws.p, l.narrow ? info : nullptr, pa.as<u32>(), pb.as<u32>()};
+  const S1Bufs bufs{recs, d.sort_b.as<u32>(), d.sort_ws.p, l.narrow ? info : nullptr, d.pa.as<u32>(), d.pb.as<u32>()};
   return s1_sort_post(d.st, d.shape, d.k, d.m, d.mercy, d.so, d.hist.as<unsigned long long>(), d.tr, bufs, n);
+}
+
+void R2sShare::s1_end() {
+  Impl &d = *d_;
+  for (DevBuf *b : {&d.s1_per_read, &d.s1_rows, &d.s1_bsum, &d.sort_b, &d.sort_ws, &d.pa, &d.pb}) b->release();
 }
 
 int R2sShare::or_planes(const void *peer_planes) {
@@ -1100,36 +1126,34 @@ int R2sShare::s2_send(const OwnerRoute &rt) {
   if (W == WW)                                                                                                        \
     k_r2s_s2_extract<WW, kS2Owner><<<grid_cap(c.n_edges, 256, 16), 256, 0, d.st>>>(c.pv, d.k, d.so.is_solid, d.m == 1, \
                                                                                  c.n_edges, nullptr, nullptr, 0, 0, 0, \
-                                                                                 nullptr, sink);
+                                                                                 nullptr, sink, rt.lo, rt.hi);
   MHB_FOR_WR(M)
 #undef M
   CK_LAUNCH();
   return MHB_OK;
 }
 
-int R2sShare::s2_own(uint32_t *items, uint64_t n, std::vector<uint8_t> *bytes, std::vector<uint64_t> *table,
-                     uint64_t *totals) {
+int R2sShare::s2_own(uint32_t *items, uint64_t n, uint64_t n_max) {
   Impl &d = *d_;
-  bytes->clear();
-  table->assign((size_t)MHB_NUM_BUCKETS * 4, 0);
-  memset(totals, 0, 16 * 8);
   if (!n) return MHB_OK;
   const uint32_t W = s2s_record_words(d.k);
-  DevBuf b, ws;
-  CKR(b.alloc((size_t)n * W * 4 + 16, "read2sdbg: stage-2 items (sort buffer)"));
-  CKR(ws.alloc(mhb_s2s_sort_workspace_bytes(n, d.k), "read2sdbg: sort workspace"));
-  S2Bufs sb;
+  CKR(d.sort_b.ensure((size_t)n_max * W * 4 + 16, "read2sdbg: stage-2 items (sort buffer)"));
+  CKR(d.sort_ws.ensure(mhb_s2s_sort_workspace_bytes(n_max, d.k), "read2sdbg: sort workspace"));
   uint64_t n_u = 0, cap_bytes = 0;
-  CKR(s2_sort_emit(d.st, d.k, items, b.as<u32>(), ws.p, sb, n, d.table.as<u64>(), d.totals.as<u64>(),
+  CKR(s2_sort_emit(d.st, d.k, items, d.sort_b.as<u32>(), d.sort_ws.p, d.s2b, n, d.table.as<u64>(), d.totals.as<u64>(),
                    d.cnt.as<unsigned long long>(), d.tr, &n_u, &cap_bytes));
-  CK(cudaMemcpyAsync(totals, d.totals.p, 16 * 8, cudaMemcpyDeviceToHost, d.st));
-  CK(cudaStreamSynchronize(d.st));
-  if (totals[0] > cap_bytes) return mhb_set_error(MHB_ERR_NOMEM, "internal: SdBG byte stream exceeds capacity");
-  bytes->resize(totals[0]);
-  if (totals[0]) CK(cudaMemcpyAsync(bytes->data(), sb.bytes.p, totals[0], cudaMemcpyDeviceToHost, d.st));
-  CK(cudaMemcpyAsync(table->data(), d.table.p, (size_t)MHB_NUM_BUCKETS * 32, cudaMemcpyDeviceToHost, d.st));
-  CK(cudaStreamSynchronize(d.st));
-  return MHB_OK;
+  return d.out.append(d.st, d.s2b.bytes.as<uint8_t>(), cap_bytes, d.table.as<u64>(), d.totals.as<u64>());
+}
+
+void R2sShare::s2_result(std::vector<uint8_t> *bytes, std::vector<uint64_t> *table, uint64_t *totals) {
+  Impl &d = *d_;
+  bytes->swap(d.out.bytes);
+  table->swap(d.out.table);
+  memcpy(totals, d.out.tot, 16 * 8);
+  d.out = SdbgStitch();
+  for (DevBuf *b : {&d.sort_b, &d.sort_ws, &d.s2b.tile_heads, &d.s2b.tile_off, &d.s2b.bsum, &d.s2b.heads, &d.s2b.scr,
+                    &d.s2b.bytes})
+    b->release();
 }
 
 int R2sShare::counting(uint64_t *hist) {

@@ -635,18 +635,22 @@ __global__ void __launch_bounds__(256) k_r2s_s1_range(PkgView pv, u32 k, u32 lo,
 }
 
 // Stage 1 on several GPUs: every record of a rank's share straight into the receive buffer of the rank that owns its
-// leading byte, in global read order.  One warp per read, lane = emission index, as k_r2s_s1_range; the lanes of a
-// batch are grouped by owner (__match_any_sync) and s_run holds, per owner, the read's records placed so far.
-//   kS1OwnerCount: per_read[o * n_reads + r] = records of read r for owner o
+// leading byte, in global read order, one round over bucket ranges at a time.  A record of bucket id b goes to owner
+// o = owner[b >> 8] only when round_lo[o] <= b <= round_hi[o] (an empty range, lo > hi, sends nothing to o); both modes
+// apply the same test, so the counts and the stores agree.  One warp per read, lane = emission index, as
+// k_r2s_s1_range; the lanes of a batch are grouped by owner (__match_any_sync) and s_run holds, per owner, the read's
+// records placed so far.
+//   kS1OwnerCount: per_read[o * n_reads + r] = records of read r for owner o in the round
 //   kS1OwnerWrite: the record goes to row my_off[o] + off[o * (n_reads + 1) + r] + its rank among read r's records for
 //                  o, of owner o's buffer rec_base[o] (narrow layout: read_info at that row of info_base[o]; the row
-//                  index the record carries is that owner-local row)
+//                  index the record carries is that owner-local row of the round)
 // The shares ascend with the rank and my_off[o] puts this rank's block after those of the lower ranks, so every owner
-// holds its records in global read order - the reference's bucket input order - without an atomic.
+// holds the records of its round in global read order - the reference's bucket input order - without an atomic.
 static constexpr int kS1MaxOwners = 16;
 enum { kS1OwnerCount = 0, kS1OwnerWrite = 1 };
 template <int NW, int MODE>
 __global__ void __launch_bounds__(256) k_r2s_s1_owners(PkgView pv, u32 k, const uint8_t *__restrict__ owner, u32 n_owners,
+                                                      const u32 *__restrict__ round_lo, const u32 *__restrict__ round_hi,
                                                       u32 *__restrict__ per_read, const u64 *__restrict__ off,
                                                       const u64 *__restrict__ rec_base, const u64 *__restrict__ info_base,
                                                       const u64 *__restrict__ my_off) {
@@ -669,16 +673,19 @@ __global__ void __launch_bounds__(256) k_r2s_s1_owners(PkgView pv, u32 k, const 
           u32 p, want;
           s1_emission(L, k, e, p, want);
           make_s1_record<NW>(s, nwords, L, k, p, want, base, rec);
-          o = __ldg(owner + (rec[0] >> 24));
+          const u32 b = rec[0] >> 16;
+          o = __ldg(owner + (b >> 8));
+          if (b < __ldg(round_lo + o) || b > __ldg(round_hi + o)) o = 0xFFFFFFFFu;  // not in o's range this round
         }
+        const bool in = o != 0xFFFFFFFFu;
         const u32 peers = __match_any_sync(0xffffffffu, o);
-        if (MODE == kS1OwnerWrite && e < n_e) {
+        if (MODE == kS1OwnerWrite && in) {
           const u64 row = my_off[o] + off[(u64)o * (pv.n_reads + 1) + r] + s_run[warp][o] + __popc(peers & lt);
           s1_store<NW>(reinterpret_cast<u32 *>(rec_base[o]), info_base ? reinterpret_cast<u64 *>(info_base[o]) : nullptr,
                        row, rec);
         }
         __syncwarp();
-        if (e < n_e && lane == (u32)__ffs(peers) - 1) s_run[warp][o] += __popc(peers);
+        if (in && lane == (u32)__ffs(peers) - 1) s_run[warp][o] += __popc(peers);
         __syncwarp();
       }
     }
@@ -1008,14 +1015,23 @@ MHB_HD u32 r2s_edge_types(const u32 *is_solid, bool sure, u64 b, u32 i, u32 L, u
 // MODE kS2Count: total number of items -> *cursor.  kS2Write: items appended at recs[*cursor ...] in no particular
 // order (whole-record sort keys).  For stage 2 in rounds: kS2Hist adds every item's 16-bit bucket id (top of word 0)
 // to hist[65536]; kS2Range appends only the items whose bucket id lies in [lo, hi].  On several GPUs, kS2Owner hands
-// every item to `sink`, which stores it in the receive buffer of the rank owning its leading byte.  One thread per
-// (k+1)-mer position.
+// an item of bucket id b to `sink`, which stores it in the receive buffer of the rank o = sink.owner[b >> 8], when
+// round_lo[o] <= b <= round_hi[o] (the round's range of o; lo > hi: nothing); each block first folds the ranges into a
+// shared table of second-byte ranges per leading byte (blocks of 256 threads).  One thread per (k+1)-mer position.
 enum { kS2Count = 0, kS2Write = 1, kS2Hist = 2, kS2Range = 3, kS2Owner = 4 };
 template <int W, int MODE>
 __global__ void __launch_bounds__(256) k_r2s_s2_extract(PkgView pv, u32 k, const u32 *__restrict__ is_solid, int sure, u64 n_edges,
                                                        u32 *__restrict__ recs, unsigned long long *__restrict__ cursor, u64 capacity,
                                                        u32 lo = 0, u32 hi = 0, unsigned long long *__restrict__ hist = nullptr,
-                                                       OwnerSink sink = {}) {
+                                                       OwnerSink sink = {}, const u32 *__restrict__ round_lo = nullptr,
+                                                       const u32 *__restrict__ round_hi = nullptr) {
+  // kS2Owner: the round's second-byte range of every leading byte B's owner, (first | last << 8) (first > last: none)
+  __shared__ u32 s_rng[MODE == kS2Owner ? 256 : 1];
+  if (MODE == kS2Owner) {
+    const u32 B = threadIdx.x, o = sink.owner[B], a = max(round_lo[o], B << 8), z = min(round_hi[o], B << 8 | 255u);
+    s_rng[B] = a <= z ? ((a & 255u) | (z & 255u) << 8) : 255u;
+    __syncthreads();
+  }
   const u32 lane = lane_id();
   u64 t0 = (u64)blockIdx.x * 256 + threadIdx.x;
   const u64 step = (u64)gridDim.x * 256;
@@ -1054,7 +1070,12 @@ __global__ void __launch_bounds__(256) k_r2s_s2_extract(PkgView pv, u32 k, const
           make_r2s_item<W>(s, nwords, k, i, strand, type, rec);
           const u32 b = rec[0] >> 16;
           if (MODE == kS2Hist) atomicAdd(&hist[b], 1ull);
-          in = MODE == kS2Owner || (b >= lo && b <= hi);
+          if (MODE == kS2Owner) {
+            const u32 x = s_rng[b >> 8], c = b & 255u;
+            in = c >= (x & 255u) && c <= (x >> 8);
+          } else {
+            in = b >= lo && b <= hi;
+          }
         }
         if (MODE == kS2Hist) continue;
         const u32 mask = __ballot_sync(0xffffffffu, in);

@@ -373,8 +373,9 @@ def set_s2s_round_limit(max_items: int = 0):
 
 
 def set_r2s_round_limit(s1: int = 0, s2: int = 0):
-    """Cap the stage-1 records / stage-2 items per round of read2sdbg (0 = derive from free device memory); independent
-    of the count and seq2sdbg caps.  The result does not depend on the caps."""
+    """Cap the stage-1 records / stage-2 items per round of read2sdbg (0 = derive from free device memory), on one GPU
+    and per owner on several (read2sdbg_run(gpus=N), whose forked workers inherit the caps); independent of the count
+    and seq2sdbg caps.  The result does not depend on the caps."""
     L = load()
     L.mhb_set_r2s_round_limit.argtypes = [C.c_uint64, C.c_uint64]
     _check(L.mhb_set_r2s_round_limit(int(s1), int(s2)))
@@ -817,7 +818,9 @@ def plan_read_shares(bin_words: np.ndarray, n_reads: int, n_ranks: int) -> list[
 def read2sdbg_run(read_lib_file: str, output_prefix: str, k: int = 21, m: int = 2, need_mercy: bool = False,
                   host_mem: float = 1e9, num_cpu_threads: int = 0, mem_flag: int = 1, gpus: int = 1) -> None:
     """gpus > 1: mhb_read2sdbg_run_multi, which forks one worker per GPU and so must be called from a process that has
-    not initialised CUDA (torch included); it writes one P.sdbg.<r> per rank."""
+    not initialised CUDA (torch included); it writes one P.sdbg.<r> per rank.  Each owner sorts its bucket range of
+    either stage in rounds when it does not fit its device at once (or exceeds set_r2s_round_limit); every rank keeps
+    its share of the reads and the whole library's bit planes resident."""
     o = Read2SdbgOpts(k, m, host_mem, num_cpu_threads, read_lib_file.encode(), output_prefix.encode(), mem_flag,
                       int(need_mercy))
     L = load()

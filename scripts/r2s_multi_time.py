@@ -9,7 +9,12 @@ same P.counting.
 When the ranks outnumber the devices they share a device, and the N-rank times then say how much the shared-device
 path costs, not how it scales: the speed-up is reported as "not measured" until the script runs on N devices.
 
-  r2s_multi_time.py [--gpus 2] [--reads 5e6] [--k 27] [--m 2] [--no-mercy] [--repeat 3] [--out DIR]
+--core-b PATH adds an N-rank arm run by another build's megahit_core (an A/B of two builds on the same library, the
+arms alternating); --no-single drops the 1-rank arm and --no-warmup the warm-up calls (a library that takes minutes
+per run).  Rank 0's round plan line is recorded with the rank lines.
+
+  r2s_multi_time.py [--gpus 2] [--reads 5e6] [--k 27] [--m 2] [--no-mercy] [--repeat 3] [--core-b PATH] [--no-single]
+                    [--no-warmup] [--out DIR]
 """
 import argparse
 import json
@@ -41,8 +46,8 @@ def make_lib(d, n_reads, read_len):
     return p
 
 
-def run_arm(libp, a, out, gpus):
-    cmd = [CORE, "read2sdbg", "-k", str(a.k), "-m", str(a.m), "--host_mem", "6e10", "--mem_flag", "1",
+def run_arm(libp, a, out, gpus, core=CORE):
+    cmd = [core, "read2sdbg", "-k", str(a.k), "-m", str(a.m), "--host_mem", "6e10", "--mem_flag", "1",
            "--num_cpu_threads", "16", "--read_lib_file", libp, "--output_prefix", out]
     cmd += [] if a.no_mercy else ["--need_mercy"]
     cmd += ["--gpus", str(gpus)] if gpus > 1 else []
@@ -51,7 +56,7 @@ def run_arm(libp, a, out, gpus):
     wall = time.time() - t0
     if r.returncode:
         sys.exit(r.stderr[-3000:])
-    ranks = [ln.split(" - ", 1)[1] for ln in r.stderr.splitlines() if " - rank " in ln]
+    ranks = [ln.split(" - ", 1)[1] for ln in r.stderr.splitlines() if " - rank " in ln or "read2sdbg plan:" in ln]
     return wall, ranks
 
 
@@ -72,6 +77,9 @@ def main():
     ap.add_argument("--m", type=int, default=2)
     ap.add_argument("--no-mercy", action="store_true")
     ap.add_argument("--repeat", type=int, default=3)
+    ap.add_argument("--core-b", default=None)
+    ap.add_argument("--no-single", action="store_true")
+    ap.add_argument("--no-warmup", action="store_true")
     ap.add_argument("--out", default=os.path.join(ROOT, "scripts", "out"))
     a = ap.parse_args()
 
@@ -86,14 +94,18 @@ def main():
         t0 = time.time()
         libp = make_lib(d, int(a.reads), a.read_len)
         print(json.dumps({"case_s": round(time.time() - t0, 1), "reads": int(a.reads)}), flush=True)
-        arms = {"1_rank": 1, f"{a.gpus}_ranks": a.gpus}
+        arms = {} if a.no_single else {"1_rank": (1, CORE)}
+        arms[f"{a.gpus}_ranks"] = (a.gpus, CORE)
+        if a.core_b:
+            arms[f"b_{a.gpus}_ranks"] = (a.gpus, os.path.abspath(a.core_b))
         times, lines, digests = {arm: [] for arm in arms}, [], {}
-        for arm, g in arms.items():
-            run_arm(libp, a, os.path.join(d, "warm"), g)
+        for arm, (g, core) in arms.items():
+            if not a.no_warmup:
+                run_arm(libp, a, os.path.join(d, "warm"), g, core)
         for rep in range(a.repeat):
-            for arm, g in arms.items():
+            for arm, (g, core) in arms.items():
                 p = os.path.join(d, arm)
-                wall, ranks = run_arm(libp, a, p, g)
+                wall, ranks = run_arm(libp, a, p, g, core)
                 digests[arm] = digest(p, a.m)
                 line = {"arm": arm, "rep": rep, "wall_s": round(wall, 3), **digests[arm], "ranks": ranks}
                 print(json.dumps(line), flush=True)
@@ -103,7 +115,7 @@ def main():
         summary = {"k": a.k, "m": a.m, "need_mercy": not a.no_mercy, "reads": int(a.reads), "read_len": a.read_len,
                    "median_s": med, "outputs_identical": len({json.dumps(x, sort_keys=True) for x in digests.values()}) == 1,
                    "speedup": ("not measured: the ranks share %d device(s)" % len(devs)) if shared
-                   else round(med["1_rank"] / med[f"{a.gpus}_ranks"], 3), **head}
+                   else round(med["1_rank"] / med[f"{a.gpus}_ranks"], 3) if "1_rank" in med else "not measured", **head}
         print(json.dumps(summary), flush=True)
         with open(os.path.join(a.out, "r2s_multi_time.json"), "w") as f:
             json.dump({"summary": summary, "lines": lines}, f, indent=1)
