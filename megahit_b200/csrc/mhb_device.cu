@@ -526,14 +526,54 @@ extern "C" int mhb_s2s_extract_range(void *stream, const mhb_dev_seqs *seqs, uin
   return launch_extract_range((cudaStream_t)stream, seqs, k, n_items, lo, hi, sink, hist256, hist_byte);
 }
 
+extern "C" int mhb_s2s_bucket_hist(void *stream, const mhb_dev_seqs *seqs, uint32_t k, uint64_t n_items, uint64_t *hist16) {
+  if (!seqs || k < 9 || k > MHB_MAX_K) return mhb_set_error(MHB_ERR_ARG, "kmer size must be >= 9 and <= 255");
+  if (!hist16) return mhb_set_error(MHB_ERR_ARG, "hist16 is NULL");
+  if (n_items == 0) return MHB_OK;
+  const BucketHistSink sink{(unsigned long long *)hist16};
+  return launch_extract_range((cudaStream_t)stream, seqs, k, n_items, 0, 65535, sink, nullptr, 0);
+}
+
+extern "C" int mhb_s2s_extract_owners_round(void *stream, const mhb_dev_seqs *seqs, uint32_t k, uint64_t n_items,
+                                            const uint8_t *owner_of_byte, const uint64_t *owner_base, uint64_t *cursor_dev,
+                                            const uint64_t *capacity_dev, const uint32_t *round_lo, const uint32_t *round_hi) {
+  if (!seqs || k < 9 || k > MHB_MAX_K) return mhb_set_error(MHB_ERR_ARG, "kmer size must be >= 9 and <= 255");
+  if (!owner_of_byte || !owner_base || !cursor_dev || !capacity_dev || !round_lo != !round_hi)
+    return mhb_set_error(MHB_ERR_ARG, "bad args");
+  if (n_items == 0) return MHB_OK;
+  const OwnerRoundSink sink{{owner_of_byte, owner_base, (unsigned long long *)cursor_dev, capacity_dev}, round_lo, round_hi};
+  return launch_extract_range((cudaStream_t)stream, seqs, k, n_items, 0, 65535, sink, nullptr, 0);
+}
+
 extern "C" int mhb_s2s_extract_owners(void *stream, const mhb_dev_seqs *seqs, uint32_t k, uint64_t n_items,
                                       const uint8_t *owner_of_byte, const uint64_t *owner_base, uint64_t *cursor_dev,
                                       const uint64_t *capacity_dev) {
-  if (!seqs || k < 9 || k > MHB_MAX_K) return mhb_set_error(MHB_ERR_ARG, "kmer size must be >= 9 and <= 255");
-  if (!owner_of_byte || !owner_base || !cursor_dev || !capacity_dev) return mhb_set_error(MHB_ERR_ARG, "bad args");
-  if (n_items == 0) return MHB_OK;
-  const OwnerSink sink{owner_of_byte, owner_base, (unsigned long long *)cursor_dev, capacity_dev};
-  return launch_extract_range((cudaStream_t)stream, seqs, k, n_items, 0, 65535, sink, nullptr, 0);
+  return mhb_s2s_extract_owners_round(stream, seqs, k, n_items, owner_of_byte, owner_base, cursor_dev, capacity_dev,
+                                      nullptr, nullptr);
+}
+
+extern "C" int mhb_s2s_edges_owners(void *stream, const uint32_t *edges, const uint8_t *aux, uint64_t n_edges,
+                                    uint64_t n_with_aux, uint32_t k, uint64_t *hist16, const uint8_t *owner_of_byte,
+                                    const uint64_t *owner_base, uint64_t *cursor_dev, const uint64_t *capacity_dev,
+                                    const uint32_t *round_lo, const uint32_t *round_hi) {
+  if (!edges || (!aux && n_with_aux) || k < 9 || k > MHB_MAX_K || n_with_aux > n_edges) return mhb_set_error(MHB_ERR_ARG, "bad args");
+  if (!hist16 && (!owner_of_byte || !owner_base || !cursor_dev || !capacity_dev || !round_lo != !round_hi))
+    return mhb_set_error(MHB_ERR_ARG, "bad args");
+  if (n_edges == 0) return MHB_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  const u32 W = s2s_record_words(k), WE = words_per_edge(k);
+  const unsigned g = grid_cap(n_edges, 256, 32);
+  const BucketHistSink hs{(unsigned long long *)hist16};
+  const OwnerRoundSink os{{owner_of_byte, owner_base, (unsigned long long *)cursor_dev, capacity_dev}, round_lo, round_hi};
+#define M(WW)                                                                                                        \
+  if (W == WW) {                                                                                                     \
+    if (hist16) k_s2s_edges_sink<WW, BucketHistSink><<<g, 256, 0, st>>>(edges, aux, n_edges, n_with_aux, WE, k, hs); \
+    else k_s2s_edges_sink<WW, OwnerRoundSink><<<g, 256, 0, st>>>(edges, aux, n_edges, n_with_aux, WE, k, os);       \
+  }
+  MHB_FOR_WR(M)
+#undef M
+  CK_LAUNCH();
+  return MHB_OK;
 }
 
 // in-place exclusive scan of n u64 values (three phases, no serial chain); total -> *total_dev

@@ -915,6 +915,17 @@ static int s2s_run(uint32_t k, SeqSource &src, uint64_t n_items, S2sOut *out) {
   return s2s_host_rounds(k, src, n_items, g_s2s_round_limit, !rounds && !stream, out);
 }
 
+// a round of a multi-GPU SdBG owner holds what one of s2s_host_rounds does: its receive buffer and the sort buffer,
+// the sort + emit workspace (at most the sort workspace plus the emit scratch) and the SdBG bytes
+extern "C" uint64_t mhb_sdbg_round_budget(uint64_t avail_bytes, uint64_t fixed_bytes, uint32_t k, uint64_t n_total) {
+  if (k < 9 || k > MHB_MAX_K) return 0;
+  const uint32_t W = s2s_record_words(k);
+  uint64_t cap = largest_round(std::max<uint64_t>(n_total, 1), fixed_bytes, avail_bytes,
+                               [&](uint64_t n) { return s2s_round_bytes(n, W, k); });
+  if (cap && g_s2s_round_limit) cap = std::min(cap, g_s2s_round_limit);
+  return cap;
+}
+
 extern "C" int mhb_set_s2s_chunk_limit(uint64_t bytes) {
   g_s2s_chunk_limit = bytes;
   return MHB_OK;

@@ -21,11 +21,12 @@
 //
 // `count` (mhb_count_run_multi): the count records go to their owners in rounds, each owner counts what it received;
 // the mercy searches are answered by the owners of the searched prefixes (mhb_mercy_probe_owned); the k_min SdBG is
-// built in the same run because the solid edges are already on the devices.  Reference behaviour reproduced:
+// built in the same run because the solid and mercy edges are already on the devices.  Reference behaviour reproduced:
 // KmerCounter::Run (sorting/kmer_counter.cpp) + SeqToSdbg::Run with need_mercy (sorting/seq_to_sdbg.cpp) at k_min;
 // files as edge_io_meta.h:25-44 / sdbg_meta.cpp:44-61 with num_files = n_gpus.
 // `seq2sdbg` for k > k_min (mhb_seq2sdbg_run_multi): the items go to their owners, which sort and emit as the count's
-// SdBG stage does (sdbg_owner_stage, sdbg_merge_info).
+// SdBG stage does (sdbg_stage, sdbg_merge_info), in rounds over ascending bucket ranges when an owner's items do not
+// fit its device at once (or exceed mhb_set_s2s_round_limit).
 // `iterate` (mhb_iterate_run_multi): each rank builds the whole flank index, runs the single-GPU read pass over its share
 // and sends its unique candidates to their owners, which sort and dedup them; the owners' ascending runs, written in
 // rank order, are the single-GPU P.edges.0.
@@ -274,42 +275,84 @@ void sdbg_publish(Exchange &X, const uint64_t *totals, const std::vector<uint8_t
   X.publish("stab", table.data(), table.size() * 8);
 }
 
-// Sort and emit the SdBG items of my receive buffer (my bucket range), close the exchange and publish the result
-void sdbg_owner_stage(Exchange &X, OwnerExchange &ex, uint32_t k, const std::string &prefix) {
-  const uint64_t n_own = ex.n_own;
-  const uint32_t W2 = mhb_s2s_record_words(k), wpt = div_ceil(k, 16);
-  uint8_t sbytes[72];
-  const uint32_t n_ssort = mhb_s2s_sort_bytes(k, sbytes);
-  std::vector<uint8_t> sdbg_bytes;
-  std::vector<uint64_t> table(65536 * 4, 0);
-  uint64_t totals[16] = {0};
-  {
-    DevBuf tmp, s, e, out, d_table, d_tot;
-    CKL(tmp.alloc((n_own * W2 + 16) * 4, "SdBG owner: sort buffer"));
-    const size_t sb = mhb_sort_workspace_bytes(std::max<uint64_t>(n_own, 1), W2), eb = mhb_s2s_emit_scratch_bytes(n_own, k);
-    CKL(s.alloc(sb, "SdBG owner: sort workspace"));
-    int in_b = 0;
-    CKL(mhb_sort_records_relaxed(nullptr, ex.mine.as<uint32_t>(), tmp.as<uint32_t>(), n_own, W2, sbytes, n_ssort, nullptr,
-                                 s.p, sb, &in_b));
-    s.release();
+// This rank's part of its device's free memory for the rounds of a stage: 92 % of it, split evenly among the ranks
+// bound to the device.  Called by every rank between two barriers, when nobody allocates.
+size_t rank_round_bytes(int rank, int world) {
+  int n_dev = 1, sharers = 0;
+  CKC(cudaGetDeviceCount(&n_dev));
+  for (int q = 0; q < world; ++q) sharers += q % n_dev == rank % n_dev;
+  return (size_t)(0.92 * (double)free_device_bytes()) / (size_t)std::max(1, sharers);
+}
 
-    CKL(e.alloc(eb, "SdBG owner: emitter scratch"));
-    const uint64_t cap_b = n_own * (4ull + 4ull * wpt) + 16;
-    CKL(out.alloc(cap_b, "SdBG owner: SdBG bytes"));
+// Rank 0: the loads of a stage's plan - the records of the largest owner, leading byte and bucket - from which a
+// round cap can be chosen, as "<label>: largest owner ..., largest leading byte ..., largest bucket ..."
+void log_loads(const Exchange &X, const OwnerExchange &ex, const char *label) {
+  if (X.rank) return;
+  std::vector<uint64_t> tot(65536, 0);
+  for (int s = 0; s < X.world; ++s)
+    for (int b = 0; b < 65536; ++b) tot[b] += ex.hist[(size_t)s * 65536 + b];
+  uint64_t owner = 0, byte = 0, bucket = 0;
+  for (int o = 0; o < X.world; ++o) {
+    uint64_t n = 0;
+    for (uint32_t b = ex.plan.bounds[o] << 8; b < ex.plan.bounds[o + 1] << 8; ++b) n += tot[b];
+    owner = std::max(owner, n);
+  }
+  for (int b = 0; b < 256; ++b) {
+    uint64_t n = 0;
+    for (int c = 0; c < 256; ++c) n += tot[b << 8 | c];
+    byte = std::max(byte, n);
+  }
+  for (uint64_t n : tot) bucket = std::max(bucket, n);
+  XINFO("%s: largest owner %llu, largest leading byte %llu, largest bucket %llu\n", label, (unsigned long long)owner,
+        (unsigned long long)byte, (unsigned long long)bucket);
+}
+
+// The SdBG stage of the count and seq2sdbg workers, from this rank's 65536-bin bucket histogram of its items (h16).
+// The plan caps every owner at its round budget (mhb_sdbg_round_budget, taken while nobody allocates); per round,
+// store(rt) puts my items of the round's bucket ranges straight into their owners' buffers, and every owner sorts and
+// emits what it received (mhb_s2s_sort_emit) and appends it to its output.  An owner's rounds ascend, so its
+// P.sdbg.<r> is in bucket order.  Then the exchange closes and the result is published.  Returns the rounds.
+template <class Store>
+int sdbg_stage(Exchange &X, const uint64_t *h16, uint32_t k, const std::string &prefix, uint64_t *n_own, Store store) {
+  const uint32_t W2 = mhb_s2s_record_words(k), wpt = div_ceil(k, 16);
+  OwnerExchange ex;
+  ex.gather(X, h16, 65536);  // ... behind which nobody allocates until the budgets are gathered
+  uint64_t n_total = 0;
+  for (uint64_t c : ex.hist) n_total += c;
+  const size_t avail = rank_round_bytes(X.rank, X.world);
+  const size_t fixed = (size_t)64 << 20;  // bucket table, totals, the exchange's small tables
+  const uint64_t budget = mhb_sdbg_round_budget(avail, fixed, k, n_total);
+  if (!budget) fail_nomem("%zu free bytes for this rank: not even a one-item SdBG round fits", avail);
+  ex.open(X, X.gather(&budget, 1).data(), W2 * 4, "SdBG owner: items received");
+  const int R = ex.plan.R;
+  if (X.rank == 0) XINFO("SdBG plan: %d round%s over bucket ranges\n", R, R > 1 ? "s" : "");
+  log_loads(X, ex, "SdBG items");
+  *n_own = ex.n_own;
+
+  SdbgStitch out;  // my rounds, in bucket order
+  {
+    const uint64_t n_max = *std::max_element(ex.own.begin(), ex.own.end());
+    const uint64_t cap_b = n_max * (4ull + 4ull * wpt) + 16;
+    const size_t ws_bytes = mhb_s2s_sort_emit_workspace_bytes(std::max<uint64_t>(n_max, 1), k);
+    DevBuf tmp, ws, bytes, d_table, d_tot;
+    CKL(tmp.alloc((n_max * W2 + 16) * 4, "SdBG owner: sort buffer"));
+    CKL(ws.alloc(ws_bytes, "SdBG owner: sort and emit workspace"));
+    CKL(bytes.alloc(cap_b, "SdBG owner: SdBG bytes"));
     CKL(d_table.alloc(65536 * 32, "SdBG owner: bucket table"));
     CKL(d_tot.alloc(128, "SdBG owner: totals"));
-    CKC(cudaMemset(d_table.p, 0, 65536 * 32));
-    CKC(cudaMemset(d_tot.p, 0, 128));
-    CKL(mhb_s2s_emit(nullptr, (in_b ? tmp : ex.mine).as<uint32_t>(), n_own, k, out.as<uint8_t>(), cap_b,
-                     d_table.as<uint64_t>(), d_tot.as<uint64_t>(), e.p, eb));
-    CKC(cudaMemcpy(totals, d_tot.p, sizeof(totals), cudaMemcpyDeviceToHost));
-    if (totals[0] > cap_b) fail("internal: SdBG byte stream exceeds capacity");
-    sdbg_bytes.resize(totals[0]);
-    if (totals[0]) CKC(cudaMemcpy(sdbg_bytes.data(), out.p, totals[0], cudaMemcpyDeviceToHost));
-    CKC(cudaMemcpy(table.data(), d_table.p, 65536 * 32, cudaMemcpyDeviceToHost));
+    for (int t = 0; t < R; ++t) {
+      ex.send(X, t, "SdBG items", store);
+      if (const uint64_t n_t = ex.own[t]) {
+        CKL(mhb_s2s_sort_emit(nullptr, ex.mine.as<uint32_t>(), tmp.as<uint32_t>(), n_t, k, nullptr, bytes.as<uint8_t>(),
+                              cap_b, d_table.as<uint64_t>(), d_tot.as<uint64_t>(), ws.p, ws_bytes));
+        CKL(out.append(nullptr, bytes.as<uint8_t>(), cap_b, d_table.as<uint64_t>(), d_tot.as<uint64_t>()));
+      }
+      if (t + 1 < R) X.barrier();  // nobody stores into my receive buffer before I have sorted it
+    }
   }
   ex.close(X);
-  sdbg_publish(X, totals, sdbg_bytes, std::move(table), prefix);
+  sdbg_publish(X, out.tot, out.bytes, std::move(out.table), prefix);
+  return R;
 }
 
 // Rank 0, once every rank's sdbg_publish is behind a barrier: the merged P.sdbg_info, one file per rank, and the
@@ -349,15 +392,6 @@ struct Job {
   std::vector<uint64_t> first;  // read shares
   std::string prefix;
 };
-
-// This rank's part of its device's free memory for the rounds of a stage: 92 % of it, split evenly among the ranks
-// bound to the device.  Called by every rank between two barriers, when nobody allocates.
-size_t rank_round_bytes(int rank, int world) {
-  int n_dev = 1, sharers = 0;
-  CKC(cudaGetDeviceCount(&n_dev));
-  for (int q = 0; q < world; ++q) sharers += q % n_dev == rank % n_dev;
-  return (size_t)(0.92 * (double)free_device_bytes()) / (size_t)std::max(1, sharers);
-}
 
 // The most count records this rank may take in one round: the largest round (round_bytes, as the single-GPU count
 // plans it) that fits rank_round_bytes, capped by mhb_set_round_limit.  Called when every share is on its device.
@@ -651,12 +685,20 @@ struct CountRank {
     CKC(cudaDeviceSynchronize());
   }
 
-  // The SdBG stage over solid + mercy edges: my items to their owners, which sort and emit their bucket range
+  // mercy() was the last reader of my share on the device; files() reads the host image
+  void release_share() {
+    for (DevBuf *b : {&bin, &roff, &eoff}) b->release();
+    memset(&reads, 0, sizeof(reads));
+  }
+
+  // The SdBG stage over solid + mercy edges, in rounds over bucket ranges when an owner's items do not fit its device
+  // at once: in every round my items go straight from the edges into their owners' buffers, and each owner sorts and
+  // emits what it received.  The owned solid edges still carry the count stage's in/out flags: the $-items the emitter
+  // is certain to discard are neither generated nor exchanged (mhb_s2s_edges_owners, DESIGN.md 4.7); under
+  // MHB_S2S_NO_PRUNE all six items of every edge go, through the sequence view of the edge records.
   void sdbg() {
-    const uint32_t W2 = mhb_s2s_record_words(k);
-    const int top2 = (int)(4 * W2 - 1);
+    const bool prune = !getenv("MHB_S2S_NO_PRUNE");
     const uint64_t n_seqs = n_solid + n_mercy;
-    uint64_t n_items = n_seqs * 6;
     mhb_dev_seqs seqs;
     memset(&seqs, 0, sizeof(seqs));
     seqs.words = all_edges;
@@ -664,40 +706,33 @@ struct CountRank {
     seqs.n_seqs = n_seqs;
     seqs.fixed_len = k + 1;
     seqs.fixed_stride = WE;
-    OwnerExchange ex;
+    const uint8_t *flags = aux.as<uint8_t>();
+    std::vector<uint64_t> h(65536);
     {
-      DevBuf recs, ws, hist;
-      CKL(recs.alloc((n_items * W2 + 16) * 4, "count: SdBG items"));
-      CKL(hist.alloc(256 * 8, "count: leading-byte histogram"));
-      uint64_t *d_hist = hist.as<uint64_t>(), *d_ns = ns.as<uint64_t>();
-      CKC(cudaMemset(d_hist, 0, 256 * 8));
-      if (getenv("MHB_S2S_NO_PRUNE")) {
-        CKL(mhb_s2s_extract(nullptr, &seqs, k, recs.as<uint32_t>(), n_items, d_hist, top2));
-      } else {
-        // the owned solid edges still carry the count stage's in/out flags: the $-items the emitter is certain to
-        // discard are neither generated nor exchanged (mhb_s2s_extract_edges_pruned, DESIGN.md 4.7)
-        CKC(cudaMemset(d_ns + 4, 0, 8));
-        CKL(mhb_s2s_extract_edges_pruned(nullptr, all_edges, aux.as<uint8_t>(), n_seqs, n_solid, k, recs.as<uint32_t>(),
-                                         n_items, d_ns + 4, d_hist, top2));
-        uint64_t kept = 0;
-        CKC(cudaMemcpy(&kept, d_ns + 4, 8, cudaMemcpyDeviceToHost));
-        if (kept > n_items) fail("internal: pruned item count exceeds 6 per edge");
-        n_items = kept;
-      }
-      const size_t ws_bytes = mhb_sort_workspace_bytes(std::max<uint64_t>(n_items, 1), W2);
-      CKL(ws.alloc(ws_bytes, "count: partition workspace"));
-      uint64_t h[256];
-      CKC(cudaMemcpy(h, d_hist, sizeof(h), cudaMemcpyDeviceToHost));
-      ex.gather(X, h, 256);
-      ex.open(X, nullptr, W2 * 4, "count: SdBG items received");
-      ex.send(X, 0, nullptr, [&](const OwnerRoute &rt) {
-        CKL(mhb_partition_scatter(nullptr, recs.as<uint32_t>(), n_items, W2, top2, rt.owner, rt.base, ws.p, ws_bytes));
-      });
+      DevBuf h16;
+      CKL(h16.alloc(65536 * 8, "count: SdBG bucket histogram"));
+      CKC(cudaMemset(h16.p, 0, 65536 * 8));
+      if (prune)
+        CKL(mhb_s2s_edges_owners(nullptr, all_edges, flags, n_seqs, n_solid, k, h16.as<uint64_t>(), nullptr, nullptr,
+                                 nullptr, nullptr, nullptr, nullptr));
+      else
+        CKL(mhb_s2s_bucket_hist(nullptr, &seqs, k, n_seqs * 6, h16.as<uint64_t>()));
+      CKC(cudaMemcpy(h.data(), h16.p, 65536 * 8, cudaMemcpyDeviceToHost));
     }
-    sdbg_owner_stage(X, ex, k, J.prefix);
-    XINFO("rank %d: %llu reads, %llu records sent, %llu owned in %d round%s, %llu solid edges; peak device memory %.1f MiB\n",
+    uint64_t n_sdbg_own = 0;
+    const int R_sdbg = sdbg_stage(X, h.data(), k, J.prefix, &n_sdbg_own, [&](const OwnerRoute &rt) {
+      if (prune)
+        CKL(mhb_s2s_edges_owners(nullptr, all_edges, flags, n_seqs, n_solid, k, nullptr, rt.owner, rt.base, rt.cursor,
+                                 rt.cap, rt.lo, rt.hi));
+      else
+        CKL(mhb_s2s_extract_owners_round(nullptr, &seqs, k, n_seqs * 6, rt.owner, rt.base, rt.cursor, rt.cap, rt.lo,
+                                         rt.hi));
+    });
+    XINFO("rank %d: %llu reads, %llu records sent, %llu owned in %d round%s, %llu solid edges, %llu SdBG items owned in "
+          "%d round%s; peak device memory %.1f MiB\n",
           r, (unsigned long long)nr, (unsigned long long)n_sent, (unsigned long long)n_own, R, R > 1 ? "s" : "",
-          (unsigned long long)n_solid, DevBuf::peak_bytes() / 1048576.0);
+          (unsigned long long)n_solid, (unsigned long long)n_sdbg_own, R_sdbg, R_sdbg > 1 ? "s" : "",
+          DevBuf::peak_bytes() / 1048576.0);
   }
 
   // The files: my bucket range of the edges; rank 0 merges the tables and writes the library-wide files
@@ -755,6 +790,7 @@ void worker(const Job &J, Exchange &X) {
   c.load();
   c.count_rounds();
   c.mercy();
+  c.release_share();
   c.sdbg();
   c.files();
 }
@@ -771,8 +807,7 @@ struct SeqJob {
 
 void s2s_worker(const SeqJob &J, Exchange &X) {
   const int W = X.world, r = X.rank;
-  const uint32_t k = J.k, W2 = mhb_s2s_record_words(k);
-  const int top2 = (int)(4 * W2 - 1);
+  const uint32_t k = J.k;
   bind_device(r, W);
 
   // ---- my share to the device ----
@@ -805,26 +840,24 @@ void s2s_worker(const SeqJob &J, Exchange &X) {
   seqs.item_off = d_io.as<uint64_t>();
   seqs.mult = mult.as<uint16_t>();
 
-  // ---- leading-byte histogram of my items -> the exchange; every item straight into its owner's buffer ----
-  OwnerExchange ex;
+  // ---- bucket histogram of my items -> the plan; per round, every item of the round's bucket ranges straight into its
+  // owner's buffer (my share stays on the device until the last round: every round extracts from it again) ----
+  std::vector<uint64_t> h(65536);
   {
-    DevBuf hist;
-    CKL(hist.alloc(256 * 8, "seq2sdbg: leading-byte histogram"));
-    CKC(cudaMemset(hist.p, 0, 256 * 8));
-    CKL(mhb_s2s_extract_range(nullptr, &seqs, k, nullptr, n_items, 0, 65535, nullptr, 0, hist.as<uint64_t>(), top2));
-    uint64_t h[256];
-    CKC(cudaMemcpy(h, hist.p, sizeof(h), cudaMemcpyDeviceToHost));
-    ex.gather(X, h, 256);
+    DevBuf h16;
+    CKL(h16.alloc(65536 * 8, "seq2sdbg: bucket histogram"));
+    CKC(cudaMemset(h16.p, 0, 65536 * 8));
+    CKL(mhb_s2s_bucket_hist(nullptr, &seqs, k, n_items, h16.as<uint64_t>()));
+    CKC(cudaMemcpy(h.data(), h16.p, 65536 * 8, cudaMemcpyDeviceToHost));
   }
-  ex.open(X, nullptr, W2 * 4, "seq2sdbg: SdBG items received");
-  ex.send(X, 0, "items", [&](const OwnerRoute &rt) {
-    CKL(mhb_s2s_extract_owners(nullptr, &seqs, k, n_items, rt.owner, rt.base, rt.cursor, rt.cap));
+  uint64_t n_own = 0;
+  const int R = sdbg_stage(X, h.data(), k, J.prefix, &n_own, [&](const OwnerRoute &rt) {
+    CKL(mhb_s2s_extract_owners_round(nullptr, &seqs, k, n_items, rt.owner, rt.base, rt.cursor, rt.cap, rt.lo, rt.hi));
   });
   for (DevBuf *b : {&words, &d_wo, &d_io, &len, &mult}) b->release();
-
-  sdbg_owner_stage(X, ex, k, J.prefix);
-  XINFO("rank %d: %llu sequences, %llu items sent, %llu owned; peak device memory %.1f MiB\n", r, (unsigned long long)n,
-        (unsigned long long)n_items, (unsigned long long)ex.n_own, DevBuf::peak_bytes() / 1048576.0);
+  XINFO("rank %d: %llu sequences, %llu items sent, %llu owned in %d round%s; peak device memory %.1f MiB\n", r,
+        (unsigned long long)n, (unsigned long long)n_items, (unsigned long long)n_own, R, R > 1 ? "s" : "",
+        DevBuf::peak_bytes() / 1048576.0);
   X.barrier();
   if (r == 0) sdbg_merge_info(X, k, J.prefix);
   X.barrier();
@@ -940,29 +973,6 @@ struct R2sJob {
   std::string prefix;
 };
 
-// Rank 0: the loads of a stage's plan - the records of the largest owner, leading byte and bucket - from which a
-// round cap (mhb_set_r2s_round_limit) can be chosen
-void log_r2s_loads(const Exchange &X, const OwnerExchange &ex, int stage) {
-  if (X.rank) return;
-  std::vector<uint64_t> tot(65536, 0);
-  for (int s = 0; s < X.world; ++s)
-    for (int b = 0; b < 65536; ++b) tot[b] += ex.hist[(size_t)s * 65536 + b];
-  uint64_t owner = 0, byte = 0, bucket = 0;
-  for (int o = 0; o < X.world; ++o) {
-    uint64_t n = 0;
-    for (uint32_t b = ex.plan.bounds[o] << 8; b < ex.plan.bounds[o + 1] << 8; ++b) n += tot[b];
-    owner = std::max(owner, n);
-  }
-  for (int b = 0; b < 256; ++b) {
-    uint64_t n = 0;
-    for (int c = 0; c < 256; ++c) n += tot[b << 8 | c];
-    byte = std::max(byte, n);
-  }
-  for (uint64_t n : tot) bucket = std::max(bucket, n);
-  XINFO("read2sdbg stage %d: largest owner %llu, largest leading byte %llu, largest bucket %llu\n", stage,
-        (unsigned long long)owner, (unsigned long long)byte, (unsigned long long)bucket);
-}
-
 void r2s_worker(const R2sJob &J, Exchange &X) {
   const int W = X.world, r = X.rank;
   const uint32_t k = J.a.k, W2 = mhb_s2s_record_words(k);
@@ -986,7 +996,7 @@ void r2s_worker(const R2sJob &J, Exchange &X) {
     if (!budget) fail_nomem("%zu free bytes for this rank: not even a one-record stage-1 round fits", rank_round_bytes(r, W));
     ex.open(X, X.gather(&budget, 1).data(), sh.s1_record_words() * 4, "read2sdbg: stage-1 records received",
             sh.s1_narrow() ? "read2sdbg: stage-1 read_info received" : nullptr);
-    log_r2s_loads(X, ex, 1);
+    log_loads(X, ex, "read2sdbg stage 1");
     R1 = ex.plan.R;
     n_s1_own = ex.n_own;
     const uint64_t n_max = *std::max_element(ex.own.begin(), ex.own.end());
@@ -1030,7 +1040,7 @@ void r2s_worker(const R2sJob &J, Exchange &X) {
   const uint64_t budget = sh.s2_round_budget(rank_round_bytes(r, W), n_s2);
   if (!budget) fail_nomem("%zu free bytes for this rank: not even a one-item stage-2 round fits", rank_round_bytes(r, W));
   ex.open(X, X.gather(&budget, 1).data(), W2 * 4, "read2sdbg: stage-2 items received");
-  log_r2s_loads(X, ex, 2);
+  log_loads(X, ex, "read2sdbg stage 2");
   const int R2 = ex.plan.R;
   if (r == 0)
     XINFO("read2sdbg plan: stage 1 in %d round%s, stage 2 in %d round%s\n", R1, R1 == 1 ? "" : "s", R2, R2 == 1 ? "" : "s");

@@ -88,6 +88,34 @@ struct RangeSink {
 };
 
 // OwnerSink (mhb_kernels.cuh): each item straight into the receive buffer of the rank owning its leading byte.
+//
+// OwnerRoundSink: the OwnerSink of one round of a multi-GPU SdBG stage.  An item of bucket id b goes to its owner
+// o = owner[b >> 8] only when lo[o] <= b <= hi[o] (an empty range, lo > hi, sends nothing to o); lo == nullptr: every
+// item goes to its owner.
+struct OwnerRoundSink {
+  OwnerSink to;
+  const u32 *lo, *hi;
+  template <int W>
+  __device__ __forceinline__ void put(bool in, const u32 (&rec)[W], u32 mask, u32 lane, u32 lt) const {
+    if (in && lo) {
+      const u32 b = rec[0] >> 16, o = __ldg(to.owner + (b >> 8));
+      in = b >= __ldg(lo + o) && b <= __ldg(hi + o);
+    }
+    to.template put<W>(in, rec, mask, lane, lt);
+  }
+};
+
+// BucketHistSink: stores nothing; hist16[bucket id] += 1 for every item (the round planner's input).  The lanes of a
+// warp holding the same bucket id add once, so a skewed set (poly-A) costs one atomic per distinct bucket.
+struct BucketHistSink {
+  unsigned long long *hist16;
+  template <int W>
+  __device__ __forceinline__ void put(bool in, const u32 (&rec)[W], u32, u32 lane, u32) const {
+    const u32 b = in ? rec[0] >> 16 : 0xFFFFFFFFu;
+    const u32 peers = __match_any_sync(0xffffffffu, b);
+    if (in && lane == (u32)__ffs(peers) - 1) atomicAdd(hist16 + b, (unsigned long long)__popc(peers));
+  }
+};
 
 // S-extract restricted to the items whose 16-bit bucket id (first eight bases) lies in [lo, hi] (A13: seq2sdbg in
 // rounds when the items of all sequences do not fit in HBM; base_engine.cpp:254-281), handed to `sink` a warp at a
@@ -205,6 +233,13 @@ __global__ void __launch_bounds__(256)
       if (s_hist[i]) atomicAdd((unsigned long long *)&hist[i], (unsigned long long)s_hist[i]);
 }
 
+// The items of an edge with count flags a (aux bit0 = no solid incoming (k+2)-mer, bit1 = no outgoing; 3 for an edge
+// without flags) that the emitter may keep: bit strand*3 + offset (the rule of k_s2s_extract_edges_pruned below)
+__device__ __forceinline__ u32 s2s_edge_keep(u32 a) {
+  const u32 no_in = a & 1u, no_out = (a >> 1) & 1u;
+  return (1u << 1) | (1u << 4) | (no_in << 0) | (no_out << 2) | (no_out << 3) | (no_in << 5);
+}
+
 // S-extract from `.edges` records WITH the in/out flags the count stage computed for them (aux bit0 = no solid
 // incoming (k+2)-mer, bit1 = no outgoing): the $-items the emitter is certain to discard are not generated at all.
 // An edge E = x0..xk yields, per strand, the items at offsets 0 ($ x0..x_{k-1}: "nothing enters this node"), 1 (the
@@ -229,11 +264,7 @@ __global__ void __launch_bounds__(256)
   for (u64 e0 = (u64)blockIdx.x * 256 + (threadIdx.x & ~31u); e0 < n_edges; e0 += (u64)gridDim.x * 256) {  // warp-uniform
     const u64 e = e0 + lane;
     u32 keep = 0;  // bit strand*3 + offset
-    if (e < n_edges) {
-      const u32 a = e < n_aux ? (u32)aux[e] : 3u;
-      const u32 no_in = a & 1u, no_out = (a >> 1) & 1u;
-      keep = (1u << 1) | (1u << 4) | (no_in << 0) | (no_out << 2) | (no_out << 3) | (no_in << 5);
-    }
+    if (e < n_edges) keep = s2s_edge_keep(e < n_aux ? (u32)aux[e] : 3u);
     const u32 cnt = (u32)__popc(keep);
     u32 inc = cnt;
 #pragma unroll
@@ -264,6 +295,32 @@ __global__ void __launch_bounds__(256)
   if (hist)
     for (int i = threadIdx.x; i < 256; i += 256)
       if (s_hist[i]) atomicAdd((unsigned long long *)&hist[i], (unsigned long long)s_hist[i]);
+}
+
+// The items k_s2s_extract_edges_pruned keeps (the same rule, s2s_edge_keep), handed to `sink` a warp at a time: one
+// put per item slot q of the six, for the lanes whose edge keeps item q.  The SdBG stage of a multi-GPU count:
+// BucketHistSink plans its rounds, OwnerRoundSink stores a round's items straight into their owners' buffers.
+template <int W, class Sink>
+__global__ void __launch_bounds__(256)
+    k_s2s_edges_sink(const u32 *__restrict__ edges, const uint8_t *__restrict__ aux, u64 n_edges, u64 n_aux, u32 we, u32 k,
+                     Sink sink) {
+  const u32 lane = threadIdx.x & 31, lt = lanemask_lt();
+  for (u64 e0 = (u64)blockIdx.x * 256 + (threadIdx.x & ~31u); e0 < n_edges; e0 += (u64)gridDim.x * 256) {  // warp-uniform
+    const u64 e = e0 + lane;
+    u32 keep = 0, mult = 0;
+    if (e < n_edges) {
+      keep = s2s_edge_keep(e < n_aux ? (u32)aux[e] : 3u);
+      mult = edges[e * we + we - 1] & 0xFFFFu;
+    }
+    for (u32 q = 0; q < 6; ++q) {
+      const bool in = (keep >> q) & 1u;
+      const u32 mask = __ballot_sync(0xffffffffu, in);
+      if (mask == 0) continue;
+      u32 rec[W];
+      if (in) make_s2s_record<W>(edges + e * we, we, k + 1, k, q / 3, q % 3, mult, rec);
+      sink.template put<W>(in, rec, mask, lane, lt);
+    }
+  }
 }
 
 // ---- record field access (seq_to_sdbg.cpp:71-97) ----

@@ -159,6 +159,7 @@ SYMBOLS = [
     "mhb_set_s2s_chunk_limit", "mhb_plan_seq_chunks", "mhb_plan_mercy_segments", "mhb_s2s_stream_stats",
     "mhb_s2s_stream_times", "mhb_selftest_s2s_stream_decide", "mhb_selftest_mercy_stream_decide",
     "mhb_selftest_mercy_auto_plan",
+    "mhb_s2s_bucket_hist", "mhb_s2s_extract_owners_round", "mhb_s2s_edges_owners", "mhb_sdbg_round_budget",
 ]
 
 
@@ -272,6 +273,12 @@ def load():
                                         C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_int]
     L.mhb_s2s_extract_owners.argtypes = [C.c_void_p, C.POINTER(DevSeqs), C.c_uint32, C.c_uint64, C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_void_p]
+    L.mhb_s2s_bucket_hist.argtypes = [C.c_void_p, C.POINTER(DevSeqs), C.c_uint32, C.c_uint64, C.c_void_p]
+    L.mhb_s2s_extract_owners_round.argtypes = L.mhb_s2s_extract_owners.argtypes + [C.c_void_p, C.c_void_p]
+    L.mhb_s2s_edges_owners.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.mhb_sdbg_round_budget.argtypes = [C.c_uint64, C.c_uint64, C.c_uint32, C.c_uint64]
+    L.mhb_sdbg_round_budget.restype = C.c_uint64
     L.mhb_selftest_count_record.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p,
                                             C.POINTER(C.c_uint32)]
     L.mhb_selftest_count_records_roll.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p,
@@ -366,10 +373,19 @@ def set_round_limit(max_records: int = 0):
 
 
 def set_s2s_round_limit(max_items: int = 0):
-    """Cap the sort items per round of the out-of-core seq2sdbg stage (0 = derive from free device memory)."""
+    """Cap the sort items per round of the out-of-core seq2sdbg stage (0 = derive from free device memory), on one GPU
+    and per owner of the SdBG stage on several (seq2sdbg_run(gpus=N) and count_run(gpus=N), whose forked workers
+    inherit the cap).  The result does not depend on the cap."""
     L = load()
     L.mhb_set_s2s_round_limit.argtypes = [C.c_uint64]
     _check(L.mhb_set_s2s_round_limit(int(max_items)))
+
+
+def sdbg_round_budget(avail_bytes: int, fixed_bytes: int, k: int, n_total: int) -> int:
+    """The most SdBG sort items one owner of a multi-GPU SdBG stage takes in one round (mhb_sdbg_round_budget, host
+    only): the largest round of at most n_total items that fits avail_bytes next to fixed_bytes, capped by
+    set_s2s_round_limit; 0 when not even one item fits."""
+    return int(load().mhb_sdbg_round_budget(int(avail_bytes), int(fixed_bytes), int(k), int(n_total)))
 
 
 def set_r2s_round_limit(s1: int = 0, s2: int = 0):

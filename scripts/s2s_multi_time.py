@@ -5,12 +5,13 @@ Every run is its own CLI process; the arms alternate within each repetition afte
 the same call: the devices (index, name, power limit) and their count; wall time per run; the peak device memory of
 every process nvidia-smi lists during the run (polled; inside a container it may list only some of them) and, for the
 N-rank runs, the peak each rank allocated as the rank itself logs it; and whether every arm gives the same canonical
-SdBG.
+SdBG.  --cap N adds an N-rank arm whose owners take at most N items per round (mhb_set_s2s_round_limit, set in a fresh
+process that then runs lib.seq2sdbg_run), so that the SdBG stage runs in rounds over bucket ranges.
 
 When the ranks outnumber the devices they share a device, and the N-rank times then say how much the shared-device
 path costs, not how it scales: the speed-up is reported as "not measured" until the script runs on N devices.
 
-  s2s_multi_time.py [--gpus 2] [--k 79] [--items 300e6] [--repeat 2] [--out DIR]
+  s2s_multi_time.py [--gpus 2] [--k 79] [--items 300e6] [--cap N] [--repeat 2] [--out DIR]
 """
 import argparse
 import json
@@ -52,11 +53,15 @@ def write_contigs(path, k, n_items, seed):
     return got, i
 
 
-def run_arm(contigs, k, out, gpus):
+def run_arm(contigs, k, out, gpus, cap=0):
     cmd = [CORE, "seq2sdbg", "--host_mem", "3e10", "--mem_flag", "1", "--output_prefix", out, "--num_cpu_threads", "16",
            "-k", str(k), "--contig", contigs]
     if gpus > 1:
         cmd += ["--gpus", str(gpus)]
+    if cap:  # no CUDA in the process that sets the cap: its workers are forked
+        cmd = [sys.executable, "-c", f"import sys\nsys.path.insert(0, {ROOT!r})\nfrom megahit_b200 import lib\n"
+               f"lib.set_s2s_round_limit({cap})\nlib.seq2sdbg_run({out!r}, {k}, contig={contigs!r}, host_mem=3e10, "
+               f"num_cpu_threads=16, gpus={gpus})\n"]
     peak, stop = {}, threading.Event()
 
     def poll():
@@ -77,7 +82,8 @@ def run_arm(contigs, k, out, gpus):
         sys.exit(r.stderr[-3000:])
     # each rank of a multi-GPU run logs the most device memory it allocated (its CUDA context not included)
     ranks = {int(m.group(1)): float(m.group(2)) for m in re.finditer(r"rank (\d+): .*peak device memory ([\d.]+) MiB", r.stderr)}
-    return wall, sorted(peak.values(), reverse=True), [ranks[i] for i in sorted(ranks)]
+    rounds = re.search(r"SdBG plan: (\d+) round", r.stderr)
+    return wall, sorted(peak.values(), reverse=True), [ranks[i] for i in sorted(ranks)], int(rounds.group(1)) if rounds else None
 
 
 def main():
@@ -85,6 +91,7 @@ def main():
     ap.add_argument("--gpus", type=int, default=2)
     ap.add_argument("--k", type=int, default=79)
     ap.add_argument("--items", type=float, default=300e6)
+    ap.add_argument("--cap", type=int, default=0, help="items per owner round of an extra N-rank arm (0 = no such arm)")
     ap.add_argument("--repeat", type=int, default=2)
     ap.add_argument("--out", default=os.path.join(ROOT, "scripts", "out"))
     a = ap.parse_args()
@@ -98,16 +105,18 @@ def main():
     with tempfile.TemporaryDirectory() as d:
         contigs = os.path.join(d, "contigs.fa")
         n_items, n_contigs = write_contigs(contigs, a.k, int(a.items), seed=4321)
-        arms = {"1_rank": 1, f"{a.gpus}_ranks": a.gpus}
+        arms = {"1_rank": (1, 0), f"{a.gpus}_ranks": (a.gpus, 0)}
+        if a.cap:
+            arms[f"{a.gpus}_ranks_cap"] = (a.gpus, a.cap)
         times, lines, shas = {arm: [] for arm in arms}, [], {}
-        for arm, g in arms.items():
-            run_arm(contigs, a.k, os.path.join(d, "warm"), g)
+        for arm, (g, c) in arms.items():
+            run_arm(contigs, a.k, os.path.join(d, "warm"), g, c)
         for rep in range(a.repeat):
-            for arm, g in arms.items():
+            for arm, (g, c) in arms.items():
                 p = os.path.join(d, arm)
-                wall, peak, rank_peak = run_arm(contigs, a.k, p, g)
+                wall, peak, rank_peak, rounds = run_arm(contigs, a.k, p, g, c)
                 shas[arm] = F.sha256(F.canonical_sdbg(p)[1])
-                line = {"arm": arm, "rep": rep, "wall_s": round(wall, 3), "peak_device_mib_per_process": peak,
+                line = {"arm": arm, "rep": rep, "wall_s": round(wall, 3), "sdbg_rounds": rounds, "peak_device_mib_per_process": peak,
                         "peak_allocated_mib_per_rank": rank_peak}
                 print(json.dumps(line), flush=True)
                 lines.append(line)
