@@ -192,8 +192,8 @@ struct CountOnDevice {
 //
 // stream: the `.bin` image stays in host memory and every pass over the reads (leading-byte histogram, second-byte
 // histograms of oversized bytes, one pass per round, mercy marks) streams it through the device in chunks
-// (ReadStream); the round buffers get the memory the resident image would have taken.  A resident call switches to
-// streaming when the library alone does not fit or when one bucket exceeds the round that fits next to it.
+// (init_read_stream); the round buffers get the memory the resident image would have taken.  A resident call switches
+// to streaming when the library alone does not fit or when one bucket exceeds the round that fits next to it.
 //
 // check: how the index checks a library whose size matches fixed-length reads.  kSampled is verified on the device
 // during the one pass only (mhb_check_fixed_len): a call known to take another plan (streamed, or a round cap below
@@ -230,10 +230,10 @@ static int count_host_rounds(const mhb_count_args *args, mhb_count_result *res, 
   // i+1 is still crossing PCIe
   static const int h2d_pieces = getenv("MHB_H2D_CHUNKS") ? atoi(getenv("MHB_H2D_CHUNKS")) : 4;
   const bool pieces = keep && h2d_pieces > 1 && ix.fixed_len >= k + 1 && n_reads >= (uint64_t)h2d_pieces * 64;
-  ReadStream rs;
+  ChunkStream rs;
   const uint64_t chunk_cap = read_chunk_limit() ? read_chunk_limit() : read_chunk_auto_bytes();
-  CKR(rs.init(args->bin, args->bin_words, n_reads, ix, stream ? chunk_cap : 0, pieces ? h2d_pieces : 1));
-  const uint64_t chunk_reads = rs.max_chunk_reads();  // reads the per-read arrays hold
+  CKR(init_read_stream(&rs, args->bin, args->bin_words, n_reads, ix, stream ? chunk_cap : 0, pieces ? h2d_pieces : 1));
+  const uint64_t chunk_reads = rs.max_chunk_units();  // reads the per-read arrays hold
   // besides the round buffers: the library (or its chunk slots), the mercy marks, the histograms and scalars
   size_t fixed = pad256(rs.device_bytes()) + pad256(65536 * 8) + pad256(256 * 8) + 4096;
   if (args->want_mercy) fixed += 2 * pad256((size_t)(chunk_reads + 1) * 4);
@@ -297,15 +297,15 @@ static int count_host_rounds(const mhb_count_args *args, mhb_count_result *res, 
 
   // one pass over the reads: fn(view of a chunk, its first read), once per chunk
   auto each_chunk = [&](const std::function<int(const mhb_dev_reads &, uint64_t)> &fn) -> int {
-    return rs.pass(st, [&](const ReadChunkView &c) {
+    return rs.pass(st, [&](const ChunkView &c) {
       mhb_dev_reads v;
-      v.bin = c.bin;
-      v.bin_words = c.bin_words;
-      v.n_reads = c.n_reads;
+      v.bin = c.words;
+      v.bin_words = c.n_words;
+      v.n_reads = c.n;
       v.fixed_len = ix.fixed_len;
-      v.rec_off = c.rec_off;
-      v.edge_off = c.aux_off;
-      return fn(v, c.first_read);
+      v.rec_off = c.at<uint64_t>(0);
+      v.edge_off = c.at<uint64_t>(1);
+      return fn(v, c.first);
     });
   };
 
@@ -585,10 +585,9 @@ void plan_seq_chunks(const uint64_t *word_off, const SeqLayout &ly, uint64_t ns,
 // The sequences of one seq2sdbg driver call as its round loop sees them, one pass at a time.  Either mhb_s2s_args
 // sequences, or `.edges`-layout records (stride words_per_edge(k), the multiplicity in the low 16 bits of the last
 // word) in host memory or already on the device, the latter possibly with the count's flags of its first records.
-// Host data is resident (uploaded once and handed over whole as one chunk) or kept in host memory and streamed through
-// two device slots in chunks that end on sequence boundaries.  A chunk of fixed-length sequences carries their words
-// and multiplicities and is viewed with fixed_len set; a variable-length one also carries word_off and item_off rebased
-// to the chunk, and len; one of edge records carries the records.
+// Host data goes through a ChunkStream, resident or streamed in chunks that end on sequence boundaries.  A chunk of
+// fixed-length sequences carries their words and multiplicities and is viewed with fixed_len set; a variable-length
+// one also carries word_off and item_off rebased to the chunk, and len; one of edge records carries the records.
 class SeqSource {
  public:
   SeqSource(const mhb_s2s_args *a, const SeqLayout &ly) : a_(a), ly_(&ly), ns_(a->n_seqs) {}
@@ -597,55 +596,48 @@ class SeqSource {
       : edges_(edges), ns_(n), stride_(words_per_edge(k)), k1_(k + 1), on_device_(on_device), aux_(aux), n_aux_(n_aux) {}
   // max_chunk_bytes = 0: resident
   int init(uint64_t max_chunk_bytes) {
-    resident_ = max_chunk_bytes == 0;
-    uint64_t max_words = word_of(ns_), max_n = ns_;
-    if (resident_) {
-      first_ = {0, ns_};
-    } else {
-      if (edges()) plan_chunks(nullptr, stride_, 0, ns_, max_chunk_bytes, &first_);
-      else plan_seq_chunks(a_->word_off, *ly_, ns_, max_chunk_bytes, &first_);
-      max_words = max_n = 0;
-      for (uint64_t i = 0; i < n_chunks(); ++i) {
-        max_n = std::max(max_n, first_[i + 1] - first_[i]);
-        max_words = std::max(max_words, word_of(first_[i + 1]) - word_of(first_[i]));
-      }
+    if (on_device_) {
+      g_s2s_st.chunks = 0;
+      return MHB_OK;
     }
-    const bool arrays = has_arrays();
-    o_wo_ = pad256(max_words * 4 + 64);
-    o_io_ = o_wo_ + (arrays ? pad256((max_n + 1) * 8) : 0);
-    o_len_ = o_io_ + (arrays ? pad256((max_n + 1) * 8) : 0);
-    o_mult_ = o_len_ + (arrays ? pad256((max_n + 1) * 4) : 0);
-    slot_bytes_ = on_device_ ? 0 : o_mult_ + (edges() ? 0 : pad256((max_n + 1) * 2));
-    g_s2s_st.chunks = n_chunks();
-    return resident_ ? MHB_OK : stager_.init(slot_bytes_, n_chunks(), &g_s2s_st);
+    ChunkStream::Input in;
+    in.n = ns_;
+    std::vector<uint64_t> first;
+    if (edges()) {
+      in.image = edges_;
+      in.stride = stride_;
+      if (max_chunk_bytes) plan_chunks(nullptr, stride_, 0, ns_, max_chunk_bytes, &first);
+    } else {
+      in.image = a_->words;
+      in.word_off = a_->word_off;
+      if (max_chunk_bytes) plan_seq_chunks(a_->word_off, *ly_, ns_, max_chunk_bytes, &first);
+      if (!max_chunk_bytes || !ly_->fixed) {  // the resident form keeps all four
+        in.side[0] = {a_->word_off, 0};
+        in.side[1] = {ly_->item_off.data(), 0};
+        in.side[2] = {a_->len, 4};
+      }
+      in.side[3] = {a_->mult, 2};
+    }
+    in.words = in.word_of(ns_);
+    return cs_.init(in, std::move(first), &g_s2s_st);
   }
   static size_t resident_bytes(uint64_t ns, uint64_t n_words) {
-    return pad256(n_words * 4 + 64) + 2 * pad256((ns + 1) * 8) + pad256((ns + 1) * 4) + pad256((ns + 1) * 2);
+    return ChunkStream::image_bytes(n_words) + 2 * ChunkStream::side_bytes(ns, 0) + ChunkStream::side_bytes(ns, 4) +
+           ChunkStream::side_bytes(ns, 2);
   }
-  size_t resident_size() const { return edges() ? pad256(word_of(ns_) * 4 + 64) : resident_bytes(ns_, ly_->n_words); }
-  size_t device_bytes() const { return (resident_ ? 1 : 2) * slot_bytes_; }
-  uint64_t n_chunks() const { return resident_ ? 0 : first_.size() - 1; }
+  size_t resident_size() const {
+    return edges() ? ChunkStream::image_bytes(ns_ * stride_) : resident_bytes(ns_, ly_->n_words);
+  }
+  size_t device_bytes() const { return on_device_ ? 0 : cs_.device_bytes(); }
+  uint64_t n_chunks() const { return cs_.n_chunks(); }
   bool on_device() const { return on_device_; }
   bool pruned() const { return aux_ != nullptr; }  // the extraction may skip the $-items the flags rule out
   // device_bytes() bytes; the resident form uploads the sequences there on st
-  int bind(char *dev, cudaStream_t st) {
-    dev_ = on_device_ ? (char *)edges_ : dev;
-    stager_.bind(dev);
-    if (!resident_ || !ns_ || on_device_) return MHB_OK;
-    CK(cudaMemcpyAsync(dev_, edges() ? edges_ : a_->words, word_of(ns_) * 4, cudaMemcpyHostToDevice, st));
-    if (edges()) return MHB_OK;
-    CK(cudaMemcpyAsync(dev_ + o_wo_, a_->word_off, (ns_ + 1) * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(dev_ + o_io_, ly_->item_off.data(), (ns_ + 1) * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(dev_ + o_len_, a_->len, ns_ * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(dev_ + o_mult_, a_->mult, ns_ * 2, cudaMemcpyHostToDevice, st));
-    return MHB_OK;
-  }
+  int bind(char *dev, cudaStream_t st) { return on_device_ ? MHB_OK : cs_.bind(dev, st); }
   // fn(view, items of the chunk) once per chunk, in order, on st
   int pass(cudaStream_t st, const std::function<int(const mhb_dev_seqs &, uint64_t)> &fn) {
-    if (resident_) return fn(view(0, dev_), items(0, ns_));
-    return stager_.pass(
-        st, [this](uint64_t i, char *h, ChunkStager::Copies *up) { return fill(i, h, up); },
-        [&](uint64_t i, const char *slot) { return fn(view(i, slot), items(first_[i], first_[i + 1])); });
+    if (on_device_) return fn(view({0, 0, ns_, edges_, ns_ * stride_, {}}), 6 * ns_);
+    return cs_.pass(st, [&](const ChunkView &c) { return fn(view(c), items(c.first, c.first + c.n)); });
   }
   // pruned(): the items of the device records that the flags do not rule out (mhb_s2s_extract_edges_pruned)
   int extract_pruned(cudaStream_t st, uint32_t *records, uint64_t capacity, uint64_t *cursor, uint64_t *hist, int hist_byte) const {
@@ -654,53 +646,19 @@ class SeqSource {
 
  private:
   bool edges() const { return stride_ != 0; }  // the records form
-  bool has_arrays() const { return !edges() && (resident_ || !ly_->fixed); }  // the resident form keeps all four
-  uint64_t word_of(uint64_t s) const { return edges() ? s * stride_ : ns_ ? a_->word_off[s] : 0; }
   uint64_t items(uint64_t b, uint64_t e) const { return edges() ? 6 * (e - b) : ly_->item_off[e] - ly_->item_off[b]; }
-  mhb_dev_seqs view(uint64_t i, const char *slot) const {
-    const uint64_t b = first_[i], e = first_[i + 1];
-    const bool arrays = has_arrays();
+  mhb_dev_seqs view(const ChunkView &c) const {
     mhb_dev_seqs v;
-    v.words = (const uint32_t *)slot;
-    v.n_words = e > b ? word_of(e) - word_of(b) : 0;  // no word_off read for an empty set
-    v.n_seqs = e - b;
+    v.words = c.words;
+    v.n_words = c.n_words;
+    v.n_seqs = c.n;
     v.fixed_len = edges() ? k1_ : ly_->fixed ? ly_->L0 : 0;
-    v.word_off = arrays ? (const uint64_t *)(slot + o_wo_) : nullptr;
-    v.item_off = arrays ? (const uint64_t *)(slot + o_io_) : nullptr;
-    v.len = arrays ? (const uint32_t *)(slot + o_len_) : nullptr;
-    v.mult = edges() ? nullptr : (const uint16_t *)(slot + o_mult_);
+    v.word_off = c.at<uint64_t>(0);
+    v.item_off = c.at<uint64_t>(1);
+    v.len = c.at<uint32_t>(2);
+    v.mult = c.at<uint16_t>(3);
     v.fixed_stride = stride_;
     return v;
-  }
-  int fill(uint64_t i, char *h, ChunkStager::Copies *up) const {
-    const uint64_t b = first_[i], e = first_[i + 1], n = e - b, w0 = word_of(b), nw = word_of(e) - w0;
-    {
-      const uint64_t bytes = nw * 4, blk = 4ull << 20, nblk = (bytes + blk - 1) / blk;
-      const char *src = (const char *)((edges() ? edges_ : a_->words) + w0);
-#pragma omp parallel for schedule(static)
-      for (long long j = 0; j < (long long)nblk; ++j) {
-        const uint64_t o = (uint64_t)j * blk;
-        memcpy(h + o, src + o, std::min(blk, bytes - o));
-      }
-    }
-    up->add(0, nw * 4);
-    if (edges()) return MHB_OK;
-    if (!ly_->fixed) {
-      uint64_t *wo = (uint64_t *)(h + o_wo_), *io = (uint64_t *)(h + o_io_);
-      const uint64_t i0 = ly_->item_off[b];
-#pragma omp parallel for schedule(static)
-      for (long long s = 0; s <= (long long)n; ++s) {
-        wo[s] = a_->word_off[b + s] - w0;
-        io[s] = ly_->item_off[b + s] - i0;
-      }
-      memcpy(h + o_len_, a_->len + b, n * 4);
-      up->add(o_wo_, (n + 1) * 8);
-      up->add(o_io_, (n + 1) * 8);
-      up->add(o_len_, n * 4);
-    }
-    memcpy(h + o_mult_, a_->mult + b, n * 2);
-    up->add(o_mult_, n * 2);
-    return MHB_OK;
   }
   const mhb_s2s_args *a_ = nullptr;
   const SeqLayout *ly_ = nullptr;
@@ -710,11 +668,7 @@ class SeqSource {
   bool on_device_ = false;
   const uint8_t *aux_ = nullptr;
   uint64_t n_aux_ = 0;
-  bool resident_ = true;
-  std::vector<uint64_t> first_;
-  size_t o_wo_ = 0, o_io_ = 0, o_len_ = 0, o_mult_ = 0, slot_bytes_ = 0;
-  char *dev_ = nullptr;
-  ChunkStager stager_;
+  ChunkStream cs_;
 };
 
 // the smallest device footprint of the rounds over resident sequences: the sequences, the tables and a one-item round
@@ -1092,19 +1046,24 @@ int mercy_from_host(uint32_t k, const uint32_t *edges, uint64_t n_edges, const C
                       (need > g_arena.cap && mhb_read_stream_decide(need, (uint64_t)arena_avail_bytes(), 0, 0));
   const size_t pw = stream ? mhb_mercy_planes_words(n_reads, max_len) : 0;
   const size_t fixed_b = mercy_stream_fixed_bytes(n_reads, c.bin.size(), max_len);
-  uint64_t start[257];
+  // streamed: the edges cut at the first edge of every segment
   std::vector<uint32_t> seg_first;
-  size_t slot_bytes = 0;
+  ChunkStream segs;
   if (stream) {
-    uint64_t target = g_s2s_chunk_limit, limit = g_s2s_chunk_limit;
+    uint64_t target = g_s2s_chunk_limit, limit = g_s2s_chunk_limit, start[257];
     if (!target) mercy_auto_segment_bytes(arena_avail_bytes(), fixed_b, &target, &limit);
     edge_byte_starts(edges, n_edges, WE, start);
     CKR(plan_mercy_segments(start, WE, target, limit, &seg_first));
-    uint64_t max_seg = 0;
-    for (size_t i = 0; i + 1 < seg_first.size(); ++i) max_seg = std::max(max_seg, start[seg_first[i + 1]] - start[seg_first[i]]);
-    slot_bytes = pad256(max_seg * WE * 4 + 16);
+    std::vector<uint64_t> first;
+    for (uint32_t b : seg_first) first.push_back(start[b]);
+    ChunkStream::Input in;
+    in.image = edges;
+    in.words = n_edges * WE;
+    in.n = n_edges;
+    in.stride = WE;
+    CKR(segs.init(in, std::move(first), &g_mercy_st));
   }
-  CKR(g_arena.reserve(stream ? fixed_b + 2 * slot_bytes : need));
+  CKR(g_arena.reserve(stream ? fixed_b + segs.device_bytes() : need));
   cudaStream_t st = 0;
   uint32_t *d_bin = g_arena.take<uint32_t>(bin_bytes / 4 + 4);
   uint64_t *d_rec_off = g_arena.take<uint64_t>(n_reads + 1);
@@ -1141,35 +1100,17 @@ int mercy_from_host(uint32_t k, const uint32_t *edges, uint64_t n_edges, const C
     const size_t core = ms_bytes - mhb_edge_lut_bytes();
     void *lut = d_ms + core;
     uint32_t *d_planes = g_arena.take<uint32_t>(pw);
-    char *d_slots = g_arena.take<char>(2 * slot_bytes);
-    const uint64_t n_seg = seg_first.size() - 1;
+    char *d_slots = g_arena.take<char>(segs.device_bytes());
     uint8_t owner[256];
-    for (uint64_t i = 0; i < n_seg; ++i)
+    for (uint64_t i = 0; i < segs.n_chunks(); ++i)
       for (uint32_t b = seg_first[i]; b < seg_first[i + 1]; ++b) owner[b] = (uint8_t)i;
     CK(cudaMemsetAsync(d_planes, 0, pw * 4, st));
-    ChunkStager stager;
-    g_mercy_st.chunks = n_seg;
-    CKR(stager.init(slot_bytes, n_seg, &g_mercy_st));
-    stager.bind(d_slots);
-    auto seg_edges = [&](uint64_t i) { return start[seg_first[i + 1]] - start[seg_first[i]]; };
-    const ChunkStager::Fill fill = [&](uint64_t i, char *h, ChunkStager::Copies *up) {
-      const uint64_t bytes = seg_edges(i) * WE * 4, blk = 4ull << 20, nblk = (bytes + blk - 1) / blk;
-      const char *src = (const char *)(edges + start[seg_first[i]] * WE);
-#pragma omp parallel for schedule(static)
-      for (long long j = 0; j < (long long)nblk; ++j) {
-        const uint64_t o = (uint64_t)j * blk;
-        memcpy(h + o, src + o, std::min(blk, bytes - o));
-      }
-      up->add(0, bytes);
-      return MHB_OK;
-    };
-    const ChunkStager::Run run = [&](uint64_t i, const char *slot) {
-      const uint32_t *d_seg = (const uint32_t *)slot;
-      CKR(mhb_edge_lut_build(st, d_seg, seg_edges(i), k, lut));
-      return mercy_probe_owned(st, &reads, d_ids, n_reads, max_len, k, d_seg, seg_edges(i), lut, owner, (uint32_t)i, d_planes,
-                               true);
-    };
-    CKR(stager.pass(st, fill, run));
+    CKR(segs.bind(d_slots, st));
+    CKR(segs.pass(st, [&](const ChunkView &c) {
+      CKR(mhb_edge_lut_build(st, c.words, c.n, k, lut));
+      return mercy_probe_owned(st, &reads, d_ids, n_reads, max_len, k, c.words, c.n, lut, owner, (uint32_t)c.index,
+                               d_planes, true);
+    }));
     CKR(mhb_mercy_count_planes(st, &reads, d_ids, n_reads, max_len, k, d_planes, 1, pw, &n_mercy, d_ms, core));
     uint32_t *d_out = nullptr;
     if (n_mercy) CKR(dest(n_mercy, &d_out));
@@ -1215,7 +1156,7 @@ extern "C" int mhb_selftest_mercy_auto_plan(const uint64_t *byte_edges, uint32_t
   memcpy(first_byte_out, first.data(), first.size() * 4);
   uint64_t max_seg = 0;
   for (size_t i = 0; i + 1 < first.size(); ++i) max_seg = std::max(max_seg, start[first[i + 1]] - start[first[i]]);
-  *slot_bytes = pad256(max_seg * words_per_edge(k) * 4 + 16);
+  *slot_bytes = ChunkStream::image_bytes(max_seg * words_per_edge(k));
   return (int)(first.size() - 1);
 }
 

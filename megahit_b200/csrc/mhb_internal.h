@@ -269,56 +269,77 @@ class ChunkStager {
   std::vector<void *> ev_;  // cudaEvent_t: 4 per chunk (copy begin/end, compute begin/end)
 };
 
-// Every pass over a read library (mhb_stream.cu), in one of two forms:
-// - resident: the library is uploaded once into the device memory the caller binds, and a pass hands it over whole;
-//   a fixed-length library may instead go up in pieces during the first pass, which hands over each piece as a chunk
-//   while the next one is still being copied;
-// - streamed: the `.bin` image stays in host memory and goes through the device in chunks that end on read boundaries.
-//   Two pinned staging buffers and two device chunk slots: while host threads fill the staging buffer of chunk i+1,
-//   chunk i uploads on a copy stream and the compute stream works on chunk i-1.
-// Either way a chunk is handed to the caller as an ordinary view: image at offset 0 of its 16-byte aligned slot, and
-// for variable-length libraries the index's two offset arrays rebased to the chunk (unit_off only when the index has it).
-struct ReadChunkView {
-  uint64_t index, first_read, n_reads;
-  const uint32_t *bin;  // device
-  uint64_t bin_words;
-  const uint64_t *rec_off, *aux_off;  // device, n_reads + 1 each (rec_off / unit_off); NULL for fixed-length libraries
-                                      // (aux_off also when the index has no unit_off)
+// A chunk of a ChunkStream on the device: units [first, first + n) of the input, its image at offset 0 of the slot
+// and each side array (offset arrays rebased to the chunk's first unit) after it; NULL where the input has none.
+struct ChunkView {
+  uint64_t index, first, n;
+  const uint32_t *words;
+  uint64_t n_words;
+  const void *side[4];
+  template <class T>
+  const T *at(int j) const { return static_cast<const T *>(side[j]); }
 };
-class ReadStream {
+// Every pass over an input held in host memory - a read library, a sequence set, sorted edges (mhb_stream.cu).  The
+// input is an image of n units, unit i at words [word_of(i), word_of(i+1)), and up to four side arrays.  It is on the
+// device in one of three forms:
+// - resident: uploaded once by bind, and a pass hands it over whole as chunk 0;
+// - resident in pieces: a fixed-stride image without side arrays goes up during the first pass in pieces, each
+//   handed over as a chunk while the next one is still being copied;
+// - streamed: it stays in host memory and goes through the two device slots of a ChunkStager in chunks that end on
+//   unit boundaries.
+// A slot holds the image, 16-byte aligned + 16 bytes for the read extraction's bulk copies, then each side array,
+// 256-byte aligned.
+class ChunkStream {
  public:
-  ReadStream() = default;
-  ReadStream(const ReadStream &) = delete;
-  ReadStream &operator=(const ReadStream &) = delete;
-  // host library and its index; max_chunk_bytes = 0: resident, otherwise streamed in chunks planned here
-  // (the index is read by every pass: it must outlive them); pieces > 1: a resident fixed-length library goes up in
-  // that many pieces of a multiple of 4 reads (16-byte aligned) during the first pass
-  int init(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, const ReadLibIndex &ix, uint64_t max_chunk_bytes,
-           uint32_t pieces = 1);
-  size_t device_bytes() const { return (resident_ ? 1 : 2) * slot_bytes_; }  // the library, or both chunk slots
-  // device_bytes() bytes, 256-byte aligned; the resident form uploads the library there on `stream`
+  struct Side {
+    const void *host = nullptr;  // NULL: no such array
+    uint32_t elem = 0;           // 0: n + 1 uint64 offsets, rebased to each chunk; else n elements of elem bytes
+  };
+  struct Input {
+    const uint32_t *image = nullptr;
+    uint64_t words = 0;                  // the whole image: what the resident form uploads and views
+    uint64_t n = 0;                      // units
+    const uint64_t *word_off = nullptr;  // n + 1 word offsets of the units, or NULL: unit i at i * stride
+    uint64_t stride = 0;
+    Side side[4];
+    uint64_t word_of(uint64_t i) const { return !n ? 0 : word_off ? word_off[i] : i * stride; }
+  };
+  ChunkStream() = default;
+  ChunkStream(const ChunkStream &) = delete;
+  ChunkStream &operator=(const ChunkStream &) = delete;
+  // first: the unit bounds of the streamed form's chunks, from the chunk planners; empty: resident.  in's arrays are
+  // read by every pass and must outlive them.  pieces > 1: a resident fixed-stride image goes up in that many pieces of
+  // a multiple of 4 units (16-byte aligned).  The chunks and passes are counted into *stats.
+  int init(const Input &in, std::vector<uint64_t> first, StreamStats *stats, uint32_t pieces = 1);
+  // the slot parts of an image of `words` words and of one side array of `units` units with elem-byte elements
+  static size_t image_bytes(uint64_t words) { return pad256(((words * 4 + 15) & ~(uint64_t)15) + 16); }
+  static size_t side_bytes(uint64_t units, uint32_t elem) { return pad256((units + 1) * (elem ? elem : 8)); }
+  size_t device_bytes() const { return (resident_ ? 1 : 2) * slot_bytes_; }  // the input, or both chunk slots
+  // device_bytes() bytes, 256-byte aligned; the resident form uploads the input there on `stream`
   int bind(void *device, void *stream);
   uint64_t n_chunks() const { return resident_ ? 0 : first_.size() - 1; }  // chunks of the stream, 0 when resident
-  uint64_t max_chunk_reads() const { return max_reads_; }
-  const std::vector<uint64_t> &first_reads() const { return first_; }  // read bounds of the views, {0, n_reads} resident
+  uint64_t max_chunk_units() const { return max_units_; }
+  const std::vector<uint64_t> &bounds() const { return first_; }  // unit bounds of the views, {0, n} resident
   // one pass: fn runs once per chunk, in order, on the compute stream `stream`, while the chunk is on the device; the
-  // resident form calls it once, with the whole library as chunk 0, and counts nothing in the stream statistics
-  int pass(void *stream, const std::function<int(const ReadChunkView &)> &fn);
+  // resident form calls it once, with the whole input as chunk 0, and counts nothing in the stream statistics
+  int pass(void *stream, const std::function<int(const ChunkView &)> &fn);
 
  private:
   int fill(uint64_t i, char *h, ChunkStager::Copies *up) const;
-  ReadChunkView view(uint64_t i, const char *slot) const;
-  bool resident_ = false;
-  const uint32_t *bin_ = nullptr;
-  uint64_t bin_words_ = 0;
-  const ReadLibIndex *ix_ = nullptr;
-  const uint64_t *aux_off_ = nullptr;
-  std::vector<uint64_t> first_, pieces_;  // pieces_: read bounds of the pieces still to upload
-  uint64_t max_reads_ = 0;
-  size_t off_at_ = 0, slot_bytes_ = 0;
+  ChunkView view(uint64_t i, const char *slot) const;
+  Input in_;
+  bool resident_ = true;
+  std::vector<uint64_t> first_, pieces_;  // pieces_: unit bounds of the pieces still to upload
+  uint64_t max_units_ = 0;
+  size_t side_at_[4] = {0, 0, 0, 0}, slot_bytes_ = 0;
   char *dev_ = nullptr;
   ChunkStager stager_;
 };
+// A read library's stream: the `.bin` image and, for a variable-length library, side 0 = rec_off and side 1 = unit_off
+// (when the index has it).  max_chunk_bytes = 0: resident, otherwise streamed in chunks that end on read boundaries;
+// pieces as ChunkStream::init, for a fixed-length library.  The index must outlive the passes.
+int init_read_stream(ChunkStream *rs, const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, const ReadLibIndex &ix,
+                     uint64_t max_chunk_bytes, uint32_t pieces = 1);
 // streaming statistics of the current host-level call (mhb_read_stream_stats)
 void read_stream_stats_reset();
 // the chunk cap: mhb_set_read_chunk_limit, or 0

@@ -205,18 +205,19 @@ int sort_unique(cudaStream_t st, u32 *a, u32 *b, uint64_t n, uint32_t w2, uint32
   return MHB_OK;
 }
 
-// The reads (ReadStream: resident, or streamed from host memory in chunks), the flank index resident: per chunk mark +
-// emit into a mark array of the chunk's bases, make the chunk's candidates unique and merge them into the running set by
-// the same sort + unique over the union.  KmerCollector is a set, so the result does not depend on the chunks.
+// The reads (init_read_stream: resident, or streamed from host memory in chunks), the flank index resident: per
+// chunk mark + emit into a mark array of the chunk's bases, make the chunk's candidates unique and merge them into the
+// running set by the same sort + unique over the union.  KmerCollector is a set, so the result does not depend on the
+// chunks.
 int iter_reads(const mhb_iterate_args *a, const ReadLibIndex &ix, const FlankTable &tab, bool stream, DevBuf *set,
                uint64_t *n_set_out, uint64_t *n_cand_out, uint64_t *n_aligned_out) {
   const uint32_t k = a->k, step = a->step, KN = k + step + 1, w2 = words_per_edge(k + step);
   const int WCc = iter_class(k, step);
   cudaStream_t st = 0;
-  ReadStream rs;
+  ChunkStream rs;
   const uint64_t cap = read_chunk_limit() ? read_chunk_limit() : read_chunk_auto_bytes();
-  CKR(rs.init(a->bin, a->bin_words, a->n_reads, ix, stream ? cap : 0));
-  const std::vector<uint64_t> &first = rs.first_reads();
+  CKR(init_read_stream(&rs, a->bin, a->bin_words, a->n_reads, ix, stream ? cap : 0));
+  const std::vector<uint64_t> &first = rs.bounds();
   auto bases_of = [&](uint64_t b, uint64_t e) { return ix.fixed_len ? (e - b) * ix.fixed_len : ix.unit_off[e] - ix.unit_off[b]; };
   uint64_t max_bases = 0;
   for (uint64_t i = 0; i + 1 < first.size(); ++i) max_bases = std::max(max_bases, bases_of(first[i], first[i + 1]));
@@ -228,16 +229,16 @@ int iter_reads(const mhb_iterate_args *a, const ReadLibIndex &ix, const FlankTab
   CKR(d_exist.alloc((max_bases / 32 + 2) * 4, "iterate: position marks"));
   DevBuf c, c2, u, u2, ws, flag, off, bsum;
   uint64_t n_cand = 0, n_set = 0, n_aligned = 0;
-  auto chunk = [&](const ReadChunkView &v) -> int {
-    IterReads rd{v.bin, v.n_reads, ix.fixed_len, v.rec_off, v.aux_off};
-    const uint64_t bw = bases_of(v.first_read, v.first_read + v.n_reads) / 32 + 2;
+  auto chunk = [&](const ChunkView &v) -> int {
+    IterReads rd{v.words, v.n, ix.fixed_len, v.at<uint64_t>(0), v.at<uint64_t>(1)};
+    const uint64_t bw = bases_of(v.first, v.first + v.n) / 32 + 2;
     CK(cudaMemsetAsync(d_exist.p, 0, bw * 4, st));
     CK(cudaMemsetAsync(cnt + 4, 0, 16, st));
-#define M(WW)                                                                                                         \
-  if (WCc == WW) {                                                                                                    \
-    k_iter_mark<WW><<<grid_cap(v.n_reads, 128, 32), 128, 0, st>>>(rd, k, step, tab, d_exist.as<u32>());               \
-    k_iter_emit<WW, false><<<grid_cap(v.n_reads, 128, 32), 128, 0, st>>>(rd, k, step, d_exist.as<u32>(), w2, nullptr, \
-                                                                       cnt + 4, 0);                                   \
+#define M(WW)                                                                                                    \
+  if (WCc == WW) {                                                                                               \
+    k_iter_mark<WW><<<grid_cap(v.n, 128, 32), 128, 0, st>>>(rd, k, step, tab, d_exist.as<u32>());               \
+    k_iter_emit<WW, false><<<grid_cap(v.n, 128, 32), 128, 0, st>>>(rd, k, step, d_exist.as<u32>(), w2, nullptr, \
+                                                                  cnt + 4, 0);                                   \
   }
     IT_FOR_WC(M)
 #undef M
@@ -252,10 +253,10 @@ int iter_reads(const mhb_iterate_args *a, const ReadLibIndex &ix, const FlankTab
     CKR(c.ensure((size_t)nc * w2 * 4 + 16, "iterate: edges"));
     CKR(c2.ensure((size_t)nc * w2 * 4 + 16, "iterate: edges (sort buffer)"));
     CK(cudaMemsetAsync(cnt + 6, 0, 8, st));
-#define M(WW)                                                                                                        \
-  if (WCc == WW)                                                                                                     \
-    k_iter_emit<WW, true><<<grid_cap(v.n_reads, 128, 32), 128, 0, st>>>(rd, k, step, d_exist.as<u32>(), w2, c.as<u32>(), \
-                                                                     cnt + 6, nc);
+#define M(WW)                                                                                                   \
+  if (WCc == WW)                                                                                                \
+    k_iter_emit<WW, true><<<grid_cap(v.n, 128, 32), 128, 0, st>>>(rd, k, step, d_exist.as<u32>(), w2, c.as<u32>(), \
+                                                                cnt + 6, nc);
     IT_FOR_WC(M)
 #undef M
     CK_LAUNCH();

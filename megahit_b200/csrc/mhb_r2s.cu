@@ -234,7 +234,7 @@ PkgChunk chunk_of(const PkgIndex &ix, uint64_t f, uint64_t e, uint32_t k) {
 }
 
 // Every pass over the package.  Resident: the package of the whole library, uploaded and reversed once, is the only
-// chunk.  Streamed: the `.bin` image stays in host memory (ReadStream); per chunk the reads are reversed into a
+// chunk.  Streamed: the `.bin` image stays in host memory (init_read_stream); per chunk the reads are reversed into a
 // chunk-sized package slot and, for variable-length libraries, the chunk's offsets are derived on the device from its
 // length words (k_r2s_chunk_geom + scan32).
 class PkgSource {
@@ -249,8 +249,8 @@ class PkgSource {
     fixed_ = ix.fixed_len != 0;
     std::vector<uint64_t> first = {0, ix.n_reads};
     if (stream) {
-      CKR(rs_.init(a->bin, a->bin_words, ix.n_reads, ix.li, chunk_bytes));
-      first = rs_.first_reads();
+      CKR(init_read_stream(&rs_, a->bin, a->bin_words, ix.n_reads, ix.li, chunk_bytes));
+      first = rs_.bounds();
     }
     for (size_t i = 0; i + 1 < first.size() && ix.n_reads; ++i) {
       chunks.push_back(chunk_of(ix, first[i], first[i + 1], k));
@@ -308,12 +308,13 @@ class PkgSource {
   }
   int each(cudaStream_t st, const ChunkFn &fn) {
     if (!streamed_) return chunks.empty() ? MHB_OK : fn(chunks[0]);
-    return rs_.pass(st, [&](const ReadChunkView &v) -> int {
+    return rs_.pass(st, [&](const ChunkView &v) -> int {
       PkgChunk c = chunks[v.index];
       const uint64_t n = c.pv.n_reads;
       if (!fixed_) {
         u32 *words = geom_.as<u32>(), *s1 = words + pad256(max_reads * 4) / 4, *edges = s1 + pad256(max_reads * 4) / 4;
-        k_r2s_chunk_geom<<<grid_cap(n, 256, 16), 256, 0, st>>>(v.bin, v.rec_off, n, k_, len_.as<u32>(), words, s1, edges);
+        k_r2s_chunk_geom<<<grid_cap(n, 256, 16), 256, 0, st>>>(v.words, v.at<uint64_t>(0), n, k_, len_.as<u32>(), words,
+                                                               s1, edges);
         CK_LAUNCH();
         u64 *bs = bsum_.as<u64>();
         CKR(scan32(st, words, n, word_off_.as<u64>(), word_off_.as<u64>() + n, bs));
@@ -323,8 +324,8 @@ class PkgSource {
         set_offsets(c.pv);
       }
       if (c.n_words) {
-        k_r2s_reverse<<<grid_cap(c.n_words, 256, 16), 256, 0, st>>>(v.bin, n, c.pv.fixed_len, v.rec_off, c.pv, pkg_.as<u32>(),
-                                                               c.n_words);
+        k_r2s_reverse<<<grid_cap(c.n_words, 256, 16), 256, 0, st>>>(v.words, n, c.pv.fixed_len, v.at<uint64_t>(0), c.pv,
+                                                               pkg_.as<u32>(), c.n_words);
         CK_LAUNCH();
       }
       c.pv.words = pkg_.as<u32>();
@@ -343,7 +344,7 @@ class PkgSource {
   const mhb_build_args *args_ = nullptr;
   uint32_t k_ = 0;
   bool streamed_ = false, fixed_ = false;
-  ReadStream rs_;
+  ChunkStream rs_;
   DevBuf lib_, pkg_, word_off_, len_, base_off_, s1_off_, edge_off_, geom_, bsum_;
 };
 
@@ -1535,7 +1536,7 @@ extern "C" int mhb_selftest_r2s_mercy_read(uint32_t fixed_len, uint64_t n_reads,
 
 // The offsets of one chunk [first, first + count) of a `.bin` library.  derive = 1: as the streamed path derives them on
 // the device, from the chunk's records alone (r2s_read_geom per read, exclusive scans; record offsets rebased to the
-// chunk as ReadStream hands them over), and *base0_out = the chunk's global base (PkgView::base0).  derive = 0:
+// chunk as the read stream hands them over), and *base0_out = the chunk's global base (PkgView::base0).  derive = 0:
 // index_pkg's arrays of the whole library sliced to the chunk and rebased (variable-length libraries only).  len_out
 // gets count entries, the offset arrays count + 1.
 extern "C" int mhb_selftest_r2s_chunk_index(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, uint32_t k,

@@ -1,7 +1,7 @@
-// mhb_stream.cu -- the host-side `.bin` index and every pass over a read library (ReadStream, mhb_internal.h): resident
-// in device memory, or, for libraries larger than device memory, kept in host memory and streamed through the device in
-// chunks that end on read boundaries.  The count and iterate stages hand each chunk to the same extraction / marking /
-// emission kernels whichever form the library takes.
+// mhb_stream.cu -- the host-side `.bin` index and every pass over an input in host memory (ChunkStream,
+// mhb_internal.h): read libraries, sequence sets and sorted edges, resident in device memory or, when larger than
+// device memory, kept in host memory and streamed through the device in chunks that end on unit boundaries.  The stages
+// hand each chunk to the same kernels whichever form the input takes.
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -245,107 +245,103 @@ int ChunkStager::upload(void *stream, const char *host, const std::vector<size_t
 }
 
 // ------------------------------------------------------------------------------------------------
-// ReadStream
+// ChunkStream
 // ------------------------------------------------------------------------------------------------
-int ReadStream::init(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, const ReadLibIndex &ix, uint64_t max_chunk_bytes,
-                     uint32_t pieces) {
-  resident_ = max_chunk_bytes == 0;
-  bin_ = bin;
-  bin_words_ = bin_words;
-  ix_ = &ix;
-  aux_off_ = ix.unit_off.empty() ? nullptr : ix.unit_off.data();  // an index without unit offsets streams none
-  uint64_t max_words = bin_words;
-  if (resident_) {
-    first_ = {0, n_reads};
-    max_reads_ = n_reads;
-  } else {
-    plan_read_chunks(ix, n_reads, max_chunk_bytes, &first_);
-    max_words = max_reads_ = 0;
+int ChunkStream::init(const Input &in, std::vector<uint64_t> first, StreamStats *stats, uint32_t pieces) {
+  in_ = in;
+  resident_ = first.empty();
+  first_ = resident_ ? std::vector<uint64_t>{0, in.n} : std::move(first);
+  uint64_t max_words = in.words;
+  max_units_ = in.n;
+  if (!resident_) {
+    max_words = max_units_ = 0;
     for (uint64_t i = 0; i < n_chunks(); ++i) {
-      max_reads_ = std::max(max_reads_, first_[i + 1] - first_[i]);
-      max_words = std::max(max_words, ix_->word_of(first_[i + 1]) - ix_->word_of(first_[i]));
+      max_units_ = std::max(max_units_, first_[i + 1] - first_[i]);
+      max_words = std::max(max_words, in.word_of(first_[i + 1]) - in.word_of(first_[i]));
     }
   }
-  // the image 16-byte aligned + 16 bytes: the extraction's bulk copies end on a 16-byte boundary
-  off_at_ = pad256(((max_words * 4 + 15) & ~(size_t)15) + 16);
-  slot_bytes_ = off_at_ + (ix_->fixed_len ? 0 : (aux_off_ ? 2 : 1) * pad256((max_reads_ + 1) * 8));
-  g_st.chunks = n_chunks();
-  pieces_.clear();
-  if (resident_ && ix.fixed_len && pieces > 1) {
-    const uint64_t per = ((n_reads + pieces - 1) / pieces + 3) & ~(uint64_t)3;
-    for (uint64_t r = 0; r < n_reads; r += per) pieces_.push_back(r);
-    pieces_.push_back(n_reads);
-    return stager_.init(0, pieces_.size() - 1, &g_st);
+  slot_bytes_ = image_bytes(max_words);
+  for (int j = 0; j < 4; ++j) {
+    side_at_[j] = slot_bytes_;
+    if (in.side[j].host) slot_bytes_ += side_bytes(max_units_, in.side[j].elem);
   }
-  return stager_.init(slot_bytes_, n_chunks(), &g_st);
+  stats->chunks = n_chunks();
+  pieces_.clear();
+  if (resident_ && pieces > 1) {
+    const uint64_t per = ((in.n + pieces - 1) / pieces + 3) & ~(uint64_t)3;
+    for (uint64_t u = 0; u < in.n; u += per) pieces_.push_back(u);
+    pieces_.push_back(in.n);
+    return stager_.init(0, pieces_.size() - 1, stats);
+  }
+  return stager_.init(slot_bytes_, n_chunks(), stats);
 }
 
-int ReadStream::bind(void *device, void *stream) {
+int ChunkStream::bind(void *device, void *stream) {
   dev_ = (char *)device;
   stager_.bind(dev_);
   if (!resident_ || !pieces_.empty()) return MHB_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  const uint64_t n_reads = first_[1];
-  if (bin_words_) CK(cudaMemcpyAsync(dev_, bin_, bin_words_ * 4, cudaMemcpyHostToDevice, st));
-  if (!ix_->fixed_len && n_reads) {
-    CK(cudaMemcpyAsync(dev_ + off_at_, ix_->rec_off.data(), (n_reads + 1) * 8, cudaMemcpyHostToDevice, st));
-    if (aux_off_)
-      CK(cudaMemcpyAsync(dev_ + off_at_ + pad256((n_reads + 1) * 8), aux_off_, (n_reads + 1) * 8, cudaMemcpyHostToDevice, st));
+  if (in_.words) CK(cudaMemcpyAsync(dev_, in_.image, in_.words * 4, cudaMemcpyHostToDevice, st));
+  for (int j = 0; j < 4 && in_.n; ++j) {
+    const Side &s = in_.side[j];
+    const size_t bytes = s.elem ? in_.n * s.elem : (in_.n + 1) * 8;
+    if (s.host) CK(cudaMemcpyAsync(dev_ + side_at_[j], s.host, bytes, cudaMemcpyHostToDevice, st));
   }
   return MHB_OK;
 }
 
-ReadChunkView ReadStream::view(uint64_t i, const char *slot) const {
-  ReadChunkView v;
+ChunkView ChunkStream::view(uint64_t i, const char *slot) const {
+  ChunkView v;
   v.index = i;
-  v.first_read = first_[i];
-  v.n_reads = first_[i + 1] - first_[i];
-  v.bin = (const uint32_t *)slot;
-  v.bin_words = resident_ ? bin_words_ : ix_->word_of(first_[i + 1]) - ix_->word_of(first_[i]);
-  v.rec_off = ix_->fixed_len ? nullptr : (const uint64_t *)(slot + off_at_);
-  v.aux_off = ix_->fixed_len || !aux_off_ ? nullptr : (const uint64_t *)(slot + off_at_ + pad256((max_reads_ + 1) * 8));
+  v.first = first_[i];
+  v.n = first_[i + 1] - first_[i];
+  v.words = (const uint32_t *)slot;
+  v.n_words = resident_ ? in_.words : in_.word_of(first_[i + 1]) - in_.word_of(first_[i]);
+  for (int j = 0; j < 4; ++j) v.side[j] = in_.side[j].host ? slot + side_at_[j] : nullptr;
   return v;
 }
 
-// chunk i into a staging buffer: its image, and for a variable-length library its offsets rebased to the chunk
-int ReadStream::fill(uint64_t i, char *h, ChunkStager::Copies *up) const {
-  const uint64_t b = first_[i], e = first_[i + 1], w0 = ix_->word_of(b), nw = ix_->word_of(e) - w0;
-  {
-    const uint64_t bytes = nw * 4, blk = 4ull << 20, nblk = (bytes + blk - 1) / blk;
+// chunk i into a staging buffer: its image, then its slice of every side array, offsets rebased to the chunk
+int ChunkStream::fill(uint64_t i, char *h, ChunkStager::Copies *up) const {
+  const uint64_t b = first_[i], n = first_[i + 1] - b, w0 = in_.word_of(b);
+  const uint64_t bytes = (in_.word_of(b + n) - w0) * 4, blk = 4ull << 20, nblk = (bytes + blk - 1) / blk;
 #pragma omp parallel for schedule(static)
-    for (long long j = 0; j < (long long)nblk; ++j) {
-      const uint64_t o = (uint64_t)j * blk;
-      memcpy(h + o, (const char *)(bin_ + w0) + o, std::min(blk, bytes - o));
+  for (long long j = 0; j < (long long)nblk; ++j) {
+    const uint64_t o = (uint64_t)j * blk;
+    memcpy(h + o, (const char *)(in_.image + w0) + o, std::min(blk, bytes - o));
+  }
+  up->add(0, bytes);
+  for (int j = 0; j < 4; ++j) {
+    const Side &s = in_.side[j];
+    if (!s.host) continue;
+    char *d = h + side_at_[j];
+    if (s.elem) {
+      memcpy(d, (const char *)s.host + b * s.elem, n * s.elem);
+      up->add(side_at_[j], n * s.elem);
+      continue;
     }
-  }
-  up->add(0, nw * 4);
-  if (ix_->fixed_len) return MHB_OK;
-  const uint64_t nr = e - b, ao_at = off_at_ + pad256((max_reads_ + 1) * 8);
-  uint64_t *ro = (uint64_t *)(h + off_at_), *ao = (uint64_t *)(h + ao_at);
-  const uint64_t r0 = ix_->rec_off[b], a0 = aux_off_ ? aux_off_[b] : 0;
+    const uint64_t *src = (const uint64_t *)s.host + b;
+    uint64_t *dst = (uint64_t *)d;
 #pragma omp parallel for schedule(static)
-  for (long long r = 0; r <= (long long)nr; ++r) {
-    ro[r] = ix_->rec_off[b + r] - r0;
-    if (aux_off_) ao[r] = aux_off_[b + r] - a0;
+    for (long long u = 0; u <= (long long)n; ++u) dst[u] = src[u] - src[0];
+    up->add(side_at_[j], (n + 1) * 8);
   }
-  up->add(off_at_, (nr + 1) * 8);
-  if (aux_off_) up->add(ao_at, (nr + 1) * 8);
   return MHB_OK;
 }
 
-int ReadStream::pass(void *stream, const std::function<int(const ReadChunkView &)> &fn) {
-  if (!dev_) return mhb_set_error(MHB_ERR_ARG, "internal: read library without device memory");
+int ChunkStream::pass(void *stream, const std::function<int(const ChunkView &)> &fn) {
+  if (!dev_) return mhb_set_error(MHB_ERR_ARG, "internal: chunk stream without device memory");
   if (resident_ && !pieces_.empty()) {
     std::vector<uint64_t> p;
     p.swap(pieces_);
     std::vector<size_t> off;
-    for (uint64_t r : p) off.push_back(ix_->word_of(r) * 4);
-    return stager_.upload(stream, (const char *)bin_, off, [&](uint64_t i, const char *piece) {
-      ReadChunkView v = view(0, piece);
+    for (uint64_t u : p) off.push_back(in_.word_of(u) * 4);
+    return stager_.upload(stream, (const char *)in_.image, off, [&](uint64_t i, const char *piece) {
+      ChunkView v = view(0, piece);
       v.index = i;
-      v.first_read = p[i];
-      v.n_reads = p[i + 1] - p[i];
-      v.bin_words = ix_->word_of(p[i + 1]) - ix_->word_of(p[i]);
+      v.first = p[i];
+      v.n = p[i + 1] - p[i];
+      v.n_words = in_.word_of(p[i + 1]) - in_.word_of(p[i]);
       return fn(v);
     });
   }
@@ -353,4 +349,19 @@ int ReadStream::pass(void *stream, const std::function<int(const ReadChunkView &
   return stager_.pass(
       stream, [this](uint64_t i, char *h, ChunkStager::Copies *up) { return fill(i, h, up); },
       [&](uint64_t i, const char *slot) { return fn(view(i, slot)); });
+}
+
+int init_read_stream(ChunkStream *rs, const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, const ReadLibIndex &ix,
+                     uint64_t max_chunk_bytes, uint32_t pieces) {
+  ChunkStream::Input in;
+  in.image = bin;
+  in.words = bin_words;
+  in.n = n_reads;
+  in.word_off = ix.fixed_len ? nullptr : ix.rec_off.data();
+  in.stride = 1 + div_ceil(ix.fixed_len, 16);
+  if (!ix.fixed_len) in.side[0].host = ix.rec_off.data();
+  if (!ix.fixed_len && !ix.unit_off.empty()) in.side[1].host = ix.unit_off.data();
+  std::vector<uint64_t> first;
+  if (max_chunk_bytes) plan_read_chunks(ix, n_reads, max_chunk_bytes, &first);
+  return rs->init(in, std::move(first), &g_st, ix.fixed_len ? pieces : 1);
 }
