@@ -594,6 +594,10 @@ int mhb_build_host(const mhb_build_args *args, mhb_build_result *res);
  * (mhb_read_stream_decide); then the `.bin` image stays in host memory and every pass streams it through the device in
  * chunks, each reversed and indexed on the device, and only the bit planes stay resident: solid (m > 1, 1 bit per base)
  * and the three mercy candidate planes (need_mercy, 3 bits per base).  mhb_read_stream_stats / _times report it.
+ * When those candidate planes do not fit next to the rest (or mhb_set_r2s_sparse_mercy(1)), the streamed form keeps the
+ * candidates as every stage-1 round's list of u64 entries (position << 2 | code: 0 = any, 1 = no in, 2 = no out),
+ * sorted by position in host memory, and the mercy step scatters each chunk's slice into chunk-sized planes; only the
+ * solid plane is then whole-library.  mhb_r2s_mercy_stats reports the form.
  * res->n_rounds_s1 / n_rounds_s2 report the plan; neither plan changes the output.  A single bucket larger than a round
  * returns MHB_ERR_NOMEM, as do bit planes and chunk buffers that alone do not fit. */
 int mhb_read2sdbg_host(const mhb_build_args *args, mhb_build_result *res);
@@ -601,6 +605,15 @@ int mhb_read2sdbg_host(const mhb_build_args *args, mhb_build_result *res);
  * memory), on one GPU and, per owner, on several (mhb_read2sdbg_run_multi).  Independent of mhb_set_round_limit /
  * mhb_set_s2s_round_limit.  The result does not depend on the caps. */
 int mhb_set_r2s_round_limit(uint64_t max_s1_records, uint64_t max_s2_items);
+/* The form of read2sdbg's mercy candidates (need_mercy): 0 = automatic - planes of the whole library, lists only when a
+ * streamed library's planes do not fit (mhb_read2sdbg_host) or when the planes of the whole library do not fit a rank
+ * (mhb_read2sdbg_run_multi: every rank takes lists when one does) -; 1 = lists whenever the library is streamed, and on
+ * every rank of a multi-GPU build.  On several GPUs each owner of stage-1 records makes sorted lists from its rounds and
+ * every rank fetches the entries inside its share into planes of its share only.  The result does not depend on it. */
+int mhb_set_r2s_sparse_mercy(int mode);
+/* The last mhb_read2sdbg_host call: *sparse = 1 when its candidates were lists, *n_entries = their entries over every
+ * round, *host_bytes = the host memory they took (8 bytes per entry).  Any pointer may be NULL. */
+int mhb_r2s_mercy_stats(int *sparse, uint64_t *n_entries, uint64_t *host_bytes);
 
 /* `megahit_core iterate` (SURVEY.md 8f N2; main_iterate.cpp:117-221, iterate/contig_flank_index.h:16-221,
  * iterate/kmer_collector.h:37-79): the iterative edges for k + step - every (k+step+1)-mer of a read whose step+1
@@ -893,6 +906,25 @@ int mhb_selftest_r2s_mercy_read(uint32_t fixed_len, uint64_t n_reads, uint64_t r
 int mhb_selftest_r2s_chunk_index(const uint32_t *bin, uint64_t bin_words, uint64_t n_reads, uint32_t k, uint64_t first,
                                  uint64_t count, int derive, uint32_t *len_out, uint64_t *word_off_out,
                                  uint64_t *base_off_out, uint64_t *s1_off_out, uint64_t *edge_off_out, uint64_t *base0_out);
+/* the form of the mercy candidates mhb_read2sdbg_host takes for a streamed library of n_bases bases, chunks of at most
+ * max_plane_words plane words and streamed_bytes of chunk buffers (host only): *planes_out / *lists_out = the device
+ * bytes the streamed form holds in either form, *sparse_out = 1 for the list form */
+int mhb_selftest_r2s_mercy_form(uint64_t n_bases, uint64_t max_plane_words, uint64_t streamed_bytes, int32_t m,
+                                int need_mercy, uint64_t free_bytes, int force, uint64_t *planes_out, uint64_t *lists_out,
+                                int *sparse_out);
+/* stage-1 Lv2Postprocess of one sorted bucket (as mhb_selftest_r2s_s1_group) in the list form: the candidates as
+ * entries (position << 2 | code) in record order, room for 2 n; *n_out = entries */
+int mhb_selftest_r2s_s1_cand(const uint32_t *recs, uint64_t n, uint32_t k, int32_t m, uint32_t fixed_len,
+                             uint64_t n_reads, uint32_t *is_solid, int64_t *counting, uint64_t *entries_out,
+                             uint64_t *n_out);
+/* the mercy step over a library whose first base is base0 (fixed_len, or the n_reads lengths len), planes on the word
+ * grid from base0 / 32: list form (entries: n_rounds sorted lists, round t ending at round_end[t]) in the chunks
+ * chunk_first[0 .. n_chunks], or plane form (entries NULL; planes = no_in, no_out, any of n_plane_words words each).
+ * mercy gets the added bits, *added_out their number. */
+int mhb_selftest_r2s_mercy_lists(uint32_t fixed_len, uint64_t n_reads, const uint32_t *len, uint64_t base0, uint32_t k,
+                                 const uint32_t *is_solid, const uint64_t *entries, const uint64_t *round_end,
+                                 uint32_t n_rounds, const uint64_t *chunk_first, uint32_t n_chunks,
+                                 const uint32_t *planes, uint64_t n_plane_words, uint32_t *mercy, uint64_t *added_out);
 /* the residency rule of mhb_read2sdbg_host on given library sizes and free device bytes (host only) */
 int mhb_selftest_r2s_stream_decide(uint64_t n_reads, uint64_t bin_words, uint32_t fixed_len, uint64_t n_words,
                                    uint64_t n_bases, uint64_t n_s1, uint64_t n_edges, uint32_t k, int32_t m, int need_mercy,

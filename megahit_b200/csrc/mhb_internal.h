@@ -415,7 +415,8 @@ struct OwnerRoute {
 // ---- read2sdbg's device pieces (mhb_r2s.cu), driven step by step by the multi-GPU worker ----
 // One rank's share [first, end) of the reads of a build, resident on the current device as one package chunk: read
 // indices are local, bases - stage-1 payload positions and bit-plane indices - global, and the bit planes (solid; with
-// need_mercy the three candidate planes after it, in one allocation) cover the whole library's word grid.  Records
+// need_mercy in the plane form the three candidate planes after it, in one allocation) cover the whole library's word
+// grid.  Records
 // reach their owners (ranks of contiguous leading-byte ranges) through an OwnerRoute, one round over ascending bucket
 // sub-ranges at a time (rt.lo / rt.hi).
 class R2sShare {
@@ -426,6 +427,18 @@ class R2sShare {
   R2sShare &operator=(const R2sShare &) = delete;
   // a: the whole library and the build's k, m, need_mercy; li: its index_read_lib (made before the fork)
   int load(const mhb_build_args *a, const ReadLibIndex &li, uint64_t first, uint64_t end);
+  // The mercy candidates of a need_mercy build: planes of the whole library, or (list form, DESIGN.md §4.9) sorted
+  // lists made by the owners of stage 1 and planes of the share only.  want_cand_lists: this rank's wish - the list
+  // form is forced (mhb_set_r2s_sparse_mercy) or the four planes of the whole library exceed avail; every rank must
+  // then bind the same form.  bind_planes allocates the planes of the form (after load, before stage 1).
+  bool want_cand_lists(size_t avail) const;
+  int bind_planes(bool lists);
+  bool cand_lists() const;
+  uint64_t base_of(uint64_t read) const;  // global base of a read of the library
+  // list form: every stage-1 round's candidates this rank owned (sorted by position), after the last s1_own; then
+  // cand_take hands over every owner's entries inside my share (any number of lists, each sorted), for mercy_count
+  const std::vector<std::vector<uint64_t>> &cand_made() const;
+  void cand_take(std::vector<std::vector<uint64_t>> *lists);
   uint32_t s1_record_words() const;  // words of a stage-1 record row
   bool s1_narrow() const;            // read_info in a side array of 8 bytes per row
   // The most stage-1 records / stage-2 items one owner takes in one round (at most n_total): the largest round whose

@@ -33,6 +33,8 @@
 // `read2sdbg` (mhb_read2sdbg_run_multi): the stage-1 records reach their owners in global read order, the owners run
 // stage 1 into planes of the whole library, every rank ORs all planes over its share's words, runs the mercy step over
 // its share and sends its stage-2 items to their owners, which sort, collapse and emit as the single-GPU read2sdbg does.
+// Where the candidate planes of the whole library do not fit, the owners make sorted candidate lists instead and every
+// rank fetches the entries of its share into candidate planes of the share (cand_exchange).
 // Both sort stages run in rounds over ascending bucket ranges when an owner's records do not fit its device at once
 // (or exceed mhb_set_r2s_round_limit), as the count's records do.
 #include <cuda_runtime.h>
@@ -973,6 +975,45 @@ struct R2sJob {
   std::string prefix;
 };
 
+// The list form's candidates to the shares they lie in: I publish my stage-1 rounds' lists back to back ("cand") and,
+// per round, the entry offsets at every share's first base ("candix": rounds x (world + 1)); every rank fetches from
+// every owner the slice of each round inside its share.  Each slice is sorted, as its round is.
+void cand_exchange(const R2sJob &J, Exchange &X, R2sShare &sh) {
+  const int W = X.world, r = X.rank;
+  const std::vector<std::vector<uint64_t>> &made = sh.cand_made();
+  std::vector<uint64_t> all, ix;
+  uint64_t n_made = 0;
+  for (const auto &v : made) {
+    for (int s = 0; s <= W; ++s) {
+      const uint64_t key = s == W ? ~0ull : sh.base_of(J.first[s]) << 2;
+      ix.push_back(all.size() + (uint64_t)(std::lower_bound(v.begin(), v.end(), key) - v.begin()));
+    }
+    all.insert(all.end(), v.begin(), v.end());
+    n_made += v.size();
+  }
+  X.publish("cand", all.data(), all.size() * 8);
+  X.publish("candix", ix.data(), ix.size() * 8);
+  std::vector<uint64_t>().swap(all);
+  X.barrier();  // every list is published
+  std::vector<std::vector<uint64_t>> mine;
+  uint64_t n_got = 0;
+  for (int o = 0; o < W; ++o) {
+    const std::vector<char> oix = X.fetch("candix", o);
+    const uint64_t *p = (const uint64_t *)oix.data();
+    const size_t rounds = oix.size() / 8 / (W + 1);
+    for (size_t t = 0; t < rounds; ++t) {
+      const uint64_t lo = p[t * (W + 1) + r], hi = p[t * (W + 1) + r + 1];
+      if (hi <= lo) continue;
+      const std::vector<char> b = X.fetch("cand", o, lo * 8, (hi - lo) * 8);
+      mine.emplace_back((const uint64_t *)b.data(), (const uint64_t *)b.data() + (hi - lo));
+      n_got += hi - lo;
+    }
+  }
+  sh.cand_take(&mine);
+  XINFO("rank %d: mercy candidates: %llu list entries made, %llu inside the share\n", r, (unsigned long long)n_made,
+        (unsigned long long)n_got);
+}
+
 void r2s_worker(const R2sJob &J, Exchange &X) {
   const int W = X.world, r = X.rank;
   const uint32_t k = J.a.k, W2 = mhb_s2s_record_words(k);
@@ -980,6 +1021,16 @@ void r2s_worker(const R2sJob &J, Exchange &X) {
   bind_device(r, W);
   R2sShare sh;
   CKL(sh.load(&J.a, *J.li, J.first[r], J.first[r + 1]));
+  // the form of the mercy candidates, the same on every rank: lists when one rank wants them (DESIGN.md §4.9)
+  const int want = sh.want_cand_lists(rank_round_bytes(r, W)) ? 1 : 0;
+  const uint64_t want64 = (uint64_t)want;
+  bool lists = false;
+  for (uint64_t w : X.gather(&want64, 1)) lists = lists || w;
+  CKL(sh.bind_planes(lists));
+  lists = sh.cand_lists();
+  if (lists)
+    XINFO("rank %d: mercy candidates as sorted lists: the solid plane of the whole library, the candidate planes of my "
+          "share only\n", r);
   std::vector<uint64_t> h16(65536);
   uint64_t n_s1_own = 0;
   int R1 = 0;
@@ -1011,6 +1062,7 @@ void r2s_worker(const R2sJob &J, Exchange &X) {
     }
     sh.s1_end();
     ex.close(X);
+    if (lists) cand_exchange(J, X, sh);
 
     // ---- plane merge: the words of my share's reads, OR-ed over every rank's planes (read through CUDA IPC) ----
     uint64_t handle[8];

@@ -200,6 +200,7 @@ struct PkgChunk {
   uint64_t s1_0 = 0, n_s1 = 0;     // stage-1 records before the chunk / in it
   uint64_t n_edges = 0;            // (k+1)-mer positions in the chunk
   uint64_t w0 = 0, w_end = 0;      // the chunk's words of the bit planes: [base0 / 32, base_end / 32 + 2)
+  uint64_t base_end = 0;           // global base after the chunk's last read
 };
 using ChunkFn = std::function<int(const PkgChunk &)>;
 using EachChunk = std::function<int(const ChunkFn &)>;  // one pass over the package: fn once per chunk, in read order
@@ -230,8 +231,64 @@ PkgChunk chunk_of(const PkgIndex &ix, uint64_t f, uint64_t e, uint32_t k) {
   }
   c.w0 = c.pv.base0 / 32;
   c.w_end = (c.pv.base0 + bases) / 32 + 2;  // the whole library: bit_words
+  c.base_end = c.pv.base0 + bases;
   return c;
 }
+
+// ---- the list form of the mercy candidates (DESIGN.md §4.9) ----
+int g_r2s_sparse_mercy = 0;  // mhb_set_r2s_sparse_mercy: 1 = lists whenever the library is streamed
+struct MercyStats {
+  int sparse = 0;
+  uint64_t n_entries = 0, host_bytes = 0;
+} g_mercy_stats;  // mhb_r2s_mercy_stats: the last mhb_read2sdbg_host call
+
+// The candidates of every stage-1 round as a list of entries (cand_entries: position << 2 | code), each sorted by
+// position, in host memory.  Duplicates are allowed: the planes they stand for are sets.
+struct CandLists {
+  std::vector<std::vector<uint64_t>> rounds;
+  uint32_t sort_bytes = 8;  // the low bytes of an entry that can be non-zero
+  void init(uint64_t n_bases) {
+    rounds.clear();
+    const uint64_t top = n_bases << 2 | 3;
+    for (sort_bytes = 1; sort_bytes < 8 && (top >> (8 * sort_bytes)); ++sort_bytes) {}
+  }
+  uint64_t n_entries() const {
+    uint64_t n = 0;
+    for (const auto &v : rounds) n += v.size();
+    return n;
+  }
+  // fn(entries, count) for the slice of every round with positions in [b0, b1) (binary search)
+  template <class F>
+  int each_slice(uint64_t b0, uint64_t b1, F fn) const {
+    for (const auto &v : rounds) {
+      const auto lo = std::lower_bound(v.begin(), v.end(), b0 << 2), hi = std::lower_bound(lo, v.end(), b1 << 2);
+      if (hi > lo) CKR(fn(&*lo, (uint64_t)(hi - lo)));
+    }
+    return MHB_OK;
+  }
+};
+
+// The chunk's candidates into three planes of plane_words words each at `planes` (no in, no out, any), on the global
+// word grid from word w0; returns o with its candidate planes pointing there.  Slices go through `stage` (device,
+// stage_cap entries) one piece at a time.
+int cand_scatter(cudaStream_t st, const CandLists &lists, uint64_t b0, uint64_t b1, uint64_t w0, u32 *planes,
+                 uint64_t plane_words, u64 *stage, uint64_t stage_cap, S1Out *o) {
+  CK(cudaMemsetAsync(planes, 0, 3 * plane_words * 4, st));
+  o->no_in = planes - w0;
+  o->no_out = planes + plane_words - w0;
+  o->any = planes + 2 * plane_words - w0;
+  const S1Out so = *o;
+  return lists.each_slice(b0, b1, [&](const uint64_t *e, uint64_t n) -> int {
+    for (uint64_t at = 0; at < n; at += stage_cap) {
+      const uint64_t piece = std::min(stage_cap, n - at);
+      CK(cudaMemcpyAsync(stage, e + at, piece * 8, cudaMemcpyHostToDevice, st));
+      k_r2s_cand_scatter<<<grid_cap(piece, 256, 16), 256, 0, st>>>(stage, piece, so);
+      CK_LAUNCH();
+    }
+    return MHB_OK;
+  });
+}
+constexpr uint64_t kCandStage = (uint64_t)1 << 20;  // entries of the staging slot of the scatter (8 MiB)
 
 // Every pass over the package.  Resident: the package of the whole library, uploaded and reversed once, is the only
 // chunk.  Streamed: the `.bin` image stays in host memory (init_read_stream); per chunk the reads are reversed into a
@@ -378,6 +435,26 @@ bool stream_decide(const ResidentPlan &p, const PkgIndex &ix, uint32_t k, int32_
   return mhb_read_stream_decide(p.resident + p.upload, free_b, no_round ? 1 : 0, chunk_limit) != 0;
 }
 
+// ---- the form of the mercy candidates (DESIGN.md §4.9) ----
+// Device bytes the streamed form holds for the whole call in either form: the solid plane (m > 1), the candidates -
+// three planes of the whole library, or (list form) three chunk-sized planes and the staging slot of the scatter -,
+// the mercy plane of a chunk, the read chunk buffers, the histogram, counters and bucket table.  The list form is taken
+// when the planes do not fit free_b, or always with force (mhb_set_r2s_sparse_mercy), and only with need_mercy.
+struct MercyForm {
+  size_t planes = 0, lists = 0;
+  bool sparse = false;
+};
+MercyForm mercy_form(uint64_t bit_words, uint64_t max_plane_words, size_t streamed_bytes, int32_t m, bool mercy,
+                     size_t free_b, int force) {
+  const size_t rest = (m > 1 ? pad256(bit_words * 4) : 0) + (mercy ? pad256(max_plane_words * 4) : 0) + streamed_bytes +
+                      pad256(65536 * 8) + pad256(64) + pad256((size_t)MHB_NUM_BUCKETS * 32) + pad256(128);
+  MercyForm f;
+  f.planes = rest + (mercy ? 3 * pad256(bit_words * 4) : 0);
+  f.lists = rest + (mercy ? pad256(3 * max_plane_words * 4) + pad256(kCandStage * 8) : 0);
+  f.sparse = mercy && (force || f.planes > free_b);
+  return f;
+}
+
 // ---- stage 1 on the device: is_solid bits, mercy planes, multiplicity histogram ----
 struct S1Side {  // the narrow layout's read_info side array and the pair buffers of its bucket partition
   DevBuf info, pa, pb;
@@ -391,7 +468,7 @@ struct S1Bufs {
   u32 *pa, *pb;
 };
 int s1_sort_post(cudaStream_t st, const PkgView &pv, uint32_t k, int32_t m, bool need_mercy, const S1Out &out,
-                 unsigned long long *d_mul_hist, PhaseTrace &tr, const S1Bufs &bufs, uint64_t n);
+                 unsigned long long *d_mul_hist, PhaseTrace &tr, const S1Bufs &bufs, uint64_t n, CandLists *lists);
 
 // Stage 1 in rounds over contiguous ranges of bucket ids, each of at most max_n records; *n_rounds counts the
 // non-empty ones.  max_n == 0: one pass, the one range over all bucket ids, known without a pass: each chunk's records
@@ -400,10 +477,11 @@ int s1_sort_post(cudaStream_t st, const PkgView &pv, uint32_t k, int32_t m, bool
 // min_ws_bytes (stage 2's share).  Otherwise one histogram pass over the library plans the ranges, then per range one
 // pass extracts the in-range records of every chunk in read order (count, scan, write at the round's cursor).  Each
 // round is sorted and post-processed alike.  A (k-1)-mer group lies in one bucket, so in one round; is_solid, the mercy
-// planes and the multiplicity histogram accumulate across rounds.
+// planes and the multiplicity histogram accumulate across rounds (lists != nullptr: each round adds its candidate list).
 int run_stage1(cudaStream_t st, const EachChunk &each, const PkgView &shape, const PkgIndex &ix, uint64_t chunk_reads,
                uint32_t k, int32_t m, bool need_mercy, const S1Out &out, unsigned long long *d_mul_hist, PhaseTrace &tr,
-               BigBufs &big, uint64_t max_n, size_t min_rec_bytes, size_t min_ws_bytes, uint32_t *n_rounds) {
+               BigBufs &big, uint64_t max_n, size_t min_rec_bytes, size_t min_ws_bytes, uint32_t *n_rounds,
+               CandLists *lists) {
   const S1Layout l = s1_layout(k);
   const uint32_t NW = l.NW, RW = l.RW;
   const bool one_pass = max_n == 0;
@@ -494,7 +572,7 @@ int run_stage1(cudaStream_t st, const EachChunk &each, const PkgView &shape, con
     if (n == 0) continue;
     tr.mark("s1.extract");
     const S1Bufs bufs{big.a.as<u32>(), big.b.as<u32>(), big.ws.p, d_info, side.pa.as<u32>(), side.pb.as<u32>()};
-    CKR(s1_sort_post(st, shape, k, m, need_mercy, out, d_mul_hist, tr, bufs, n));
+    CKR(s1_sort_post(st, shape, k, m, need_mercy, out, d_mul_hist, tr, bufs, n, lists));
     ++*n_rounds;
   }
   if (seen != ix.n_s1)
@@ -503,9 +581,57 @@ int run_stage1(cudaStream_t st, const EachChunk &each, const PkgView &shape, con
   return MHB_OK;
 }
 
-// stable bucket partition, kmsort emulation and Lv2Postprocess of the n records in bufs.a
+// The candidate bytes of a post-processed round of n records (recs) -> the round's entries, sorted by position, appended
+// to lists.  Count -> scan32 -> write in record order; entries in `spare` (the other record buffer) when they fit, and
+// the stable radix sort on the position bytes into recs, which the write leaves unused.
+int cand_round(cudaStream_t st, const uint8_t *cand, uint64_t n, u32 *recs, u32 *spare, const S1Layout &l,
+               const S1Bufs &bufs, CandLists *lists) {
+  const uint64_t n_tiles = (n + kCandTile - 1) / kCandTile;
+  const size_t rec_bytes = (size_t)n * l.RW * 4;  // the least either record buffer holds
+  DevBuf tile_n, tile_off, bsum, ent, srt, ws;
+  CKR(tile_n.alloc(n_tiles * 4, "read2sdbg: candidate counts"));
+  CKR(tile_off.alloc((n_tiles + 1) * 8, "read2sdbg: candidate offsets"));
+  CKR(bsum.alloc((n_tiles / 4096 + 4) * 8, "read2sdbg: scan sums"));
+  k_r2s_cand_count<<<(unsigned)n_tiles, 256, 0, st>>>(cand, n, tile_n.as<u32>());
+  CK_LAUNCH();
+  CKR(scan32(st, tile_n.as<u32>(), n_tiles, tile_off.as<u64>(), tile_off.as<u64>() + n_tiles, bsum.as<u64>()));
+  uint64_t cnt = 0;
+  CK(cudaMemcpyAsync(&cnt, tile_off.as<u64>() + n_tiles, 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  lists->rounds.emplace_back(cnt);
+  if (!cnt) return MHB_OK;
+  u64 *e = (u64 *)spare;
+  if (cnt * 8 > rec_bytes) {
+    CKR(ent.alloc(cnt * 8, "read2sdbg: candidate entries"));
+    e = ent.as<u64>();
+  }
+  k_r2s_cand_write<<<(unsigned)n_tiles, 256, 0, st>>>(cand, n, recs, l.narrow ? bufs.info : nullptr, l.RW, l.NW,
+                                                      tile_off.as<u64>(), e);
+  CK_LAUNCH();
+  u32 *sb = recs;
+  if (cnt * 8 > rec_bytes) {
+    CKR(srt.alloc(cnt * 8, "read2sdbg: candidate entries (sort buffer)"));
+    sb = srt.as<u32>();
+  }
+  const size_t ws_need = mhb_sort_workspace_bytes(cnt, 2);
+  void *w = bufs.ws;
+  if (ws_need > s1_ws_bytes(n, l)) {
+    CKR(ws.alloc(ws_need, "read2sdbg: candidate sort workspace"));
+    w = ws.p;
+  }
+  static const uint8_t pos_bytes[8] = {4, 5, 6, 7, 0, 1, 2, 3};  // low word first: the entry's bytes, least significant first
+  int in_b = 0;
+  CKR(mhb_sort_records(st, (u32 *)e, sb, cnt, 2, pos_bytes, lists->sort_bytes, nullptr, w, ws_need, &in_b));
+  CK(cudaMemcpyAsync(lists->rounds.back().data(), in_b ? (const void *)sb : (const void *)e, cnt * 8,
+                     cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return MHB_OK;
+}
+
+// stable bucket partition, kmsort emulation and Lv2Postprocess of the n records in bufs.a; lists != nullptr: the
+// candidates go to a new round of lists instead of the planes of out
 int s1_sort_post(cudaStream_t st, const PkgView &pv, uint32_t k, int32_t m, bool need_mercy, const S1Out &out,
-                 unsigned long long *d_mul_hist, PhaseTrace &tr, const S1Bufs &bufs, uint64_t n) {
+                 unsigned long long *d_mul_hist, PhaseTrace &tr, const S1Bufs &bufs, uint64_t n, CandLists *lists) {
   const S1Layout l = s1_layout(k);
   const uint32_t NW = l.NW, RW = l.RW;
   DevBuf bstart, segs0, segs1, counter, bnd;
@@ -548,6 +674,7 @@ int s1_sort_post(cudaStream_t st, const PkgView &pv, uint32_t k, int32_t m, bool
   int level = 0;
   DevBuf todo, src16;
   u32 *d_todo = nullptr;
+  if (lists) CKR(src16.alloc((size_t)n * 2 + 64, "read2sdbg: kmsort source indices"));  // then the candidate bytes
   if (!km_global) {
     // level 0 on shared-memory tags: bucket sizes decide the tag capacity of a CTA
     std::vector<uint64_t> h_b(MHB_NUM_BUCKETS + 1);
@@ -560,7 +687,7 @@ int s1_sort_post(cudaStream_t st, const PkgView &pv, uint32_t k, int32_t m, bool
     if (const char *e = getenv("MHB_R2S_KM_CAP")) cap = std::max(1024u, (uint32_t)atoi(e) & ~1023u);  // tests: force the fall-back
     CKR(todo.alloc((n / 32 + 2) * 4, "read2sdbg: unsorted-range marks"));
     CK(cudaMemsetAsync(todo.p, 0, (n / 32 + 2) * 4, st));
-    CKR(src16.alloc((size_t)n * 2 + 64, "read2sdbg: kmsort source indices"));
+    CKR(src16.ensure((size_t)n * 2 + 64, "read2sdbg: kmsort source indices"));
     d_todo = todo.as<u32>();
     u32 *other = in_b ? a : b;
 #define M(WW)                                                                                                           \
@@ -624,13 +751,15 @@ int s1_sort_post(cudaStream_t st, const PkgView &pv, uint32_t k, int32_t m, bool
 #undef M
   CK_LAUNCH();
   tr.mark("s1.kmsort.finish");
+  uint8_t *const cand = lists ? src16.as<uint8_t>() : nullptr;  // the kmsort source indices are dead by now
 #define M(WW)                                                                                                          \
   if (RW == WW)                                                                                                        \
     k_r2s_s1_post<WW><<<grid_cap(n, 256, 32), 256, 0, st>>>(recs, l.narrow ? bufs.info : nullptr, n, NW, k, m, \
-                                                            pv, out, need_mercy ? 1 : 0, d_mul_hist);
+                                                            pv, out, need_mercy ? 1 : 0, d_mul_hist, cand);
   MHB_FOR_RW(M)
 #undef M
   CK_LAUNCH();
+  if (lists) CKR(cand_round(st, cand, n, recs, recs == a ? b : a, l, bufs, lists));
   tr.mark("s1.post");
   CK(cudaStreamSynchronize(st));
   return MHB_OK;
@@ -701,15 +830,28 @@ int result_bytes(const mhb_build_args *args, mhb_build_result *res) {
 // chunk-sized plane on the global word grid (d_mplane - w0) and are OR-ed into the solid plane over the chunk's words
 // right away: no read of another chunk looks at them, and a boundary word shared with the next chunk gets nothing
 // but this chunk's bits.  The chunk's solid bits are then final, so its stage-2 items are counted in the same pass.
+// List form (cl): the chunk's slice of every round's candidate list is scattered into the chunk-sized candidate planes
+// first (the same word grid), and the unchanged mercy kernel reads those.
+struct CandPlanes {  // the list form's chunk-sized candidate planes and staging slot
+  const CandLists *lists = nullptr;
+  u32 *planes = nullptr;  // 3 x plane_words
+  uint64_t plane_words = 0;
+  u64 *stage = nullptr;
+  uint64_t stage_cap = 0;
+};
 int mercy_count_pass(cudaStream_t st, const EachChunk &each, uint32_t k, int32_t m, bool mercy, const S1Out &so,
-                     u32 *d_mplane, unsigned long long *d_counter, PhaseTrace &tr, uint64_t *n_items, uint64_t *n_mercy) {
+                     u32 *d_mplane, unsigned long long *d_counter, PhaseTrace &tr, uint64_t *n_items, uint64_t *n_mercy,
+                     const CandPlanes &cl) {
   const uint32_t W = s2s_record_words(k);
   CK(cudaMemsetAsync(d_counter, 0, 8, st));
   if (int rc_ = each([&](const PkgChunk &c) -> int {
     if (mercy) {
       const uint64_t nw = c.w_end - c.w0;
+      S1Out o = so;
+      if (cl.lists)
+        CKR(cand_scatter(st, *cl.lists, c.pv.base0, c.base_end, c.w0, cl.planes, cl.plane_words, cl.stage, cl.stage_cap, &o));
       CK(cudaMemsetAsync(d_mplane, 0, nw * 4, st));
-      k_r2s_mercy<<<grid_cap(c.pv.n_reads, 256, 16), 256, 0, st>>>(c.pv, k, so, d_mplane - c.w0, d_counter + 1);
+      k_r2s_mercy<<<grid_cap(c.pv.n_reads, 256, 16), 256, 0, st>>>(c.pv, k, o, d_mplane - c.w0, d_counter + 1);
       CK_LAUNCH();
       k_r2s_or_words<<<grid_cap(nw, 256, 16), 256, 0, st>>>(so.is_solid + c.w0, d_mplane, nw);
       CK_LAUNCH();
@@ -867,6 +1009,7 @@ struct R2sShare::Impl {
   uint32_t k = 0;
   int32_t m = 0;
   bool mercy = false;  // need_mercy with a stage 1
+  bool sparse = false; // the candidates as lists (bind_planes)
   PkgIndex ix;         // the whole library
   PkgChunk c;          // the share, package words in pkg
   PkgView shape;       // the library's shape for the post-processing of stage 1
@@ -877,6 +1020,8 @@ struct R2sShare::Impl {
   DevBuf sort_b, sort_ws, pa, pb;        // the owner's sort buffer, workspace and narrow pairs, for the largest round
   S2Bufs s2b;
   SdbgStitch out;                        // the owner's stage-2 rounds
+  CandLists made, got;                   // list form: my stage-1 rounds' candidates, and those of my share
+  DevBuf cplanes, stage;                 // list form: the share's candidate planes and the staging slot of their scatter
   S1Out so;
   PhaseTrace tr;
   cudaStream_t st = 0;
@@ -967,19 +1112,6 @@ int R2sShare::load(const mhb_build_args *a, const ReadLibIndex &li, uint64_t fir
   c.pv.words = d.pkg.as<u32>();
   d.bit_words = ix.n_bases / 32 + 2;
   memset(&d.so, 0, sizeof(d.so));
-  if (d.m > 1) {  // m == 1: stage 2 takes every edge and never reads the solid plane
-    d.n_planes = d.mercy ? 4 : 1;
-    const size_t pb = (size_t)d.n_planes * d.bit_words * 4;
-    CKR(d.planes.alloc(pb, "read2sdbg: bit planes of the whole library"));
-    CK(cudaMemsetAsync(d.planes.p, 0, pb, st));
-    d.so.is_solid = d.planes.as<u32>();
-    if (d.mercy) {
-      d.so.no_in = d.so.is_solid + d.bit_words;
-      d.so.no_out = d.so.no_in + d.bit_words;
-      d.so.any = d.so.no_out + d.bit_words;
-      CKR(d.mplane.alloc((c.w_end - c.w0) * 4, "read2sdbg: mercy plane of the share"));
-    }
-  }
   CKR(d.hist.alloc(65536 * 8, "read2sdbg: multiplicity histogram"));
   CK(cudaMemsetAsync(d.hist.p, 0, 65536 * 8, st));
   CKR(d.cnt.alloc(64, "read2sdbg: counters"));
@@ -988,6 +1120,50 @@ int R2sShare::load(const mhb_build_args *a, const ReadLibIndex &li, uint64_t fir
   CKR(d.totals.alloc(16 * 8, "read2sdbg: totals"));
   CK(cudaStreamSynchronize(st));
   return MHB_OK;
+}
+
+bool R2sShare::want_cand_lists(size_t avail) const {
+  const Impl &d = *d_;
+  return d.mercy && (g_r2s_sparse_mercy || 4 * pad256(d.bit_words * 4) > avail);
+}
+
+int R2sShare::bind_planes(bool lists) {
+  Impl &d = *d_;
+  const PkgChunk &c = d.c;
+  const cudaStream_t st = d.st;
+  d.sparse = lists && d.mercy;
+  if (d.m > 1) {  // m == 1: stage 2 takes every edge and never reads the solid plane
+    d.n_planes = d.mercy && !d.sparse ? 4 : 1;
+    const size_t pb = (size_t)d.n_planes * d.bit_words * 4;
+    CKR(d.planes.alloc(pb, d.sparse ? "read2sdbg: solid plane of the whole library" : "read2sdbg: bit planes of the whole library"));
+    CK(cudaMemsetAsync(d.planes.p, 0, pb, st));
+    d.so.is_solid = d.planes.as<u32>();
+    if (d.mercy && !d.sparse) {
+      d.so.no_in = d.so.is_solid + d.bit_words;
+      d.so.no_out = d.so.no_in + d.bit_words;
+      d.so.any = d.so.no_out + d.bit_words;
+    }
+    if (d.mercy) CKR(d.mplane.alloc((c.w_end - c.w0) * 4, "read2sdbg: mercy plane of the share"));
+    if (d.sparse) {
+      CKR(d.cplanes.alloc(3 * (c.w_end - c.w0) * 4, "read2sdbg: mercy candidate planes of the share"));
+      CKR(d.stage.alloc(kCandStage * 8, "read2sdbg: mercy candidate staging slot"));
+      d.made.init(d.ix.n_bases);
+    }
+  }
+  CK(cudaStreamSynchronize(st));
+  return MHB_OK;
+}
+
+bool R2sShare::cand_lists() const { return d_->sparse; }
+uint64_t R2sShare::base_of(uint64_t read) const {
+  const PkgIndex &ix = d_->ix;
+  return ix.fixed_len ? read * ix.fixed_len : ix.base_off[read];
+}
+const std::vector<std::vector<uint64_t>> &R2sShare::cand_made() const { return d_->made.rounds; }
+void R2sShare::cand_take(std::vector<std::vector<uint64_t>> *lists) {
+  Impl &d = *d_;
+  std::vector<std::vector<uint64_t>>().swap(d.made.rounds);
+  d.got.rounds.swap(*lists);
 }
 
 int R2sShare::s1_hist(uint64_t *hist) {
@@ -1064,7 +1240,8 @@ int R2sShare::s1_own(uint32_t *recs, uint64_t *info, uint64_t n, uint64_t n_max)
     CKR(d.pb.ensure((size_t)n_max * 8 + 16, "read2sdbg: bucket partition pairs (sort buffer)"));
   }
   const S1Bufs bufs{recs, d.sort_b.as<u32>(), d.sort_ws.p, l.narrow ? info : nullptr, d.pa.as<u32>(), d.pb.as<u32>()};
-  return s1_sort_post(d.st, d.shape, d.k, d.m, d.mercy, d.so, d.hist.as<unsigned long long>(), d.tr, bufs, n);
+  return s1_sort_post(d.st, d.shape, d.k, d.m, d.mercy, d.so, d.hist.as<unsigned long long>(), d.tr, bufs, n,
+                      d.sparse ? &d.made : nullptr);
 }
 
 void R2sShare::s1_end() {
@@ -1091,8 +1268,21 @@ int R2sShare::mercy_count(uint64_t *n_items, uint64_t *n_mercy) {
   *n_items = *n_mercy = 0;
   if (!d.c.pv.n_reads) return MHB_OK;
   const EachChunk each = [&](const ChunkFn &fn) { return fn(d.c); };
-  return mercy_count_pass(d.st, each, d.k, d.m, d.mercy, d.so, d.mplane.as<u32>(), d.cnt.as<unsigned long long>(), d.tr,
-                          n_items, n_mercy);
+  CandPlanes cp;
+  if (d.sparse) {
+    cp.lists = &d.got;
+    cp.planes = d.cplanes.as<u32>();
+    cp.plane_words = d.c.w_end - d.c.w0;
+    cp.stage = d.stage.as<u64>();
+    cp.stage_cap = kCandStage;
+  }
+  CKR(mercy_count_pass(d.st, each, d.k, d.m, d.mercy, d.so, d.mplane.as<u32>(), d.cnt.as<unsigned long long>(), d.tr,
+                       n_items, n_mercy, cp));
+  if (d.sparse) {
+    for (DevBuf *b : {&d.cplanes, &d.stage}) b->release();
+    std::vector<std::vector<uint64_t>>().swap(d.got.rounds);
+  }
+  return MHB_OK;
 }
 
 int R2sShare::s2_hist(uint64_t *hist) {
@@ -1222,17 +1412,20 @@ extern "C" int mhb_read2sdbg_host(const mhb_build_args *args, mhb_build_result *
   PkgSource src;
   CKR(src.plan(args, ix, k, stream, read_chunk_limit() ? read_chunk_limit() : read_chunk_auto_bytes()));
   const char *held = stream ? "the bit planes and read chunk buffers leave" : "the resident read library leaves";
-  if (stream) {  // resident: the solid plane, the mercy planes (the fourth one chunk-sized) and the chunk buffers
-    const size_t solid_b = m > 1 ? pad256(bit_words * 4) : 0,
-                 mercy_b = mercy ? 3 * pad256(bit_words * 4) + pad256(src.max_plane_words * 4) : 0;
-    const size_t need = solid_b + mercy_b + src.streamed_bytes() + pad256(65536 * 8) + pad256(64) +
-                        pad256((size_t)MHB_NUM_BUCKETS * 32) + pad256(128);
+  MercyForm form;
+  if (stream) {  // resident: the solid plane, the mercy candidates (planes or lists), a chunk's mercy plane, the chunk buffers
+    form = mercy_form(bit_words, src.max_plane_words, src.streamed_bytes(), m, mercy, free_device_bytes(), g_r2s_sparse_mercy);
+    const size_t need = form.sparse ? form.lists : form.planes;
     if (need > free_device_bytes())
       return mhb_set_error(MHB_ERR_NOMEM,
-                           "read2sdbg: the streamed read library needs %zu bytes of device memory (solid plane %zu, "
-                           "mercy planes %zu, read chunk buffers %zu), %zu are free",
-                           need, solid_b, mercy_b, src.streamed_bytes(), free_device_bytes());
+                           "read2sdbg: the streamed read library needs %zu bytes of device memory (mercy candidates as "
+                           "%s, read chunk buffers %zu), %zu are free",
+                           need, form.sparse ? "lists" : "planes", src.streamed_bytes(), free_device_bytes());
   }
+  g_mercy_stats = MercyStats();
+  g_mercy_stats.sparse = form.sparse ? 1 : 0;
+  CandLists lists;
+  lists.init(ix.n_bases);
   CKR(src.bind(st, ix));
   tr.mark("h2d.upload+reverse");
   const EachChunk each = [&](const ChunkFn &fn) { return src.each(st, fn); };
@@ -1259,15 +1452,26 @@ extern "C" int mhb_read2sdbg_host(const mhb_build_args *args, mhb_build_result *
   BigBufs big;
   S1Out so;
   memset(&so, 0, sizeof(so));
+  CandPlanes cp;
+  DevBuf d_cplanes, d_stage;
   so.is_solid = d_solid.as<u32>();
   if (s1_runs) {
-    if (mercy) {
+    if (mercy && !form.sparse) {
       CKR(d_planes.alloc(bit_words * 4 * 3, "read2sdbg: mercy candidate planes"));
       CK(cudaMemsetAsync(d_planes.p, 0, bit_words * 4 * 3, st));
       so.no_in = d_planes.as<u32>();
       so.no_out = so.no_in + bit_words;
       so.any = so.no_out + bit_words;
-      CKR(d_mplane.alloc(src.max_plane_words * 4, "read2sdbg: mercy plane of a chunk"));
+    }
+    if (mercy) CKR(d_mplane.alloc(src.max_plane_words * 4, "read2sdbg: mercy plane of a chunk"));
+    if (mercy && form.sparse) {  // the list form: chunk-sized candidate planes and the staging slot of their scatter
+      cp.lists = &lists;
+      cp.plane_words = src.max_plane_words;
+      cp.stage_cap = kCandStage;
+      CKR(d_cplanes.alloc(3 * cp.plane_words * 4, "read2sdbg: mercy candidate planes of a chunk"));
+      CKR(d_stage.alloc(cp.stage_cap * 8, "read2sdbg: mercy candidate staging slot"));
+      cp.planes = d_cplanes.as<u32>();
+      cp.stage = d_stage.as<u64>();
     }
     // one pass when the records fit (and no cap is set), else rounds over bucket ranges
     const size_t avail = (size_t)(0.92 * (double)free_device_bytes());
@@ -1286,19 +1490,26 @@ extern "C" int mhb_read2sdbg_host(const mhb_build_args *args, mhb_build_result *
       }
     }
     CKR(run_stage1(st, each, shape, ix, src.max_reads, k, m, mercy, so, d_hist.as<unsigned long long>(), tr, big, max_n,
-                   min_rec, min_ws, &res->n_rounds_s1));
+                   min_rec, min_ws, &res->n_rounds_s1, form.sparse ? &lists : nullptr));
   }
 
   // ---- the mercy step and the stage-2 item count, then stage 2 ----
   const bool mercy_runs = s1_runs && mercy;
   uint64_t n_items = 0;
+  if (cp.lists) {
+    g_mercy_stats.n_entries = lists.n_entries();
+    g_mercy_stats.host_bytes = g_mercy_stats.n_entries * 8;
+  }
   if (mercy_runs || ix.n_edges)
-    CKR(mercy_count_pass(st, each, k, m, mercy_runs, so, d_mplane.as<u32>(), d_counter, tr, &n_items, &res->n_mercy));
+    CKR(mercy_count_pass(st, each, k, m, mercy_runs, so, d_mplane.as<u32>(), d_counter, tr, &n_items, &res->n_mercy, cp));
   if (s1_runs) {
     CK(cudaMemcpyAsync(res->counting, d_hist.p, 65536 * 8, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     d_planes.release();
     d_mplane.release();
+    d_cplanes.release();
+    d_stage.release();
+    std::vector<std::vector<uint64_t>>().swap(lists.rounds);
   }
   res->n_sort_items = n_items;
   if (n_items) {
@@ -1620,5 +1831,112 @@ extern "C" int mhb_selftest_r2s_s1_plan(uint32_t k, uint64_t n_s1, uint64_t max_
   *rec_words_out = l.RW;
   if (s1_plan_round(l, n_s1, max_reads, (size_t)avail, limit, max_n_out))
     return mhb_set_error(MHB_ERR_NOMEM, "read2sdbg: no room for a stage-1 round");
+  return MHB_OK;
+}
+
+extern "C" int mhb_set_r2s_sparse_mercy(int mode) {
+  if (mode < 0 || mode > 1) return mhb_set_error(MHB_ERR_ARG, "mhb_set_r2s_sparse_mercy: 0 = automatic, 1 = lists");
+  g_r2s_sparse_mercy = mode;
+  return MHB_OK;
+}
+
+extern "C" int mhb_r2s_mercy_stats(int *sparse, uint64_t *n_entries, uint64_t *host_bytes) {
+  if (sparse) *sparse = g_mercy_stats.sparse;
+  if (n_entries) *n_entries = g_mercy_stats.n_entries;
+  if (host_bytes) *host_bytes = g_mercy_stats.host_bytes;
+  return MHB_OK;
+}
+
+// The form of the mercy candidates mhb_read2sdbg_host takes for a streamed library (mercy_form)
+extern "C" int mhb_selftest_r2s_mercy_form(uint64_t n_bases, uint64_t max_plane_words, uint64_t streamed_bytes, int32_t m,
+                                           int need_mercy, uint64_t free_bytes, int force, uint64_t *planes_out,
+                                           uint64_t *lists_out, int *sparse_out) {
+  const MercyForm f = mercy_form(n_bases / 32 + 2, max_plane_words, (size_t)streamed_bytes, m, need_mercy && m > 1,
+                                 (size_t)free_bytes, force);
+  *planes_out = f.planes;
+  *lists_out = f.lists;
+  *sparse_out = f.sparse ? 1 : 0;
+  return MHB_OK;
+}
+
+// Stage-1 Lv2Postprocess of one sorted bucket (wide layout) in the list form: the candidate bytes of the group walk,
+// then every record's entries in record order (k_r2s_cand_write); *n_out = entries written (room for 2 n)
+extern "C" int mhb_selftest_r2s_s1_cand(const uint32_t *recs, uint64_t n, uint32_t k, int32_t m, uint32_t fixed_len,
+                                        uint64_t n_reads, uint32_t *is_solid, int64_t *counting, uint64_t *entries_out,
+                                        uint64_t *n_out) {
+  const uint32_t nw = r2s_s1_key_words(k), rw = nw + 2;
+  PkgView pv;
+  memset(&pv, 0, sizeof(pv));
+  pv.fixed_len = fixed_len;
+  pv.n_reads = n_reads;
+  S1Out o{is_solid, nullptr, nullptr, nullptr};
+  std::vector<uint8_t> cand(n, 0xFF);
+  for (u64 g = 0; g < n;) {
+    u32 hv[16], nh;
+    g = s1_group(recs, nullptr, n, g, rw, nw, k, m, pv, o, true, hv, nh, cand.data());
+    for (u32 q = 0; q < nh; ++q) counting[hv[q] > MHB_MAX_MUL ? MHB_MAX_MUL : hv[q]]++;
+  }
+  uint64_t at = 0;
+  for (u64 i = 0; i < n; ++i) {
+    if (cand[i] == 0xFF) return mhb_set_error(MHB_ERR_CUDA, "record %llu got no candidate byte", (unsigned long long)i);
+    at += cand_entries(cand[i], s1_info(recs + i * rw, nw, nullptr), entries_out + at);
+  }
+  *n_out = at;
+  return MHB_OK;
+}
+
+// The mercy step over a library in chunks, as mercy_count_pass runs it.  Library: fixed_len, or the n_reads lengths
+// len[] (a zero-length read as one base), its first base at global base0.  is_solid and mercy: bit planes on the word
+// grid from word base0 / 32.  List form (entries != nullptr): n_rounds lists back to back, round t ends at
+// round_end[t], each sorted; per chunk [chunk_first[i], chunk_first[i + 1]) the slice of every list in its base range is
+// scattered into chunk-sized candidate planes, and the reads of the chunk run r2s_mercy_read on them.  Plane form
+// (entries == nullptr): planes holds no_in, no_out, any, each n_plane_words words on the same grid as is_solid.
+extern "C" int mhb_selftest_r2s_mercy_lists(uint32_t fixed_len, uint64_t n_reads, const uint32_t *len, uint64_t base0,
+                                            uint32_t k, const uint32_t *is_solid, const uint64_t *entries,
+                                            const uint64_t *round_end, uint32_t n_rounds, const uint64_t *chunk_first,
+                                            uint32_t n_chunks, const uint32_t *planes, uint64_t n_plane_words,
+                                            uint32_t *mercy, uint64_t *added_out) {
+  PkgView pv;
+  memset(&pv, 0, sizeof(pv));
+  pv.fixed_len = fixed_len;
+  pv.n_reads = n_reads;
+  pv.base0 = base0;
+  std::vector<uint64_t> base_off(n_reads + 1, 0);
+  if (!fixed_len) {
+    for (uint64_t r = 0; r < n_reads; ++r) base_off[r + 1] = base_off[r] + std::max<uint32_t>(len[r], 1);
+    pv.len = len;
+    pv.base_off = base_off.data();
+  }
+  const uint64_t g0 = base0 / 32;  // the callers' planes start at this word
+  S1Out o{const_cast<u32 *>(is_solid) - g0, nullptr, nullptr, nullptr};
+  u32 *const mer = mercy - g0;
+  *added_out = 0;
+  if (!entries) {
+    o.no_in = const_cast<u32 *>(planes) - g0;
+    o.no_out = o.no_in + n_plane_words;
+    o.any = o.no_out + n_plane_words;
+    for (uint64_t r = 0; r < n_reads; ++r) *added_out += r2s_mercy_read(pv, r, k, o, mer);
+    return MHB_OK;
+  }
+  CandLists lists;
+  for (uint32_t t = 0; t < n_rounds; ++t)
+    lists.rounds.emplace_back(entries + (t ? round_end[t - 1] : 0), entries + round_end[t]);
+  for (uint32_t i = 0; i < n_chunks; ++i) {
+    const uint64_t f = chunk_first[i], e = chunk_first[i + 1];
+    if (f > e || e > n_reads) return mhb_set_error(MHB_ERR_ARG, "bad chunk bounds");
+    if (f == e) continue;
+    const uint64_t b0 = pv.base(f), b1 = pv.base(e);  // base_off has n_reads + 1 entries
+    const uint64_t w0 = b0 / 32, nw = b1 / 32 + 2 - w0;
+    std::vector<u32> cp(3 * nw, 0);
+    S1Out c = o;
+    c.no_in = cp.data() - w0;
+    c.no_out = cp.data() + nw - w0;
+    c.any = cp.data() + 2 * nw - w0;
+    CKR(lists.each_slice(b0, b1, [&](const uint64_t *s, uint64_t n) -> int {
+      for (uint64_t q = 0; q < n; ++q) cand_mark(c, s[q]);
+      return MHB_OK;
+    }));
+    for (uint64_t r = f; r < e; ++r) *added_out += r2s_mercy_read(pv, r, k, c, mer);
+  }
   return MHB_OK;
 }

@@ -378,10 +378,33 @@ MHB_HD u64 s1_info(const u32 *r, u32 nw, const u64 *info) {
   return info ? info[r[nw]] : ((u64)r[nw] << 32) | r[nw + 1];
 }
 
+// ---- the list form of the mercy candidates (DESIGN.md §4.9): one u64 entry per marked position, position << 2 | code
+// (code 0 = any, 1 = no in, 2 = no out; 1 and 2 imply any), as Read2SdbgS1 writes P.mercy_cand.* ----
+// Per stage-1 record the group walk leaves one candidate byte: (left code + 1) | (right code + 1) << 2, 0 = none.
+MHB_HD u32 cand_count(u32 c) { return ((c & 3u) ? 1u : 0u) + ((c >> 2) ? 1u : 0u); }
+// the entries of a record with candidate byte c and read_info `info` (full_offset << 6 | prev << 3 | next), left first
+MHB_HD u32 cand_entries(u32 c, u64 info, u64 *out) {
+  const u64 full = info >> 6, pos = full >> 1;
+  const bool fwd = (full & 1) == 0;
+  u32 n = 0;
+  if (c & 3u) out[n++] = (fwd ? pos - 1 : pos) << 2 | ((c & 3u) - 1);
+  if (c >> 2) out[n++] = (fwd ? pos : pos - 1) << 2 | ((c >> 2) - 1);
+  return n;
+}
+// one entry into the three candidate planes (indexed by global base; the caller shifts them to its word grid)
+MHB_HD void cand_mark(const S1Out &o, u64 e) {
+  const u64 pos = e >> 2;
+  const u32 code = (u32)(e & 3);
+  bit_or(o.any, pos);
+  if (code == 1) bit_or(o.no_in, pos);
+  if (code == 2) bit_or(o.no_out, pos);
+}
+
 // walks the group [g0, end) twice: tallies, then per-record outputs.  Returns the group's end.  hist_vals[0..n_hist)
 // (room for 16) receives the occurrence count of every distinct (k+1)-mer of the group (edge_counter_.Add, :430-432).
+// With need_mercy the candidates go to the planes of o, or - cand != nullptr, the list form - to cand[record].
 MHB_HD u64 s1_group(const u32 *recs, const u64 *info, u64 n, u64 g0, u32 rw, u32 nw, u32 k, int m, const PkgView &pv,
-                    const S1Out &o, bool need_mercy, u32 *hist_vals, u32 &n_hist) {
+                    const S1Out &o, bool need_mercy, u32 *hist_vals, u32 &n_hist, uint8_t *cand = nullptr) {
   n_hist = 0;
   const u32 *first = recs + g0 * rw;
   u32 cht[40];  // count_head_tail, index head<<3|tail <= 36
@@ -445,6 +468,10 @@ MHB_HD u64 s1_group(const u32 *recs, const u64 *info, u64 n, u64 g0, u32 rw, u32
         else if ((has_out >> tail) & 1u)
           rc = 1 + (int)strand;
       }
+    }
+    if (cand) {
+      cand[q] = (uint8_t)((lc + 1) | (rc + 1) << 2);
+      continue;
     }
     if (lc >= 0) {
       bit_or(o.any, l_off);
@@ -969,7 +996,7 @@ static constexpr int kS1HistSmem = 2048;
 template <int RW>
 __global__ void __launch_bounds__(256) k_r2s_s1_post(const u32 *__restrict__ recs, const u64 *__restrict__ info, u64 n, u32 nw,
                                                     u32 k, int m, PkgView pv, S1Out o, int need_mercy,
-                                                    unsigned long long *__restrict__ mul_hist) {
+                                                    unsigned long long *__restrict__ mul_hist, uint8_t *__restrict__ cand) {
   __shared__ u32 s_hist[kS1HistSmem];
   for (int i = threadIdx.x; i < kS1HistSmem; i += 256) s_hist[i] = 0;
   __syncthreads();
@@ -977,7 +1004,7 @@ __global__ void __launch_bounds__(256) k_r2s_s1_post(const u32 *__restrict__ rec
     const bool head = i == 0 || s1_diff_km1(recs + (i - 1) * RW, recs + i * RW, k);
     if (head) {
       u32 hv[16], nh;
-      s1_group(recs, info, n, i, RW, nw, k, m, pv, o, need_mercy != 0, hv, nh);
+      s1_group(recs, info, n, i, RW, nw, k, m, pv, o, need_mercy != 0, hv, nh, cand);
       for (u32 q = 0; q < nh; ++q) {
         const u32 c = hv[q];
         if (c < (u32)kS1HistSmem) atomicAdd(&s_hist[c], 1u);
@@ -1001,6 +1028,59 @@ __global__ void __launch_bounds__(256) k_r2s_mercy(PkgView pv, u32 k, S1Out o, u
 
 __global__ void __launch_bounds__(256) k_r2s_or_words(u32 *__restrict__ dst, const u32 *__restrict__ src, u64 n_words) {
   for (u64 t = (u64)blockIdx.x * 256 + threadIdx.x; t < n_words; t += (u64)gridDim.x * 256) dst[t] |= src[t];
+}
+
+// ---- the list form of the candidates: count -> scan32 -> write over the candidate bytes of a stage-1 round, tiles of
+// kCandTile records (kCandPer consecutive records per thread), entries in record order ----
+static constexpr int kCandPer = 4, kCandTile = 256 * kCandPer;
+__global__ void __launch_bounds__(256) k_r2s_cand_count(const uint8_t *__restrict__ cand, u64 n, u32 *__restrict__ tile_n) {
+  __shared__ u32 s_w[8];
+  const u64 i0 = (u64)blockIdx.x * kCandTile + (u64)threadIdx.x * kCandPer;
+  u32 c = 0;
+  for (int j = 0; j < kCandPer; ++j)
+    if (i0 + j < n) c += cand_count(cand[i0 + j]);
+  for (int d = 16; d; d >>= 1) c += __shfl_xor_sync(0xffffffffu, c, d);
+  if (lane_id() == 0) s_w[threadIdx.x >> 5] = c;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    u32 t = 0;
+    for (int w = 0; w < 8; ++w) t += s_w[w];
+    tile_n[blockIdx.x] = t;
+  }
+}
+
+// recs: the round's records (rw words, read_info as s1_info reads it); tile_off: the scan of k_r2s_cand_count's tiles
+__global__ void __launch_bounds__(256) k_r2s_cand_write(const uint8_t *__restrict__ cand, u64 n, const u32 *__restrict__ recs,
+                                                        const u64 *__restrict__ info, u32 rw, u32 nw,
+                                                        const u64 *__restrict__ tile_off, u64 *__restrict__ out) {
+  __shared__ u32 s_w[8];
+  const u64 i0 = (u64)blockIdx.x * kCandTile + (u64)threadIdx.x * kCandPer;
+  u32 c = 0;
+  for (int j = 0; j < kCandPer; ++j)
+    if (i0 + j < n) c += cand_count(cand[i0 + j]);
+  // exclusive prefix of c over the block: inclusive warp scan, then the sums of the warps before
+  const u32 lane = lane_id(), warp = threadIdx.x >> 5;
+  u32 inc = c;
+  for (int d = 1; d < 32; d <<= 1) {
+    const u32 v = __shfl_up_sync(0xffffffffu, inc, d);
+    if (lane >= (u32)d) inc += v;
+  }
+  if (lane == 31) s_w[warp] = inc;
+  __syncthreads();
+  u64 at = tile_off[blockIdx.x] + inc - c;
+  for (u32 w = 0; w < warp; ++w) at += s_w[w];
+  for (int j = 0; j < kCandPer; ++j) {
+    const u64 i = i0 + j;
+    if (i >= n || !cand[i]) continue;
+    u64 e[2];
+    const u32 ne = cand_entries(cand[i], s1_info(recs + i * rw, nw, info), e);
+    for (u32 q = 0; q < ne; ++q) out[at++] = e[q];
+  }
+}
+
+// the n entries e[] into the candidate planes of o (each on the caller's word grid, indexed by global base)
+__global__ void __launch_bounds__(256) k_r2s_cand_scatter(const u64 *__restrict__ e, u64 n, S1Out o) {
+  for (u64 t = (u64)blockIdx.x * 256 + threadIdx.x; t < n; t += (u64)gridDim.x * 256) cand_mark(o, e[t]);
 }
 
 // stage-2 items of edge position t (global index over all reads): which $-variants exist (read_to_sdbg_s2.cpp:389-431)

@@ -149,6 +149,8 @@ SYMBOLS = [
     "mhb_iterate_host", "mhb_iterate_run", "mhb_iterate_run_multi", "mhb_plan_read_shares", "mhb_selftest_iterate", "mhb_s2s_extract_edges_pruned", "mhb_s2s_emit_fmt", "mhb_read2sdbg_host", "mhb_read2sdbg_run", "mhb_read2sdbg_run_multi", "mhb_plan_r2s_owners", "mhb_selftest_r2s_s1_record", "mhb_selftest_r2s_item",
     "mhb_selftest_kmsort", "mhb_selftest_kmsort_smem", "mhb_selftest_r2s_s1_group", "mhb_selftest_r2s_mercy_read",
     "mhb_selftest_r2s_chunk_index", "mhb_selftest_r2s_stream_decide",
+    "mhb_set_r2s_sparse_mercy", "mhb_r2s_mercy_stats", "mhb_selftest_r2s_mercy_form", "mhb_selftest_r2s_s1_cand",
+    "mhb_selftest_r2s_mercy_lists",
     "mhb_selftest_kmsort_narrow", "mhb_selftest_r2s_s1_plan", "mhb_selftest_read2sdbg_narrow", "mhb_selftest_iterate_narrow",
     "mhb_buildlib_host", "mhb_buildlib_free", "mhb_set_buildlib_chunk", "mhb_buildlib_run", "mhb_selftest_fastx",
     "mhb_s2s_sort", "mhb_s2s_sort_workspace_bytes", "mhb_s2s_sort_hist_byte", "mhb_s2s_sort_stats",
@@ -395,6 +397,81 @@ def set_r2s_round_limit(s1: int = 0, s2: int = 0):
     L = load()
     L.mhb_set_r2s_round_limit.argtypes = [C.c_uint64, C.c_uint64]
     _check(L.mhb_set_r2s_round_limit(int(s1), int(s2)))
+
+
+def set_r2s_sparse_mercy(mode: int = 0):
+    """read2sdbg's mercy candidates: 0 = automatic (planes of the whole library unless they do not fit), 1 = sorted
+    position lists whenever the library is streamed and on every rank of read2sdbg_run(gpus=N), whose forked workers
+    inherit the setting.  The result does not depend on it."""
+    L = load()
+    L.mhb_set_r2s_sparse_mercy.argtypes = [C.c_int]
+    _check(L.mhb_set_r2s_sparse_mercy(int(mode)))
+
+
+def r2s_mercy_stats() -> dict:
+    """The mercy candidates of the last read2sdbg_host call: sparse (lists rather than planes), list entries over every
+    stage-1 round, and the host bytes they took."""
+    L = load()
+    sp, n, b = C.c_int(), C.c_uint64(), C.c_uint64()
+    L.mhb_r2s_mercy_stats.argtypes = [C.POINTER(C.c_int), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
+    _check(L.mhb_r2s_mercy_stats(C.byref(sp), C.byref(n), C.byref(b)))
+    return {"sparse": bool(sp.value), "n_entries": n.value, "host_bytes": b.value}
+
+
+def r2s_mercy_form(n_bases: int, max_plane_words: int, streamed_bytes: int, m: int, need_mercy: bool, free_bytes: int,
+                   force: int = 0) -> dict:
+    """The form of read2sdbg's mercy candidates on a streamed library (host code): the device bytes of the streamed
+    form with candidate planes and with candidate lists, and whether the lists are taken."""
+    L = load()
+    pl, li, sp = C.c_uint64(), C.c_uint64(), C.c_int()
+    L.mhb_selftest_r2s_mercy_form.argtypes = [C.c_uint64, C.c_uint64, C.c_uint64, C.c_int32, C.c_int, C.c_uint64, C.c_int,
+                                              C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_int)]
+    _check(L.mhb_selftest_r2s_mercy_form(n_bases, max_plane_words, streamed_bytes, m, int(need_mercy), free_bytes,
+                                         int(force), C.byref(pl), C.byref(li), C.byref(sp)))
+    return {"planes": pl.value, "lists": li.value, "sparse": bool(sp.value)}
+
+
+def selftest_r2s_s1_cand(recs: np.ndarray, k: int, m: int, fixed_len: int, n_reads: int, is_solid: np.ndarray,
+                         counting: np.ndarray) -> np.ndarray:
+    """Stage-1 Lv2Postprocess of one sorted bucket in the list form (host code): the candidate entries
+    (position << 2 | code) in record order; is_solid and counting are updated in place."""
+    L = load()
+    recs = np.ascontiguousarray(recs, np.uint32)
+    out = np.zeros(2 * len(recs) + 1, np.uint64)
+    n = C.c_uint64()
+    L.mhb_selftest_r2s_s1_cand.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_int32, C.c_uint32, C.c_uint64,
+                                           C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
+    _check(L.mhb_selftest_r2s_s1_cand(recs.ctypes.data, len(recs), k, m, fixed_len, n_reads, is_solid.ctypes.data,
+                                      counting.ctypes.data, out.ctypes.data, C.byref(n)))
+    return out[:n.value].copy()
+
+
+def selftest_r2s_mercy_lists(k: int, is_solid: np.ndarray, n_reads: int, fixed_len: int = 0, lens=None, base0: int = 0,
+                             rounds=None, chunk_first=None, planes=None) -> tuple[np.ndarray, int]:
+    """The mercy step (host code) over a library whose first base is base0, with is_solid on the word grid from
+    base0 // 32: from the candidate lists `rounds` (each sorted) in the chunks chunk_first, or from the candidate
+    planes (3, words) on that grid.  Returns (the added bits on the grid, their number)."""
+    L = load()
+    is_solid = np.ascontiguousarray(is_solid, np.uint32)
+    mercy = np.zeros_like(is_solid)
+    lens_a = np.ascontiguousarray(lens if lens is not None else [0], np.uint32)
+    added = C.c_uint64()
+    L.mhb_selftest_r2s_mercy_lists.argtypes = [C.c_uint32, C.c_uint64, C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p,
+                                               C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p,
+                                               C.c_uint64, C.c_void_p, C.POINTER(C.c_uint64)]
+    if planes is not None:
+        planes = np.ascontiguousarray(planes, np.uint32)
+        _check(L.mhb_selftest_r2s_mercy_lists(fixed_len, n_reads, lens_a.ctypes.data, base0, k, is_solid.ctypes.data,
+                                              None, None, 0, None, 0, planes.ctypes.data, planes.shape[1],
+                                              mercy.ctypes.data, C.byref(added)))
+        return mercy, added.value
+    ent = np.ascontiguousarray(np.concatenate([np.asarray(r, np.uint64) for r in rounds] + [np.zeros(1, np.uint64)]))
+    ends = np.cumsum([len(r) for r in rounds]).astype(np.uint64)
+    cf = np.ascontiguousarray(chunk_first, np.uint64)
+    _check(L.mhb_selftest_r2s_mercy_lists(fixed_len, n_reads, lens_a.ctypes.data, base0, k, is_solid.ctypes.data,
+                                          ent.ctypes.data, ends.ctypes.data, len(rounds), cf.ctypes.data, len(cf) - 1,
+                                          None, 0, mercy.ctypes.data, C.byref(added)))
+    return mercy, added.value
 
 
 def plan_read_chunks(bin_words: np.ndarray, n_reads: int, max_chunk_bytes: int) -> list[int]:
