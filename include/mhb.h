@@ -772,8 +772,10 @@ int mhb_buildlib_run(const char *lib_file, const char *out_prefix);
  * searched prefixes, and - because the solid edges are already on the devices - the k_min SdBG is built in the same
  * run: every rank's pruned edge items (mhb_s2s_edges_owners) go straight into their owners' buffers, in rounds over
  * ascending bucket sub-ranges when an owner's items do not fit its device at once (or exceed mhb_set_s2s_round_limit),
- * and each owner sorts and emits every round into P.sdbg.<r> in bucket order.  What stays resident on every rank
- * through the SdBG stage: its solid and mercy edges (its share of the reads is released after the mercy search).
+ * and each owner sorts and emits every round into P.sdbg.<r> in bucket order.  A rank's share of the reads stays on
+ * its device when it fits next to the smallest round (mhb_read_stream_decide), and is streamed from host memory in
+ * chunks otherwise or under mhb_set_read_chunk_limit; it is released after the mercy marks.  What stays resident on
+ * every rank through the SdBG stage: its solid and mercy edges.
  * Rank 0 logs both plans ("count plan: R rounds ...", "SdBG plan: R rounds ...") and the SdBG loads.  Files: rank r
  * writes P.edges.<r> and P.sdbg.<r>, rank 0 the merged P.edges.info (num_files = n_gpus, edge_io_meta.h:25-44), P.sdbg_info
  * (sdbg_meta.cpp:44-61), P.cand, P.counting, and the marker P.sdbg_fused ("k need_mercy n_gpus") that lets a following
@@ -806,9 +808,10 @@ int mhb_plan_count_owner_rounds(const uint64_t *hist16, uint32_t n_ranks, uint64
  * other in P.sdbg.<r>, so the canonical stream and the files are those of one round.  Rank 0 writes the merged
  * P.sdbg_info (num_files = n_gpus, sdbg_meta.cpp:44-61) and logs the plan ("SdBG plan: R rounds over bucket ranges")
  * and the loads ("SdBG items: largest owner ..., largest leading byte ..., largest bucket ...").  A single bucket
- * larger than one round is MHB_ERR_NOMEM, naming the bucket and the rank, before any receive buffer exists.  What stays
- * resident on every rank: its share of the sequences; a share that does not fit returns MHB_ERR_NOMEM.  The caller
- * must not have initialised CUDA in this process. */
+ * larger than one round is MHB_ERR_NOMEM, naming the bucket and the rank, before any receive buffer exists.  A rank's
+ * share of the sequences stays on its device when it fits next to the smallest round (mhb_read_stream_decide), and is
+ * streamed from host memory in chunks otherwise or under mhb_set_s2s_chunk_limit.  The caller must not have
+ * initialised CUDA in this process. */
 int mhb_seq2sdbg_run_multi(const mhb_seq2sdbg_opts *opts, int n_gpus);
 /* The shares of mhb_seq2sdbg_run_multi (host only): n_ranks contiguous runs [first[r], first[r+1]) of the n_seqs
  * sequences (lengths len), every cut at the sequence boundary whose item count (2 * (len - k + 2) per sequence of length

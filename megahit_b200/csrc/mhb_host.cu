@@ -884,6 +884,7 @@ extern "C" int mhb_set_s2s_chunk_limit(uint64_t bytes) {
   g_s2s_chunk_limit = bytes;
   return MHB_OK;
 }
+uint64_t s2s_chunk_limit() { return g_s2s_chunk_limit; }
 
 extern "C" int mhb_s2s_stream_stats(int mercy, uint64_t *n_chunks, uint64_t *n_passes, uint64_t *n_rounds, uint64_t *h2d_bytes) {
   const StreamStats &s = mercy ? g_mercy_st : g_s2s_st;

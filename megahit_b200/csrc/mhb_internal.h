@@ -346,6 +346,8 @@ void read_stream_stats_reset();
 uint64_t read_chunk_limit();
 // the chunk size of a library that is streamed because it does not fit (no cap set)
 uint64_t read_chunk_auto_bytes();
+// the sequence chunk cap of seq2sdbg: mhb_set_s2s_chunk_limit, or 0 (mhb_host.cu)
+uint64_t s2s_chunk_limit();
 
 // host container mirroring what SeqPackage holds for seq2sdbg: word-aligned package-orientation sequences (mhb_files.cpp)
 struct HostSeqs {

@@ -3,7 +3,8 @@
 //
 // One worker PROCESS per GPU (forked before CUDA is touched; libmhb keeps per-process state: arena, kernel attributes),
 // with no Python, torch or NCCL underneath.  The parent loads the input and deals it in contiguous shares (reads
-// balanced on bases, sequences on items); rank order is input order.
+// balanced on bases, sequences on items); rank order is input order.  The count and seq2sdbg workers read their shares
+// through a chunk stream: on the device when a share fits, otherwise streamed from the host copy they inherit.
 //
 // Every stage moves its records to their owners with one exchange (OwnerExchange):
 //   1. every rank all-gathers its 65536-bin bucket histogram (a stage that histograms leading bytes puts byte b in
@@ -52,6 +53,8 @@
 #include <unistd.h>
 
 #include <algorithm>
+#include <numeric>
+#include <optional>
 #include <string>
 #include <vector>
 
@@ -286,6 +289,28 @@ size_t rank_round_bytes(int rank, int world) {
   return (size_t)(0.92 * (double)free_device_bytes()) / (size_t)std::max(1, sharers);
 }
 
+// An XINFO line in one write: the lines of ranks that log at the same time stay whole
+#define RANK_INFO(...) rank_info(__LINE__, __VA_ARGS__)
+void rank_info(int line, const char *fmt, ...) {
+  char buf[1024];
+  int n = snprintf(buf, sizeof(buf), "INFO  %-30s: %4d - ", "megahit_b200", line);
+  va_list ap;
+  va_start(ap, fmt);
+  n += vsnprintf(buf + n, sizeof(buf) - n, fmt, ap);
+  va_end(ap);
+  fflush(stderr);
+  if (write(2, buf, std::min<size_t>((size_t)n, sizeof(buf) - 1)) < 0) return;
+}
+
+// How a rank's share went through its device, for its log line: "resident", or "in <c> chunks, <p> passes in <t> ms"
+std::string share_form(const StreamStats &st) {
+  if (!st.chunks) return "resident";
+  char buf[96];
+  snprintf(buf, sizeof(buf), "in %llu chunks, %llu passes in %.1f ms", (unsigned long long)st.chunks,
+           (unsigned long long)st.passes, st.pass_ms);
+  return buf;
+}
+
 // Rank 0: the loads of a stage's plan - the records of the largest owner, leading byte and bucket - from which a
 // round cap can be chosen, as "<label>: largest owner ..., largest leading byte ..., largest bucket ..."
 void log_loads(const Exchange &X, const OwnerExchange &ex, const char *label) {
@@ -408,6 +433,29 @@ uint64_t count_round_budget(int rank, int world, uint64_t n_total, uint32_t k, i
   return cap;
 }
 
+// A small read library in host memory (an image of n reads and its index) to the device, for the mercy kernels: bufs[0]
+// the image, bufs[1] / bufs[2] the read and edge offsets of variable-length reads
+mhb_dev_reads upload_reads(const std::vector<uint32_t> &img, uint64_t n, const ReadLibIndex &ix, DevBuf *bufs,
+                           const char *what) {
+  mhb_dev_reads v;
+  memset(&v, 0, sizeof(v));
+  CKL(bufs[0].alloc((img.size() + 16) * 4, what));
+  if (!img.empty()) CKC(cudaMemcpy(bufs[0].p, img.data(), img.size() * 4, cudaMemcpyHostToDevice));
+  v.bin = bufs[0].as<uint32_t>();
+  v.bin_words = img.size();
+  v.n_reads = n;
+  v.fixed_len = ix.fixed_len;
+  if (!ix.fixed_len) {
+    for (int j = 1; j < 3; ++j) {
+      CKL(bufs[j].alloc((n + 1) * 8, what));
+      CKC(cudaMemcpy(bufs[j].p, (j == 1 ? ix.rec_off : ix.unit_off).data(), (n + 1) * 8, cudaMemcpyHostToDevice));
+    }
+    v.rec_off = bufs[1].as<uint64_t>();
+    v.edge_off = bufs[2].as<uint64_t>();
+  }
+  return v;
+}
+
 struct CountRank {
   const Job &J;
   Exchange &X;
@@ -415,8 +463,9 @@ struct CountRank {
   const uint32_t k, WR, WE;
   const int32_t m;
   const uint64_t r0, nr, w0;  // my share of the reads, and its first image word
-  mhb_dev_reads reads;        // ... on the device
-  DevBuf bin, roff, eoff, mul, ns;
+  ReadLibIndex six;           // its index, rebased to the share
+  std::optional<ChunkStream> rs;  // ... resident on the device or streamed from the inherited host image
+  DevBuf lib, mul, ns;        // lib: the stream's device memory
   uint8_t owner[256];         // the count's owner of every leading byte, which also answers the mercy searches
   int R = 1;
   uint64_t n_sent = 0, n_own = 0;
@@ -433,38 +482,61 @@ struct CountRank {
         m(J_.m), r0(J_.first[X_.rank]), nr(J_.first[X_.rank + 1] - r0), w0(J_.ix->word_of(r0)) {}
   const uint32_t *read_at(uint64_t i) const { return J.bin + J.ix->word_of(r0 + i); }  // my read i, at its length word
 
-  // my share to the device: the image slice and, for variable-length reads, its rebased offsets
+  // My share as a chunk stream over the inherited host image (J.bin + w0, for variable-length reads with offsets
+  // rebased to the share): resident when it fits, next to the mercy marks and the smallest count round, in what this
+  // rank may use (mhb_read_stream_decide, the rule of the single-GPU count); otherwise, or when mhb_set_read_chunk_limit
+  // is set, streamed through the device in chunks that end on read boundaries.  Every pass over my reads goes through it.
   void load() {
     const ReadLibIndex &ix = *J.ix;
     const uint64_t nw = ix.word_of(r0 + nr) - w0;
-    CKL(bin.alloc((nw + 16) * 4, "count: reads"));
-    if (nw) CKC(cudaMemcpy(bin.p, J.bin + w0, nw * 4, cudaMemcpyHostToDevice));
-    memset(&reads, 0, sizeof(reads));
-    reads.bin = bin.as<uint32_t>();
-    reads.bin_words = nw;
-    reads.n_reads = nr;
-    reads.fixed_len = ix.fixed_len;
+    six.fixed_len = ix.fixed_len;
+    six.n_units = ix.fixed_len > k ? nr * (ix.fixed_len - k) : 0;
     if (!ix.fixed_len) {
-      std::vector<uint64_t> ro(nr + 1), eo(nr + 1);
+      six.rec_off.resize(nr + 1);
+      six.unit_off.resize(nr + 1);
       for (uint64_t i = 0; i <= nr; ++i) {
-        ro[i] = ix.rec_off[r0 + i] - w0;
-        eo[i] = ix.unit_off[r0 + i] - ix.unit_off[r0];
+        six.rec_off[i] = ix.rec_off[r0 + i] - w0;
+        six.unit_off[i] = ix.unit_off[r0 + i] - ix.unit_off[r0];
       }
-      CKL(roff.alloc((nr + 1) * 8, "count: read offsets"));
-      CKL(eoff.alloc((nr + 1) * 8, "count: edge offsets"));
-      CKC(cudaMemcpy(roff.p, ro.data(), (nr + 1) * 8, cudaMemcpyHostToDevice));
-      CKC(cudaMemcpy(eoff.p, eo.data(), (nr + 1) * 8, cudaMemcpyHostToDevice));
-      reads.rec_off = roff.as<uint64_t>();
-      reads.edge_off = eoff.as<uint64_t>();
+      six.n_units = six.unit_off[nr];
     }
+    X.barrier();  // every rank has its context: nobody allocates until the free memory is read
+    const size_t avail = rank_round_bytes(r, W);
+    X.barrier();
+    const size_t share = ChunkStream::image_bytes(nw) + (ix.fixed_len ? 0 : 2 * ChunkStream::side_bytes(nr, 0));
+    const size_t marks = 2 * pad256((nr + 1) * 4) + pad256((nr + 1) * 8);  // first, last, candidates: either form
+    const size_t smallest = ((size_t)64 << 20) + round_bytes(1, WR, WE, m, k);  // as count_round_budget plans it
+    const bool stream = mhb_read_stream_decide(share + marks + smallest, avail, 0, read_chunk_limit()) != 0;
+    read_stream_stats_reset();
+    rs.emplace();
+    CKL(init_read_stream(&*rs, J.bin + w0, nw, nr, six,
+                         stream ? (read_chunk_limit() ? read_chunk_limit() : read_chunk_auto_bytes()) : 0));
+    CKL(lib.alloc(rs->device_bytes(), stream ? "count: read chunk buffers" : "count: reads"));
+    CKL(rs->bind(lib.p, nullptr));
     CKL(mul.alloc(65536 * 8, "count: multiplicity histogram"));
     CKL(ns.alloc(8 * 8, "count: counters"));
     CKC(cudaMemset(mul.p, 0, 65536 * 8));
     CKC(cudaMemset(ns.p, 0, 64));
   }
 
+  // one pass over my share: fn(a chunk as a read library, the share's index of its first read), once per chunk
+  void each_chunk(const std::function<int(const mhb_dev_reads &, uint64_t)> &fn) {
+    CKL(rs->pass(nullptr, [&](const ChunkView &c) {
+      mhb_dev_reads v;
+      v.bin = c.words;
+      v.bin_words = c.n_words;
+      v.n_reads = c.n;
+      v.fixed_len = six.fixed_len;
+      v.rec_off = c.at<uint64_t>(0);
+      v.edge_off = c.at<uint64_t>(1);
+      return fn(v, c.first);
+    }));
+  }
+
   // The count rounds: my records of the round straight into their owners, then every owner counts what it received.
-  // The plan caps every owner at its round budget.
+  // The plan caps every owner at its round budget.  The histogram and every round are one pass over my share: the
+  // route's cursors keep counting across the launches of a round, and the owner counts the same multiset of records
+  // whatever the chunks.
   void count_rounds() {
     OwnerExchange ex;
     {
@@ -472,8 +544,10 @@ struct CountRank {
       DevBuf h16;
       CKL(h16.alloc(65536 * 8, "count: bucket histogram"));
       CKC(cudaMemset(h16.p, 0, 65536 * 8));
-      CKL(mhb_count_extract_owners(nullptr, &reads, k, h16.as<uint64_t>(), nullptr, nullptr, nullptr, nullptr, nullptr,
-                                   nullptr));
+      each_chunk([&](const mhb_dev_reads &v, uint64_t) {
+        return mhb_count_extract_owners(nullptr, &v, k, h16.as<uint64_t>(), nullptr, nullptr, nullptr, nullptr, nullptr,
+                                        nullptr);
+      });
       CKC(cudaMemcpy(h.data(), h16.p, 65536 * 8, cudaMemcpyDeviceToHost));
       h16.release();
       ex.gather(X, h.data(), 65536);  // ... behind which every share is on its device: what is left the rounds may take
@@ -499,7 +573,9 @@ struct CountRank {
       uint64_t *d_ns = ns.as<uint64_t>();
       for (int t = 0; t < R; ++t) {
         ex.send(X, t, "count records", [&](const OwnerRoute &rt) {
-          CKL(mhb_count_extract_owners(nullptr, &reads, k, nullptr, rt.owner, rt.base, rt.cursor, rt.cap, rt.lo, rt.hi));
+          each_chunk([&](const mhb_dev_reads &v, uint64_t) {
+            return mhb_count_extract_owners(nullptr, &v, k, nullptr, rt.owner, rt.base, rt.cursor, rt.cap, rt.lo, rt.hi);
+          });
         });
         const uint64_t n_t = ex.own[t];
         uint64_t s_t = 0;
@@ -591,22 +667,24 @@ struct CountRank {
       const size_t tb = mhb_tipset_bytes(n_tip_all, k);
       CKL(tipset.alloc(tb, "count: tip set"));
       CKL(mhb_tipset_build(nullptr, d_te.as<uint32_t>(), d_ta.as<uint8_t>(), n_tip_all, k, tipset.p, tb, n_tip_all));
-      CKL(mhb_count_mark_mercy(nullptr, &reads, k, tipset.p, tb, n_tip_all, first.as<uint32_t>(), last.as<uint32_t>()));
+      each_chunk([&](const mhb_dev_reads &v, uint64_t c0) {  // every chunk marks its reads at its first read
+        return mhb_count_mark_mercy(nullptr, &v, k, tipset.p, tb, n_tip_all, first.as<uint32_t>() + c0,
+                                    last.as<uint32_t>() + c0);
+      });
       const size_t csb = mhb_mercy_candidates_scratch_bytes(nr);
       CKL(cs.alloc(csb, "count: candidate scratch"));
       CKL(mhb_mercy_candidates(nullptr, first.as<uint32_t>(), last.as<uint32_t>(), nr, d_cand, &n_cand, cs.p, csb));
     }
     cand_ids.resize(n_cand);
     if (n_cand) CKC(cudaMemcpy(cand_ids.data(), d_cand, n_cand * 8, cudaMemcpyDeviceToHost));
-    {  // number of reads with both marks set (the "(%d)" of the reference's log line) + my candidate reads as their
-       // image words (length word + payload)
+    std::vector<uint32_t> cr;  // my candidate reads as their image words (length word + payload), in read order
+    {  // number of reads with both marks set (the "(%d)" of the reference's log line) + my candidate reads
       std::vector<uint32_t> f(nr), l(nr);
       if (nr) {
         CKC(cudaMemcpy(f.data(), first.p, nr * 4, cudaMemcpyDeviceToHost));
         CKC(cudaMemcpy(l.data(), last.p, nr * 4, cudaMemcpyDeviceToHost));
       }
       for (uint64_t i = 0; i < nr; ++i) has_tips += f[i] != MHB_SENTINEL_OFFSET && l[i] != MHB_SENTINEL_OFFSET;
-      std::vector<uint32_t> cr;
       for (uint64_t c = 0; c < n_cand; ++c) {
         const uint32_t *rd = read_at(cand_ids[c]);
         cr.insert(cr.end(), rd, rd + 1 + div_ceil(rd[0], 16));
@@ -634,23 +712,8 @@ struct CountRank {
     uint32_t L = 0;
     for (uint64_t c = 0; c < n_cand_all; ++c) L = std::max(L, all[cix.word_of(c)]);
     {
-      DevBuf call, croff, ceoff, lut, planes;
-      CKL(call.alloc((all.size() + 16) * 4, "count: candidate reads of every rank"));
-      CKC(cudaMemcpy(call.p, all.data(), all.size() * 4, cudaMemcpyHostToDevice));
-      mhb_dev_reads greads;
-      memset(&greads, 0, sizeof(greads));
-      greads.bin = call.as<uint32_t>();
-      greads.bin_words = all.size();
-      greads.n_reads = n_cand_all;
-      greads.fixed_len = cix.fixed_len;
-      if (!cix.fixed_len) {
-        CKL(croff.alloc((n_cand_all + 1) * 8, "count: candidate read offsets"));
-        CKL(ceoff.alloc((n_cand_all + 1) * 8, "count: candidate edge offsets"));
-        CKC(cudaMemcpy(croff.p, cix.rec_off.data(), (n_cand_all + 1) * 8, cudaMemcpyHostToDevice));
-        CKC(cudaMemcpy(ceoff.p, cix.unit_off.data(), (n_cand_all + 1) * 8, cudaMemcpyHostToDevice));
-        greads.rec_off = croff.as<uint64_t>();
-        greads.edge_off = ceoff.as<uint64_t>();
-      }
+      DevBuf call[3], lut, planes;
+      const mhb_dev_reads greads = upload_reads(all, n_cand_all, cix, call, "count: candidate reads of every rank");
       CKL(lut.alloc(mhb_edge_lut_bytes(), "count: edge lookup table"));
       CKL(mhb_edge_lut_build(nullptr, d_edges, n_solid, k, lut.p));
       const size_t pw_all = mhb_mercy_planes_words(n_cand_all, L);
@@ -670,12 +733,22 @@ struct CountRank {
       const std::vector<char> v = X.fetch("planes", s, cand_off[r] * pw1 * 4, pw_mine * 4);
       memcpy(mine.data() + (size_t)s * pw_mine, v.data(), pw_mine * 4);
     }
-    DevBuf d_mine, ms;
+    // my candidates as a library of their own, the image published as "cand": candidate c is its read c, so the
+    // last steps read no more than the candidates, whether my share is resident or streamed
+    ReadLibIndex mix;
+    CKL(index_read_lib(cr.data(), cr.size(), n_cand, k, &mix, FixedCheck::kSerial));
+    DevBuf mbuf[3], d_mine, ms;
+    const mhb_dev_reads creads = upload_reads(cr, n_cand, mix, mbuf, "count: my candidate reads");
+    {
+      std::vector<uint64_t> ids(n_cand);
+      std::iota(ids.begin(), ids.end(), 0ull);
+      CKC(cudaMemcpy(d_cand, ids.data(), n_cand * 8, cudaMemcpyHostToDevice));
+    }
     CKL(d_mine.alloc(mine.size() * 4, "count: mercy answers about my candidates"));
     CKC(cudaMemcpy(d_mine.p, mine.data(), mine.size() * 4, cudaMemcpyHostToDevice));
     const size_t msb = mhb_mercy_edges_scratch_bytes(n_cand, L) - mhb_edge_lut_bytes();
     CKL(ms.alloc(msb, "count: mercy edge scratch"));
-    CKL(mhb_mercy_count_planes(nullptr, &reads, d_cand, n_cand, L, k, d_mine.as<uint32_t>(), (uint32_t)W, pw_mine, &n_mercy,
+    CKL(mhb_mercy_count_planes(nullptr, &creads, d_cand, n_cand, L, k, d_mine.as<uint32_t>(), (uint32_t)W, pw_mine, &n_mercy,
                                ms.p, msb));
     if (!n_mercy) return;
     if (n_solid + n_mercy > cap_all) {  // reads overlapping only at their ends: more mercy than solid edges
@@ -683,14 +756,14 @@ struct CountRank {
       CKC(cudaMemcpy(big.p, d_edges, n_solid * WE * 4, cudaMemcpyDeviceToDevice));
       all_edges = big.as<uint32_t>();
     }
-    CKL(mhb_mercy_edges_write(nullptr, &reads, d_cand, n_cand, L, k, all_edges + n_solid * WE, n_mercy, n_mercy, ms.p, msb));
+    CKL(mhb_mercy_edges_write(nullptr, &creads, d_cand, n_cand, L, k, all_edges + n_solid * WE, n_mercy, n_mercy, ms.p, msb));
     CKC(cudaDeviceSynchronize());
   }
 
-  // mercy() was the last reader of my share on the device; files() reads the host image
+  // the marks were the last pass over my share: its stream goes; files() reads the host image
   void release_share() {
-    for (DevBuf *b : {&bin, &roff, &eoff}) b->release();
-    memset(&reads, 0, sizeof(reads));
+    rs.reset();
+    lib.release();
   }
 
   // The SdBG stage over solid + mercy edges, in rounds over bucket ranges when an owner's items do not fit its device
@@ -730,11 +803,14 @@ struct CountRank {
         CKL(mhb_s2s_extract_owners_round(nullptr, &seqs, k, n_seqs * 6, rt.owner, rt.base, rt.cursor, rt.cap, rt.lo,
                                          rt.hi));
     });
-    XINFO("rank %d: %llu reads, %llu records sent, %llu owned in %d round%s, %llu solid edges, %llu SdBG items owned in "
-          "%d round%s; peak device memory %.1f MiB\n",
-          r, (unsigned long long)nr, (unsigned long long)n_sent, (unsigned long long)n_own, R, R > 1 ? "s" : "",
-          (unsigned long long)n_solid, (unsigned long long)n_sdbg_own, R_sdbg, R_sdbg > 1 ? "s" : "",
-          DevBuf::peak_bytes() / 1048576.0);
+    StreamStats st;
+    mhb_read_stream_stats(&st.chunks, &st.passes, &st.h2d_bytes);
+    mhb_read_stream_times(nullptr, nullptr, nullptr, &st.pass_ms);
+    RANK_INFO("rank %d: %llu reads, %llu records sent, %llu owned in %d round%s, %llu solid edges, %llu SdBG items owned "
+              "in %d round%s; reads %s; peak device memory %.1f MiB\n",
+              r, (unsigned long long)nr, (unsigned long long)n_sent, (unsigned long long)n_own, R, R > 1 ? "s" : "",
+              (unsigned long long)n_solid, (unsigned long long)n_sdbg_own, R_sdbg, R_sdbg > 1 ? "s" : "",
+              share_form(st).c_str(), DevBuf::peak_bytes() / 1048576.0);
   }
 
   // The files: my bucket range of the edges; rank 0 merges the tables and writes the library-wide files
@@ -812,54 +888,83 @@ void s2s_worker(const SeqJob &J, Exchange &X) {
   const uint32_t k = J.k;
   bind_device(r, W);
 
-  // ---- my share to the device ----
+  // ---- my share as a chunk stream over the inherited sequences: their words and, rebased to the share (and by the
+  // stream to each chunk), word offsets, item offsets, lengths and multiplicities.  Resident when it fits, next to the
+  // smallest SdBG round, in what this rank may use (mhb_read_stream_decide); otherwise, or when mhb_set_s2s_chunk_limit
+  // is set, streamed through the device in chunks that end on sequence boundaries ----
   const HostSeqs &S = *J.seqs;
   const uint64_t s0 = J.first[r], n = J.first[r + 1] - s0, w0 = S.word_off[s0], nw = S.word_off[s0 + n] - w0;
   std::vector<uint64_t> wo(n + 1), io(n + 1, 0);
   for (uint64_t i = 0; i <= n; ++i) wo[i] = S.word_off[s0 + i] - w0;
   for (uint64_t i = 0; i < n; ++i) io[i + 1] = io[i] + seq_items(S.len[s0 + i], k);
   const uint64_t n_items = io[n];
-  DevBuf words, d_wo, d_io, len, mult;
-  CKL(words.alloc((nw + 16) * 4, "seq2sdbg: sequences"));
-  CKL(d_wo.alloc((n + 1) * 8, "seq2sdbg: word offsets"));
-  CKL(d_io.alloc((n + 1) * 8, "seq2sdbg: item offsets"));
-  CKL(len.alloc((n + 1) * 4, "seq2sdbg: lengths"));
-  CKL(mult.alloc((n + 1) * 2, "seq2sdbg: multiplicities"));
-  if (nw) CKC(cudaMemcpy(words.p, S.words.data() + w0, nw * 4, cudaMemcpyHostToDevice));
-  CKC(cudaMemcpy(d_wo.p, wo.data(), (n + 1) * 8, cudaMemcpyHostToDevice));
-  CKC(cudaMemcpy(d_io.p, io.data(), (n + 1) * 8, cudaMemcpyHostToDevice));
-  if (n) {
-    CKC(cudaMemcpy(len.p, S.len.data() + s0, n * 4, cudaMemcpyHostToDevice));
-    CKC(cudaMemcpy(mult.p, S.mult.data() + s0, n * 2, cudaMemcpyHostToDevice));
-  }
-  mhb_dev_seqs seqs;
-  memset(&seqs, 0, sizeof(seqs));
-  seqs.words = words.as<uint32_t>();
-  seqs.n_words = nw;
-  seqs.n_seqs = n;
-  seqs.word_off = d_wo.as<uint64_t>();
-  seqs.len = len.as<uint32_t>();
-  seqs.item_off = d_io.as<uint64_t>();
-  seqs.mult = mult.as<uint16_t>();
-
-  // ---- bucket histogram of my items -> the plan; per round, every item of the round's bucket ranges straight into its
-  // owner's buffer (my share stays on the device until the last round: every round extracts from it again) ----
-  std::vector<uint64_t> h(65536);
+  ChunkStream::Input in;
+  in.image = S.words.data() + w0;
+  in.words = nw;
+  in.n = n;
+  in.word_off = wo.data();
+  in.side[0] = {wo.data(), 0};
+  in.side[1] = {io.data(), 0};
+  in.side[2] = {S.len.data() + s0, 4};
+  in.side[3] = {S.mult.data() + s0, 2};
+  X.barrier();  // every rank has its context: nobody allocates until the free memory is read
+  const size_t avail = rank_round_bytes(r, W);
+  X.barrier();
+  const size_t share = ChunkStream::image_bytes(nw) + 2 * ChunkStream::side_bytes(n, 0) + ChunkStream::side_bytes(n, 4) +
+                       ChunkStream::side_bytes(n, 2);
+  const size_t fixed = (size_t)64 << 20;  // as sdbg_stage plans its rounds
+  const int no_round = mhb_sdbg_round_budget(avail, share + fixed, k, 1) == 0;
+  const bool stream = mhb_read_stream_decide(share, avail, no_round, s2s_chunk_limit()) != 0;
+  std::vector<uint64_t> first;  // a sequence costs its words, two offsets, its length and its multiplicity
+  if (stream)
+    plan_chunks(wo.data(), 0, 8 + 8 + 4 + 2, n, s2s_chunk_limit() ? s2s_chunk_limit() : read_chunk_auto_bytes(), &first);
+  StreamStats st;
+  DevBuf dev;
   {
-    DevBuf h16;
-    CKL(h16.alloc(65536 * 8, "seq2sdbg: bucket histogram"));
-    CKC(cudaMemset(h16.p, 0, 65536 * 8));
-    CKL(mhb_s2s_bucket_hist(nullptr, &seqs, k, n_items, h16.as<uint64_t>()));
-    CKC(cudaMemcpy(h.data(), h16.p, 65536 * 8, cudaMemcpyDeviceToHost));
+    ChunkStream cs;
+    CKL(cs.init(in, std::move(first), &st));
+    CKL(dev.alloc(cs.device_bytes(), stream ? "seq2sdbg: sequence chunk buffers" : "seq2sdbg: sequences"));
+    CKL(cs.bind(dev.p, nullptr));
+    // one pass over my share: fn(a chunk as a sequence set, its items), once per chunk
+    auto each_chunk = [&](const std::function<int(const mhb_dev_seqs &, uint64_t)> &fn) {
+      CKL(cs.pass(nullptr, [&](const ChunkView &c) {
+        mhb_dev_seqs v;
+        memset(&v, 0, sizeof(v));
+        v.words = c.words;
+        v.n_words = c.n_words;
+        v.n_seqs = c.n;
+        v.word_off = c.at<uint64_t>(0);
+        v.item_off = c.at<uint64_t>(1);
+        v.len = c.at<uint32_t>(2);
+        v.mult = c.at<uint16_t>(3);
+        return fn(v, io[c.first + c.n] - io[c.first]);
+      }));
+    };
+
+    // ---- bucket histogram of my items -> the plan; per round, every item of the round's bucket ranges straight into
+    // its owner's buffer, one pass over my share (it stays on the device, or in host memory, until the last round:
+    // every round extracts from it again) ----
+    std::vector<uint64_t> h(65536);
+    {
+      DevBuf h16;
+      CKL(h16.alloc(65536 * 8, "seq2sdbg: bucket histogram"));
+      CKC(cudaMemset(h16.p, 0, 65536 * 8));
+      each_chunk([&](const mhb_dev_seqs &v, uint64_t n_v) {
+        return mhb_s2s_bucket_hist(nullptr, &v, k, n_v, h16.as<uint64_t>());
+      });
+      CKC(cudaMemcpy(h.data(), h16.p, 65536 * 8, cudaMemcpyDeviceToHost));
+    }
+    uint64_t n_own = 0;
+    const int R = sdbg_stage(X, h.data(), k, J.prefix, &n_own, [&](const OwnerRoute &rt) {
+      each_chunk([&](const mhb_dev_seqs &v, uint64_t n_v) {
+        return mhb_s2s_extract_owners_round(nullptr, &v, k, n_v, rt.owner, rt.base, rt.cursor, rt.cap, rt.lo, rt.hi);
+      });
+    });
+    RANK_INFO("rank %d: %llu sequences, %llu items sent, %llu owned in %d round%s; sequences %s; peak device memory "
+              "%.1f MiB\n", r, (unsigned long long)n, (unsigned long long)n_items, (unsigned long long)n_own, R,
+              R > 1 ? "s" : "", share_form(st).c_str(), DevBuf::peak_bytes() / 1048576.0);
   }
-  uint64_t n_own = 0;
-  const int R = sdbg_stage(X, h.data(), k, J.prefix, &n_own, [&](const OwnerRoute &rt) {
-    CKL(mhb_s2s_extract_owners_round(nullptr, &seqs, k, n_items, rt.owner, rt.base, rt.cursor, rt.cap, rt.lo, rt.hi));
-  });
-  for (DevBuf *b : {&words, &d_wo, &d_io, &len, &mult}) b->release();
-  XINFO("rank %d: %llu sequences, %llu items sent, %llu owned in %d round%s; peak device memory %.1f MiB\n", r,
-        (unsigned long long)n, (unsigned long long)n_items, (unsigned long long)n_own, R, R > 1 ? "s" : "",
-        DevBuf::peak_bytes() / 1048576.0);
+  dev.release();
   X.barrier();
   if (r == 0) sdbg_merge_info(X, k, J.prefix);
   X.barrier();
